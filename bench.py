@@ -8,6 +8,7 @@ L2O-DM (LSTM-20x2, identity preprocess) on separable Rastrigin, 1M coordinates P
 unroll T=100.  Synthetic data, random-init weights (seeded).
 
   python bench.py --gpus 1 --steps 5 --warmup 3
+  python bench.py --gpus 1 --steps 5 --warmup 3 --dump-outputs out/   # + the last timed step's outputs as .npy
   torchrun --nproc-per-node N ... bench.py --gpus N ...
   python bench.py --impl reference ...     # the CPU oracle (port of the reference's algorithm) on host cores
 """
@@ -30,6 +31,12 @@ import torch  # noqa: E402
 FLOP_PER_UPDATE_INFER = {"dm_identity": 9800.0, "dm_logsign": 9960.0, "rnnprop": 12920.0}  # SURVEY.md 8(d)
 C_SF_BYTES = 320  # LSTM-20x2 checkpoint row per coordinate-update
 METRIC = "coordinate-updates/sec (N_params x unroll_steps)"
+# Roofline denominators: NVIDIA's H100 SXM data sheet (dense, for a card allowed 700 W).  They are not measured here; a
+# card run at a lower power limit (reported under "clocks") sustains less than these.
+PEAK_HBM_GBS = 3350.0
+PEAK_BF16_TFLOPS = 989.0
+PEAK_SOURCE = "NVIDIA H100 SXM data sheet (dense, 700 W), not measured"
+DUMP_LIMIT_BYTES = 64 << 20   # --dump-outputs: total size cap; larger outputs are dumped as a fixed, seeded sample
 
 
 def parse():
@@ -49,7 +56,46 @@ def parse():
                     help="coordinates of the CPU-oracle sample (0 = best of the workload's default sample sizes)")
     ap.add_argument("--scaling", default="weak", choices=["weak", "strong"],
                     help="weak: --coords per GPU (default 1M each); strong: --coords in TOTAL (default 1M) sharded over the ranks")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the timed path computed in its last step as DIR/<name>.npy "
+                         "(rank 0; inputs are seeded, so two builds can be compared output for output)")
     return ap.parse_args()
+
+
+def _sample(t, limit_elems):
+    """t flattened, or a fixed, seeded sample of limit_elems of its elements (sorted indices) when it is larger."""
+    flat = t.detach().reshape(-1)
+    if flat.numel() <= limit_elems:
+        return flat
+    idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:limit_elems].sort().values
+    return flat[idx.to(flat.device)]
+
+
+def dump_outputs(path, arrays):
+    """Write each array as path/<name>.npy in float32 (float64 stays float64); at most DUMP_LIMIT_BYTES in all."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    total = 0
+    for name, t in arrays.items():
+        a = t.detach().cpu().numpy() if torch.is_tensor(t) else np.asarray(t)
+        a = a.astype(np.float64 if a.dtype == np.float64 else np.float32, copy=False)
+        total += a.nbytes
+        if total > DUMP_LIMIT_BYTES:
+            raise SystemExit("--dump-outputs: %s would exceed %d bytes" % (name, DUMP_LIMIT_BYTES))
+        np.save(os.path.join(path, name + ".npy"), a)
+
+
+def program_outputs(prog):
+    """What Session.run([fx, update, step]) computed in its last call: the fx trajectory of the unroll (fx[T] is the
+    value returned), the updated optimizee parameters, and per optimizer net its weights after the meta-step, the
+    meta-gradient, and per run the carried LSTM state (samples when larger than 4M / 2M elements)."""
+    out = {"fx": prog.last_fx.double(), "x": _sample(prog.X, 4 << 20)}
+    for k, net in prog.nets.items():
+        out["theta_" + k] = net.theta
+        out["dtheta_" + k] = prog.dtheta[k]
+    for i, r in enumerate(prog.runs):
+        out["state_%d" % i] = _sample(r.state, 2 << 20)
+    return out
 
 
 # ------------------------------------------------------------------------------------------------
@@ -102,8 +148,10 @@ def make_problem(name, coords, rank, shard=None):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clock / throttle-reason sampler (B200_PROFILING.md): one streaming `nvidia-smi -lms` process; only
-    samples whose arrival time falls inside [t_begin, t_end] of the timed region are summarised."""
+    """Read-only nvidia-smi sampler of the card's name, power limit, SM clock and clock-event reasons: one streaming
+    `nvidia-smi -lms` query process, terminated by stop(); only samples whose arrival time falls inside
+    [t_begin, t_end] of the timed region are summarised.  An absolute rate means little without the card and its power
+    limit, so both go into the JSON line."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -112,13 +160,13 @@ class ClockSampler(threading.Thread):
 
     def run(self):
         q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
-             "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+             "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit,name")
         try:
             self.proc = subprocess.Popen(["nvidia-smi", "-i", str(self.index), "--query-gpu=" + q,
                                           "--format=csv,noheader,nounits", "-lms", "50"], stdout=subprocess.PIPE, text=True)
             for line in self.proc.stdout:
                 parts = [p.strip() for p in line.strip().split(",")]
-                if len(parts) >= 6:
+                if len(parts) >= 8:
                     self.samples.append((time.perf_counter(), parts))
         except Exception:
             pass
@@ -127,38 +175,35 @@ class ClockSampler(threading.Thread):
         if self.proc is not None:
             try:
                 self.proc.terminate()
+                self.proc.wait(timeout=10)
             except Exception:
-                pass
+                self.proc.kill()
 
     def summary(self):
         inside = [p for (ts, p) in self.samples if self.t_begin is not None and self.t_begin <= ts <= self.t_end]
         use = inside if inside else [p for (_, p) in self.samples]
         if not use:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["unsampled"]}
+            return {"gpu": torch.cuda.get_device_name(self.index), "power_limit_w": None, "sm_mhz": None,
+                    "sm_max_mhz": None, "reasons": ["unsampled"]}
         sm = sorted(int(float(s[0])) for s in use)
         reasons = set()
         for s in use:
             for name, val in zip(["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"], s[2:6]):
                 if val.lower().startswith("active"):
                     reasons.add(name)
-        return {"sm_mhz": sm[len(sm) // 2], "sm_max_mhz": int(float(use[0][1])), "reasons": sorted(reasons),
-                "samples": len(sm), "samples_in_timed_region": len(inside)}
-
-
-def _peaks():
-    try:
-        return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        return {}
+        try:
+            plim = float(use[0][6])
+        except ValueError:
+            plim = None
+        return {"gpu": use[0][7], "power_limit_w": plim, "sm_mhz": sm[len(sm) // 2], "sm_max_mhz": int(float(use[0][1])),
+                "reasons": sorted(reasons), "samples": len(sm), "samples_in_timed_region": len(inside)}
 
 
 def external_roofline(prog, netkind, T, t_unroll):
     """HBM roofline of the step-at-a-time (external-gradient) regime, SURVEY.md 8(d): one `l2o_step` launch moves
     652 B (668 B RNNProp) per coordinate; the BPTT sweep re-reads 328 B.  The step kernel and the BPTT kernel are timed
     ALONE here with CUDA events on this workload's own buffers (inside the captured graph they cannot be bracketed)."""
-    from open_l2o_b200 import engine as eng
-    peaks = _peaks()
-    peak = float(peaks.get("hbm_gbs", 6500.0))
+    peak = PEAK_HBM_GBS
     r = prog.runs[0]
     h = r.net.handle
     n = r.n
@@ -193,17 +238,9 @@ def external_roofline(prog, netkind, T, t_unroll):
     t_bwd = timed(lambda: h.unroll_bwd(r.net.theta, n, T, in_seq, r.ckpt, dth, g_rec=r.g_rec, **prog._bwd_extra(r)), 3)
     sb, bb = STEP_BYTES[netkind], BWD_BYTES[netkind]
     ach = sb * n / t_step / 1e9
-    step_traffic = None   # measured DRAM bytes of one l2o_step launch (ncu --set full capture of the DM step kernel)
-    if netkind != "rnnprop":
-        try:
-            tj = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-            step_traffic = tj["step_dram_bytes_per_coord_update"] * n
-        except Exception:
-            pass
     ws = (T + 1) * slot * 4
     return {"bound": "hbm", "kernel": "l2o_step (one coordinate-wise LSTM step, state in HBM)", "achieved": ach,
-            "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": step_traffic,
-            "algorithmic_bytes_per_coord_update": sb, "step_us": 1e6 * t_step, "coord_updates_per_s_step_kernel": n / t_step,
+            "peak": peak, "unit": "GB/s", "frac": ach / peak, "algorithmic_bytes_per_coord_update": sb, "step_us": 1e6 * t_step, "coord_updates_per_s_step_kernel": n / t_step,
             "bptt": {"kernel": "l2o_unroll_bwd over the T checkpoint slots", "ms": 1e3 * t_bwd,
                      "algorithmic_bytes_per_coord_update": bb, "achieved": bb * n * T / t_bwd / 1e9,
                      "frac": bb * n * T / t_bwd / 1e9 / peak, "coord_updates_per_s": n * T / t_bwd},
@@ -211,8 +248,7 @@ def external_roofline(prog, netkind, T, t_unroll):
                              "achieved": (sb + bb) * n * T / t_unroll / 1e9,
                              "frac": (sb + bb) * n * T / t_unroll / 1e9 / peak,
                              "note": "whole unroll incl. the optimizee's own forward/backward (torch autograd) and Adam"},
-            "working_set_bytes": ws, "l2_resident": bool(ws < 126e6),
-            "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback 6.5 TB/s (B200_PROFILING.md)"}
+            "working_set_bytes": ws, "l2_resident": bool(ws < 50e6), "peak_source": PEAK_SOURCE}
 
 
 def quick_measure(workload, steps, warmup, with_cpu=True):
@@ -268,10 +304,11 @@ def quick_measure(workload, steps, warmup, with_cpu=True):
     return out
 
 
-def quick_measure_hrnn(steps, warmup, T=20, batch=128):
+def quick_measure_hrnn(steps, warmup, T=20, batch=128, dump=None):
     """BASELINE config #4: L2O-Scale HierarchicalRNN [10,20,20] optimizing a ConvNet on CIFAR-shaped synthetic data
     (354,218 coordinates, unroll 20; inference path = the update step; SURVEY.md 8(f) row 1).  Also times the
-    step's three kernels alone on a large synthetic state for the HBM roofline of the per-coordinate kernel."""
+    step's three kernels alone on a large synthetic state for the HBM roofline of the per-coordinate kernel.
+    dump: directory for --dump-outputs (the last timed unroll's loss and ConvNet parameters)."""
     from open_l2o_b200 import engine as eng, hierarchical_rnn as hr
     from open_l2o_b200.scale_problems import ConvNet
     dev = torch.device("cuda", torch.cuda.current_device())
@@ -300,6 +337,9 @@ def quick_measure_hrnn(steps, warmup, T=20, batch=128):
     t = e0.elapsed_time(e1) / 1e3
     n = opt.N
     launches = int(eng.launch_count() - l0)
+    if dump:
+        dump_outputs(dump, {"loss": torch.as_tensor([float(loss)], dtype=torch.float64),
+                            "params": torch.cat([p.detach().reshape(-1) for p in params])})
     # the optimizer step alone (3 launches), same state
     e0.record()
     for _ in range(steps * T):
@@ -333,7 +373,7 @@ def quick_measure_hrnn(steps, warmup, T=20, batch=128):
         t_mt = e0.elapsed_time(e1) / 1e3 / reps
         out["meta_train"] = {"ms_per_meta_step": 1e3 * t_mt, "coordinate_updates_per_s": n * T / t_mt,
                              "meta_objective": float(meta),
-                             "what": "one unroll of T steps forward (tcgen05 step kernel) + BPTT (l2o_hrnn_coord_bwd, per-tensor "
+                             "what": "one unroll of T steps forward (tensor-core step kernel) + BPTT (l2o_hrnn_coord_bwd, per-tensor "
                                      "pieces by torch autograd) + RMSProp on the 8,349 optimizer weights; eager, no CUDA graph"}
         del tr
     except Exception as ex:   # reported, never fatal for the headline line
@@ -357,18 +397,12 @@ def quick_measure_hrnn(steps, warmup, T=20, batch=128):
     t_big = e0.elapsed_time(e1) / 1e3 / reps
     nbig = opt2.N
     bytes_per = 192.0   # coord kernel 88 B read + 88 B written, apply kernel 16 B (DESIGN.md 3.4)
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    peak = float(peaks.get("hbm_gbs", 6500.0))
+    peak = PEAK_HBM_GBS
     ach = bytes_per * nbig / t_big / 1e9
     out["roofline"] = {"bound": "hbm", "kernel": "l2o::hrnn::tcg::coord_tc_kernel + tensor_kernel + apply_kernel (one l2o_hrnn_step)",
-                       "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": 174.41 * nbig,   # dram bytes of coord_tc_kernel per launch (ncu --set full, profiles/r02j_hrnn_coord_tc.raw.csv)
+                       "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
                        "coords": nbig, "ms": 1e3 * t_big, "coord_updates_per_s": nbig / t_big,
-                       "algorithmic_bytes_per_coord_update": bytes_per,
-                       "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback 6.5 TB/s"}
+                       "algorithmic_bytes_per_coord_update": bytes_per, "peak_source": PEAK_SOURCE}
     del opt2, big, g
     torch.cuda.empty_cache()
     return out
@@ -510,10 +544,12 @@ def run_reference(args):
 def main():
     args = parse()
     if args.impl == "reference":
+        if args.dump_outputs:
+            raise SystemExit("--dump-outputs dumps the GPU path; --impl reference has none")
         return run_reference(args)
     if args.workload == "hrnn_convnet":   # side workload: its own line (N=1 only)
         torch.cuda.set_device(0)
-        print(json.dumps(quick_measure_hrnn(steps=args.steps, warmup=args.warmup)))
+        print(json.dumps(quick_measure_hrnn(steps=args.steps, warmup=args.warmup, dump=args.dump_outputs)))
         return
 
     import torch.distributed as dist
@@ -595,6 +631,8 @@ def main():
     launches = eng.launch_count() - l0
     t_dev = e0.elapsed_time(e1) / 1e3
     sampler.stop()
+    if args.dump_outputs and rank == 0:   # before any later section runs the program again
+        dump_outputs(args.dump_outputs, program_outputs(prog))
     tt = torch.tensor([t_dev], dtype=torch.float64, device=dev)
     if distributed:
         dist.all_reduce(tt, op=dist.ReduceOp.MAX)
@@ -621,7 +659,7 @@ def main():
     roof = None
     if prog.fused is not None and args.workload == "rastrigin":
         fw, bw = [], []
-        for _ in range(max(2, min(args.steps, 3))):
+        for _ in range(args.steps):
             prog.fx_buf.zero_()
             xw = prog.X.clone()
             st = r.state.clone()
@@ -639,45 +677,22 @@ def main():
             fw.append(kf0.elapsed_time(kf1) / 1e3)
             bw.append(kb0.elapsed_time(kb1) / 1e3)
         t_f, t_b = sum(fw) / len(fw), sum(bw) / len(bw)
-        peaks = {}
-        try:
-            peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        except Exception:
-            pass
-        peak = float(peaks.get("bf16_tflops", 1700.0))   # burst figure: the kernels are timed alone (launch, sync)
+        peak = PEAK_BF16_TFLOPS
         fl = FLOP_PER_UPDATE_INFER[netkind]
         ach_b = 2.0 * fl * r.n * T / t_b / 1e12          # backward = two more GEMMs of the forward's shape
         ach_f = fl * r.n * T / t_f / 1e12
-        traffic, traffic_src = None, None
-        try:
-            tj = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-            traffic = tj["unroll_bwd_dram_bytes_per_coord_update"] * r.n * T
-            traffic_src = tj.get("source")
-        except Exception:
-            pass
         alg_bytes = (C_SF_BYTES + 8) * r.n * T      # checkpoint row + g_rec + in_seq per coordinate-update (read)
-        roof = {"bound": "tensor", "kernel": "tcb2::unroll_bwd2_kernel (layer-pipelined tcgen05 BPTT)", "achieved": ach_b, "peak": peak,
-                "unit": "TFLOP/s", "frac": ach_b / peak, "traffic": traffic, "traffic_source": traffic_src,
-                "algorithmic_bytes": alg_bytes,
-                "peak_source": "MEASURED_PEAKS.json bf16_tflops (burst: kernel timed alone)" if peaks else "fallback 1.7 PF (B200_PROFILING.md)",
-                "fwd_kernel": {"name": "tc::unroll_fwd_kernel (tcgen05)", "achieved": ach_f, "frac": ach_f / peak,
+        roof = {"bound": "tensor", "kernel": "tcb::unroll_bwd_kernel (wgmma BPTT)", "achieved": ach_b, "peak": peak,
+                "unit": "TFLOP/s", "frac": ach_b / peak, "algorithmic_bytes": alg_bytes,
+                "hbm_frac_of_algorithmic_bytes": alg_bytes / t_b / 1e9 / PEAK_HBM_GBS, "peak_source": PEAK_SOURCE,
+                "fwd_kernel": {"name": "tc::unroll_fwd_kernel (wgmma)", "achieved": ach_f, "frac": ach_f / peak,
                                "ms": 1e3 * t_f, "coord_updates_per_s": r.n * T / t_f},
                 "bwd_ms": 1e3 * t_b, "bwd_coord_updates_per_s": r.n * T / t_b,
                 "alg_flop_per_coord_update": {"fwd": fl, "bwd": 2 * fl},
-                "algorithmic_bytes_8d_fused": 8.0 * r.n * T,
-                "traffic_over_8d_fused": (traffic / (8.0 * r.n * T)) if traffic else None,
-                "traffic_note": "SURVEY.md 8(d) puts the fused regime at 4-8 B per coordinate-update (inference: g in, "
-                                "x out).  TRAINING by recompute must also write (forward) and read (BPTT) the "
-                                "checkpoint row: 320 B + g 4 B + net input 4 B = 328 B per coordinate-update per "
-                                "direction = `algorithmic_bytes`; the measured DRAM traffic is ~41x the 8 B figure and "
-                                "1.01x the checkpoint figure",
                 "notes": "fp32 parity => 3xTF32 for the gate recompute and dX (tf32 = 1/2 the bf16 rate: a 100%-busy tensor "
-                         "pipe reads 1/6 of this peak) and bf16 hi/lo for dW^T; ncu r02e: tensor pipe 28%, issue slots "
-                         "36%, XU 28%, warps active 31% in the BPTT kernel (profiles/r02_ncu_summary.json); the kernel is "
-                         "bound by instruction issue inside the two overlapping layer phases (130 warp-instructions per "
-                         "coordinate-update, 30% of them operand splitting) and by the serial MMA round trips of each chain; "
-                         "the activation pipe (320 MUFU ops per coordinate-update forward, 400 backward) caps the path "
-                         "near 1.4e10 upd/s/GPU"}
+                         "pipe reads 1/6 of this peak) and bf16 hi/lo for dW^T.  TRAINING by recompute writes (forward) "
+                         "and reads (BPTT) the checkpoint row: 320 B + g 4 B + net input 4 B per coordinate-update = "
+                         "`algorithmic_bytes`"}
 
     if roof is None:      # external-gradient workloads: HBM roofline of the step kernel (+ BPTT) on this workload
         roof = external_roofline(prog, netkind, T, t_dev / args.steps)
@@ -686,7 +701,7 @@ def main():
     infer = None
     if prog.fused is not None and args.workload == "rastrigin":
         ts = []
-        for _ in range(max(2, min(args.steps, 3))):
+        for _ in range(args.steps):
             xw = prog.X.clone()
             st = r.state.clone()
             kf0.record()
@@ -739,11 +754,11 @@ def main():
         also = []
         for w in ("mlp", "lasso", "rnnprop_mlp", "quadratic"):
             try:
-                also.append(quick_measure(w, steps=max(args.steps, 5), warmup=max(args.warmup, 3)))
+                also.append(quick_measure(w, steps=args.steps, warmup=args.warmup))
             except Exception as ex:  # the headline line must survive a failure of a side measurement
                 also.append({"workload": WORKLOADS[w][0], "error": repr(ex)[:200]})
         try:
-            also.append(quick_measure_hrnn(steps=max(args.steps, 5), warmup=max(args.warmup, 3)))
+            also.append(quick_measure_hrnn(steps=args.steps, warmup=args.warmup))
         except Exception as ex:
             also.append({"workload": "L2O-Scale HierarchicalRNN (BASELINE config #4)", "error": repr(ex)[:200]})
 
@@ -760,7 +775,7 @@ def main():
                            else "external-gradient (torch autograd)"),
                        "engine": args.engine, "parallelism": "dp%d (coordinates sharded)" % world,
                        "net_scale": NET_SCALE[args.workload], "theta_check": theta_check,
-                       "l2_policy": "working set (checkpoints %.1f GB/GPU) >> 126 MB L2" % (r.ckpt.numel() * 4 / 1e9),
+                       "l2_policy": "working set (checkpoints %.1f GB/GPU) >> 50 MB L2" % (r.ckpt.numel() * 4 / 1e9),
                        "last_fx": cost},
             "clocks": sampler.summary(), "e2e": e2e, "gpu_launches": int(launches), "roofline": roof,
             "cpu_baseline": cpu, "infer": infer, "also": also,

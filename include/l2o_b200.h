@@ -1,5 +1,5 @@
 /*
- * l2o_b200 — C-ABI of the B200-native coordinate-wise LSTM learned-optimizer engine.
+ * l2o_b200 — C-ABI of the H100-native (sm_90a) coordinate-wise LSTM learned-optimizer engine.
  *
  * The reference (VITA-Group/Open-L2O, L2O-DM / L2O-RNNProp) is pure Python/TensorFlow and has no
  * FFI; the seam this library sits behind is the reference's own operator surface.  Each entry point
@@ -62,7 +62,7 @@ extern "C" {
 
 #define L2O_ENGINE_AUTO 0
 #define L2O_ENGINE_FFMA 1   /* exact-fp32 CUDA-core kernels */
-#define L2O_ENGINE_TC 2     /* tcgen05 (3xTF32 error-compensated) kernels */
+#define L2O_ENGINE_TC 2     /* tensor-core wgmma (3xTF32 error-compensated) kernels */
 
 typedef struct l2o_net* l2o_handle;
 

@@ -99,8 +99,8 @@ class L2OError(RuntimeError):
     pass
 
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-std=c++17", "-O3", "-lineinfo",
-              "-I" + INCLUDE, "-I" + CSRC, "-Xcompiler", "-fPIC"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]   # H100 (Hopper); the kernels use wgmma / TMA (sm_90a only)
+NVCC_FLAGS = ARCH + ["-std=c++17", "-O3", "-lineinfo", "-I" + INCLUDE, "-I" + CSRC, "-Xcompiler", "-fPIC"]
 OBJ_DIR = os.path.join(_ROOT, "build", "obj")
 
 
@@ -114,7 +114,7 @@ def sources():
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile every CUDA translation unit in-tree for sm_100a (nvcc cross-compiles without a GPU) and link
+    """Compile every CUDA translation unit in-tree for sm_90a (nvcc cross-compiles without a GPU) and link
     ``libl2o_b200.so``.  Objects are rebuilt only when a source/header is newer."""
     from concurrent.futures import ThreadPoolExecutor
     os.makedirs(OBJ_DIR, exist_ok=True)
@@ -141,7 +141,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         rebuilt = [o for o in ex.map(compile_one, jobs) if o]
     objs = [j[1] for j in jobs]
     if rebuilt or not os.path.exists(LIB_PATH) or os.path.getmtime(LIB_PATH) < max(os.path.getmtime(o) for o in objs):
-        cmd = ["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", LIB_PATH] + objs
+        cmd = ["nvcc"] + ARCH + ["-shared", "-o", LIB_PATH] + objs
         if verbose:
             print(" ".join(cmd), file=sys.stderr)
         r = subprocess.run(cmd, capture_output=True, text=True)

@@ -46,7 +46,7 @@ __device__ __forceinline__ float sigmoid_acc(float x) { return __frcp_rn(1.0f + 
 __device__ __forceinline__ float tanh_acc(float x) { return tanhf(x); }
 __device__ __forceinline__ float elu_acc(float a) { return a > 0.f ? a : expm1f(a); }
 
-// ---- fast activations for the tcgen05 engine: branch-free, 2 MUFU each (ex2.approx 2^-22 rel, rcp.approx 1 ulp);
+// ---- fast activations for the tensor-core engine: branch-free, 2 MUFU each (ex2.approx 2^-22 rel, rcp.approx 1 ulp);
 // measured against the oracle the end-to-end error stays ~1e-6 (tests/test_tc_gpu.py) -----------------------------
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;

@@ -1,7 +1,7 @@
 // Exact-fp32 CUDA-core engine: one thread owns one coordinate; the shared [K x 4H] gate weights
 // live in shared memory and are read with warp-uniform 128-bit loads; the coordinate's (h, c)
 // state stays in registers across the whole T-step unroll.  This engine is the always-available
-// parity anchor for the tcgen05 engine (cwlstm_tc.cuh) and serves the small test-only net shapes.
+// parity anchor for the tensor-core engine (cwlstm_tc.cuh) and serves the small test-only net shapes.
 //
 // Reference semantics: DM/networks.py:207-232, DM/meta.py:319-376 (forward); SURVEY.md Appendix B
 // (backward, derived from DM/meta.py:319-376 with second_derivatives=False).

@@ -1,106 +1,68 @@
-// tcgen05 engine (sm_100a): the [coords x K] x [K x 4H] gate contraction on the 5th-gen tensor cores.
+// Tensor-core engine (sm_90a): the [coords x K] x [K x 4H] gate contractions of the LSTM-20x2 on Hopper's warpgroup
+// MMA (wgmma), forward unroll / single step.  The BPTT kernel (cwlstm_tc_bwd.cuh) shares the operand layout below.
 //
-// Design (DESIGN.md "tcgen05 engine"):
-//  * CTA = 2 tiles of 128 coordinates (8 epilogue warps, thread == coordinate == TMEM lane) + 1 warp
-//    that allocates TMEM, stages the weights and issues every tcgen05.mma (single elected thread).
-//  * A operand = the coordinate's [features | 1 | h1 | h2] row, kept IN TENSOR MEMORY (TS-mode MMA):
-//    the epilogue thread that produced h' writes it straight into its own TMEM lane with tcgen05.st,
-//    so the recurrent state never touches shared or global memory between unroll steps; the cell
-//    state c stays in registers.
-//  * B operand = gate weights in shared memory, canonical K-major no-swizzle core-matrix layout,
-//    staged ONCE per CTA by a TMA bulk copy (cp.async.bulk) of a pre-arranged image.
-//  * fp32 parity on tf32 tensor cores: error-compensated 3xTF32 -- A = Ah + Al, B = Bh + Bl with
-//    Ah/Bh exactly representable in tf32; D = Ah.Bh + Al.Bh + Ah.Bl accumulated in fp32 in TMEM.
-//    Biases ride along as a constant-1 column of A.
-//  * accumulators come back with tcgen05.ld (gate columns interleaved i,j,f,o per hidden unit so one
-//    x16 load = 4 complete units); sigmoid/tanh/c/h/output-linear/x+=delta are fused in the epilogue.
-//  * (round 2) warps of the issuer warpgroup: 16 = polling MMA issuer (split accumulators D1 | D2, K-steps whose
-//    operand columns are already final are issued one epilogue early), 17 = TMA producer of the next pair's state rows
-//    (step regime), 18 = TMA store warp (checkpoint / state rows staged in shared memory by the epilogue threads).
+// Design (DESIGN.md "tensor-core engine"):
+//  * A warpgroup (128 threads) owns a tile of 64 coordinates = the M of one wgmma.  Thread (warp w, lane l) holds the
+//    coordinates 16w + l/4 and 16w + l/4 + 8 (the rows of its accumulator fragment); the four threads of a quad
+//    (q = l % 4) split the hidden units: thread q owns units [5q, 5q + 5) of both layers.
+//  * A operand = the coordinate's [features | 1 | h1 | h2] row, kept IN REGISTERS as wgmma A fragments (register-A
+//    mode): fragment column c belongs to thread c % 4, so a 20-vector starting at column `base` stores unit 5q + s at
+//    column base + 4s + q.  The thread that produced h' writes it straight into its own fragment registers; the
+//    recurrent state never touches shared or global memory between unroll steps, the cell state c stays in registers.
+//  * B operand = gate weights in shared memory (K-major, no swizzle, 8x16-byte core matrices), staged once per CTA
+//    with one TMA bulk copy (cp.async.bulk + mbarrier) of a pre-arranged image.  Gate column order: unit 5q + s has
+//    its (i, j) pre-activations in accumulator columns 16s + 2q + {0, 1} and (f, o) in 16s + 8 + 2q + {0, 1}, i.e. in
+//    the accumulator registers of the thread that owns the unit.
+//  * fp32 parity on tf32 tensor cores: error-compensated 3xTF32 -- A = Ah + Al, B = Bh + Bl; D = Al.Bh + Ah.Bl + Ah.Bh
+//    accumulated in fp32.  Biases ride along as a constant-1 column of A.
+//  * sigmoid / tanh / c / h / output linear / x += delta are fused in the epilogue; the output layer's partial sums
+//    over the thread's 5 units are combined with two quad shuffles.
 #pragma once
 #include "cwlstm_common.cuh"
 
 namespace l2o {
 namespace tc {
 
-constexpr int kTiles = 2;                    // coordinate tiles per CTA
-constexpr int kTileCoords = 128 * kTiles;    // coordinates per CTA pass
-constexpr int kEpiThreads = 256 * kTiles;    // a thread PAIR per coordinate (hidden units 0..11 | 12..19)
-constexpr int kThreads = kEpiThreads + 128;  // + the warpgroup that holds the MMA / alloc warp (3 idle warps)
-constexpr int kFwdEpiRegs = 104, kFwdIssuerRegs = 64;  // setmaxnreg targets; 512 x 104 + 128 x 64 = the launch allocation 640 x 96 (no spare registers on the SM)
 constexpr int kH = 20;
-constexpr int kN = 4 * kH;                   // 80 gate columns
-constexpr int kXC = 4;                       // feature chunk: cols [0, kXC): features, then the constant 1
-constexpr int kColH1 = kXC;                  // A columns of h1: [4, 24)
-constexpr int kColH2 = kXC + kH;             // A columns of h2: [24, 44)
-constexpr int kACols = 48;                   // 44 used + 4 zero pad columns
-constexpr int kK1 = 24;                      // layer-1 K range: cols [0, 24) = [features | 1 | h1]
-constexpr int kK2 = 48;                      // layer-2 K range: cols [0, 48)  (feature rows zero, 1-col = b2, pad rows zero)
-constexpr int kTileCols = kN + 2 * kACols;   // default geometry without split accumulators; kernels use Geo<C>::TileCols
-constexpr int kTmemCols = 512;
-constexpr int kB1Floats = kK1 * kN;          // 1920
-constexpr int kB2Floats = kK2 * kN;          // 3840
-constexpr int kImgFloats = 2 * (kB1Floats + kB2Floats);  // forward image: B1h | B1l | B2h | B2l
-constexpr int kImgBytes = kImgFloats * 4;    // 46080
-// transposed (input-major) images for the BPTT dX contractions: T[n' = input][k' = gate], K-major
-constexpr int kT1Rows = 32, kT2Rows = 48;
-constexpr int kT1Floats = kT1Rows * kN, kT2Floats = kT2Rows * kN;
-constexpr int kImgAllFloats = kImgFloats + 2 * (kT1Floats + kT2Floats);  // + T1h | T1l | T2h | T2l
-constexpr int kImgAllBytes = kImgAllFloats * 4;  // 97280
-// Per-net geometry of the FORWARD kernel's A operand and weight image.  LSTM-20x2 with <= 3 features (identity,
-// LogAndSign): the constants above.  RNNProp (fc(2->20)+ELU, DM/networks.py:180-183,219): the feature chunk widens to
-// 24 columns [u(20) | 1 | 0 0 0], the row becomes [chunk | h1 | h2] = 64 columns; layer 1 contracts columns [0,48)
-// (the h2 units 0..3 at 44..47 meet zero weight rows) and layer 2 columns [16,64) (u16..19 meet zero rows, the
-// constant 1 at column 20 carries b2) -- both K = 48, the same trick the BPTT kernel uses for its Z2.
+constexpr int kN = 4 * kH;        // 80 gate columns
+constexpr int kTile = 64;         // coordinates per warpgroup tile (wgmma M)
+constexpr int kU = 5;             // hidden units per thread
+constexpr int kFwdWG = 3;         // warpgroups per forward CTA (they share the weight image)
+constexpr int kFwdThreads = 128 * kFwdWG;
+template <int N>
+struct IC {
+  static constexpr int value = N;
+};
+
+// Operand-row geometry.  LSTM-20x2 with <= 3 features (identity, LogAndSign): [f0..f(F-1), 1, 0.. | h1 | h2 | 0 0 0 0]
+// = 48 columns, layer 1 contracts k-blocks 0..2 (columns 0..23), layer 2 k-blocks 0..5 (the feature columns meet zero
+// rows, the constant 1 carries b2).  RNNProp (fc(2->20)+ELU, DM/networks.py:180-183,219): [u(20) | 1 0 0 0 | h1 | h2] =
+// 64 columns, layer 1 contracts columns 0..47 (h2 units in 44..47 meet zero rows), layer 2 columns 16..63 (u in 16..19
+// meet zero rows, the 1 at column 20 carries b2).  BPTT dX widths: 24 columns per 20-vector (slot 2j + e of thread q =
+// accumulator column 8j + 2q + e, slot 5 is padding); dX2 = [dh1n | dh2p], dX1 = [dh1p] (+ [de] for fc nets).
 template <class C>
 struct Geo {
   static constexpr bool FC = C::FC;
-  static constexpr int XC = FC ? 24 : kXC;
-  static constexpr int ColH1 = XC, ColH2 = XC + kH;
-  static constexpr int ACols = FC ? 64 : kACols;
-  static constexpr int K1 = FC ? 48 : kK1;
-  static constexpr int K2 = 48;
-  static constexpr int A2Off = FC ? 16 : 0;          // first A column of the layer-2 contraction
-  // Split accumulators (nets whose row fits): layer 1 accumulates in D1, layer 2 in D2, so the part of a layer's
-  // contraction whose operand columns are already final (layer 2: the h2 columns, layer 1 of the NEXT step: the h1
-  // columns) is issued one epilogue early and only 9 / 3 of the 18 / 9 MMAs stay on the step's critical path.
-  static constexpr bool SplitD = !FC;
-  static constexpr int DCols = SplitD ? 2 * kN : kN;
-  static constexpr int TileCols = DCols + 2 * ACols;  // D1 [| D2] | A_hi | A_lo
-  static constexpr int B1Floats = K1 * kN, B2Floats = K2 * kN;
-  static constexpr int ImgFloats = 2 * (B1Floats + B2Floats);
-  static constexpr int ImgBytes = ImgFloats * 4;
-  static_assert(kTiles * TileCols <= kTmemCols, "TMEM budget");
+  static constexpr int ColH1 = FC ? 24 : 4, ColH2 = FC ? 44 : 24;
+  static constexpr int ColOne = FC ? 20 : C::F;
+  static constexpr int KB = FC ? 8 : 6;                        // k-blocks of 8 columns in the operand row
+  static constexpr int L1Lo = 0, L1Hi = FC ? 6 : 3;           // layer-1 k-blocks [L1Lo, L1Hi)
+  static constexpr int L2Lo = FC ? 2 : 0, L2Hi = KB;          // layer-2 k-blocks
+  static constexpr int K1 = 8 * (L1Hi - L1Lo), K2 = 8 * (L2Hi - L2Lo);
+  static constexpr int N1 = FC ? 48 : 24, N2 = 48;
+  static constexpr int B1Floats = K1 * kN, B2Floats = K2 * kN, T1Floats = kN * N1, T2Floats = kN * N2;
+  static constexpr int FwdFloats = 2 * (B1Floats + B2Floats);                 // B1h | B1l | B2h | B2l
+  static constexpr int AllFloats = FwdFloats + 2 * (T1Floats + T2Floats);     // + T1h | T1l | T2h | T2l
   static_assert(!FC || C::F == 20, "fc preprocessing: dim 20");
+  static_assert(FC || C::F <= 3, "feature chunk: at most 3 features");
 };
-#ifdef L2O_TC_FDBG
-// progress words in host-mapped memory (scripts/tc_fwd_prof.cu, hang diagnosis): CTA 0 only
-__device__ volatile int* g_fdbg;
-#define L2O_FDBG(slot, val) do { if (blockIdx.x == 0 && g_fdbg) g_fdbg[slot] = (val); } while (0)
-#else
-#define L2O_FDBG(slot, val) do { } while (0)
-#endif
-#ifdef L2O_TC_FPROF
-// timeline instrumentation (scripts/tc_fwd_prof.cu only): clock64 stamps of CTA 0; role 0 / 1 = tile 0 half 0 / half 1
-// (warp 0 / 4, lane 0), 2 = tile 1 half 0 (warp 8), 3 = issuer (tag in the low 3 bits)
-__device__ long long g_fprof[4 * 4096];
-__device__ int g_fprof_n[4];
-#define L2O_FPROF(role, tag) \
-  do { if (blockIdx.x == 0) { int k_ = g_fprof_n[role]; if (k_ < 4096) { g_fprof[(role) * 4096 + k_] = (clock64() << 3) | (tag); g_fprof_n[role] = k_ + 1; } } } while (0)
-#else
-#define L2O_FPROF(role, tag) do { } while (0)
-#endif
-constexpr uint32_t kSBO = 128;               // bytes between 8-row (N) core-matrix groups
-constexpr uint32_t kLBO = (kN / 8) * 128;    // bytes between 16-byte K chunks
+constexpr int kImgMaxFloats = Geo<Cfg<L2O_PRE_FC, 2, 20, 20, 20>>::AllFloats;
 
 // ------------------------------------------------------------------ PTX wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
@@ -118,19 +80,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       "r"(parity)
       : "memory");
 }
-__device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {   // non-blocking probe
-  uint32_t ok;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.b32 %0, 1, 0, p;\n\t"
-      "}\n"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void tma_bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
@@ -139,436 +88,264 @@ __device__ __forceinline__ void tma_bulk_g2s(void* dst, const void* src, uint32_
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot)), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(ncols) : "memory");
-}
-// warp-uniform leader election: the whole warp runs the issuing code (operands stay in uniform registers),
-// only the elected lane's tcgen05.mma / commit takes effect
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "elect.sync _|p, 0xFFFFFFFF;\n\t"
-      "selp.b32 %0, 1, 0, p;\n\t"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]   (kind::tf32, M=128, K=8)
-__device__ __forceinline__ void mma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  tc_wait_ld();
-#pragma unroll
-  for (int k = 0; k < 16; ++k) v[k] = __uint_as_float(r[k]);
-}
-__device__ __forceinline__ void tmem_st4(uint32_t taddr, float a, float b, float c, float d) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1,%2,%3,%4};" ::"r"(taddr), "r"(__float_as_uint(a)),
-               "r"(__float_as_uint(b)), "r"(__float_as_uint(c)), "r"(__float_as_uint(d))
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st2(uint32_t taddr, float a, float b) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x2.b32 [%0], {%1,%2};" ::"r"(taddr), "r"(__float_as_uint(a)),
-               "r"(__float_as_uint(b))
-               : "memory");
-}
-// Asynchronous TMEM -> register load of N consecutive columns of this thread's lane (N = 2, 4, 8, 16).  The caller
-// issues tc_wait_ld() before reading v (several loads may be in flight behind one wait).
-template <int N>
-__device__ __forceinline__ void tmem_ldn(uint32_t taddr, float* v) {
-  static_assert(N == 2 || N == 4 || N == 8 || N == 16, "unsupported TMEM load width");
-  uint32_t r[N];
-  if constexpr (N == 2) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x2.b32 {%0,%1}, [%2];" : "=r"(r[0]), "=r"(r[1]) : "r"(taddr) : "memory");
-  } else if constexpr (N == 4) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0,%1,%2,%3}, [%4];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-                 : "r"(taddr)
-                 : "memory");
-  } else if constexpr (N == 8) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr)
-                 : "memory");
-  } else {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
+// One thread stages `bytes` (multiple of 16, 16-byte aligned) of global memory into shared memory with the TMA engine;
+// every thread of the CTA then waits on the barrier.  `bar` must have been initialised (count 1) and fenced.
+__device__ __forceinline__ void stage_image(float* dst, const float* src, uint32_t bytes, uint64_t* bar) {
+  if (threadIdx.x == 0) {
+    mbar_expect_tx(bar, bytes);
+    tma_bulk_g2s(dst, src, bytes, bar);
   }
-#pragma unroll
-  for (int k = 0; k < N; ++k) v[k] = __uint_as_float(r[k]);  // register renames only; values are valid after the wait
+  mbar_wait(bar, 0);
 }
 
-// ---- thread-pair work split -------------------------------------------------------------------------------------
-// A coordinate is served by a PAIR of epilogue threads (same TMEM lane, warps w and w+4).  Half 0 owns hidden units
-// [0, kSplit) of both layers, half 1 the rest plus the per-coordinate scalar work (optimizee / preprocessing / output
-// layer), which is worth about two units — hence 12 | 8 (measured: 10 | 10 is 4 % slower, it only adds x2 accesses).
-// Each half walks its units in chunks of 4 (or 2) units, so that every chunk is a naturally aligned group for the
-// 8/16-byte global and shared accesses and for the x2/x4 (one column per unit) and x8/x16 (four gate columns per
-// unit) TMEM accesses.  f(K0, NC): K0 = index of the chunk's first unit in the thread's arrays (unit = U0 + K0),
-// NC = units in the chunk; both are compile-time constants (IC<>).
-#ifndef L2O_SPLIT_UNITS
-#define L2O_SPLIT_UNITS 12
-#endif
-constexpr int kSplit = L2O_SPLIT_UNITS;
-static_assert(kSplit == 12 || kSplit == 10, "supported thread-pair splits: 12|8 and 10|10");
-template <int HALF>
-struct HalfUnits {
-  static constexpr int U0 = HALF == 0 ? 0 : kSplit;
-  static constexpr int NU = HALF == 0 ? kSplit : kH - kSplit;
-};
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
-struct IC {
-  static constexpr int value = N;
-};
-template <int HALF, class F>
-__device__ __forceinline__ void for_chunks(F&& f) {
-  if constexpr (kSplit == 12) {
-    f(IC<0>{}, IC<4>{});
-    f(IC<4>{}, IC<4>{});
-    if constexpr (HALF == 0) f(IC<8>{}, IC<4>{});
-  } else if constexpr (HALF == 0) {
-    f(IC<0>{}, IC<4>{});
-    f(IC<4>{}, IC<4>{});
-    f(IC<8>{}, IC<2>{});
-  } else {
-    f(IC<0>{}, IC<2>{});
-    f(IC<2>{}, IC<4>{});
-    f(IC<6>{}, IC<4>{});
-  }
+__device__ __forceinline__ void wg_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-#define L2O_CHUNK(K0, NC, k0c, ncc)                 \
-  constexpr int K0 = decltype(k0c)::value;          \
-  constexpr int NC = decltype(ncc)::value
-// global <-> register copies of the thread's units (p already points at unit U0 of the coordinate's row)
-template <int HALF>
-__device__ __forceinline__ void load_units(const float* __restrict__ p, float* v) {
-  for_chunks<HALF>([&](auto k0c, auto ncc) {
-    L2O_CHUNK(K0, NC, k0c, ncc);
-    if constexpr (NC == 4) {
-      const float4 t = *reinterpret_cast<const float4*>(p + K0);
-      v[K0] = t.x; v[K0 + 1] = t.y; v[K0 + 2] = t.z; v[K0 + 3] = t.w;
-    } else {
-      const float2 t = *reinterpret_cast<const float2*>(p + K0);
-      v[K0] = t.x; v[K0 + 1] = t.y;
-    }
-  });
+
+// shared-memory matrix descriptor (wgmma), no swizzle: start >> 4 | LBO >> 4 << 16 | SBO >> 4 << 32
+__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
+  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32);
 }
-// the same from a shared-window address (explicit ld.shared: no generic-window check per access)
-template <int HALF>
-__device__ __forceinline__ void load_units_smem(uint32_t sa, float* v) {
-  for_chunks<HALF>([&](auto k0c, auto ncc) {
-    L2O_CHUNK(K0, NC, k0c, ncc);
-    if constexpr (NC == 4) {
-      asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
-                   : "=f"(v[K0]), "=f"(v[K0 + 1]), "=f"(v[K0 + 2]), "=f"(v[K0 + 3])
-                   : "r"(sa + 4u * K0));
-    } else {
-      asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v[K0]), "=f"(v[K0 + 1]) : "r"(sa + 4u * K0));
-    }
-  });
+// descriptor of a K-major tf32 image with N columns (core matrices: 8 rows of N x 16 bytes of K; N-groups 128 B apart,
+// K-chunks of 4 (N/8) * 128 B apart) and its start-address increment per K = 8 step (descriptor units of 16 B)
+__device__ __forceinline__ uint64_t img_desc(const float* p, int ncols) {
+  return make_desc(smem_u32(p), (uint32_t)(ncols / 8) * 128u, 128u);
 }
-template <int HALF>
-__device__ __forceinline__ void store_units(float* __restrict__ p, const float* v) {
-  for_chunks<HALF>([&](auto k0c, auto ncc) {
-    L2O_CHUNK(K0, NC, k0c, ncc);
-    if constexpr (NC == 4) *reinterpret_cast<float4*>(p + K0) = make_float4(v[K0], v[K0 + 1], v[K0 + 2], v[K0 + 3]);
-    else *reinterpret_cast<float2*>(p + K0) = make_float2(v[K0], v[K0 + 1]);
-  });
+__host__ __device__ constexpr uint64_t img_kstep(int ncols) { return (uint64_t)((2 * (ncols / 8) * 128) >> 4); }
+
+#define L2O_ACC8(b) "+f"(d[b]), "+f"(d[b + 1]), "+f"(d[b + 2]), "+f"(d[b + 3]), "+f"(d[b + 4]), "+f"(d[b + 5]), \
+                    "+f"(d[b + 6]), "+f"(d[b + 7])
+// D[64 x 80] (+)= A[64 x 8] (registers, tf32) . B[8 x 80] (shared, tf32, K-major)
+__device__ __forceinline__ void mma_rs_n80(float* d, const uint32_t* a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %45, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n80k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,"
+      "%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39}, "
+      "{%40,%41,%42,%43}, %44, p, 1, 1;\n\t}\n"
+      : L2O_ACC8(0), L2O_ACC8(8), L2O_ACC8(16), L2O_ACC8(24), L2O_ACC8(32)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
 }
-// the same into a shared-window address (explicit st.shared)
-template <int HALF>
-__device__ __forceinline__ void sts_units(uint32_t sa, const float* v) {
-  for_chunks<HALF>([&](auto k0c, auto ncc) {
-    L2O_CHUNK(K0, NC, k0c, ncc);
-    if constexpr (NC == 4) {
-      asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(sa + 4u * K0), "f"(v[K0]), "f"(v[K0 + 1]), "f"(v[K0 + 2]),
-                   "f"(v[K0 + 3])
-                   : "memory");
-    } else {
-      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(sa + 4u * K0), "f"(v[K0]), "f"(v[K0 + 1]) : "memory");
-    }
-  });
+// D[64 x 48] (+)= A[64 x 8] (registers) . B[8 x 48]
+__device__ __forceinline__ void mma_rs_n48(float* d, const uint32_t* a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %29, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n48k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, "
+      "{%24,%25,%26,%27}, %28, p, 1, 1;\n\t}\n"
+      : L2O_ACC8(0), L2O_ACC8(8), L2O_ACC8(16)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
 }
-// TMA bulk store shared -> global (one thread; bulk async-group completion)
-__device__ __forceinline__ void bulk_s2g(float* dst, uint32_t src_s, uint32_t bytes) {
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(src_s), "r"(bytes) : "memory");
+// D[64 x 24] (+)= A[64 x 8] (registers) . B[8 x 24]
+__device__ __forceinline__ void mma_rs_n24(float* d, const uint32_t* a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %17, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n24k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11}, "
+      "{%12,%13,%14,%15}, %16, p, 1, 1;\n\t}\n"
+      : L2O_ACC8(0), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
 }
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void mma_rs(float* d, const uint32_t* a, uint64_t b, uint32_t acc) {
+  static_assert(N == 80 || N == 48 || N == 24, "wgmma width");
+  if constexpr (N == 80) mma_rs_n80(d, a, b, acc);
+  else if constexpr (N == 48) mma_rs_n48(d, a, b, acc);
+  else mma_rs_n24(d, a, b, acc);
+}
+
 __device__ __forceinline__ float to_tf32(float x) {
   uint32_t r;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
   return __uint_as_float(r);
 }
-// Error-compensated operand split for 3xTF32: the tensor core reads only the top 19 bits of an fp32 operand (sign,
-// 8 exponent, 10 mantissa bits — it truncates, verified on B200: passing x itself gives bit-identical results to
-// passing the explicitly truncated x), so the "hi" operand is x as is and lo = x - trunc19(x) (exact in fp32,
-// |lo| < 2^-10 |x|; its own truncation leaves a 2^-21 relative residual).  2 instructions per value instead of the 5
-// of cvt.rna.tf32.f32 + subtract.  Measured error of d-theta after T=100 against the fp64 oracle: 7.9e-7 (rna
-// split: 5.2e-7; the fp32 oracle itself: 9.7e-7).  -DL2O_SPLIT_RNA restores round-to-nearest for the hi part.
-__device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
-#if defined(L2O_SPLIT_RNA)
-  hi = __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
-  lo = x - hi;
-#else
-  hi = x;
-  lo = x - __uint_as_float(__float_as_uint(x) & 0xFFFFE000u);
-#endif
+// Error-compensated operand split for 3xTF32: hi = x truncated to tf32 (sign, 8 exponent, 10 mantissa bits), lo = the
+// exact remainder (|lo| < 2^-10 |x|; its own truncation leaves a 2^-21 relative residual).  hi + lo == x exactly.
+__device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
+  hi = __float_as_uint(x) & 0xFFFFE000u;
+  lo = __float_as_uint(x - __uint_as_float(hi));
 }
 
-// instruction descriptor: D=f32, A=B=tf32, both K-major, N, M=128 (cute/arch/mma_sm100_desc.hpp InstrDescriptor)
-__host__ __device__ constexpr uint32_t make_idesc(int n) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
+// ------------------------------------------------------------------ operand / accumulator maps
+// 20-vector slot s of thread q at column base + 4s + q  <->  unit 5q + s
+__host__ __device__ constexpr int vec_unit(int c, int base) { return 5 * ((c - base) & 3) + ((c - base) >> 2); }
+__host__ __device__ constexpr int unit_col(int u, int base) { return base + 4 * (u % 5) + u / 5; }
+// MMA gate column n -> reference gate column (gate * 20 + unit, snt.LSTM i|j|f|o blocks)
+__host__ __device__ constexpr int gate_ref_col(int n) {
+  return (2 * ((n >> 3) & 1) + (n & 1)) * kH + 5 * ((n & 7) >> 1) + (n >> 4);
 }
-// shared-memory matrix descriptor, K-major, SWIZZLE_NONE (cute SmemDescriptor): addr>>4 | LBO>>4 <<16 | SBO>>4 <<32 |
-// version 1 << 46
-__device__ __forceinline__ uint64_t make_bdesc(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(kLBO >> 4) << 16) | ((uint64_t)(kSBO >> 4) << 32) |
-         (1ull << 46);
+// physical K index of the dX contractions -> MMA gate column.  The dZ accumulators are reused as A fragments
+// (k-block j: a0|a1 = accumulator column 8j + 2q, a2|a3 = 8j + 2q + 1), so physical k = 8j + p carries gate column
+// 8j + 2 (p % 4) + p / 4.
+__host__ __device__ constexpr int dx_gate_col(int k) { return (k & ~7) + 2 * (k & 3) + ((k >> 2) & 1); }
+// dX output column -> (20-vector group, unit), unit -1 = padding slot
+__host__ __device__ constexpr int dx_group(int c) { return c / 24; }
+__host__ __device__ constexpr int dx_unit(int c) {
+  return 2 * ((c % 24) >> 3) + (c & 1) >= 5 ? -1 : 5 * ((c & 7) >> 1) + 2 * ((c % 24) >> 3) + (c & 1);
+}
+// index of (k, n) in a K-major tf32 image with ncols columns
+__host__ __device__ constexpr int img_index(int k, int n, int ncols) {
+  return ((k >> 2) * (ncols / 8) + (n >> 3)) * 32 + (n & 7) * 4 + (k & 3);
 }
 
-// ------------------------------------------------------------------ weight image
-// Image layout per matrix (K rows, kN cols): float index ((k/4)*(kN/8) + n/8)*32 + (n%8)*4 + k%4, where the
-// MMA column n = 4*u + gate (gate 0..3 = i,j,f,o of hidden unit u) -- one tcgen05.ld x16 = 4 whole units.
-__device__ __forceinline__ int img_index(int k, int n) { return ((k >> 2) * (kN / 8) + (n >> 3)) * 32 + (n & 7) * 4 + (k & 3); }
-
-// transposed image index: rows n' (inputs, NR of them), K = gate (kN): ((k'/4)*(NR/8) + n'/8)*32 + (n'%8)*4 + k'%4
-__device__ __forceinline__ int timg_index(int nrows, int nprime, int kprime) {
-  return ((kprime >> 2) * (nrows / 8) + (nprime >> 3)) * 32 + (nprime & 7) * 4 + (kprime & 3);
-}
-
-// value of the extended weight matrix of layer `l2` at (row k of that layer's contraction range, interleaved gate
-// column n); A column = k (layer 1) or Geo::A2Off + k (layer 2)
+// value of the extended weight matrix of layer `l2` at (operand-row column c, MMA gate column n)
 template <class C>
-__device__ __forceinline__ float ext_weight(const float* __restrict__ theta, bool l2, int k, int n) {
+__device__ __forceinline__ float ext_weight(const float* __restrict__ theta, bool l2, int c, int n) {
   using G = Geo<C>;
-  const int u = n >> 2, g = n & 3;
-  const int col = g * kH + u;  // reference gate-column order i|j|f|o blocks (snt.LSTM split)
-  const int ac = l2 ? G::A2Off + k : k;
-  if (ac == C::F) return theta[(l2 ? C::O_B2 : C::O_B1) + col];
+  const int col = gate_ref_col(n);
+  if (c == G::ColOne) return theta[(l2 ? C::O_B2 : C::O_B1) + col];
+  const bool in_h1 = c >= G::ColH1 && c < G::ColH1 + kH, in_h2 = c >= G::ColH2 && c < G::ColH2 + kH;
   if (!l2) {
-    if (ac < C::F) return theta[C::O_W1 + ac * C::G1 + col];
-    if (ac >= G::ColH1 && ac < G::ColH1 + kH) return theta[C::O_W1 + (C::F + ac - G::ColH1) * C::G1 + col];
+    if (in_h1) return theta[C::O_W1 + (C::F + vec_unit(c, G::ColH1)) * C::G1 + col];
+    if (G::FC && c < kH) return theta[C::O_W1 + vec_unit(c, 0) * C::G1 + col];
+    if (!G::FC && c < C::F) return theta[C::O_W1 + c * C::G1 + col];
     return 0.f;
   }
-  if (ac >= G::ColH1 && ac < G::ColH1 + 2 * kH) return theta[C::O_W2 + (ac - G::ColH1) * C::G2 + col];
+  if (in_h1) return theta[C::O_W2 + vec_unit(c, G::ColH1) * C::G2 + col];
+  if (in_h2) return theta[C::O_W2 + (kH + vec_unit(c, G::ColH2)) * C::G2 + col];
   return 0.f;
 }
-
-// BPTT operand layout (cwlstm_tc_bwd.cuh): A row = [h1p (0..19) | features,1 (20..23) | h1n (24..43) | h2p (44..63)];
-// Z1 contracts columns [0,24), Z2 columns [16,64).  Value of the extended weight matrix at (row k of that
-// contraction range, interleaved gate column n).
-constexpr int kBColXC = 20, kBColH1N = 24, kBColH2P = 44, kBZ2Start = 16;
+// operand-row column of dX output column c of layer l2
 template <class C>
-__device__ __forceinline__ float ext_weight_bwd(const float* __restrict__ theta, bool l2, int k, int n) {
-  const int u = n >> 2, g = n & 3;
-  const int col = g * kH + u;
-  if (!l2) {
-    if (k < kH) return theta[C::O_W1 + (C::F + k) * C::G1 + col];
-    if (k < kBColXC + C::F) return theta[C::O_W1 + (k - kBColXC) * C::G1 + col];
-    if (k == kBColXC + C::F) return theta[C::O_B1 + col];
-    return 0.f;
-  }
-  const int acol = kBZ2Start + k;  // A column
-  if (acol == kBColXC + C::F) return theta[C::O_B2 + col];
-  if (acol >= kBColH1N && acol < kBColH1N + 2 * kH) return theta[C::O_W2 + (acol - kBColH1N) * C::G2 + col];
-  return 0.f;
+__host__ __device__ constexpr int dx_operand_col(bool l2, int c) {
+  using G = Geo<C>;
+  return l2 ? unit_col(dx_unit(c), dx_group(c) == 0 ? G::ColH1 : G::ColH2)
+            : unit_col(dx_unit(c), dx_group(c) == 0 ? G::ColH1 : 0);
 }
 
-// fc(20) nets run the BPTT as two single-chain passes (cwlstm_tc_bwd2.cuh), each with its matrix in the layer-2 slots
-// (B2' | T2) of its own image.  pass 0: layer 2, A = [0..3 zero | 4 one | 5..7 zero | 8..27 h1n | 28..47 h2p];
-// pass 1: layer 1, A = [h1p 0..19 | fc outputs 20..39 | 40 one | 41..47 zero].
-template <class C>
-__device__ __forceinline__ float ext_weight_bwd_fc(const float* __restrict__ theta, int pass, int k, int n) {
-  const int u = n >> 2, g = n & 3;
-  const int col = g * kH + u;
-  if (pass == 0) {
-    if (k == 4) return theta[C::O_B2 + col];
-    if (k >= 8 && k < 8 + 2 * kH) return theta[C::O_W2 + (k - 8) * C::G2 + col];
-    return 0.f;
-  }
-  if (k < kH) return theta[C::O_W1 + (C::F + k) * C::G1 + col];
-  if (k < 2 * kH) return theta[C::O_W1 + (k - kH) * C::G1 + col];
-  if (k == 2 * kH) return theta[C::O_B1 + col];
-  return 0.f;
-}
-
-// mode 0: forward image (B1 | B2, hi/lo);  mode 1: BPTT image (B1' | B2' in the BPTT operand order, then T1 | T2)
-constexpr float kLog2e = 1.4426950408889634f;
+// Weight image: B1h | B1l | B2h | B2l (forward) and, with_transposed, T1h | T1l | T2h | T2l (BPTT dX contractions,
+// K = 80 gates in the physical order of dx_gate_col, N = N1 / N2 dX columns).  B_l rows = operand-row columns
+// 8 L_lLo .. 8 L_lHi - 1.
 template <class C>
 __global__ void prep_weights_kernel(const float* __restrict__ theta, float* __restrict__ img, int with_transposed) {
   static_assert(C::H1 == kH && C::H2 == kH && (C::F <= 3 || C::FC), "tc engine: LSTM-20x2, F <= 3 or fc(20)");
   using G = Geo<C>;
-  if (!with_transposed) {   // forward image: B1h | B1l | B2h | B2l in the net's own geometry
-    float* b1h = img;
-    float* b1l = img + G::B1Floats;
-    float* b2h = img + 2 * G::B1Floats;
-    float* b2l = img + 2 * G::B1Floats + G::B2Floats;
-    const int nfwd = (G::K1 + G::K2) * kN;
-    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < nfwd; e += gridDim.x * blockDim.x) {
+  const int nb = (G::K1 + G::K2) * kN;
+  const int nt = with_transposed ? kN * (G::N1 + G::N2) : 0;
+  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < nb + nt; e += gridDim.x * blockDim.x) {
+    float w;
+    float* hi;
+    int off, idx;
+    if (e < nb) {
       const bool l2 = e >= G::K1 * kN;
       const int ee = l2 ? e - G::K1 * kN : e;
       const int k = ee / kN, n = ee % kN;
-      const float w = ext_weight<C>(theta, l2, k, n);
-      const float hi = to_tf32(w);
-      const int idx = img_index(k, n);
-      (l2 ? b2h : b1h)[idx] = hi;
-      (l2 ? b2l : b1l)[idx] = to_tf32(w - hi);
+      w = ext_weight<C>(theta, l2, 8 * (l2 ? G::L2Lo : G::L1Lo) + k, n);
+      hi = img + (l2 ? 2 * G::B1Floats : 0);
+      off = l2 ? G::B2Floats : G::B1Floats;
+      idx = img_index(k, n, kN);
+    } else {
+      const int e2 = e - nb;
+      const bool l2 = e2 >= kN * G::N1;
+      const int nc = l2 ? G::N2 : G::N1;
+      const int ee = l2 ? e2 - kN * G::N1 : e2;
+      const int k = ee / nc, n = ee % nc;
+      w = dx_unit(n) < 0 ? 0.f : ext_weight<C>(theta, l2, dx_operand_col<C>(l2, n), dx_gate_col(k));
+      hi = img + G::FwdFloats + (l2 ? 2 * G::T1Floats : 0);
+      off = l2 ? G::T2Floats : G::T1Floats;
+      idx = img_index(k, n, nc);
     }
-    return;
-  }
-  if constexpr (!C::FC) {   // BPTT image (B1' | B2' in the BPTT operand order, then T1 | T2)
-    float* b1h = img;
-    float* b1l = img + kB1Floats;
-    float* b2h = img + 2 * kB1Floats;
-    float* b2l = img + 2 * kB1Floats + kB2Floats;
-    float* t1h = img + kImgFloats;
-    float* t1l = t1h + kT1Floats;
-    float* t2h = t1l + kT1Floats;
-    float* t2l = t2h + kT2Floats;
-    const int nfwd = (kK1 + kK2) * kN;
-    const int ntr = (kT1Rows + kT2Rows) * kN;
-    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < nfwd + ntr; e += gridDim.x * blockDim.x) {
-      float hi, lo;
-      if (e < nfwd) {
-        const bool l2 = e >= kK1 * kN;
-        const int ee = l2 ? e - kK1 * kN : e;
-        const int k = ee / kN, n = ee % kN;
-        const float w = ext_weight_bwd<C>(theta, l2, k, n);
-        hi = to_tf32(w);
-        lo = w - hi;
-        const int idx = img_index(k, n);
-        (l2 ? b2h : b1h)[idx] = hi;
-        (l2 ? b2l : b1l)[idx] = to_tf32(lo);
-      } else {
-        const int e2 = e - nfwd;
-        const bool l2 = e2 >= kT1Rows * kN;
-        const int ee = l2 ? e2 - kT1Rows * kN : e2;
-        const int k = ee / kN, n = ee % kN;  // k = input row (n'), n = gate (k')
-        const float w = (k < (l2 ? kK2 : kK1)) ? ext_weight_bwd<C>(theta, l2, k, n) : 0.f;
-        hi = to_tf32(w);
-        lo = w - hi;
-        const int idx = timg_index(l2 ? kT2Rows : kT1Rows, k, n);
-        (l2 ? t2h : t1h)[idx] = hi;
-        (l2 ? t2l : t1l)[idx] = to_tf32(lo);
-      }
-    }
-  } else {   // fc nets: one image per pass, only the layer-2 slots are read
-    const int per = kK2 * kN + kT2Rows * kN;
-    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < 2 * per; e += gridDim.x * blockDim.x) {
-      const int pass = e / per, r = e % per;
-      const bool tr = r >= kK2 * kN;
-      const int ee = tr ? r - kK2 * kN : r;
-      const int k = ee / kN, n = ee % kN;   // k = operand row (A column), n = interleaved gate column
-      const float w = ext_weight_bwd_fc<C>(theta, pass, k, n);
-      const float hi = to_tf32(w), lo = to_tf32(w - hi);
-      float* base = img + (size_t)pass * kImgAllFloats;
-      if (!tr) {
-        const int idx = img_index(k, n);
-        base[2 * kB1Floats + idx] = hi;
-        base[2 * kB1Floats + kB2Floats + idx] = lo;
-      } else {
-        const int idx = timg_index(kT2Rows, k, n);
-        base[kImgFloats + 2 * kT1Floats + idx] = hi;
-        base[kImgFloats + 2 * kT1Floats + kT2Floats + idx] = lo;
-      }
-    }
+    const float h = to_tf32(w);
+    hi[idx] = h;
+    hi[off + idx] = to_tf32(w - h);
   }
 }
 
+// ------------------------------------------------------------------ operand fragments
+// Register-A fragments of one operand row: f[kb][hf * 2 + rh] = column 8 kb + 4 hf + q of row rh (rh 0: coordinate
+// 16w + l/4, rh 1: + 8).
+template <int KB>
+struct Frag {
+  uint32_t hi[KB][4], lo[KB][4];
+  __device__ __forceinline__ void zero() {
+#pragma unroll
+    for (int k = 0; k < KB; ++k)
+#pragma unroll
+      for (int r = 0; r < 4; ++r) { hi[k][r] = 0u; lo[k][r] = 0u; }
+  }
+  // this thread's column of the 4-column group starting at column c (c % 4 == 0; a compile-time value after
+  // unrolling, so the register index is static)
+  __device__ __forceinline__ void put_at(int c, int rh, float v) {
+    split_tf32(v, hi[c / 8][((c / 4) & 1) * 2 + rh], lo[c / 8][((c / 4) & 1) * 2 + rh]);
+  }
+  __device__ __forceinline__ float get_at(int c, int rh) const {   // hi + lo == the value put
+    return __uint_as_float(hi[c / 8][((c / 4) & 1) * 2 + rh]) + __uint_as_float(lo[c / 8][((c / 4) & 1) * 2 + rh]);
+  }
+  template <int COL>
+  __device__ __forceinline__ void put(int rh, float v) {
+    static_assert(COL % 4 == 0 && COL / 8 < KB, "fragment column");
+    put_at(COL, rh, v);
+  }
+  // the thread's 5 units of a 20-vector starting at column BASE
+  template <int BASE>
+  __device__ __forceinline__ void put_vec(int rh, const float* v) {
+    static_assert(BASE % 4 == 0 && (BASE + 19) / 8 < KB, "fragment column");
+#pragma unroll
+    for (int s = 0; s < kU; ++s) put_at(BASE + 4 * s, rh, v[s]);
+  }
+};
+
+// 3xTF32 contraction of k-blocks [LO, HI) of the operand row against a K-major image (hi at bh, lo at bl)
+template <int N, int KB, int LO, int HI>
+__device__ __forceinline__ void mma3(float* d, const Frag<KB>& f, uint64_t bh, uint64_t bl) {
+  constexpr uint64_t step = img_kstep(N);
+#pragma unroll
+  for (int kb = LO; kb < HI; ++kb) {
+    const uint64_t o = (uint64_t)(kb - LO) * step;
+    mma_rs<N>(d, f.lo[kb], bh + o, kb > LO ? 1u : 0u);
+    mma_rs<N>(d, f.hi[kb], bl + o, 1u);
+    mma_rs<N>(d, f.hi[kb], bh + o, 1u);
+  }
+}
+
+// accumulator register of (unit slot s, gate g in i|j|f|o, row rh)
+__host__ __device__ constexpr int acc_idx(int s, int g, int rh) { return 4 * (2 * s + (g >> 1)) + 2 * rh + (g & 1); }
+
 // ------------------------------------------------------------------ epilogue helpers
-// One LSTM unit, pointwise, from the four accumulator columns (pre-activations i, j, f, o) of the unit.  7 MUFU ops
-// (5 ex2 + 2 rcp) instead of the 10 of five separate sigmoid/tanh evaluations: the whole cell update shares ONE
-// reciprocal,  c' = sigma(f) c + sigma(i) tanh(j) = [c (1+Ei)(1+Ej) + (1-Ej)(1+Ef)] / [(1+Ei)(1+Ej)(1+Ef)],
+// One LSTM unit, pointwise, from the pre-activations (i, j, f, o) of the unit.  7 MUFU ops (5 ex2 + 2 rcp) instead of
+// the 10 of five separate sigmoid/tanh evaluations: the whole cell update shares ONE reciprocal,
+//   c' = sigma(f+1) c + sigma(i) tanh(j) = [c (1+Ei)(1+Ej) + (1-Ej)(1+Ef)] / [(1+Ei)(1+Ej)(1+Ef)],
 // and tanh(c') sigma(o) = (1-Ec) / ((1+Ec)(1+Eo)) another.  The exponents are clamped to 2^40 so the triple product
-// stays finite (sigma / tanh are saturated to 1e-12 there).  The activation pipe is the forward kernel's busiest unit
-// (ncu: XU 62 % with the 8-MUFU form).  -DL2O_MUFU8 restores the two-reciprocal cell update.  (Folding the -log2(e)
-// factors into the weight images was measured too: -0.7 % time, 1.5x the d-theta error — not kept.)
+// stays finite (sigma / tanh are saturated to 1e-12 there).
+constexpr float kLog2e = 1.4426950408889634f;
 __device__ __forceinline__ void lstm_point_fwd(float zi, float zj, float zf, float zo, float& c, float& h) {
-#if defined(L2O_MUFU8)
-  const float Ei = ex2_approx(fminf(-kLog2e * zi, 63.f));
-  const float Ej = ex2_approx(fminf(-2.f * kLog2e * zj, 63.f));
-  const float f = rcp_approx(1.0f + ex2_approx(fmaf(-kLog2e, zf, -kLog2e)));
-  const float ij = (1.0f - Ej) * rcp_approx((1.0f + Ei) * (1.0f + Ej));
-  const float cn = fmaf(f, c, ij);
-#else
   const float Ei = ex2_approx(fminf(-kLog2e * zi, 40.f));
   const float Ej = ex2_approx(fminf(-2.f * kLog2e * zj, 40.f));
   const float Qf = 1.0f + ex2_approx(fminf(fmaf(-kLog2e, zf, -kLog2e), 40.f));
   const float Pij = (1.0f + Ei) * (1.0f + Ej);
   const float cn = fmaf(c, Pij, (1.0f - Ej) * Qf) * rcp_approx(Pij * Qf);
-#endif
   c = cn;
   const float Ec = ex2_approx(fminf(-2.f * kLog2e * cn, 63.f));
   const float Eo = ex2_approx(fminf(-kLog2e * zo, 63.f));
   h = (1.0f - Ec) * rcp_approx((1.0f + Ec) * (1.0f + Eo));
 }
-// write 4 values (hi/lo split) to A_hi / A_lo columns [col, col+4)
-__device__ __forceinline__ void st_split4(uint32_t a_hi, uint32_t a_lo, int col, const float* v) {
-  float h0, h1, h2, h3, l0, l1, l2, l3;
-  split_tf32(v[0], h0, l0);
-  split_tf32(v[1], h1, l1);
-  split_tf32(v[2], h2, l2);
-  split_tf32(v[3], h3, l3);
-  tmem_st4(a_hi + col, h0, h1, h2, h3);
-  tmem_st4(a_lo + col, l0, l1, l2, l3);
-}
-__device__ __forceinline__ void st_split2(uint32_t a_hi, uint32_t a_lo, int col, const float* v) {
-  float h0, h1, l0, l1;
-  split_tf32(v[0], h0, l0);
-  split_tf32(v[1], h1, l1);
-  tmem_st2(a_hi + col, h0, h1);
-  tmem_st2(a_lo + col, l0, l1);
-}
-// the thread's NU per-unit values -> A_hi / A_lo columns [col0, col0+NU)  (col0 = column of the thread's first unit)
-template <int HALF>
-__device__ __forceinline__ void st_split_units(uint32_t a_hi, uint32_t a_lo, int col0, const float* v) {
-  for_chunks<HALF>([&](auto k0c, auto ncc) {
-    L2O_CHUNK(K0, NC, k0c, ncc);
-    if constexpr (NC == 4) st_split4(a_hi, a_lo, col0 + K0, v + K0);
-    else st_split2(a_hi, a_lo, col0 + K0, v + K0);
-  });
+// elu as the forward and backward kernels both evaluate it: a (a > 0) | expm1(a), with a short Taylor sum near zero
+// where 2^x - 1 cancels
+__device__ __forceinline__ float elu_fast(float av) {
+  const float em = ex2_approx(kLog2e * av) - 1.0f;
+  const float ep = av * fmaf(av, fmaf(av, fmaf(av, 1.0f / 24.0f, 1.0f / 6.0f), 0.5f), 1.0f);
+  return av > 0.f ? av : (av > -0.0625f ? ep : em);
 }
 
-__device__ __forceinline__ void lstm_unit_fwd(const float* z, float& c, float& h) {
-  lstm_point_fwd(z[0], z[1], z[2], z[3], c, h);
+// the thread's 5 units of a [n][20] row-major array (p already points at the coordinate's row)
+__device__ __forceinline__ void load5(const float* __restrict__ p, int q, float* v) {
+#pragma unroll
+  for (int s = 0; s < kU; ++s) v[s] = p[5 * q + s];
+}
+__device__ __forceinline__ void store5(float* __restrict__ p, int q, const float* v) {
+#pragma unroll
+  for (int s = 0; s < kU; ++s) p[5 * q + s] = v[s];
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+// value of row rh (0 | 1) from the quad thread that computed it (threads q = 0 / 1 of the quad; 2 / 3 duplicate them)
+__device__ __forceinline__ float from_row(float v, int lane, int rh) {
+  return __shfl_sync(0xffffffffu, v, (lane & ~3) | rh);
 }
 
 // internal (non-ABI) extras of a launch: RNNProp's bias-correction exponent p = float(step0 + t) may come from a
@@ -580,368 +357,50 @@ struct FwdExtra {
 };
 
 template <class C>
-struct Smem {
-  float img[Geo<C>::ImgFloats];   // must stay first (16B-aligned TMA destination, descriptor base)
+struct SmemF {
+  float img[Geo<C>::FwdFloats];   // must stay first (16-byte aligned TMA destination)
   float wo[kH + 4];               // linear/w, linear/b
   float win[64];                  // fc nets: input_projection/w [2][20] then /b [20]
-  float ypart[kTiles][2][128];    // output-layer partial sums exchanged inside a thread pair
   uint64_t wbar;
-  uint64_t a_ready[kTiles];
-  uint64_t d_ready[kTiles];
-  uint64_t full[2], empty[2];     // STAGE: state rows of a tile pair landed in / drained from staging buffer b
-  uint64_t st_ready[kTiles][2];   // staged stores: a tile's new (h, c) rows of layer l are in shared memory (256 arrivals)
-  uint64_t st_free[kTiles][2];    // store warp -> epilogue: the TMA engine has read the layer's staging rows
-  uint32_t tmem_slot;
-  uint32_t pad;
+  uint64_t pad;
   double fx[1];                   // [T+1], dynamic tail
 };
-// STAGE (l2o_step, T = 1): the (h, c) rows of the NEXT tile pair are pulled into shared memory by TMA bulk copies while
-// the current pair computes, so the HBM read of the 320 B/coordinate state overlaps the epilogue instead of preceding
-// it.  Two buffers x kTiles tiles x 4 arrays (h1, c1, h2, c2) x [128][kH] floats = 160 KB after the fx tail.
-constexpr int kStageArr = 128 * kH;                       // floats per (tile, array)
-constexpr int kStageFloats = 2 * kTiles * 4 * kStageArr;  // 40960 floats
-// dynamic tail after Smem<C>: fx [T+1] doubles | (fc nets) Adam bias corrections [T][2] floats | staging buffers
+// dynamic tail after SmemF<C>: fx [T+1] doubles | (fc nets) Adam bias corrections [T][2] floats
 template <class C>
 __host__ __device__ constexpr size_t adamc_offset(int T) {
-  return (sizeof(Smem<C>) + (size_t)(T + 1) * sizeof(double) + 15) & ~(size_t)15;
+  return (sizeof(SmemF<C>) + (size_t)(T + 1) * sizeof(double) + 15) & ~(size_t)15;
 }
 template <class C>
-__host__ __device__ constexpr size_t stage_offset(int T) {
-  return (adamc_offset<C>(T) + (C::FC ? (size_t)T * 2 * sizeof(float) : 0) + 127) & ~(size_t)127;
+__host__ __device__ constexpr size_t fwd_smem_bytes(int T) {
+  return adamc_offset<C>(T) + (C::FC ? (size_t)T * 2 * sizeof(float) : 0);
 }
 
-// Epilogue of one thread: coordinate `row` of tile `tile`, hidden units [U0, U0+NU) of both layers.
-template <class C, int HALF, bool STAGE>
-__device__ __forceinline__ void fwd_epilogue(const l2o_unroll_args& a, const NetRt& rt, Smem<C>& S, uint32_t tmem_base,
-                                             float* __restrict__ state_out, int warp, int lane,
-                                             const float* __restrict__ stage, const float* __restrict__ adamc) {
-  using G = Geo<C>;
-  constexpr int kTileCols = G::TileCols, kACols = G::ACols, kColH1 = G::ColH1, kColH2 = G::ColH2;  // shadow the defaults
-  constexpr int U0 = HalfUnits<HALF>::U0;
-  constexpr int NU = HalfUnits<HALF>::NU;
-  const int tile = warp >> 3;          // warps 0-7: tile 0, 8-15: tile 1
-  const int q = warp & 3;              // TMEM lane quarter
-  const int row = q * 32 + lane;       // coordinate within the tile
-  const int T = a.T;
-  const int64_t n = a.n;
-  const int64_t npairs = (n + kTileCoords - 1) / kTileCoords;
-  const bool in_kernel_opt = a.opt_kind != L2O_OPT_NONE;
-  const bool want_fx = in_kernel_opt && a.fx != nullptr;
-  const uint32_t lane_off = (uint32_t)(q * 32) << 16;
-  const uint32_t t_d = tmem_base + lane_off + tile * kTileCols;
-  const uint32_t t_d2 = t_d + (G::SplitD ? kN : 0);   // layer-2 accumulators
-  const uint32_t t_ah = t_d + G::DCols;
-  const uint32_t t_al = t_ah + kACols;
-  uint32_t pd = 0;  // d_ready parity
-  const int64_t slot = n * C::SF;
-  double imit = 0.0;
-  if (HALF == 1 && kColH2 + kH < kACols) {  // zero the pad columns of A once (zero weight rows, but must be finite)
-    tmem_st4(t_ah + kColH2 + kH, 0.f, 0.f, 0.f, 0.f);
-    tmem_st4(t_al + kColH2 + kH, 0.f, 0.f, 0.f, 0.f);
-  }
-  const bool adam_mode = C::NIN == 2 && a.m != nullptr;   // fused RNNProp features (DM/meta_rnnprop_train.py:383-388)
-  uint32_t pfull[2] = {0, 0};
-  int kpair = 0;
-  // Staged stores: with checkpoints (training) or in the step regime every step writes this thread's 2 x NU x 2 new
-  // state values; as float4 stores at an 80-byte row stride a warp-level store touches 20 cache lines, and the LSU
-  // queue backs up on the step's critical path (ncu: mio_throttle 15 %, about 2 K cycles between the pair barrier and the
-  // next step).  Instead the rows go to shared memory (conflict-free st.shared.v4) and a warp of the issuer warpgroup
-  // writes each tile's 10 KB (h | c) blocks with TMA bulk stores.  kTst 1: dedicated staging (single-buffered per layer,
-  // st_free handshake); STAGE: the ring slot the rows were loaded from (same addresses per thread), released to the
-  // producer by the store warp.
-  const bool tst = STAGE || a.ckpt != nullptr;
-  uint32_t pfree[2] = {0, 0};
-  bool staged_before = false;
-  // Step-at-a-time regime (STAGE): the parameter and the first input of the NEXT pair are loaded one pair ahead, so
-  // their DRAM latency hides behind this pair's two MMA round trips (the state rows already arrive through the TMA ring).
-  constexpr bool kAheadIn = STAGE;   // in_seq[i] is the first input of step 0 in every input layout
-  float x_ahead = 0.f, in_ahead = 0.f;
-  if (STAGE && HALF == 1) {
-    const int64_t i0 = (int64_t)blockIdx.x * kTileCoords + tile * 128 + row;
-    if (i0 < n) {
-      if (a.x) x_ahead = a.x[i0];
-      if (kAheadIn && !in_kernel_opt) in_ahead = a.in_seq[i0];
-    }
-  }
-  for (int64_t pair = blockIdx.x; pair < npairs; pair += gridDim.x, ++kpair) {
-    const int64_t i = pair * kTileCoords + tile * 128 + row;
-    const bool act = i < n;
-    const float x_cur = x_ahead, in_cur = in_ahead;
-    if (STAGE && HALF == 1) {
-      const int64_t inx = i + (int64_t)gridDim.x * kTileCoords;
-      if (inx < n) {
-        if (a.x) x_ahead = a.x[inx];
-        if (kAheadIn && !in_kernel_opt) in_ahead = a.in_seq[inx];
-      }
-    }
-    if constexpr (!STAGE) {  // pull the NEXT pair's state rows towards L2: with T = 1 the loads below are the critical path
-      const int64_t inx = i + (int64_t)gridDim.x * kTileCoords;
-      if (inx < n) {
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(a.state + inx * kH + U0));
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(a.state + (n + inx) * kH + U0));
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(a.state + 2 * n * kH + inx * kH + U0));
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(a.state + 2 * n * kH + (n + inx) * kH + U0));
-        if (HALF == 1) {
-          if (a.x) asm volatile("prefetch.global.L2 [%0];" ::"l"(a.x + inx));
-          if (!in_kernel_opt) asm volatile("prefetch.global.L2 [%0];" ::"l"(a.in_seq + inx));
-        }
-      }
-    }
-    float c1[NU], c2[NU];
-    float x = 0.f, oa = 0.f, ob = 0.f;
-    float am = 0.f, av = 0.f;   // RNNProp Adam moments of this coordinate (half 1)
-    if (HALF == 1 && adam_mode && act) { am = a.m[i]; av = a.v[i]; }
-    {
-      float h1[NU], h2[NU];
-#pragma unroll
-      for (int k = 0; k < NU; ++k) { h1[k] = 0.f; h2[k] = 0.f; c1[k] = 0.f; c2[k] = 0.f; }
-      if constexpr (STAGE) {
-        const int buf = kpair & 1;
-        mbar_wait(&S.full[buf], pfull[buf]);
-        pfull[buf] ^= 1;
-        if (act) {
-          const uint32_t sb = smem_u32(stage) + 4u * (uint32_t)(((buf * kTiles + tile) * 4) * kStageArr + row * kH + U0);
-          load_units_smem<HALF>(sb, h1);
-          load_units_smem<HALF>(sb + 4u * kStageArr, c1);
-          load_units_smem<HALF>(sb + 8u * kStageArr, h2);
-          load_units_smem<HALF>(sb + 12u * kStageArr, c2);
-        }
-        // (the slot is reused as the staging area of this pair's stores; the store warp releases it to the producer)
-      }
-      if (act) {
-        if constexpr (!STAGE) {
-          load_units<HALF>(a.state + i * kH + U0, h1);
-          load_units<HALF>(a.state + (n + i) * kH + U0, c1);
-          load_units<HALF>(a.state + 2 * n * kH + i * kH + U0, h2);
-          load_units<HALF>(a.state + 2 * n * kH + (n + i) * kH + U0, c2);
-        }
-        if (a.ckpt) {
-          store_units<HALF>(a.ckpt + i * kH + U0, h1);
-          store_units<HALF>(a.ckpt + (n + i) * kH + U0, c1);
-          store_units<HALF>(a.ckpt + 2 * n * kH + i * kH + U0, h2);
-          store_units<HALF>(a.ckpt + 2 * n * kH + (n + i) * kH + U0, c2);
-        }
-        if (HALF == 1) x = STAGE ? x_cur : (a.x ? a.x[i] : 0.f);   // only half 1 carries the parameter
-        if (in_kernel_opt) { oa = a.opt_a[i]; ob = a.opt_b[i]; }
-      }
-      st_split_units<HALF>(t_ah, t_al, kColH1 + U0, h1);
-      st_split_units<HALF>(t_ah, t_al, kColH2 + U0, h2);
-    }
-    const int prole = (lane == 0 && (warp == 0 || warp == 4 || warp == 8)) ? (warp == 0 ? 0 : (warp == 4 ? 1 : 2)) : -1;
-    (void)prole;
-    for (int t = 0; t < T; ++t) {
-      if (prole >= 0) L2O_FPROF(prole, 0);
-      if (prole >= 0) L2O_FDBG(prole * 4, (kpair << 16) | (t << 4) | 0);
-      // ---- gradient + preprocessing -> feature chunk of A (half 1 owns the per-coordinate scalars) ----------
-      float fval = 0.f;
-      if (HALF == 1) {
-        float raw0 = 0.f, raw1 = 0.f;
-        if (act) {
-          if (in_kernel_opt) {
-            optimizee_eval(a.opt_kind, x, oa, ob, a.opt_alpha, a.opt_fscale, fval, raw0);
-            if (a.g_rec) a.g_rec[(int64_t)t * n + i] = raw0;
-          } else if (C::NIN == 2 && !adam_mode) {   // operator surface: (m~, g~) given
-            raw0 = (kAheadIn && t == 0) ? in_cur : a.in_seq[((int64_t)t * 2) * n + i];
-            raw1 = a.in_seq[((int64_t)t * 2 + 1) * n + i];
-          } else {
-            raw0 = (kAheadIn && t == 0) ? in_cur : a.in_seq[(int64_t)t * n + i];
-          }
-        }
-        if constexpr (C::FC) {
-          if (adam_mode) {   // m' = b1 m + (1-b1) g ; v' = b2 v + (1-b2) g^2 ; m~ = m^/(sqrt(v^)+1e-8) ; g~ = g/(sqrt(v^)+1e-8)
-            const float g = raw0;
-            am = a.beta1 * am + (1.0f - a.beta1) * g;
-            av = a.beta2 * av + (1.0f - a.beta2) * g * g;
-            const float mh = am / adamc[2 * t], vh = av / adamc[2 * t + 1];   // 1 - beta^p, tabulated per step
-            const float den = sqrtf(vh) + 1e-8f;
-            raw0 = mh / den;
-            raw1 = g / den;
-          }
-          if (act && a.feat_rec) {
-            a.feat_rec[((int64_t)t * 2) * n + i] = raw0;
-            a.feat_rec[((int64_t)t * 2 + 1) * n + i] = raw1;
-          }
-          // u = elu([m~, g~] Win + bin) (DM/networks.py:219), then the constant 1 and three zero columns
-#pragma unroll
-          for (int k4 = 0; k4 < 5; ++k4) {
-            float u[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const int j = 4 * k4 + e;
-              const float av_ = fmaf(raw1, S.win[20 + j], fmaf(raw0, S.win[j], S.win[40 + j]));
-              // elu: a (a > 0) | expm1(a); near zero the 2^x - 1 form cancels, so a short Taylor sum takes over
-              const float em = ex2_approx(kLog2e * av_) - 1.0f;
-              const float ep = av_ * fmaf(av_, fmaf(av_, fmaf(av_, 1.0f / 24.0f, 1.0f / 6.0f), 0.5f), 1.0f);
-              u[e] = av_ > 0.f ? av_ : (av_ > -0.0625f ? ep : em);
-            }
-            st_split4(t_ah, t_al, 4 * k4, u);
-          }
-          tmem_st4(t_ah + 20, 1.0f, 0.f, 0.f, 0.f);
-          tmem_st4(t_al + 20, 0.f, 0.f, 0.f, 0.f);
-        } else {
-          float u[4] = {0.f, 0.f, 0.f, 0.f};
-          float dummy[C::F];
-          preprocess<C>(nullptr, rt, raw0, 0.f, dummy);
-#pragma unroll
-          for (int k = 0; k < C::F; ++k) u[k] = dummy[k];
-          u[C::F] = 1.0f;  // bias column
-          st_split4(t_ah, t_al, 0, u);
-        }
-      }
-      tc_wait_st();
-      tc_fence_before();
-      mbar_arrive(&S.a_ready[tile]);
-      if (prole >= 0) L2O_FPROF(prole, 1);
-      if (HALF == 1 && want_fx) {
-        const double ws = warp_sum_d((double)fval);
-        if (lane == 0) atomicAdd(&S.fx[t], ws);
-      }
-      // ---- layer 1 epilogue ---------------------------------------------------------------
-      mbar_wait(&S.d_ready[tile], pd);
-      pd ^= 1;
-      tc_fence_after();
-      if (prole >= 0) L2O_FPROF(prole, 2);
-      if (prole >= 0) L2O_FDBG(prole * 4, (kpair << 16) | (t << 4) | 2);
-      float hrow[NU];
-      {
-        float z[4 * NU];  // this thread's 40 gate pre-activations: three loads in flight behind one wait
-        for_chunks<HALF>([&](auto k0c, auto ncc) {
-          L2O_CHUNK(K0, NC, k0c, ncc);
-          tmem_ldn<4 * NC>(t_d + 4 * (U0 + K0), z + 4 * K0);
-        });
-        tc_wait_ld();
-#pragma unroll
-        for (int k = 0; k < NU; ++k) lstm_unit_fwd(z + 4 * k, c1[k], hrow[k]);
-      }
-      st_split_units<HALF>(t_ah, t_al, kColH1 + U0, hrow);
-      tc_wait_st();
-      tc_fence_before();
-      mbar_arrive(&S.a_ready[tile]);
-      if (prole >= 0) L2O_FPROF(prole, 3);
-      if (prole >= 0) L2O_FDBG(prole * 4, (kpair << 16) | (t << 4) | 3);
-      // shared address of this thread's slice of the tile's staging block (arrays h1 | c1 | h2 | c2)
-      const uint32_t sst = smem_u32(stage) + 4u * (uint32_t)((((STAGE ? (kpair & 1) : 0) * kTiles + tile) * 4) * kStageArr + row * kH + U0);
-      if (tst) {
-        if (staged_before) {   // the previous layer-1 rows have been read (also keeps this barrier pair in lockstep with
-          mbar_wait(&S.st_free[tile][0], pfree[0]);   // the polling store warp: never more than one phase ahead)
-          pfree[0] ^= 1;
-        }
-        if (act) {
-          sts_units<HALF>(sst, hrow);
-          sts_units<HALF>(sst + 4u * kStageArr, c1);
-        }
-        fence_proxy_async();
-        mbar_arrive(&S.st_ready[tile][0]);
-        if (prole >= 0) L2O_FDBG(prole * 4 + 1, (kpair << 16) | (t << 4) | 1);
-      } else if (act) {
-        if (t == T - 1) store_units<HALF>(state_out + i * kH + U0, hrow);  // final hidden state of layer 1
-      }
-      // ---- layer 2 epilogue + output linear + parameter add ---------------------------------
-      mbar_wait(&S.d_ready[tile], pd);
-      pd ^= 1;
-      tc_fence_after();
-      if (prole >= 0) L2O_FPROF(prole, 4);
-      if (prole >= 0) L2O_FDBG(prole * 4, (kpair << 16) | (t << 4) | 4);
-      float yp = 0.f;
-      {
-        float z[4 * NU];
-        for_chunks<HALF>([&](auto k0c, auto ncc) {
-          L2O_CHUNK(K0, NC, k0c, ncc);
-          tmem_ldn<4 * NC>(t_d2 + 4 * (U0 + K0), z + 4 * K0);
-        });
-        tc_wait_ld();
-#pragma unroll
-        for (int k = 0; k < NU; ++k) {
-          lstm_unit_fwd(z + 4 * k, c2[k], hrow[k]);
-          yp = fmaf(hrow[k], S.wo[U0 + k], yp);
-        }
-      }
-      st_split_units<HALF>(t_ah, t_al, kColH2 + U0, hrow);
-      // exchange the output-layer partial sums inside the thread pair (named barrier: the tile's 256 threads)
-      S.ypart[tile][HALF][row] = yp;
-      if (prole >= 0) L2O_FPROF(prole, 5);
-      asm volatile("bar.sync %0, 256;" ::"r"(1 + tile) : "memory");
-      if (prole >= 0) L2O_FPROF(prole, 6);
-      if (prole >= 0) L2O_FDBG(prole * 4, (kpair << 16) | (t << 4) | 6);
-      const float y = (S.ypart[tile][0][row] + S.ypart[tile][1][row]) + S.wo[kH];
-      const float d = rt.tanh_output ? tanh_acc(y) * rt.scale : y * rt.scale;
-      x += d;
-      if (tst) {
-        if (staged_before) {
-          mbar_wait(&S.st_free[tile][1], pfree[1]);
-          pfree[1] ^= 1;
-        }
-        if (act) {
-          sts_units<HALF>(sst + 8u * kStageArr, hrow);
-          sts_units<HALF>(sst + 12u * kStageArr, c2);
-        }
-        fence_proxy_async();
-        mbar_arrive(&S.st_ready[tile][1]);
-        if (prole >= 0) L2O_FDBG(prole * 4 + 1, (kpair << 16) | (t << 4) | 2);
-        staged_before = true;
-      }
-      if (act) {
-        if (!tst && t == T - 1) store_units<HALF>(state_out + 2 * n * kH + i * kH + U0, hrow);  // final hidden state of layer 2
-        if (HALF == 1) {
-          if (a.delta_seq) a.delta_seq[(int64_t)t * n + i] = d;
-          if (a.labels) {
-            const float r = a.labels[(int64_t)t * n + i] - d;
-            imit += 0.5 * (double)r * (double)r;
-          }
-        }
-      }
-    }
-    // ---- tile epilogue: final cell state / x / f(x_T), g_T ------------------------------------
-    {
-      float fval = 0.f;
-      if (act) {
-        if (HALF == 1 && in_kernel_opt) {
-          float gT;
-          optimizee_eval(a.opt_kind, x, oa, ob, a.opt_alpha, a.opt_fscale, fval, gT);
-          if (a.g_rec) a.g_rec[(int64_t)T * n + i] = gT;
-        }
-        if (T > 0 && !tst) {
-          store_units<HALF>(state_out + (n + i) * kH + U0, c1);
-          store_units<HALF>(state_out + 2 * n * kH + (n + i) * kH + U0, c2);
-        }
-        if (HALF == 1 && a.x) a.x[i] = x;
-        if (HALF == 1 && adam_mode) { a.m[i] = am; a.v[i] = av; }
-      }
-      if (HALF == 1 && want_fx) {
-        const double ws = warp_sum_d((double)fval);
-        if (lane == 0) atomicAdd(&S.fx[T], ws);
-      }
-    }
-  }
-  if (HALF == 1 && a.labels && a.imit_loss) {
-    const double ws = warp_sum_d(imit);
-    if (lane == 0) atomicAdd(a.imit_loss, ws / (double)a.n_total);
-  }
-}
-
-template <class C, bool STAGE>
-__global__ void __launch_bounds__(kThreads, 1) unroll_fwd_kernel(l2o_unroll_args a, NetRt rt, const float* __restrict__ img,
-                                                                  float* __restrict__ state_out, FwdExtra ex) {
+// ------------------------------------------------------------------ forward kernel
+// Forward unroll of T steps (T = 1 with an out-of-place state_out: the l2o_step regime).  Per warpgroup tile: state
+// rows in, then per step  features -> layer-1 MMAs -> layer-1 epilogue -> layer-2 MMAs -> layer-2 epilogue + output
+// layer + parameter add.  The three warpgroups of a CTA run independent tiles, so one warpgroup's MMA round trip
+// overlaps the others' epilogues.
+template <class C>
+__global__ void __launch_bounds__(kFwdThreads, 1) unroll_fwd_kernel(l2o_unroll_args a, NetRt rt, const float* __restrict__ img,
+                                                                     float* __restrict__ state_out, FwdExtra ex) {
   using G = Geo<C>;
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  Smem<C>& S = *reinterpret_cast<Smem<C>*>(smem_raw);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  SmemF<C>& S = *reinterpret_cast<SmemF<C>*>(smem_raw);
   const int T = a.T;
   const int64_t n = a.n;
-  const int64_t npairs = (n + kTileCoords - 1) / kTileCoords;
-  const bool want_fx = a.opt_kind != L2O_OPT_NONE && a.fx != nullptr;
-  constexpr int kIssuerWarp = kEpiThreads / 32;
+  const bool in_kernel_opt = a.opt_kind != L2O_OPT_NONE;
+  const bool want_fx = in_kernel_opt && a.fx != nullptr;
+  const bool adam_mode = C::NIN == 2 && a.m != nullptr;   // fused RNNProp features (DM/meta_rnnprop_train.py:383-388)
+  float* adamc = reinterpret_cast<float*>(smem_raw + adamc_offset<C>(T));
 
-  if (threadIdx.x == 0) L2O_FDBG(30, 1);
   if (want_fx)
     for (int t = threadIdx.x; t <= T; t += blockDim.x) S.fx[t] = 0.0;
   if (threadIdx.x < kH) S.wo[threadIdx.x] = a.theta[C::O_WO + threadIdx.x];
   if (threadIdx.x == kH) S.wo[kH] = a.theta[C::O_BO];
-  float* adamc = reinterpret_cast<float*>(smem_raw + adamc_offset<C>(T));
   if constexpr (C::FC) {
     static_assert(!C::FC || C::NIN == 2, "fc nets here are RNNprop nets (two inputs)");
-    if (threadIdx.x < 60) S.win[threadIdx.x] = a.theta[C::O_WIN + threadIdx.x];   // w [2][20] then b [20] (contiguous)
-    if (a.m != nullptr) {   // 1 - beta^p per step, p = float(step + t) (DM/meta_rnnprop_train.py:384,386)
+    if (threadIdx.x >= 32 && threadIdx.x < 92) S.win[threadIdx.x - 32] = a.theta[C::O_WIN + threadIdx.x - 32];
+    if (adam_mode) {   // 1 - beta^p per step, p = float(step + t) (DM/meta_rnnprop_train.py:384,386)
       const int step0 = ex.step_ptr ? *ex.step_ptr + ex.t_offset : a.step0;
       for (int t = threadIdx.x; t < T; t += blockDim.x) {
         const float p = (ex.step_ptr == nullptr && ex.p_fixed > 0.f) ? ex.p_fixed : (float)(step0 + t);
@@ -950,261 +409,240 @@ __global__ void __launch_bounds__(kThreads, 1) unroll_fwd_kernel(l2o_unroll_args
       }
     }
   }
-  if (warp == kIssuerWarp) {
-    if (lane == 0) {
-      mbar_init(&S.wbar, 1);
-#pragma unroll
-      for (int k = 0; k < kTiles; ++k) {
-        mbar_init(&S.a_ready[k], 256);
-        mbar_init(&S.d_ready[k], 1);
-      }
-      mbar_init(&S.full[0], 1);
-      mbar_init(&S.full[1], 1);
-      mbar_init(&S.empty[0], kTiles);   // released by the store warp, once per tile
-      mbar_init(&S.empty[1], kTiles);
-      for (int k = 0; k < kTiles; ++k) {
-        mbar_init(&S.st_ready[k][0], 256);
-        mbar_init(&S.st_ready[k][1], 256);
-        mbar_init(&S.st_free[k][0], 1);
-        mbar_init(&S.st_free[k][1], 1);
-      }
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc(&S.tmem_slot, kTmemCols);
-    tmem_relinquish();
-    if (lane == 0) {
-      mbar_expect_tx(&S.wbar, G::ImgBytes);
-      tma_bulk_g2s(S.img, img, G::ImgBytes, &S.wbar);
-    }
+  if (threadIdx.x == 0) {
+    mbar_init(&S.wbar, 1);
+    fence_barrier_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = S.tmem_slot;
+  stage_image(S.img, img, G::FwdFloats * 4, &S.wbar);
 
-  if (warp < kIssuerWarp) {
-    // =============================== epilogue warps: a thread pair per coordinate ===============================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kFwdEpiRegs));
-    const float* stage = reinterpret_cast<const float*>(smem_raw + stage_offset<C>(T));
-    if (((warp >> 2) & 1) == 0) fwd_epilogue<C, 0, STAGE>(a, rt, S, tmem_base, state_out, warp, lane, stage, adamc);
-    else fwd_epilogue<C, 1, STAGE>(a, rt, S, tmem_base, state_out, warp, lane, stage, adamc);
-  } else if (warp > kIssuerWarp) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kFwdIssuerRegs));  // idle warps of the issuer warpgroup
-    if (warp == kIssuerWarp + 2 && (STAGE || a.ckpt != nullptr)) {
-      // ---- store warp: per tile the events alternate "layer-1 rows staged" / "layer-2 rows staged"; each becomes two
-      // (at t = T-1 four) 10 KB TMA bulk stores: checkpoint slot t+1 and, after the last step, the state arena
-      const uint32_t sst0 = smem_u32(smem_raw + stage_offset<C>(T));
-      const int64_t slot = n * C::SF;
-      uint32_t ps[kTiles][2] = {{0, 0}, {0, 0}};
-      int k = 0;
-      for (int64_t pair = blockIdx.x; pair < npairs; pair += gridDim.x, ++k) {
-        int ev[kTiles] = {0, 0};
-        while (ev[0] < 2 * T || ev[1] < 2 * T) {
+  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const int g = lane >> 2, q = lane & 3, own = q & 1;
+  const uint64_t b1h = img_desc(S.img, kN), b1l = img_desc(S.img + G::B1Floats, kN);
+  const uint64_t b2h = img_desc(S.img + 2 * G::B1Floats, kN), b2l = img_desc(S.img + 2 * G::B1Floats + G::B2Floats, kN);
+  const int64_t ntiles = (n + kTile - 1) / kTile;
+  const int64_t slot = n * C::SF;
+  const float bo = S.wo[kH];
+  float wo[kU];
 #pragma unroll
-          for (int tile = 0; tile < kTiles; ++tile) {
-            if (ev[tile] >= 2 * T || !mbar_test(&S.st_ready[tile][ev[tile] & 1], ps[tile][ev[tile] & 1])) continue;
-            const int e = ev[tile]++;
-            const int t = e >> 1, layer = e & 1;
-            ps[tile][layer] ^= 1;
-            if (lane == 0) L2O_FDBG(16 + tile, (k << 16) | e);
-            if (lane == 0) {
-              const int64_t base = pair * kTileCoords + tile * 128;
-              const int64_t cnt = n - base < 0 ? 0 : (n - base > 128 ? 128 : n - base);
-              if (cnt > 0) {
-                const uint32_t bytes = (uint32_t)cnt * kH * 4u;
-                const uint32_t src_h = sst0 + 4u * (uint32_t)((((STAGE ? (k & 1) : 0) * kTiles + tile) * 4 + 2 * layer) * kStageArr);
-                const uint32_t src_c = src_h + 4u * kStageArr;
-                const int64_t loff = (int64_t)layer * 2 * n * kH;
-                if (a.ckpt) {
-                  float* ck = a.ckpt + (int64_t)(t + 1) * slot + loff;
-                  bulk_s2g(ck + base * kH, src_h, bytes);
-                  bulk_s2g(ck + (n + base) * kH, src_c, bytes);
-                }
-                if (t == T - 1) {
-                  bulk_s2g(state_out + loff + base * kH, src_h, bytes);
-                  bulk_s2g(state_out + loff + (n + base) * kH, src_c, bytes);
-                }
-              }
-              bulk_commit();
-              bulk_wait_read0();
-              mbar_arrive(&S.st_free[tile][layer]);
-              L2O_FDBG(18 + tile, (k << 16) | e);
-              if constexpr (STAGE) {
-                if (layer == 1 && t == T - 1) mbar_arrive(&S.empty[k & 1]);   // the ring slot may be refilled
-              }
-            }
-            __syncwarp();
-          }
+  for (int s = 0; s < kU; ++s) wo[s] = S.wo[5 * q + s];
+  double imit = 0.0;
+  float d[kN / 2];   // gate accumulators (the first MMA of each layer overwrites them)
+#pragma unroll
+  for (int k = 0; k < kN / 2; ++k) d[k] = 0.f;
+
+  for (int64_t tile = (int64_t)blockIdx.x * kFwdWG + wg; tile < ntiles; tile += (int64_t)gridDim.x * kFwdWG) {
+    const int64_t r0 = tile * kTile + warp * 16 + g;
+    const int64_t row[2] = {r0, r0 + 8};
+    const bool act[2] = {row[0] < n, row[1] < n};
+    const int64_t io = own ? row[1] : row[0];   // the row whose per-coordinate scalars this thread computes
+    const bool oact = io < n;
+    const bool writer = q < 2 && oact;
+    Frag<G::KB> A;
+    A.zero();
+    float c1[2][kU], c2[2][kU];
+#pragma unroll
+    for (int rh = 0; rh < 2; ++rh) {
+      float h1[kU] = {0.f, 0.f, 0.f, 0.f, 0.f}, h2[kU] = {0.f, 0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+      for (int s = 0; s < kU; ++s) { c1[rh][s] = 0.f; c2[rh][s] = 0.f; }
+      if (act[rh]) {
+        const int64_t i = row[rh];
+        load5(a.state + i * kH, q, h1);
+        load5(a.state + (n + i) * kH, q, c1[rh]);
+        load5(a.state + 2 * n * kH + i * kH, q, h2);
+        load5(a.state + 2 * n * kH + (n + i) * kH, q, c2[rh]);
+        if (a.ckpt) {
+          store5(a.ckpt + i * kH, q, h1);
+          store5(a.ckpt + (n + i) * kH, q, c1[rh]);
+          store5(a.ckpt + 2 * n * kH + i * kH, q, h2);
+          store5(a.ckpt + 2 * n * kH + (n + i) * kH, q, c2[rh]);
+        }
+        if (T == 0 && state_out != a.state) {
+          store5(state_out + i * kH, q, h1);
+          store5(state_out + (n + i) * kH, q, c1[rh]);
+          store5(state_out + 2 * n * kH + i * kH, q, h2);
+          store5(state_out + 2 * n * kH + (n + i) * kH, q, c2[rh]);
         }
       }
-      if (lane == 0) bulk_wait0();
+      A.template put_vec<G::ColH1>(rh, h1);
+      A.template put_vec<G::ColH2>(rh, h2);
     }
-    if constexpr (STAGE) {
-      if (warp == kIssuerWarp + 1) {
-        // ---- state-row producer: TMA bulk copies of pair k+0, k+1 ... into the two staging buffers -------------------
-        float* stage = reinterpret_cast<float*>(smem_raw + stage_offset<C>(T));
-        uint32_t pempty[2] = {0, 0};
-        int k = 0;
-        for (int64_t pair = blockIdx.x; pair < npairs; pair += gridDim.x, ++k) {
-          const int buf = k & 1;
-          if (k >= 2) {
-            mbar_wait(&S.empty[buf], pempty[buf]);
-            pempty[buf] ^= 1;
+    if constexpr (G::FC) {   // the constant 1 of the fc row; DM rows carry theirs in the feature chunk
+      A.template put<G::ColOne>(0, q == 0 ? 1.0f : 0.f);
+      A.template put<G::ColOne>(1, q == 0 ? 1.0f : 0.f);
+    }
+    float x = 0.f, oa = 0.f, ob = 0.f, am = 0.f, av = 0.f;
+    if (oact) {
+      if (a.x) x = a.x[io];
+      if (in_kernel_opt) { oa = a.opt_a[io]; ob = a.opt_b[io]; }
+      if (adam_mode) { am = a.m[io]; av = a.v[io]; }
+    }
+
+    for (int t = 0; t < T; ++t) {
+      // ---- gradient + preprocessing of the own row, then the feature columns of both rows -------------------------
+      float fval = 0.f, raw0 = 0.f, raw1 = 0.f;
+      if (oact) {
+        if (in_kernel_opt) {
+          optimizee_eval(a.opt_kind, x, oa, ob, a.opt_alpha, a.opt_fscale, fval, raw0);
+          if (a.g_rec && q < 2) a.g_rec[(int64_t)t * n + io] = raw0;
+        } else if (C::NIN == 2 && !adam_mode) {   // operator surface: (m~, g~) given
+          raw0 = a.in_seq[((int64_t)t * 2) * n + io];
+          raw1 = a.in_seq[((int64_t)t * 2 + 1) * n + io];
+        } else {
+          raw0 = a.in_seq[(int64_t)t * n + io];
+        }
+      }
+      if constexpr (G::FC) {
+        if (adam_mode) {   // m' = b1 m + (1-b1) g ; v' = b2 v + (1-b2) g^2 ; m~ = m^/(sqrt(v^)+1e-8) ; g~ = g/(sqrt(v^)+1e-8)
+          const float gg = raw0;
+          am = a.beta1 * am + (1.0f - a.beta1) * gg;
+          av = a.beta2 * av + (1.0f - a.beta2) * gg * gg;
+          const float mh = am / adamc[2 * t], vh = av / adamc[2 * t + 1];
+          const float den = sqrtf(vh) + 1e-8f;
+          raw0 = mh / den;
+          raw1 = gg / den;
+        }
+        if (writer && a.feat_rec) {
+          a.feat_rec[((int64_t)t * 2) * n + io] = raw0;
+          a.feat_rec[((int64_t)t * 2 + 1) * n + io] = raw1;
+        }
+        // u = elu([m~, g~] Win + bin) (DM/networks.py:219) for the thread's 5 fc outputs of both rows
+#pragma unroll
+        for (int rh = 0; rh < 2; ++rh) {
+          const float m0 = from_row(raw0, lane, rh), m1 = from_row(raw1, lane, rh);
+          float u[kU];
+#pragma unroll
+          for (int s = 0; s < kU; ++s) {
+            const int j = 5 * q + s;
+            u[s] = elu_fast(fmaf(m1, S.win[kH + j], fmaf(m0, S.win[j], S.win[2 * kH + j])));
           }
-          if (lane == 0) {
-            uint32_t total = 0;
+          A.template put_vec<0>(rh, u);
+        }
+      } else {
+        float f[C::F];
+        preprocess<C>(nullptr, rt, raw0, raw1, f);
 #pragma unroll
-            for (int tile = 0; tile < kTiles; ++tile) {
-              const int64_t base = pair * kTileCoords + tile * 128;
-              const int64_t cnt = n - base < 0 ? 0 : (n - base > 128 ? 128 : n - base);
-              total += (uint32_t)cnt * 4u * kH * 4u;
-            }
-            mbar_expect_tx(&S.full[buf], total);
+        for (int rh = 0; rh < 2; ++rh) {
+          float v = q == C::F ? 1.0f : 0.f;
 #pragma unroll
-            for (int tile = 0; tile < kTiles; ++tile) {
-              const int64_t base = pair * kTileCoords + tile * 128;
-              const int64_t cnt = n - base < 0 ? 0 : (n - base > 128 ? 128 : n - base);
-              if (cnt > 0) {
-#pragma unroll
-                for (int arr = 0; arr < 4; ++arr)
-                  tma_bulk_g2s(stage + (size_t)((buf * kTiles + tile) * 4 + arr) * kStageArr,
-                               a.state + (int64_t)arr * n * kH + base * kH, (uint32_t)cnt * kH * 4u, &S.full[buf]);
-              }
-            }
+          for (int k = 0; k < C::F; ++k) {
+            const float fk = from_row(f[k], lane, rh);
+            if (q == k) v = fk;
           }
-          __syncwarp();
+          A.template put<0>(rh, v);
+        }
+      }
+      if (want_fx) {
+        const double ws = warp_sum_d(q < 2 ? (double)fval : 0.0);
+        if (lane == 0) atomicAdd(&S.fx[t], ws);
+      }
+      // ---- layer 1 ---------------------------------------------------------------------------------------------------
+      wg_fence();
+      mma3<kN, G::KB, G::L1Lo, G::L1Hi>(d, A, b1h, b1l);
+      wg_commit();
+      wg_wait<0>();
+#pragma unroll
+      for (int rh = 0; rh < 2; ++rh) {
+        float h[kU];
+#pragma unroll
+        for (int s = 0; s < kU; ++s)
+          lstm_point_fwd(d[acc_idx(s, 0, rh)], d[acc_idx(s, 1, rh)], d[acc_idx(s, 2, rh)], d[acc_idx(s, 3, rh)], c1[rh][s], h[s]);
+        A.template put_vec<G::ColH1>(rh, h);
+        if (act[rh]) {
+          const int64_t i = row[rh];
+          if (a.ckpt) {
+            float* ck = a.ckpt + (int64_t)(t + 1) * slot;
+            store5(ck + i * kH, q, h);
+            store5(ck + (n + i) * kH, q, c1[rh]);
+          }
+          if (t == T - 1) {
+            store5(state_out + i * kH, q, h);
+            store5(state_out + (n + i) * kH, q, c1[rh]);
+          }
+        }
+      }
+      // ---- layer 2 + output layer + parameter add --------------------------------------------------------------------
+      wg_fence();
+      mma3<kN, G::KB, G::L2Lo, G::L2Hi>(d, A, b2h, b2l);
+      wg_commit();
+      wg_wait<0>();
+      float y[2];
+#pragma unroll
+      for (int rh = 0; rh < 2; ++rh) {
+        float h[kU];
+        float yp = 0.f;
+#pragma unroll
+        for (int s = 0; s < kU; ++s) {
+          lstm_point_fwd(d[acc_idx(s, 0, rh)], d[acc_idx(s, 1, rh)], d[acc_idx(s, 2, rh)], d[acc_idx(s, 3, rh)], c2[rh][s], h[s]);
+          yp = fmaf(h[s], wo[s], yp);
+        }
+        A.template put_vec<G::ColH2>(rh, h);
+        y[rh] = quad_sum(yp) + bo;
+        if (act[rh]) {
+          const int64_t i = row[rh];
+          if (a.ckpt) {
+            float* ck = a.ckpt + (int64_t)(t + 1) * slot + 2 * n * kH;
+            store5(ck + i * kH, q, h);
+            store5(ck + (n + i) * kH, q, c2[rh]);
+          }
+          if (t == T - 1) {
+            store5(state_out + 2 * n * kH + i * kH, q, h);
+            store5(state_out + 2 * n * kH + (n + i) * kH, q, c2[rh]);
+          }
+        }
+      }
+      const float yo = own ? y[1] : y[0];
+      const float dl = rt.tanh_output ? tanh_acc(yo) * rt.scale : yo * rt.scale;
+      x += dl;
+      if (writer) {
+        if (a.delta_seq) a.delta_seq[(int64_t)t * n + io] = dl;
+        if (a.labels) {
+          const float r = a.labels[(int64_t)t * n + io] - dl;
+          imit += 0.5 * (double)r * (double)r;
         }
       }
     }
-  } else {
-    // =============================== MMA issuer warp ===============================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kFwdIssuerRegs));
-    // The whole warp runs this loop (warp-uniform => descriptors live in uniform registers and the UTCHMMA issue
-    // rate matches the tensor pipe); elect.sync picks the one lane whose tcgen05.mma / commit take effect.
-    mbar_wait(&S.wbar, 0);  // weights landed (TMA complete_tx)
-    const uint32_t idesc = make_idesc(kN);
-    const uint32_t img_s = smem_u32(S.img);
-    const uint64_t b1h = make_bdesc(img_s);
-    const uint64_t b1l = make_bdesc(img_s + G::B1Floats * 4);
-    const uint64_t b2h = make_bdesc(img_s + 2 * G::B1Floats * 4);
-    const uint64_t b2l = make_bdesc(img_s + (2 * G::B1Floats + G::B2Floats) * 4);
-    constexpr uint64_t kStep = (2 * kLBO) >> 4;  // descriptor start-address increment per K=8 chunk
-    uint32_t pa[kTiles] = {0, 0};
-    if constexpr (G::SplitD) {
-      // Polling issuer over the two tiles; per tile the events alternate A(t) (features + h2 final: layer 1's last
-      // K-step, commit, then layer 2's h2 K-steps early) and B(t) (h1' final: layer 2's remaining K-steps, commit, then
-      // the NEXT step's layer-1 h1 K-steps early).  K-step 0 of both layers holds the feature chunk + h1 units 0..3.
-      constexpr int kS1 = G::K1 / 8, kS2 = G::K2 / 8, kS2Early = (G::ColH2 + 7) / 8;   // 3, 6, 3
-      static_assert(G::A2Off == 0 && kS1 == 3 && kS2 == 6 && kS2Early == 3, "split-accumulator schedule: DM row layout");
-      auto kstep = [&](uint32_t d, uint32_t ah, uint32_t al, uint64_t bh, uint64_t bl, int kc, uint32_t acc) {
-        mma_tf32_ts(d, al + 8 * kc, bh + kc * kStep, idesc, acc);
-        mma_tf32_ts(d, ah + 8 * kc, bl + kc * kStep, idesc, 1u);
-        mma_tf32_ts(d, ah + 8 * kc, bh + kc * kStep, idesc, 1u);
-      };
-      for (int64_t pair = blockIdx.x; pair < npairs; pair += gridDim.x) {
-        int ev[kTiles] = {0, 0};
-        while (ev[0] < 2 * T || ev[1] < 2 * T) {
-#pragma unroll
-          for (int tile = 0; tile < kTiles; ++tile) {
-            if (ev[tile] >= 2 * T || !mbar_test(&S.a_ready[tile], pa[tile])) continue;
-            pa[tile] ^= 1;
-            const int e = ev[tile]++;
-            const int t = e >> 1;
-            if (lane == 0) L2O_FPROF(3, (tile << 1) | (e & 1));
-            if (lane == 0) L2O_FDBG(20 + tile, e);
-            const uint32_t t_d = tmem_base + tile * G::TileCols, t_d2 = t_d + kN;
-            const uint32_t t_ah = t_d + G::DCols, t_al = t_ah + G::ACols;
-            tc_fence_after();
-            if (elect_one()) {
-              if ((e & 1) == 0) {
-                if (t == 0) {   // first step of a pair: nothing was issued ahead
-                  kstep(t_d, t_ah, t_al, b1h, b1l, 1, 0u);
-                  kstep(t_d, t_ah, t_al, b1h, b1l, 2, 1u);
-                }
-                kstep(t_d, t_ah, t_al, b1h, b1l, 0, 1u);
-                tc_commit(&S.d_ready[tile]);
-#pragma unroll
-                for (int kc = kS2Early; kc < kS2; ++kc) kstep(t_d2, t_ah, t_al, b2h, b2l, kc, kc > kS2Early ? 1u : 0u);
-              } else {
-#pragma unroll
-                for (int kc = 0; kc < kS2Early; ++kc) kstep(t_d2, t_ah, t_al, b2h, b2l, kc, 1u);
-                tc_commit(&S.d_ready[tile]);
-                if (t + 1 < T) {
-                  kstep(t_d, t_ah, t_al, b1h, b1l, 1, 0u);
-                  kstep(t_d, t_ah, t_al, b1h, b1l, 2, 1u);
-                }
-              }
-            }
-            __syncwarp();
-          }
-        }
+    // ---- tile epilogue: x, f(x_T), g_T, Adam moments ---------------------------------------------------------------
+    float fval = 0.f;
+    if (writer) {
+      if (in_kernel_opt) {
+        float gT;
+        optimizee_eval(a.opt_kind, x, oa, ob, a.opt_alpha, a.opt_fscale, fval, gT);
+        if (a.g_rec) a.g_rec[(int64_t)T * n + io] = gT;
       }
-    } else
-    for (int64_t pair = blockIdx.x; pair < npairs; pair += gridDim.x) {
-      for (int t = 0; t < T; ++t) {
-#pragma unroll
-        for (int layer = 0; layer < 2; ++layer) {
-#pragma unroll
-          for (int tile = 0; tile < kTiles; ++tile) {
-            const uint32_t t_d = tmem_base + tile * G::TileCols;
-            const uint32_t t_ah = t_d + G::DCols;
-            const uint32_t t_al = t_ah + G::ACols;
-            mbar_wait(&S.a_ready[tile], pa[tile]);
-            pa[tile] ^= 1;
-            tc_fence_after();
-            if (elect_one()) {
-              if (layer == 0) {
-#pragma unroll
-                for (int kc = 0; kc < G::K1 / 8; ++kc) {
-                  mma_tf32_ts(t_d, t_al + 8 * kc, b1h + kc * kStep, idesc, kc > 0 ? 1u : 0u);
-                  mma_tf32_ts(t_d, t_ah + 8 * kc, b1l + kc * kStep, idesc, 1u);
-                  mma_tf32_ts(t_d, t_ah + 8 * kc, b1h + kc * kStep, idesc, 1u);
-                }
-              } else {
-#pragma unroll
-                for (int kc = 0; kc < G::K2 / 8; ++kc) {
-                  mma_tf32_ts(t_d, t_al + G::A2Off + 8 * kc, b2h + kc * kStep, idesc, kc > 0 ? 1u : 0u);
-                  mma_tf32_ts(t_d, t_ah + G::A2Off + 8 * kc, b2l + kc * kStep, idesc, 1u);
-                  mma_tf32_ts(t_d, t_ah + G::A2Off + 8 * kc, b2h + kc * kStep, idesc, 1u);
-                }
-              }
-              tc_commit(&S.d_ready[tile]);
-            }
-            __syncwarp();
-          }
-        }
-      }
+      if (a.x) a.x[io] = x;
+      if (adam_mode) { a.m[io] = am; a.v[io] = av; }
+    }
+    if (want_fx) {
+      const double ws = warp_sum_d((double)fval);
+      if (lane == 0) atomicAdd(&S.fx[T], ws);
     }
   }
-  // ---- teardown ----
-  tc_fence_before();
+  if (a.labels && a.imit_loss) {
+    const double ws = warp_sum_d(imit);
+    if (lane == 0) atomicAdd(a.imit_loss, ws / (double)a.n_total);
+  }
   __syncthreads();
-  tc_fence_after();
   if (want_fx)
     for (int t = threadIdx.x; t <= T; t += blockDim.x) atomicAdd(&a.fx[t], S.fx[t]);
-  if (warp == kIssuerWarp) tmem_dealloc(tmem_base, kTmemCols);
 }
 
 }  // namespace tc
 
-// ------------------------------------------------------------------ host side (called from l2o_capi.cu)
+// ------------------------------------------------------------------ host side (called from l2o_tc.cu)
 template <class C>
 int tc_launch_fwd(const NetRt& rt, const l2o_unroll_args& a, float* img, cudaStream_t st, int sms, float* state_out = nullptr,
-                  bool stage = false, tc::FwdExtra ex = tc::FwdExtra{nullptr, 0, 0.f}, bool prep = true) {
-  if (prep) tc::prep_weights_kernel<C><<<8, 256, 0, st>>>(a.theta, img, 0);
-  // stage: TMA-prefetched state rows (the l2o_step path, T = 1); needs 16-byte aligned arrays (n * 80 B always is)
-  stage = stage && (reinterpret_cast<uintptr_t>(a.state) % 16 == 0);
-  auto k = stage ? tc::unroll_fwd_kernel<C, true> : tc::unroll_fwd_kernel<C, false>;
-  // + the TMA state ring (step regime) or the staging area of the checkpoint stores (training unroll)
-  const size_t smem = tc::stage_offset<C>(a.T) +
-                      (stage ? (size_t)tc::kStageFloats * sizeof(float)
-                             : (a.ckpt ? (size_t)tc::kTiles * 4 * tc::kStageArr * sizeof(float) : 0)) + 128;
+                  tc::FwdExtra ex = tc::FwdExtra{nullptr, 0, 0.f}, bool prep = true) {
+  if (prep) tc::prep_weights_kernel<C><<<16, 256, 0, st>>>(a.theta, img, 0);
+  auto k = tc::unroll_fwd_kernel<C>;
+  const size_t smem = tc::fwd_smem_bytes<C>(a.T);
   if (smem > 227 * 1024) return L2O_E_INVALID;
   if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return L2O_E_CUDA;
-  const int64_t npairs = (a.n + tc::kTileCoords - 1) / tc::kTileCoords;
-  const int grid = (int)(npairs < sms ? npairs : sms);
-  k<<<grid, tc::kThreads, smem, st>>>(a, rt, img, state_out ? state_out : a.state, ex);
+  const int64_t ntiles = (a.n + tc::kTile - 1) / tc::kTile;
+  const int64_t ctas = (ntiles + tc::kFwdWG - 1) / tc::kFwdWG;
+  const int grid = (int)(ctas < sms ? ctas : sms);
+  k<<<grid, tc::kFwdThreads, smem, st>>>(a, rt, img, state_out ? state_out : a.state, ex);
   return cudaGetLastError() == cudaSuccess ? L2O_OK : L2O_E_CUDA;
 }
 

@@ -1,14 +1,22 @@
-// tcgen05 BPTT kernel (sm_100a) for the LSTM-20x2 coordinate-wise optimizer (meta-loss mode).
+// Tensor-core BPTT kernel (sm_90a, wgmma) through a T-step unroll of the LSTM-20x2 (cwlstm_tc.cuh operand layout).
 //
-// Per 128-coordinate tile and per time step (descending), every contraction runs on the tensor cores with
-// error-compensated 3xTF32 and fp32 accumulation in tensor memory:
-//   Z1 = A_F[0:32].B1, Z2 = A_F[0:48].B2      gate recompute from the checkpointed (h, c)   TS-mode (A in TMEM)
-//   dX2 = dZ2.W2^T (N=48), dX1 = dZ1.W1^T (N=32) TS-mode; B = the SAME forward weight image, addressed MN-major
-//   dW2^T += dZ2^T.X2, dW1^T += dZ1^T.X1        SS-mode over MN-major operands staged in shared memory by the
-//                                               epilogue threads; accumulators stay in TMEM for the whole kernel
-// CTA = one tile: 8 epilogue warps (thread pair per coordinate: hidden units 0..11 | 12..19) + 1 MMA-issuer warp.
-// Semantics: SURVEY.md Appendix B (derived from DM/meta.py:319-376, second_derivatives=False).
+// Per warpgroup tile of 64 coordinates, walking t = T-1 .. 0 from the checkpoints:
+//   layer 2:  Z2 = [1 | h1n | h2p] . B2  (3xTF32, register-A)  -> gates, output layer, LSTM backward -> dZ2
+//             dX2 = dZ2 . W2^T           (3xTF32, the dZ2 accumulators reused as A fragments)  -> dh1n(t), dh2p carry
+//   layer 1:  Z1 = [u, 1 | h1p] . B1 -> LSTM backward with dh1 = carry + dh1n(t) -> dZ1;  dX1 = dZ1 . W1^T -> dh1p carry
+//   dW:       dW^T rows += X^T . dZ over the tile's coordinates, on the bf16 tensor cores from shared-memory staging
+//             (x = hi + lo, hi = bf16_rn(x), lo = bf16_rn(x - hi); products hi.hi + hi.lo + lo.hi, fp32 accumulate).
+//             Both layers share ONE 64 x 80 accumulator: the operand rows of layer 2 (h1n 0..19 | h2p 20..39 | 1 40) and
+//             of layer 1 (h1p 41..60 | features 61.. | 1) are disjoint, and each layer's staged X^T keeps the other
+//             layer's rows at zero, so the two K = 64 contractions add into disjoint accumulator rows.  The accumulators
+//             are drained into the fp64 dtheta after every tile (bounded fp32 accumulation length).
+// fc(20) nets (RNNProp) run the two layers as two passes over time (MODE 1: layer 2, exporting dX2[h1n] to the
+// caller's hand-over buffer; MODE 2: layer 1 with the fc layer's own gradient), DM nets both layers in one pass (MODE 0).
+// Semantics: SURVEY.md Appendix B (derived from DM/meta.py:319-376, second_derivatives=False); imitation mode
+// DM/meta_dm_train.py:472-475.
 #pragma once
+#include <cuda_bf16.h>
+
 #include "cwlstm_tc.cuh"
 
 namespace l2o {
@@ -16,566 +24,448 @@ namespace tcb {
 
 using namespace tc;
 
-constexpr int kEpi = 256;
-constexpr int kThreadsB = kEpi + 128;
-#ifndef L2O_EPI_REGS
-#define L2O_EPI_REGS 224
-#endif
-constexpr int kEpiRegs = L2O_EPI_REGS, kIssuerRegs = 40;
-// TMEM column map.  The A operand of the gate recompute is ALIASED into the dZ operand region: it is dead once Z1/Z2
-// have completed (before dZ2 is written) and is rewritten only after the previous step's dX1 MMAs have drained.
-constexpr int cD1 = 0;                   // Z1 accumulators (read by the layer-1 backward phase)
-constexpr int cD2 = 80;                  // Z2 accumulators, then dX2 / dX1 results (aliased)
-constexpr int cAZh = 160, cAZl = 240;    // dZ rows (80 gate columns), hi / lo
-constexpr int cAh = cAZh, cAl = cAZl;    // A rows [h1p | u,1 | h1n | h2p] (64 columns), hi / lo -- aliased
-constexpr int cW2 = 320;                 // dW2^T accumulator: lanes = gate rows, 48 feature columns
-constexpr int cW1 = 368;                 // dW1^T accumulator: 32 feature columns
-// The layer-1 input rows [h1p | u,1] get their own (non-aliased) copy: the issuer runs Z2 first and commits it alone,
-// so the epilogue starts the layer-2 backward (which overwrites the aliased region with dZ2) while the Z1 MMAs are
-// still reading A1; Z1 is needed only by the layer-1 phase and is covered by the dX2 commit.
-constexpr int cA1h = 400, cA1l = 424;    // 24 columns each
-static_assert(cA1l + 24 <= kTmemCols, "TMEM budget");
-// Staged operand Y = [X (48 feature slots) | dZ (80 gate slots)] per coordinate, MN-major SWIZZLE_128B_BASE32B
-// (the only shared-memory layout the tensor core accepts for MN-major tf32; address map verified on the B200 with
-// scripts/umma_probe.cu):  byte(mn, c) = (c/4)*kYSBO + (mn/32)*kYLBO + (c%4)*128 + (((mn%32)/8) ^ (c%4))*32 + (mn%8)*4
-// The SAME buffer is the A operand (M = 128 slots) and the B operand (N = 48 / 32 feature slots) of
-// dW^T-block = Y^T.Y : rows 48..127 (gate slots) x cols 0..47 (feature slots) is dZ^T.X.
-constexpr int kYSlots = 128;
-constexpr int kYX = 0, kYZ = 48;                 // slot bases of X and dZ inside a Y row
-constexpr uint32_t kYLBO = 512;                  // bytes between 32-slot MN atoms
-constexpr uint32_t kYSBO = 4 * 512;              // bytes between 4-coordinate K atoms
-constexpr int kYFloats = 128 * kYSlots;          // 16384 floats = 64 KB per hi / lo buffer
+constexpr int kBwdWG = 2;                       // warpgroups per CTA (they share the weight image)
+constexpr int kBwdThreads = 128 * kBwdWG;
+// staged dW operands per warpgroup (bf16, K-major: the 64 coordinates of the tile are the contraction index)
+constexpr uint32_t kXaLBO = 8 * 128;            // X^T: 64 rows (8 core-matrix groups) per 8 coordinates
+constexpr uint32_t kXbLBO = 10 * 128;           // dZ^T: 80 rows
+constexpr uint32_t kXaBytes = 8 * kXaLBO;       // per hi / lo
+constexpr uint32_t kXbBytes = 8 * kXbLBO;
+// dW accumulator rows
+constexpr int kRowH1N = 0, kRowH2P = 20, kRowOne2 = 40;                 // layer 2 (and MODE 2: h1p | e | 1)
+constexpr int kRowH1P = 41, kRowFeat = 61;                              // layer 1 of DM nets (MODE 0)
 
-#ifdef L2O_TC_PROF
-// timeline instrumentation (scripts/tc_bwd_prof.cu only): clock64 stamps of CTA 0 at every phase boundary
-__device__ long long g_prof[3 * 2048];
-#define L2O_PROF(role, idx) \
-  do { if (blockIdx.x == 0 && (idx) < 2048) g_prof[(role) * 2048 + (idx)] = clock64(); } while (0)
-#else
-#define L2O_PROF(role, idx) do { } while (0)
-#endif
-
-struct SmemB {
-  float y_hi[kYFloats];        // 1024-B aligned (first member)
-  float y_lo[kYFloats];
-  float img[kImgAllFloats];    // B1h|B1l|B2h|B2l (forward, K-major) | T1h|T1l|T2h|T2l (transposed, K-major)
-  float wo[kH + 4];
-  uint64_t wbar, a_ready, d_ready, w_done;
-  uint32_t tmem_slot, pad;
-};
-static_assert(sizeof(SmemB) + 1024 <= 227 * 1024, "shared memory budget");
-
-__host__ __device__ constexpr uint32_t make_idesc_ex(int n, int a_mn, int b_mn) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) |
-         ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
+__device__ __forceinline__ uint32_t xa_off(int m, int k) {
+  return (uint32_t)((m >> 3) * 128 + (k >> 3) * (int)kXaLBO + (m & 7) * 16 + (k & 7) * 2);
 }
-// layout_type: 0 = no swizzle (interleave), 1 = SWIZZLE_128B_BASE32B   (cute::UMMA::LayoutType)
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo, uint32_t layout_type = 0) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32) |
-         (1ull << 46) | ((uint64_t)layout_type << 61);
+__device__ __forceinline__ uint32_t xb_off(int nn, int k) {
+  return (uint32_t)((nn >> 3) * 128 + (k >> 3) * (int)kXbLBO + (nn & 7) * 16 + (k & 7) * 2);
 }
-__device__ __forceinline__ void mma_tf32_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
+__device__ __forceinline__ void split_bf16(float x, uint16_t& hi, uint16_t& lo) {
+  const __nv_bfloat16 h = __float2bfloat16_rn(x);
+  hi = __bfloat16_as_ushort(h);
+  lo = __bfloat16_as_ushort(__float2bfloat16_rn(x - __bfloat162float(h)));
+}
+__device__ __forceinline__ void sts16(uint32_t sa, uint16_t v) {
+  asm volatile("st.shared.u16 [%0], %1;" ::"r"(sa), "h"(v) : "memory");
+}
+// value v at (row, coordinate) of a staged hi / lo pair (lo at +lo_off bytes)
+__device__ __forceinline__ void stage_bf16(uint32_t base, uint32_t off, uint32_t lo_off, float v) {
+  uint16_t h, l;
+  split_bf16(v, h, l);
+  sts16(base + off, h);
+  sts16(base + lo_off + off, l);
+}
+// D[64 x 80] += A[64 x 16] (shared, bf16, K-major) . B[16 x 80] (shared, bf16, K-major)
+__device__ __forceinline__ void mma_ss_bf16_n80(float* d, uint64_t a, uint64_t b) {
   asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %42, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n80k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,"
+      "%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39}, "
+      "%40, %41, p, 1, 1, 0, 0;\n\t}\n"
+      : L2O_ACC8(0), L2O_ACC8(8), L2O_ACC8(16), L2O_ACC8(24), L2O_ACC8(32)
+      : "l"(a), "l"(b), "r"(1));
 }
-__device__ __forceinline__ void tmem_ld4(uint32_t taddr, float* v) {
-  uint32_t r[4];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(taddr)
-               : "memory");
-  tc_wait_ld();
-#pragma unroll
-  for (int k = 0; k < 4; ++k) v[k] = __uint_as_float(r[k]);
-}
-__device__ __forceinline__ float4 split4_hi(const float* v, float4& lo) {
-  float h0, h1, h2, h3;
-  split_tf32(v[0], h0, lo.x);
-  split_tf32(v[1], h1, lo.y);
-  split_tf32(v[2], h2, lo.z);
-  split_tf32(v[3], h3, lo.w);
-  return make_float4(h0, h1, h2, h3);
-}
-// 4 values -> TMEM A columns (hi/lo) and, optionally, the MN-major smem staging (hi/lo) at float index `sidx`
-__device__ __forceinline__ void put4(uint32_t t_hi, uint32_t t_lo, int col, const float* v, float* s_hi, float* s_lo,
-                                     int sidx, bool to_tmem, bool to_smem) {
-  float4 lo;
-  const float4 hi = split4_hi(v, lo);
-  if (to_tmem) {
-    tmem_st4(t_hi + col, hi.x, hi.y, hi.z, hi.w);
-    tmem_st4(t_lo + col, lo.x, lo.y, lo.z, lo.w);
-  }
-  if (to_smem) {
-    *reinterpret_cast<float4*>(s_hi + sidx) = hi;
-    *reinterpret_cast<float4*>(s_lo + sidx) = lo;
-  }
-}
-// float index of the 16-byte group holding slots [mn, mn+4) (mn % 4 == 0) of coordinate c in a Y buffer
-__device__ __forceinline__ int y_sidx(int c, int mn) {
-  return (c >> 2) * (int)(kYSBO / 4) + (mn >> 5) * (int)(kYLBO / 4) + (c & 3) * 32 + ((((mn & 31) >> 3) ^ (c & 3)) << 3) + (mn & 7);
-}
-__device__ __forceinline__ int dz_sidx(int c, int unit) { return y_sidx(c, kYZ + 4 * unit); }
-__device__ __forceinline__ int x_sidx(int c, int grp) { return y_sidx(c, kYX + 4 * grp); }
+// named barrier over the 128 threads of warpgroup wg
+__device__ __forceinline__ void wg_bar(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 
-// activated gates of 4 units from 16 interleaved accumulator columns
-__device__ __forceinline__ void gates4(const float* z, float* g) {
-#pragma unroll
-  for (int u = 0; u < 4; ++u) {
-    g[4 * u + 0] = sigmoid_fast(z[4 * u + 0]);
-    g[4 * u + 1] = tanh_fast(z[4 * u + 1]);
-    g[4 * u + 2] = sigmoid_fast(z[4 * u + 2] + 1.0f);
-    g[4 * u + 3] = sigmoid_fast(z[4 * u + 3]);
-  }
-}
-// LSTM pointwise backward for one unit; g = (i, j, f, o) -> overwritten with (dz_i, dz_j, dz_f, dz_o)
-__device__ __forceinline__ void unit_bwd(float* g, float cprev, float tcn, float dh, float& dc) {
-  const float i = g[0], j = g[1], f = g[2], o = g[3];
+// LSTM pointwise backward for one unit from the pre-activations (i, j, f, o) -> overwritten with dz; c: previous cell
+// state; dh: gradient of h'; dc: carry in (gradient of c') / out (gradient of c).  hn: h' (the output layer needs it).
+__device__ __forceinline__ void unit_bwd(float& zi, float& zj, float& zf, float& zo, float cprev, float dh, float& dc, float& hn) {
+  const float i = sigmoid_fast(zi), j = tanh_fast(zj), f = sigmoid_fast(zf + 1.0f), o = sigmoid_fast(zo);
+  const float cn = fmaf(f, cprev, i * j);
+  const float tcn = tanh_fast(cn);
+  hn = tcn * o;
   const float dho = dh * o;
   const float dcv = fmaf(dho, fmaf(-tcn, tcn, 1.0f), dc);
-  g[0] = (dcv * j) * fmaf(-i, i, i);           // sigma' = i - i^2
-  g[1] = (dcv * i) * fmaf(-j, j, 1.0f);        // tanh'  = 1 - j^2
-  g[2] = (dcv * cprev) * fmaf(-f, f, f);
-  g[3] = (dho * tcn) * (1.0f - o);             // dh tcn o (1 - o)
+  zi = (dcv * j) * fmaf(-i, i, i);           // sigma' = i - i^2
+  zj = (dcv * i) * fmaf(-j, j, 1.0f);        // tanh'  = 1 - j^2
+  zf = (dcv * cprev) * fmaf(-f, f, f);
+  zo = (dho * tcn) * (1.0f - o);             // dh tcn o (1 - o)
   dc = dcv * f;
 }
 
-template <class C, int HALF>
-__device__ __forceinline__ void epilogue(const l2o_bwd_args& a, const NetRt& rt, SmemB& S, uint32_t tmem_base, int warp,
-                                         int lane) {
-  constexpr int U0 = HALF == 0 ? 0 : 12;  // first hidden unit owned by this thread
-  constexpr int NU = HALF == 0 ? 12 : 8;  // number of owned units (multiples of 4: whole x16 accumulator loads)
-  const int q = warp & 3;
-  const int c = q * 32 + lane;  // coordinate within the tile == TMEM lane
-  const uint32_t tl = tmem_base + ((uint32_t)(q * 32) << 16);
-  const uint32_t tD1 = tl + cD1, tD2 = tl + cD2, tAh = tl + cAh, tAl = tl + cAl, tAZh = tl + cAZh, tAZl = tl + cAZl;
-  const uint32_t tA1h = tl + cA1h, tA1l = tl + cA1l;
-  const int T = a.T;
-  const int64_t n = a.n;
-  const int64_t slot = n * C::SF;
-  const int64_t ntiles = (n + 127) / 128;
-  uint32_t pd = 0;  // parity of d_ready (Z1+Z2, dX2, dX1 in turn)
-  int pi = 0;       // profile event index
-  const bool prof = (q == 0 && lane == 0);
-  (void)pi; (void)prof;
-  bool dx1_pending = false;  // a dX1 batch whose completion has not been consumed yet
-  // w_done completes exactly twice per step: dW2 (even completion, parity 0) then dW1 (odd, parity 1)
-  float acc_wo[NU], acc_bo = 0.f;
-#pragma unroll
-  for (int k = 0; k < NU; ++k) acc_wo[k] = 0.f;
-  if (HALF == 0) {  // zero the persistent dW accumulators (lane = gate row)
-#pragma unroll
-    for (int k = 0; k < (48 + 32) / 4; ++k) tmem_st4(tl + cW2 + 4 * k, 0.f, 0.f, 0.f, 0.f);
+// theta index of dW accumulator row m, gate column n (-1: padding row)
+template <class C, int MODE>
+__device__ __forceinline__ int dw_index(int m, int n) {
+  const int col = gate_ref_col(n);
+  if (MODE == 2) {   // fc nets, layer 1: h1p | e | 1  (lstm_1/w_gates rows: the 20 fc outputs first, then h1)
+    if (m < kRowH2P) return C::O_W1 + (C::F + m) * C::G1 + col;
+    if (m < kRowOne2) return C::O_W1 + (m - kRowH2P) * C::G1 + col;
+    return m == kRowOne2 ? C::O_B1 + col : -1;
   }
-  tc_wait_st();
+  if (m < kRowOne2) return C::O_W2 + m * C::G2 + col;   // h1n rows 0..19, h2p rows 20..39 of lstm_2/w_gates
+  if (m == kRowOne2) return C::O_B2 + col;
+  if (MODE == 0) {
+    if (m < kRowFeat) return C::O_W1 + (C::F + m - kRowH1P) * C::G1 + col;
+    if (m < kRowFeat + C::F) return C::O_W1 + (m - kRowFeat) * C::G1 + col;
+    if (m == kRowFeat + C::F) return C::O_B1 + col;
+  }
+  return -1;
+}
 
-  for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    const int64_t i = tile * 128 + c;
-    const bool act = i < n;
-    float dh1c[NU], dc1c[NU], dh2c[NU], dc2c[NU];
+template <class C, int MODE>
+struct SmemB {
+  float img[Geo<C>::AllFloats];   // B1h|B1l|B2h|B2l|T1h|T1l|T2h|T2l; must stay first (TMA destination)
+  float wo[kH + 4];
+  float win[64];
+  uint64_t wbar, pad;
+};
+template <class C, int MODE>
+__host__ __device__ constexpr uint32_t stage_bytes() {   // per warpgroup: Xa (layer 2) [| Xa (layer 1)] | Xb, hi + lo each
+  return (MODE == 0 ? 4 : 2) * kXaBytes + 2 * kXbBytes;
+}
+template <class C, int MODE>
+__host__ __device__ constexpr size_t bwd_smem_bytes() {
+  return ((sizeof(SmemB<C, MODE>) + 1023) & ~(size_t)1023) + (size_t)kBwdWG * stage_bytes<C, MODE>();
+}
+
+// MODE 0: both layers (DM nets); 1: layer 2 only, dX2[h1n] exported to a.scratch [T][n][20]; 2: layer 1 of an fc net,
+// dX2[h1n] read from a.scratch.
+template <class C, int MODE>
+__global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args a, NetRt rt, const float* __restrict__ img) {
+  using G = Geo<C>;
+  static_assert(MODE == 0 ? !C::FC : C::FC, "DM nets: one pass; fc nets: two passes");
+  static_assert(MODE != 0 || kRowFeat + C::F < 64, "dW rows of both layers fit one 64-row accumulator");
+  extern __shared__ __align__(1024) unsigned char smem_raw[];
+  SmemB<C, MODE>& S = *reinterpret_cast<SmemB<C, MODE>*>(smem_raw);
+  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const int g = lane >> 2, q = lane & 3;
+  const uint32_t stage = smem_u32(smem_raw) + (uint32_t)((sizeof(SmemB<C, MODE>) + 1023) & ~(size_t)1023) +
+                         (uint32_t)wg * stage_bytes<C, MODE>();
+  constexpr uint32_t kXa2 = 0, kXa1 = 2 * kXaBytes;                          // MODE 0 only has kXa1
+  constexpr uint32_t kXb = (MODE == 0 ? 4 : 2) * kXaBytes;
+  constexpr bool kL2 = MODE != 2, kL1 = MODE != 1;
+
+  // zero the staging (rows of the other layer stay zero for the whole kernel)
+  for (uint32_t o = threadIdx.x * 4; o < kBwdWG * stage_bytes<C, MODE>(); o += blockDim.x * 4)
+    asm volatile("st.shared.u32 [%0], 0;" ::"r"(stage - (uint32_t)wg * stage_bytes<C, MODE>() + o) : "memory");
+  if (threadIdx.x < kH) S.wo[threadIdx.x] = a.theta[C::O_WO + threadIdx.x];
+  if constexpr (C::FC) {
+    if (threadIdx.x >= 32 && threadIdx.x < 92) S.win[threadIdx.x - 32] = a.theta[C::O_WIN + threadIdx.x - 32];
+  }
+  if (threadIdx.x == 0) {
+    mbar_init(&S.wbar, 1);
+    fence_barrier_init();
+  }
+  fence_proxy_async();
+  __syncthreads();
+  stage_image(S.img, img, G::AllFloats * 4, &S.wbar);
+
+  const uint64_t b1h = img_desc(S.img, kN), b1l = img_desc(S.img + G::B1Floats, kN);
+  const uint64_t b2h = img_desc(S.img + 2 * G::B1Floats, kN), b2l = img_desc(S.img + 2 * G::B1Floats + G::B2Floats, kN);
+  const float* tbase = S.img + G::FwdFloats;
+  const uint64_t t1h = img_desc(tbase, G::N1), t1l = img_desc(tbase + G::T1Floats, G::N1);
+  const uint64_t t2h = img_desc(tbase + 2 * G::T1Floats, G::N2), t2l = img_desc(tbase + 2 * G::T1Floats + G::T2Floats, G::N2);
+  const uint64_t xbh = make_desc(stage + kXb, kXbLBO, 128), xbl = make_desc(stage + kXb + kXbBytes, kXbLBO, 128);
+  const uint64_t xa2h = make_desc(stage + kXa2, kXaLBO, 128), xa2l = make_desc(stage + kXa2 + kXaBytes, kXaLBO, 128);
+  const uint64_t xa1h = make_desc(stage + (MODE == 0 ? kXa1 : kXa2), kXaLBO, 128);
+  const uint64_t xa1l = make_desc(stage + (MODE == 0 ? kXa1 : kXa2) + kXaBytes, kXaLBO, 128);
+
+  const int T = a.T;
+  const int64_t n = a.n, slot = n * C::SF;
+  const int64_t ntiles = (n + tc::kTile - 1) / tc::kTile;
+  const bool imit = a.labels != nullptr;
+  const float inv_nt = imit ? 1.0f / (float)a.n_total : 0.f;
+  float wo[kU];
 #pragma unroll
-    for (int k = 0; k < NU; ++k) { dh1c[k] = 0.f; dc1c[k] = 0.f; dh2c[k] = 0.f; dc2c[k] = 0.f; }
-    // dDelta_t: meta-loss mode = running suffix sum of the recorded gradients (SURVEY.md App. B); imitation mode =
-    // (delta_t - label_t) / N_total from the forward pass's recorded deltas (DM/meta_dm_train.py:472-475)
-    const bool imit = a.labels != nullptr;
-    const float inv_nt = imit ? 1.0f / (float)a.n_total : 0.f;
-    float lam = (act && !imit) ? a.g_rec[(int64_t)T * n + i] : 0.f;
+  for (int s = 0; s < kU; ++s) wo[s] = S.wo[5 * q + s];
+  float acc_wo[kU] = {0.f, 0.f, 0.f, 0.f, 0.f}, acc_bo = 0.f;
+  float aw0[kU] = {0.f, 0.f, 0.f, 0.f, 0.f}, aw1[kU] = {0.f, 0.f, 0.f, 0.f, 0.f}, ab[kU] = {0.f, 0.f, 0.f, 0.f, 0.f};
+  float dw[kN / 2];
+#pragma unroll
+  for (int k = 0; k < kN / 2; ++k) dw[k] = 0.f;
+  const int kx = warp * 16 + g;   // staged coordinate index of row rh = kx + 8 rh
+
+  Frag<G::KB> A;
+  // X^T rows of this thread's units of the 20-vector at operand column `col`: row base + 5q + s, coordinate kx + 8 rh
+  auto stage_vec = [&](uint32_t xh, int base, int rh, int col) {
+#pragma unroll
+    for (int s = 0; s < kU; ++s) stage_bf16(xh, xa_off(base + 5 * q + s, kx + 8 * rh), kXaBytes, A.get_at(col + 4 * s, rh));
+  };
+  auto stage_dz = [&](const float* z) {
+#pragma unroll
+    for (int j = 0; j < kN / 8; ++j)
+#pragma unroll
+      for (int rh = 0; rh < 2; ++rh)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) stage_bf16(stage + kXb, xb_off(8 * j + 2 * q + e, kx + 8 * rh), kXbBytes, z[4 * j + 2 * rh + e]);
+  };
+  // dX_l = dZ_l . W_l^T (3xTF32; the dZ accumulators as A fragments, cwlstm_tc.cuh dx_gate_col) then the dW batch
+  auto dx_dw = [&](auto ncols, float* z, float* x, uint64_t th, uint64_t tl, uint64_t xah, uint64_t xal) {
+    constexpr int NX = decltype(ncols)::value;
+    uint32_t fh[kN / 8][4], fl[kN / 8][4];
+#pragma unroll
+    for (int j = 0; j < kN / 8; ++j) {
+      split_tf32(z[4 * j + 0], fh[j][0], fl[j][0]);
+      split_tf32(z[4 * j + 2], fh[j][1], fl[j][1]);
+      split_tf32(z[4 * j + 1], fh[j][2], fl[j][2]);
+      split_tf32(z[4 * j + 3], fh[j][3], fl[j][3]);
+    }
+    constexpr uint64_t step = img_kstep(NX);
+    wg_fence();
+#pragma unroll
+    for (int j = 0; j < kN / 8; ++j) {
+      mma_rs<NX>(x, fl[j], th + j * step, j > 0 ? 1u : 0u);
+      mma_rs<NX>(x, fh[j], tl + j * step, 1u);
+      mma_rs<NX>(x, fh[j], th + j * step, 1u);
+    }
+    wg_commit();
+    constexpr uint64_t sa = (2 * kXaLBO) >> 4, sb = (2 * kXbLBO) >> 4;
+#pragma unroll
+    for (int kk = 0; kk < tc::kTile / 16; ++kk) {
+      mma_ss_bf16_n80(dw, xal + kk * sa, xbh + kk * sb);
+      mma_ss_bf16_n80(dw, xah + kk * sa, xbl + kk * sb);
+      mma_ss_bf16_n80(dw, xah + kk * sa, xbh + kk * sb);
+    }
+    wg_commit();
+    wg_wait<1>();   // dX done; the dW batch may still run (the next wait<0> retires it)
+  };
+  auto flush_dw = [&]() {
+    wg_wait<0>();
+#pragma unroll
+    for (int j = 0; j < kN / 8; ++j)
+#pragma unroll
+      for (int rh = 0; rh < 2; ++rh)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float& v = dw[4 * j + 2 * rh + e];
+          const int idx = dw_index<C, MODE>(warp * 16 + g + 8 * rh, 8 * j + 2 * q + e);
+          if (idx >= 0 && v != 0.f) atomicAdd(&a.dtheta[idx], (double)v);
+          v = 0.f;
+        }
+  };
+
+  for (int64_t tile = (int64_t)blockIdx.x * kBwdWG + wg; tile < ntiles; tile += (int64_t)gridDim.x * kBwdWG) {
+    const int64_t r0 = tile * tc::kTile + warp * 16 + g;
+    const int64_t row[2] = {r0, r0 + 8};
+    const bool act[2] = {row[0] < n, row[1] < n};
+    float dc2[2][kU], dh2c[2][kU], dc1[2][kU], dh1c[2][kU];
+#pragma unroll
+    for (int rh = 0; rh < 2; ++rh)
+#pragma unroll
+      for (int s = 0; s < kU; ++s) { dc2[rh][s] = 0.f; dh2c[rh][s] = 0.f; dc1[rh][s] = 0.f; dh1c[rh][s] = 0.f; }
+    float lam[2];
+#pragma unroll
+    for (int rh = 0; rh < 2; ++rh) lam[rh] = (kL2 && act[rh] && !imit) ? a.g_rec[(int64_t)T * n + row[rh]] : 0.f;
+    A.zero();
+    A.template put<(G::ColOne & ~3)>(0, q == (G::ColOne & 3) ? 1.0f : 0.f);
+    A.template put<(G::ColOne & ~3)>(1, q == (G::ColOne & 3) ? 1.0f : 0.f);
 
     for (int t = T - 1; t >= 0; --t) {
       const float* ck = a.ckpt + (int64_t)t * slot;
-      // ---------------- P0: checkpoint rows -> A = [h1p | u,1 | h1n | h2p] ----------------
-      // h1n(t), the layer-1 output of step t, IS the checkpointed h1 of slot t+1: no layer-1 recompute is needed to
-      // form the layer-2 input, so Z1 and Z2 are issued back to back.  Loads go out before the dX1 wait.
-      float u4[4] = {0.f, 0.f, 0.f, 0.f};
-      float h1p[NU], h1n[NU], h2p[NU], c1p[NU], c2p[NU];
+      float z[kN / 2];
+      float dh1n[2][kU];
+      // ================================= layer 2 =================================
+      if constexpr (kL2) {
+        float c2p[2][kU], dy[2];
 #pragma unroll
-      for (int k = 0; k < NU; ++k) { h1p[k] = 0.f; h1n[k] = 0.f; h2p[k] = 0.f; c1p[k] = 0.f; c2p[k] = 0.f; }
-      float raw0 = 0.f;
-      if (HALF == 1 && act) raw0 = a.in_seq[(int64_t)t * n + i];  // only half 1 owns the feature chunk
-      if (imit && act) lam = (a.delta_seq[(int64_t)t * n + i] - a.labels[(int64_t)t * n + i]) * inv_nt;
-      if (act) {
-        load_vec<NU>(ck + i * kH + U0, h1p);
-        load_vec<NU>(ck + slot + i * kH + U0, h1n);
-        load_vec<NU>(ck + 2 * n * kH + i * kH + U0, h2p);
-        load_vec<NU>(ck + (n + i) * kH + U0, c1p);
-        load_vec<NU>(ck + 2 * n * kH + (n + i) * kH + U0, c2p);
-        if (t > 0) {  // pull the following step's rows towards L2
-          const float* nk = ck - slot;
-          asm volatile("prefetch.global.L2 [%0];" ::"l"(nk + i * kH + U0));
-          asm volatile("prefetch.global.L2 [%0];" ::"l"(nk + 2 * n * kH + i * kH + U0));
-          asm volatile("prefetch.global.L2 [%0];" ::"l"(nk + (n + i) * kH + U0));
-          asm volatile("prefetch.global.L2 [%0];" ::"l"(nk + 2 * n * kH + (n + i) * kH + U0));
-          if (HALF == 1) {
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(a.in_seq + (int64_t)(t - 1) * n + i));
-            if (!imit) asm volatile("prefetch.global.L2 [%0];" ::"l"(a.g_rec + (int64_t)(t - 1) * n + i));
+        for (int rh = 0; rh < 2; ++rh) {
+          float h1n[kU] = {0.f, 0.f, 0.f, 0.f, 0.f}, h2p[kU] = {0.f, 0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+          for (int s = 0; s < kU; ++s) c2p[rh][s] = 0.f;
+          float dtanh = 1.0f;
+          if (act[rh]) {
+            const int64_t i = row[rh];
+            load5(ck + slot + i * kH, q, h1n);   // h1n(t) IS the checkpointed h1 of slot t+1
+            load5(ck + 2 * n * kH + i * kH, q, h2p);
+            load5(ck + 2 * n * kH + (n + i) * kH, q, c2p[rh]);
+            if (imit) lam[rh] = (a.delta_seq[(int64_t)t * n + i] - a.labels[(int64_t)t * n + i]) * inv_nt;
+            if (rt.tanh_output) {   // delta = scale tanh(y): the recorded delta gives tanh' without y
+              const float th = a.delta_seq[(int64_t)t * n + i] / rt.scale;
+              dtanh = fmaf(-th, th, 1.0f);
+            }
+          }
+          dy[rh] = rt.scale * lam[rh] * dtanh;
+          A.template put_vec<G::ColH1>(rh, h1n);
+          A.template put_vec<G::ColH2>(rh, h2p);
+        }
+        wg_fence();
+        mma3<kN, G::KB, G::L2Lo, G::L2Hi>(z, A, b2h, b2l);
+        wg_commit();
+        wg_wait<0>();   // also retires every earlier dW batch of this warp
+        if (q == 0) acc_bo += dy[0] + dy[1];
+#pragma unroll
+        for (int rh = 0; rh < 2; ++rh)
+#pragma unroll
+          for (int s = 0; s < kU; ++s) {
+            float hn;
+            unit_bwd(z[acc_idx(s, 0, rh)], z[acc_idx(s, 1, rh)], z[acc_idx(s, 2, rh)], z[acc_idx(s, 3, rh)], c2p[rh][s],
+                     fmaf(wo[s], dy[rh], dh2c[rh][s]), dc2[rh][s], hn);
+            acc_wo[s] = fmaf(hn, dy[rh], acc_wo[s]);
+          }
+        wg_bar(wg);   // every warp has retired the previous dW batch: the staging may be overwritten
+#pragma unroll
+        for (int rh = 0; rh < 2; ++rh) {
+          stage_vec(stage + kXa2, kRowH1N, rh, G::ColH1);
+          stage_vec(stage + kXa2, kRowH2P, rh, G::ColH2);
+          if (q == 0) stage_bf16(stage + kXa2, xa_off(kRowOne2, kx + 8 * rh), kXaBytes, 1.0f);
+        }
+        stage_dz(z);
+        fence_proxy_async();
+        wg_bar(wg);
+        float x2[G::N2 / 2];
+        dx_dw(IC<G::N2>{}, z, x2, t2h, t2l, xa2h, xa2l);
+#pragma unroll
+        for (int rh = 0; rh < 2; ++rh)
+#pragma unroll
+          for (int s = 0; s < kU; ++s) {
+            // dX column of slot s: 8 (s / 2) + 2q + (s % 2) in group 0 (h1n), + 24 in group 1 (h2p)
+            dh1n[rh][s] = x2[4 * (s >> 1) + 2 * rh + (s & 1)];
+            dh2c[rh][s] = x2[4 * (3 + (s >> 1)) + 2 * rh + (s & 1)];
+          }
+        if constexpr (MODE == 1) {
+#pragma unroll
+          for (int rh = 0; rh < 2; ++rh)
+            if (act[rh]) store5(a.scratch + ((int64_t)t * n + row[rh]) * kH, q, dh1n[rh]);
+        }
+#pragma unroll
+        for (int rh = 0; rh < 2; ++rh)
+          if (!imit && act[rh]) lam[rh] += a.g_rec[(int64_t)t * n + row[rh]];
+      }
+      // ================================= layer 1 =================================
+      if constexpr (kL1) {
+        float c1p[2][kU];
+        float r0v[2] = {0.f, 0.f}, r1v[2] = {0.f, 0.f};
+        float ep[2][kU];   // fc nets: elu'(a) of the thread's fc outputs
+#pragma unroll
+        for (int rh = 0; rh < 2; ++rh) {
+          float h1p[kU] = {0.f, 0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+          for (int s = 0; s < kU; ++s) c1p[rh][s] = 0.f;
+          if (act[rh]) {
+            const int64_t i = row[rh];
+            load5(ck + i * kH, q, h1p);
+            load5(ck + (n + i) * kH, q, c1p[rh]);
+            if constexpr (MODE == 2) {
+              load5(a.scratch + ((int64_t)t * n + i) * kH, q, dh1n[rh]);
+              r0v[rh] = a.in_seq[((int64_t)t * 2) * n + i];
+              r1v[rh] = a.in_seq[((int64_t)t * 2 + 1) * n + i];
+            } else {
+              r0v[rh] = a.in_seq[(int64_t)t * n + i];
+            }
+          } else if constexpr (MODE == 2) {
+#pragma unroll
+            for (int s = 0; s < kU; ++s) dh1n[rh][s] = 0.f;
+          }
+          A.template put_vec<G::ColH1>(rh, h1p);
+          if constexpr (MODE == 2) {
+            // e = elu([m~, g~] Win + bin) for the thread's units, as the forward kernel computes it
+            float e[kU];
+#pragma unroll
+            for (int s = 0; s < kU; ++s) {
+              const int u = 5 * q + s;
+              const float av = fmaf(r1v[rh], S.win[kH + u], fmaf(r0v[rh], S.win[u], S.win[2 * kH + u]));
+              e[s] = elu_fast(av);
+              ep[rh][s] = av > 0.f ? 1.0f : e[s] + 1.0f;   // elu' = exp(a) on the negative side
+            }
+            A.template put_vec<0>(rh, e);
+          } else {
+            float f[C::F];
+            preprocess<C>(nullptr, rt, r0v[rh], 0.f, f);
+            float v = q == C::F ? 1.0f : 0.f;
+#pragma unroll
+            for (int k = 0; k < C::F; ++k)
+              if (q == k) v = f[k];
+            A.template put<0>(rh, v);
           }
         }
-      }
-      if (HALF == 1) {
-        float uu[C::F];
-        preprocess<C>(nullptr, rt, raw0, 0.f, uu);
+        wg_fence();
+        mma3<kN, G::KB, G::L1Lo, G::L1Hi>(z, A, b1h, b1l);
+        wg_commit();
+        wg_wait<0>();
 #pragma unroll
-        for (int k = 0; k < C::F; ++k) u4[k] = uu[k];
-        u4[C::F] = 1.0f;
-      }
-      if (prof) { L2O_PROF(HALF, pi); ++pi; }
-      if (dx1_pending) {  // previous step's dX1 = dZ1 . W1^T : carries, and the dZ operand region becomes free
-        mbar_wait(&S.d_ready, pd);
-        pd ^= 1;
-        tc_fence_after();
-        dx1_pending = false;
-        if (t != T - 1) {
+        for (int rh = 0; rh < 2; ++rh)
 #pragma unroll
-          for (int g4 = 0; g4 < NU / 4; ++g4) {
-            float v[4];
-            tmem_ld4(tD2 + U0 + 4 * g4, v);
+          for (int s = 0; s < kU; ++s) {
+            float hn;
+            unit_bwd(z[acc_idx(s, 0, rh)], z[acc_idx(s, 1, rh)], z[acc_idx(s, 2, rh)], z[acc_idx(s, 3, rh)], c1p[rh][s],
+                     dh1c[rh][s] + dh1n[rh][s], dc1[rh][s], hn);
+          }
+        wg_bar(wg);
 #pragma unroll
-            for (int u = 0; u < 4; ++u) dh1c[4 * g4 + u] = v[u];
+        for (int rh = 0; rh < 2; ++rh) {
+          if constexpr (MODE == 2) {
+            stage_vec(stage + kXa2, kRowH1N, rh, G::ColH1);   // h1p
+            stage_vec(stage + kXa2, kRowH2P, rh, 0);          // e
+            if (q == 0) stage_bf16(stage + kXa2, xa_off(kRowOne2, kx + 8 * rh), kXaBytes, 1.0f);
+          } else {
+            stage_vec(stage + kXa1, kRowH1P, rh, G::ColH1);
+            if (q <= C::F) stage_bf16(stage + kXa1, xa_off(kRowFeat + q, kx + 8 * rh), kXaBytes, A.get_at(0, rh));
           }
         }
-      }
-      if (prof) { L2O_PROF(HALF, pi); ++pi; }
-      if (HALF == 1) {  // the feature chunk feeds both layers' bias row: aliased copy (Z2) + A1 copy (Z1)
-        put4(tAh, tAl, kBColXC, u4, nullptr, nullptr, 0, true, false);
-        put4(tA1h, tA1l, kBColXC, u4, nullptr, nullptr, 0, true, false);
-      }
+        stage_dz(z);
+        fence_proxy_async();
+        wg_bar(wg);
+        float x1[G::N1 / 2];
+        dx_dw(IC<G::N1>{}, z, x1, t1h, t1l, xa1h, xa1l);
 #pragma unroll
-      for (int g4 = 0; g4 < NU / 4; ++g4) {
-        put4(tA1h, tA1l, U0 + 4 * g4, h1p + 4 * g4, nullptr, nullptr, 0, true, false);
-        // aliased columns 16..19 sit inside Z2's contraction range (zero weight rows): keep them finite
-        if (U0 + 4 * g4 == kBZ2Start) put4(tAh, tAl, kBZ2Start, h1p + 4 * g4, nullptr, nullptr, 0, true, false);
-        put4(tAh, tAl, kBColH1N + U0 + 4 * g4, h1n + 4 * g4, nullptr, nullptr, 0, true, false);
-        put4(tAh, tAl, kBColH2P + U0 + 4 * g4, h2p + 4 * g4, nullptr, nullptr, 0, true, false);
-      }
-      tc_wait_st();
-      tc_fence_before();
-      mbar_arrive(&S.a_ready);
-      if (prof) { L2O_PROF(HALF, pi); ++pi; }
-      // ---------------- P2: layer-2 gates + output layer + layer-2 backward ----------------
-      mbar_wait(&S.d_ready, pd);
-      pd ^= 1;
-      tc_fence_after();
-      if (prof) { L2O_PROF(HALF, pi); ++pi; }
-      const float dy = rt.scale * lam;  // dDelta_t = sum_{tau>t} g_tau ; linear output (tanh_output handled by FFMA engine)
-      if (HALF == 1) acc_bo += dy;
-      // staging buffers must be free: the dW1 MMAs of the previous step have completed
-      mbar_wait(&S.w_done, 1);  // passes trivially on the fresh barrier (first step)
-      if (prof) { L2O_PROF(HALF, pi); ++pi; }
-      {
+        for (int rh = 0; rh < 2; ++rh)
 #pragma unroll
-        for (int g4 = 0; g4 < NU / 4; ++g4) {
-          float z[16], g[16];
-          tmem_ld16(tD2 + 4 * U0 + 16 * g4, z);
-          gates4(z, g);
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const int k = 4 * g4 + u;
-            const float cn = fmaf(g[4 * u + 2], c2p[k], g[4 * u + 0] * g[4 * u + 1]);
-            const float tcn = tanh_fast(cn);
-            const float h2n = tcn * g[4 * u + 3];
-            acc_wo[k] = fmaf(h2n, dy, acc_wo[k]);
-            const float dh = fmaf(S.wo[U0 + k], dy, dh2c[k]);
-            unit_bwd(g + 4 * u, c2p[k], tcn, dh, dc2c[k]);
-            // dz of this unit: one 16-byte group of the MN-major staging + 4 TMEM columns
-            put4(tAZh, tAZl, 4 * (U0 + k), g + 4 * u, S.y_hi, S.y_lo, dz_sidx(c, U0 + k), true, true);
+          for (int s = 0; s < kU; ++s) {
+            dh1c[rh][s] = x1[4 * (s >> 1) + 2 * rh + (s & 1)];
+            if constexpr (MODE == 2) {   // da = de * elu'(a);  dWin += [m~, g~]^T da, dbin += da
+              const float da = x1[4 * (3 + (s >> 1)) + 2 * rh + (s & 1)] * ep[rh][s];
+              aw0[s] = fmaf(r0v[rh], da, aw0[s]);
+              aw1[s] = fmaf(r1v[rh], da, aw1[s]);
+              ab[s] += da;
+            }
           }
-        }
-        // X2 row = A columns 16..63 = [h1p tail (unused) | u,1 | h1n | h2p]  (slot = column - 16)
-        if (HALF == 1) put4(0, 0, 0, u4, S.y_hi, S.y_lo, x_sidx(c, (kBColXC - kBZ2Start) / 4), false, true);
-#pragma unroll
-        for (int g4 = 0; g4 < NU / 4; ++g4) {
-          put4(0, 0, 0, h1n + 4 * g4, S.y_hi, S.y_lo, x_sidx(c, (kBColH1N - kBZ2Start + U0) / 4 + g4), false, true);
-          put4(0, 0, 0, h2p + 4 * g4, S.y_hi, S.y_lo, x_sidx(c, (kBColH2P - kBZ2Start + U0) / 4 + g4), false, true);
-        }
       }
-      fence_proxy_async();
-      tc_wait_st();
-      tc_fence_before();
-      mbar_arrive(&S.a_ready);
-      if (prof) { L2O_PROF(HALF, pi); ++pi; }
-      // ---------------- P3: layer-1 backward ----------------
-      mbar_wait(&S.d_ready, pd);
-      pd ^= 1;
-      tc_fence_after();
-      if (prof) { L2O_PROF(HALF, pi); ++pi; }
-      float dh1[NU];
+    }
+    flush_dw();
+  }
+  wg_wait<0>();
+  // ---- output layer (layer-2 passes) and fc layer (MODE 2) gradients: per-thread sums over the warp's rows -----------
+  auto red8 = [&](float v) {   // sum over the 8 lanes with the same q
 #pragma unroll
-      for (int g4 = 0; g4 < NU / 4; ++g4) {  // dX2 columns are in Z2 contraction order: 8.. = h1n, 28.. = h2p
-        float v[4];
-        tmem_ld4(tD2 + (kBColH1N - kBZ2Start) + U0 + 4 * g4, v);
+    for (int o = 4; o < 32; o <<= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+  };
 #pragma unroll
-        for (int u = 0; u < 4; ++u) dh1[4 * g4 + u] = v[u] + dh1c[4 * g4 + u];
-        tmem_ld4(tD2 + (kBColH2P - kBZ2Start) + U0 + 4 * g4, v);
-#pragma unroll
-        for (int u = 0; u < 4; ++u) dh2c[4 * g4 + u] = v[u];
+  for (int s = 0; s < kU; ++s) {
+    const int u = 5 * q + s;
+    if constexpr (kL2) {
+      const float v = red8(acc_wo[s]);
+      if (lane < 4) atomicAdd(&a.dtheta[C::O_WO + u], (double)v);
+    }
+    if constexpr (MODE == 2) {
+      const float v0 = red8(aw0[s]), v1 = red8(aw1[s]), vb = red8(ab[s]);
+      if (lane < 4) {
+        atomicAdd(&a.dtheta[C::O_WIN + u], (double)v0);
+        atomicAdd(&a.dtheta[C::O_WIN + C::F + u], (double)v1);
+        atomicAdd(&a.dtheta[C::O_BIN + u], (double)vb);
       }
-      {
-        // compute dz1 and feed the dX1 A operand (TMEM) first; the shared staging is touched only after the dW2 MMAs
-        // have drained, so their ~2K cycles overlap with this phase's arithmetic instead of stalling it
-        float dz1[4 * NU];
-#pragma unroll
-        for (int g4 = 0; g4 < NU / 4; ++g4) {
-          float z[16];
-          tmem_ld16(tD1 + 4 * U0 + 16 * g4, z);
-          gates4(z, dz1 + 16 * g4);
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const int k = 4 * g4 + u;
-            float* g = dz1 + 16 * g4 + 4 * u;
-            const float cn = fmaf(g[2], c1p[k], g[0] * g[1]);
-            const float tcn = tanh_fast(cn);
-            unit_bwd(g, c1p[k], tcn, dh1[k], dc1c[k]);
-            put4(tAZh, tAZl, 4 * (U0 + k), g, nullptr, nullptr, 0, true, false);
-          }
-        }
-        mbar_wait(&S.w_done, 0);  // dW2 MMAs done: staging may be overwritten
-        if (prof) { L2O_PROF(HALF, pi); ++pi; }
-        // X1 row = A columns 0..23 = [h1p | u,1]
-#pragma unroll
-        for (int g4 = 0; g4 < NU / 4; ++g4) {
-#pragma unroll
-          for (int u = 0; u < 4; ++u)
-            put4(0, 0, 0, dz1 + 16 * g4 + 4 * u, S.y_hi, S.y_lo, dz_sidx(c, U0 + 4 * g4 + u), false, true);
-          put4(0, 0, 0, h1p + 4 * g4, S.y_hi, S.y_lo, x_sidx(c, U0 / 4 + g4), false, true);
-        }
-        if (HALF == 1) put4(0, 0, 0, u4, S.y_hi, S.y_lo, x_sidx(c, kBColXC / 4), false, true);
-      }
-      fence_proxy_async();
-      tc_wait_st();
-      tc_fence_before();
-      mbar_arrive(&S.a_ready);
-      dx1_pending = true;
-      if (prof) { L2O_PROF(HALF, pi); ++pi; }
-      if (act && !imit) lam += a.g_rec[(int64_t)t * n + i];
     }
   }
-  if (dx1_pending) {  // drain the last dX1 completion so the barrier phase bookkeeping stays consistent
-    mbar_wait(&S.d_ready, pd);
-    pd ^= 1;
-  }
-  // ---------------- flush: output-layer gradient from registers ----------------
-#pragma unroll
-  for (int k = 0; k < NU; ++k) {
-    float v = acc_wo[k];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if (lane == 0) atomicAdd(&a.dtheta[C::O_WO + U0 + k], (double)v);
-  }
-  if (HALF == 1) {
-    float v = acc_bo;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if constexpr (kL2) {
+    const float v = red8(acc_bo);
     if (lane == 0) atomicAdd(&a.dtheta[C::O_BO], (double)v);
   }
-  // ---------------- flush: dW^T accumulators (lane = interleaved gate row) ----------------
-  mbar_wait(&S.w_done, 1);  // last dW1 MMAs complete
-  tc_fence_after();
-  if (HALF == 0) {
-    const int m = c - kYZ;  // Y slot -> interleaved gate row 4u+g (slots below kYZ hold the unused X^T.X block)
-    const int col = (m & 3) * kH + (m >> 2);
-#pragma unroll
-    for (int k4 = 0; k4 < 48 / 4; ++k4) {
-      float v[4];
-      tmem_ld4(tl + cW2 + 4 * k4, v);
-      if (m >= 0 && m < kN) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int k = 4 * k4 + e;
-          int idx = -1;  // slot k <-> A column kBZ2Start + k
-          const int acol = kBZ2Start + k;
-          if (acol == kBColXC + C::F) idx = C::O_B2 + col;
-          else if (acol >= kBColH1N && acol < kBColH1N + 2 * kH) idx = C::O_W2 + (acol - kBColH1N) * C::G2 + col;
-          if (idx >= 0) atomicAdd(&a.dtheta[idx], (double)v[e]);
-        }
-      }
-    }
-#pragma unroll
-    for (int k4 = 0; k4 < 32 / 4; ++k4) {
-      float v[4];
-      tmem_ld4(tl + cW1 + 4 * k4, v);
-      if (m >= 0 && m < kN) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int k = 4 * k4 + e;
-          int idx = -1;  // slot k <-> A column k
-          if (k < kH) idx = C::O_W1 + (C::F + k) * C::G1 + col;
-          else if (k < kBColXC + C::F) idx = C::O_W1 + (k - kBColXC) * C::G1 + col;
-          else if (k == kBColXC + C::F) idx = C::O_B1 + col;
-          if (idx >= 0) atomicAdd(&a.dtheta[idx], (double)v[e]);
-        }
-      }
-    }
-  }
-}
-
-template <class C>
-__global__ void __launch_bounds__(kThreadsB, 1) unroll_bwd_kernel(l2o_bwd_args a, NetRt rt, const float* __restrict__ img) {
-  extern __shared__ __align__(1024) unsigned char smem_raw[];
-  SmemB& S = *reinterpret_cast<SmemB*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int T = a.T;
-  const int64_t ntiles = (a.n + 127) / 128;
-
-  for (int k = threadIdx.x; k < kYFloats; k += blockDim.x) { S.y_hi[k] = 0.f; S.y_lo[k] = 0.f; }
-  if (threadIdx.x < kH) S.wo[threadIdx.x] = a.theta[C::O_WO + threadIdx.x];
-  if (warp == kEpi / 32) {
-    if (lane == 0) {
-      mbar_init(&S.wbar, 1);
-      mbar_init(&S.a_ready, kEpi);
-      mbar_init(&S.d_ready, 1);
-      mbar_init(&S.w_done, 1);
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc(&S.tmem_slot, kTmemCols);
-    tmem_relinquish();
-    if (lane == 0) {
-      mbar_expect_tx(&S.wbar, kImgAllBytes);
-      tma_bulk_g2s(S.img, img, kImgAllBytes, &S.wbar);
-    }
-  }
-  fence_proxy_async();
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = S.tmem_slot;
-
-  if (warp < kEpi / 32) {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kEpiRegs));
-    if (warp < 4) epilogue<C, 0>(a, rt, S, tmem_base, warp, lane);
-    else epilogue<C, 1>(a, rt, S, tmem_base, warp, lane);
-  } else if (warp > kEpi / 32) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kIssuerRegs));
-  } else {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kIssuerRegs));
-    mbar_wait(&S.wbar, 0);
-    {  // warp-uniform issuer (see cwlstm_tc.cuh): elect.sync predicates the MMAs / commits to one lane
-      const uint32_t img_s = smem_u32(S.img);
-      // forward (K-major) views
-      const uint64_t b1h = make_bdesc(img_s), b1l = make_bdesc(img_s + kB1Floats * 4);
-      const uint64_t b2h = make_bdesc(img_s + 2 * kB1Floats * 4), b2l = make_bdesc(img_s + (2 * kB1Floats + kB2Floats) * 4);
-      // transposed images (K-major, no swizzle): T[n' = input][k' = gate]; 16-byte K chunk stride = (rows/8)*128
-      const uint32_t t_s = img_s + kImgFloats * 4;
-      constexpr uint32_t kT1LBO = (kT1Rows / 8) * 128, kT2LBO = (kT2Rows / 8) * 128;
-      const uint64_t t1h = make_desc(t_s, kT1LBO, 128), t1l = make_desc(t_s + kT1Floats * 4, kT1LBO, 128);
-      const uint64_t t2h = make_desc(t_s + 2 * kT1Floats * 4, kT2LBO, 128);
-      const uint64_t t2l = make_desc(t_s + (2 * kT1Floats + kT2Floats) * 4, kT2LBO, 128);
-      // staged Y (MN-major SWIZZLE_128B_BASE32B): both operands of the dW products
-      const uint64_t yh = make_desc(smem_u32(S.y_hi), kYLBO, kYSBO, 1), yl = make_desc(smem_u32(S.y_lo), kYLBO, kYSBO, 1);
-      constexpr uint32_t id_fwd = make_idesc_ex(kN, 0, 0);
-      constexpr uint32_t id_dx2 = make_idesc_ex(48, 0, 0), id_dx1 = make_idesc_ex(32, 0, 0);
-      constexpr uint32_t id_dw2 = make_idesc_ex(48, 1, 1), id_dw1 = make_idesc_ex(32, 1, 1);
-      constexpr uint64_t kFwdStep = (2 * kLBO) >> 4;      // K-major: 8 k = two 16-byte chunks
-      constexpr uint64_t kT1Step = (2 * kT1LBO) >> 4, kT2Step = (2 * kT2LBO) >> 4;  // 8 gates = two 16-byte chunks
-      constexpr uint64_t kYStep = (2 * kYSBO) >> 4;       // 8 coordinates = two K atoms
-      const uint32_t tD1 = tmem_base + cD1, tD2 = tmem_base + cD2, tAh = tmem_base + cAh, tAl = tmem_base + cAl;
-      const uint32_t tAZh = tmem_base + cAZh, tAZl = tmem_base + cAZl, tW2 = tmem_base + cW2, tW1 = tmem_base + cW1;
-      const uint32_t tA1h = tmem_base + cA1h, tA1l = tmem_base + cA1l;
-      uint32_t pa = 0;
-      int pi = 0;
-      (void)pi;
-      for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        for (int t = T - 1; t >= 0; --t) {
-          // Z2 = A[16:64].B2' first, committed alone (the layer-2 phase starts on it); then Z1 = A1[0:24].B1', which
-          // only the layer-1 phase reads, after the dX2 commit.  Both depend only on checkpointed rows.
-          mbar_wait(&S.a_ready, pa); pa ^= 1; tc_fence_after();
-          L2O_PROF(2, pi); ++pi;
-          if (elect_one()) {
-#pragma unroll
-            for (int kc = 0; kc < kK2 / 8; ++kc) {
-              mma_tf32_ts(tD2, tAl + kBZ2Start + 8 * kc, b2h + kc * kFwdStep, id_fwd, kc > 0 ? 1u : 0u);
-              mma_tf32_ts(tD2, tAh + kBZ2Start + 8 * kc, b2l + kc * kFwdStep, id_fwd, 1u);
-              mma_tf32_ts(tD2, tAh + kBZ2Start + 8 * kc, b2h + kc * kFwdStep, id_fwd, 1u);
-            }
-            tc_commit(&S.d_ready);
-#pragma unroll
-            for (int kc = 0; kc < kK1 / 8; ++kc) {
-              mma_tf32_ts(tD1, tA1l + 8 * kc, b1h + kc * kFwdStep, id_fwd, kc > 0 ? 1u : 0u);
-              mma_tf32_ts(tD1, tA1h + 8 * kc, b1l + kc * kFwdStep, id_fwd, 1u);
-              mma_tf32_ts(tD1, tA1h + 8 * kc, b1h + kc * kFwdStep, id_fwd, 1u);
-            }
-          }
-          __syncwarp();
-          L2O_PROF(2, pi); ++pi;
-          // dX2 = dZ2 . W2^T   and   dW2^T += dZ2^T . X2
-          mbar_wait(&S.a_ready, pa); pa ^= 1; tc_fence_after();
-          L2O_PROF(2, pi); ++pi;
-          if (elect_one()) {
-#pragma unroll
-            for (int kc = 0; kc < kN / 8; ++kc) {
-              mma_tf32_ts(tD2, tAZl + 8 * kc, t2h + kc * kT2Step, id_dx2, kc > 0 ? 1u : 0u);
-              mma_tf32_ts(tD2, tAZh + 8 * kc, t2l + kc * kT2Step, id_dx2, 1u);
-              mma_tf32_ts(tD2, tAZh + 8 * kc, t2h + kc * kT2Step, id_dx2, 1u);
-            }
-            tc_commit(&S.d_ready);
-          }
-          __syncwarp();
-          L2O_PROF(2, pi); ++pi;
-          if (elect_one()) {
-#pragma unroll
-            for (int kb = 0; kb < 16; ++kb) {
-              mma_tf32_ss(tW2, yl + kb * kYStep, yh + kb * kYStep, id_dw2, 1u);
-              mma_tf32_ss(tW2, yh + kb * kYStep, yl + kb * kYStep, id_dw2, 1u);
-              mma_tf32_ss(tW2, yh + kb * kYStep, yh + kb * kYStep, id_dw2, 1u);
-            }
-            tc_commit(&S.w_done);
-          }
-          __syncwarp();
-          L2O_PROF(2, pi); ++pi;
-          // dX1 = dZ1 . W1^T   and   dW1^T += dZ1^T . X1
-          mbar_wait(&S.a_ready, pa); pa ^= 1; tc_fence_after();
-          L2O_PROF(2, pi); ++pi;
-          if (elect_one()) {
-#pragma unroll
-            for (int kc = 0; kc < kN / 8; ++kc) {
-              mma_tf32_ts(tD2, tAZl + 8 * kc, t1h + kc * kT1Step, id_dx1, kc > 0 ? 1u : 0u);
-              mma_tf32_ts(tD2, tAZh + 8 * kc, t1l + kc * kT1Step, id_dx1, 1u);
-              mma_tf32_ts(tD2, tAZh + 8 * kc, t1h + kc * kT1Step, id_dx1, 1u);
-            }
-            tc_commit(&S.d_ready);
-          }
-          __syncwarp();
-          L2O_PROF(2, pi); ++pi;
-          if (elect_one()) {
-#pragma unroll
-            for (int kb = 0; kb < 16; ++kb) {
-              mma_tf32_ss(tW1, yl + kb * kYStep, yh + kb * kYStep, id_dw1, 1u);
-              mma_tf32_ss(tW1, yh + kb * kYStep, yl + kb * kYStep, id_dw1, 1u);
-              mma_tf32_ss(tW1, yh + kb * kYStep, yh + kb * kYStep, id_dw1, 1u);
-            }
-            tc_commit(&S.w_done);
-          }
-          __syncwarp();
-          L2O_PROF(2, pi); ++pi;
-        }
-      }
-    }
-    __syncwarp();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == kEpi / 32) tmem_dealloc(tmem_base, kTmemCols);
 }
 
 }  // namespace tcb
 
 template <class C>
-int tc_launch_bwd(const NetRt& rt, const l2o_bwd_args& a, float* img, cudaStream_t st, int sms) {
-  tc::prep_weights_kernel<C><<<8, 256, 0, st>>>(a.theta, img, 1);
-  auto k = tcb::unroll_bwd_kernel<C>;
-  const size_t smem = sizeof(tcb::SmemB) + 1024;
-  if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return L2O_E_CUDA;
-  const int64_t ntiles = (a.n + 127) / 128;
-  const int grid = (int)(ntiles < sms ? ntiles : sms);
-  k<<<grid, tcb::kThreadsB, smem, st>>>(a, rt, img);
-  return cudaGetLastError() == cudaSuccess ? L2O_OK : L2O_E_CUDA;
+int tc_launch_bwd(const NetRt& rt, const l2o_bwd_args& a, float* img, cudaStream_t st, int sms, bool prep = true) {
+  if (prep) tc::prep_weights_kernel<C><<<16, 256, 0, st>>>(a.theta, img, 1);
+  const int64_t ntiles = (a.n + tc::kTile - 1) / tc::kTile;
+  const int64_t ctas = (ntiles + tcb::kBwdWG - 1) / tcb::kBwdWG;
+  const int grid = (int)(ctas < sms ? ctas : sms);
+  auto launch = [&](auto kern, size_t smem) {
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return L2O_E_CUDA;
+    kern<<<grid, tcb::kBwdThreads, smem, st>>>(a, rt, img);
+    return cudaGetLastError() == cudaSuccess ? L2O_OK : L2O_E_CUDA;
+  };
+  if constexpr (C::FC) {
+    // two passes over time: layer 2 (exporting dX2[h1n] to a.scratch), then layer 1 fed by it
+    int rc = launch(tcb::unroll_bwd_kernel<C, 1>, tcb::bwd_smem_bytes<C, 1>());
+    if (rc != L2O_OK) return rc;
+    return launch(tcb::unroll_bwd_kernel<C, 2>, tcb::bwd_smem_bytes<C, 2>());
+  } else {
+    return launch(tcb::unroll_bwd_kernel<C, 0>, tcb::bwd_smem_bytes<C, 0>());
+  }
 }
 
 }  // namespace l2o

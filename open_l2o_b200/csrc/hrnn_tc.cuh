@@ -1,16 +1,16 @@
-// HierarchicalRNN per-parameter level on the sm_100a tensor cores (included by l2o_hrnn.cu, inside namespace l2o::hrnn).
+// HierarchicalRNN per-parameter level on the sm_90a tensor cores (included by l2o_hrnn.cu, inside namespace l2o::hrnn).
 //
 // Same arithmetic as coord_kernel (HR:444-540 features, rnn_cells.py:46-68 BiasGRU(10), HR:606-706 readouts); the
-// two GRU products run as error-compensated 3xTF32 tcgen05.mma with the per-coordinate operand rows in TMEM (TS mode):
+// two GRU products run as error-compensated 3xTF32 wgmma with the per-coordinate operand rows staged in shared memory:
 //   MMA 1  D[128 x 48] = A1[128 x 24] . B1[24 x 48]     A1 = [feat 0..11 | h 12..21 | 1 | 0]
-//          D columns: r 0..9 | u 16..25 | candidate (feature part + bc) 32..41        (9 instructions: 3 K-steps x hi/lo)
-//   MMA 2  D[:, 32..47] += A2[128 x 16] . B2[16 x 16]   A2 = [r*h 0..9 | 0]           (6 instructions)
-// A persistent CTA of 128 threads (thread = TMEM lane = coordinate) walks tiles of 128 coordinates: the 21 state planes
-// and the gradient of the NEXT tile stream into a shared-memory ring with 4-byte cp.async (tensor boundaries are not
-// 16-byte aligned, and every thread only ever reads what it copied itself, so no barrier guards the ring); the per-tensor
-// sums stay in registers across tiles and go through the warp butterfly + fp64 atomics every kFlushTiles tiles.
-// 4 CTAs per SM (128 TMEM columns, 35 KB of shared memory, <= 128 registers) overlap each other's MMA round trips.
-// Against the FFMA kernel: 660 FFMA + 220 LDS + 240 reduction instructions per coordinate become ~90.
+//          D columns: r 0..9 | u 16..25 | candidate (feature part + bc) 32..41        (per 64-row half: 3 K-steps x 3)
+//   MMA 2  D[:, 32..47] += A2[128 x 16] . B2[16 x 16]   A2 = [r*h 0..9 | 0]           (the same accumulator registers)
+// A persistent CTA of 128 threads (one warpgroup; thread = coordinate) walks tiles of 128 coordinates: the 21 state
+// planes and the gradient of the NEXT tile stream into a shared-memory ring with 4-byte cp.async (tensor boundaries are
+// not 16-byte aligned, and every thread only ever reads what it copied itself, so no barrier guards the ring).  The
+// accumulator fragments come back to their coordinate's thread through a padded shared-memory row buffer.  The
+// per-tensor sums stay in registers across tiles and go through the warp butterfly + fp64 atomics every kFlushTiles
+// tiles.
 #pragma once
 
 namespace tcg {
@@ -24,25 +24,23 @@ constexpr int kB1Floats = kKA * kND;
 constexpr int kB2Floats = kKA2 * kND2;
 constexpr int kPlanesIn = kPlanes + 1;  // + the gradient
 constexpr int kStages = 2;
-constexpr int kTmemCols = 128;
-constexpr int cD = 0, cA1H = 48, cA1L = 72, cA2H = 96, cA2L = 112;
+constexpr int kDStride = kND + 4;       // row stride of the accumulator buffer (conflict-free row reads)
+constexpr uint32_t kALBO = (kTile / 8) * 128;   // K-major operand rows: 16 row groups of 128 B per 4 columns
 constexpr int kFlushTiles = 8;
-constexpr int kCtasPerSm = 4;
+constexpr int kCtasPerSm = 2;
 
 struct SmemG {
+  float a1h[kKA * kTile], a1l[kKA * kTile];     // K-major core-matrix layout (first: 16-byte aligned)
+  float a2h[kKA2 * kTile], a2l[kKA2 * kTile];
   float b1h[kB1Floats], b1l[kB1Floats], b2h[kB2Floats], b2l[kB2Floats];
+  float dbuf[kTile * kDStride];
   float ring[kStages][kPlanesIn][kTile];
   float4 ro[H0];     // readout weights (Wu, Ws, Wi, Wl)[k]   (HR:609-611,645-651,663-666)
   float cst[12];     // bs | bi | bl | sigmoid(lr momentum) | offset | grad-shortcut weights 5..8
   double red[kTile / 32][kAcc];
-  uint64_t bar1, bar2;
-  uint32_t tmem_slot;
 };
 
 __device__ __forceinline__ int b_index(int nn, int k, int n) { return ((k >> 2) * (nn / 8) + (n >> 3)) * 32 + (n & 7) * 4 + (k & 3); }
-__device__ __forceinline__ uint64_t b_desc(uint32_t saddr, uint32_t lbo) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(128u >> 4) << 32) | (1ull << 46);
-}
 __device__ __forceinline__ void cp_async4(uint32_t saddr, const float* g) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(saddr), "l"(g) : "memory");
 }
@@ -54,19 +52,32 @@ __device__ __forceinline__ float lds(uint32_t saddr) {
   asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(saddr));
   return v;
 }
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const float* v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr),
-               "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-               "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7]))
-               : "memory");
-}
-// 8 operand columns: hi = the value itself (the tensor core truncates to tf32), lo = the truncated remainder
-__device__ __forceinline__ void st_split8(uint32_t t_hi, uint32_t t_lo, const float* v) {
-  float lo[8];
+// 4 operand columns [4c, 4c + 4) of this thread's row into the hi / lo images: hi = truncated tf32, lo = the remainder
+__device__ __forceinline__ void st_split4(float* hi, float* lo, int c, int row, const float* v) {
+  uint32_t h[4], l[4];
 #pragma unroll
-  for (int k = 0; k < 8; ++k) lo[k] = v[k] - __uint_as_float(__float_as_uint(v[k]) & 0xFFFFE000u);
-  tmem_st8(t_hi, v);
-  tmem_st8(t_lo, lo);
+  for (int k = 0; k < 4; ++k) split_tf32(v[k], h[k], l[k]);
+  const int o = c * (int)(kALBO / 4) + row * 4;
+  *reinterpret_cast<uint4*>(hi + o) = make_uint4(h[0], h[1], h[2], h[3]);
+  *reinterpret_cast<uint4*>(lo + o) = make_uint4(l[0], l[1], l[2], l[3]);
+}
+// D[64 x N] (+)= A[64 x 8] (shared, tf32, K-major) . B[8 x N] (shared)
+__device__ __forceinline__ void mma_ss_n48(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n48k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, "
+      "%24, %25, p, 1, 1;\n\t}\n"
+      : L2O_ACC8(0), L2O_ACC8(8), L2O_ACC8(16)
+      : "l"(a), "l"(b), "r"(acc));
+}
+__device__ __forceinline__ void mma_ss_n16(float* d, uint64_t a, uint64_t b) {   // always accumulates
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1;\n\t}\n"
+      : L2O_ACC8(0)
+      : "l"(a), "l"(b), "r"(1));
 }
 
 // weight value of the extended matrices (theta layout: l2o_hrnn.cu O_* offsets)
@@ -91,10 +102,12 @@ __global__ void __launch_bounds__(kTile, kCtasPerSm) coord_tc_kernel(const float
                                                                      float* __restrict__ state, int64_t n,
                                                                      const BlockEnt* __restrict__ blocks, int ntiles,
                                                                      Workspace w) {
-  __shared__ __align__(128) SmemG S;
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  SmemG& S = *reinterpret_cast<SmemG*>(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int gq = lane >> 2, q = lane & 3;
 
-  // ---- one-time setup: weight images (hi/lo, K-major core-matrix layout), readout constants, barriers, TMEM
+  // ---- one-time setup: weight images (hi/lo, K-major core-matrix layout), readout constants
   for (int e = tid; e < kB1Floats + kB2Floats; e += kTile) {
     const bool second = e >= kB1Floats;
     const int ee = second ? e - kB1Floats : e;
@@ -116,24 +129,13 @@ __global__ void __launch_bounds__(kTile, kCtasPerSm) coord_tc_kernel(const float
 #pragma unroll
     for (int s = 0; s < NS; ++s) S.cst[5 + s] = theta[O_G2D + s];
   }
-  if (tid == 0) {
-    mbar_init(&S.bar1, 1);
-    mbar_init(&S.bar2, 1);
-    fence_barrier_init();
-  }
-  if (warp == 0) {
-    tmem_alloc(&S.tmem_slot, kTmemCols);
-    tmem_relinquish();
-  }
-  fence_proxy_async();   // the image was written with generic stores; the MMA reads it through the async proxy
-  tc_fence_before();
+  fence_proxy_async();   // the images are written with generic stores; the MMA reads them through the async proxy
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tbase = S.tmem_slot + ((uint32_t)(warp * 32) << 16);
-  const uint32_t tD = tbase + cD, tA1H = tbase + cA1H, tA1L = tbase + cA1L, tA2H = tbase + cA2H, tA2L = tbase + cA2L;
-  const uint32_t idesc1 = make_idesc(kND), idesc2 = make_idesc(kND2);
-  const uint64_t d1h = b_desc(smem_u32(S.b1h), (kND / 8) * 128), d1l = b_desc(smem_u32(S.b1l), (kND / 8) * 128);
-  const uint64_t d2h = b_desc(smem_u32(S.b2h), (kND2 / 8) * 128), d2l = b_desc(smem_u32(S.b2l), (kND2 / 8) * 128);
+  const uint64_t d1h = make_desc(smem_u32(S.b1h), (kND / 8) * 128, 128), d1l = make_desc(smem_u32(S.b1l), (kND / 8) * 128, 128);
+  const uint64_t d2h = make_desc(smem_u32(S.b2h), (kND2 / 8) * 128, 128), d2l = make_desc(smem_u32(S.b2l), (kND2 / 8) * 128, 128);
+  const uint64_t a1h = make_desc(smem_u32(S.a1h), kALBO, 128), a1l = make_desc(smem_u32(S.a1l), kALBO, 128);
+  const uint64_t a2h = make_desc(smem_u32(S.a2h), kALBO, 128), a2l = make_desc(smem_u32(S.a2l), kALBO, 128);
+  constexpr uint64_t kStepA = (2 * kALBO) >> 4, kHalfA = (8 * 128) >> 4;    // per K = 8 / per 64-row half
   constexpr uint64_t kStep1 = (2 * (kND / 8) * 128) >> 4, kStep2 = (2 * (kND2 / 8) * 128) >> 4;
   const uint32_t ring_s = smem_u32(&S.ring[0][0][0]) + tid * 4;
   constexpr uint32_t kStageBytes = kPlanesIn * kTile * 4;
@@ -173,9 +175,32 @@ __global__ void __launch_bounds__(kTile, kCtasPerSm) coord_tc_kernel(const float
     if (tid < kAcc) atomicAdd(&w.acc[tensor * kAcc + tid], ((S.red[0][tid] + S.red[1][tid]) + S.red[2][tid]) + S.red[3][tid]);
     __syncthreads();
   };
+  // accumulator fragments of both 64-row halves -> the row buffer, columns [8 J0, 8 J1)
+  auto put_acc = [&](const float (&d)[2][kND / 2], int j0, int j1) {
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+      for (int j = 0; j < kND / 8; ++j)
+        if (j >= j0 && j < j1)
+#pragma unroll
+          for (int rh = 0; rh < 2; ++rh) {
+            const int r = 64 * hf + 16 * warp + gq + 8 * rh;
+            *reinterpret_cast<float2*>(&S.dbuf[r * kDStride + 8 * j + 2 * q]) = make_float2(d[hf][4 * j + 2 * rh], d[hf][4 * j + 2 * rh + 1]);
+          }
+  };
+  auto get10 = [&](int col, float* z) {   // columns [col, col + 10) of this thread's row
+    const float* p = &S.dbuf[tid * kDStride + col];
+    const float4 x0 = *reinterpret_cast<const float4*>(p), x1 = *reinterpret_cast<const float4*>(p + 4);
+    const float2 x2 = *reinterpret_cast<const float2*>(p + 8);
+    z[0] = x0.x; z[1] = x0.y; z[2] = x0.z; z[3] = x0.w; z[4] = x1.x; z[5] = x1.y; z[6] = x1.z; z[7] = x1.w; z[8] = x2.x; z[9] = x2.y;
+  };
 
   const float mean_llr = *w.mean_log_lr;
-  uint32_t par = 0;
+  float d[2][kND / 2];
+#pragma unroll
+  for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+    for (int k = 0; k < kND / 2; ++k) d[hf][k] = 0.f;
   int cur_tensor = -1, since = 0, it = 0;
   if ((int)blockIdx.x < ntiles) prefetch(blockIdx.x, 0);
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
@@ -244,27 +269,24 @@ __global__ void __launch_bounds__(kTile, kCtasPerSm) coord_tc_kernel(const float
     a[F + H0] = 1.0f;
     a[F + H0 + 1] = 0.f;
 #pragma unroll
-    for (int q = 0; q < kKA / 8; ++q) st_split8(tA1H + 8 * q, tA1L + 8 * q, a + 8 * q);
+    for (int c = 0; c < kKA / 4; ++c) st_split4(S.a1h, S.a1l, c, tid, a + 4 * c);
     if (act) {
 #pragma unroll
       for (int k = 0; k < F; ++k) vals[H0 + k] += a[k];   // features as fed to the gates (HR:582-587 mean of [h' | feat])
     }
-    tc_wait_st();
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-      tc_fence_after();
-      if (elect_one()) {
+    fence_proxy_async();
+    __syncthreads();   // A1 complete; the previous tile's reads of the row buffer are done
+    wg_fence();
 #pragma unroll
-        for (int kc = 0; kc < kKA / 8; ++kc) {
-          mma_tf32_ts(tD, tA1L + 8 * kc, d1h + kc * kStep1, idesc1, kc > 0 ? 1u : 0u);
-          mma_tf32_ts(tD, tA1H + 8 * kc, d1l + kc * kStep1, idesc1, 1u);
-          mma_tf32_ts(tD, tA1H + 8 * kc, d1h + kc * kStep1, idesc1, 1u);
-        }
-        tc_commit(&S.bar1);
+    for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+      for (int kc = 0; kc < kKA / 8; ++kc) {
+        const uint64_t oa = hf * kHalfA + kc * kStepA;
+        mma_ss_n48(d[hf], a1l + oa, d1h + kc * kStep1, kc > 0 ? 1u : 0u);
+        mma_ss_n48(d[hf], a1h + oa, d1l + kc * kStep1, 1u);
+        mma_ss_n48(d[hf], a1h + oa, d1h + kc * kStep1, 1u);
       }
-      __syncwarp();
-    }
+    wg_commit();
     const float4* b0 = reinterpret_cast<const float4*>(w.bias0 + be.tensor * kB0Stride);
     float bq[12];
     {
@@ -272,46 +294,40 @@ __global__ void __launch_bounds__(kTile, kCtasPerSm) coord_tc_kernel(const float
       bq[0] = q0.x; bq[1] = q0.y; bq[2] = q0.z; bq[3] = q0.w; bq[4] = q1.x; bq[5] = q1.y; bq[6] = q1.z; bq[7] = q1.w;
       bq[8] = q2.x; bq[9] = q2.y; bq[10] = q2.z; bq[11] = q2.w;
     }
-    mbar_wait(&S.bar1, par);
-    tc_fence_after();
+    wg_wait<0>();
+    put_acc(d, 0, 4);   // r | u (columns 0..31)
+    __syncthreads();
     // ---- reset gate, A2 = [r*h | 0]
     {
       float z[16];
-      tmem_ldn<8>(tD, z);
-      tmem_ldn<2>(tD + 8, z + 8);
-      tc_wait_ld();
+      get10(0, z);
 #pragma unroll
       for (int k = 0; k < H0; ++k) z[k] = sigmoid_fast(z[k] + bq[k]) * h[k];
 #pragma unroll
       for (int k = H0; k < 16; ++k) z[k] = 0.f;
-      st_split8(tA2H, tA2L, z);
-      st_split8(tA2H + 8, tA2L + 8, z + 8);
-    }
-    tc_wait_st();
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-      tc_fence_after();
-      if (elect_one()) {
 #pragma unroll
-        for (int kc = 0; kc < kKA2 / 8; ++kc) {
-          mma_tf32_ts(tD + kColC, tA2L + 8 * kc, d2h + kc * kStep2, idesc2, 1u);
-          mma_tf32_ts(tD + kColC, tA2H + 8 * kc, d2l + kc * kStep2, idesc2, 1u);
-          mma_tf32_ts(tD + kColC, tA2H + 8 * kc, d2h + kc * kStep2, idesc2, 1u);
-        }
-        tc_commit(&S.bar2);
-      }
-      __syncwarp();
+      for (int c = 0; c < kKA2 / 4; ++c) st_split4(S.a2h, S.a2l, c, tid, z + 4 * c);
     }
+    fence_proxy_async();
+    __syncthreads();
+    wg_fence();
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+      for (int kc = 0; kc < kKA2 / 8; ++kc) {
+        const uint64_t oa = hf * kHalfA + kc * kStepA;
+        mma_ss_n16(d[hf] + 16, a2l + oa, d2h + kc * kStep2);
+        mma_ss_n16(d[hf] + 16, a2h + oa, d2l + kc * kStep2);
+        mma_ss_n16(d[hf] + 16, a2h + oa, d2h + kc * kStep2);
+      }
+    wg_commit();
     // ---- update gate while MMA 2 runs (columns 16..25 are not touched by it)
     float u[H0];
     {
       const float4 q3 = __ldg(b0 + 3), q4 = __ldg(b0 + 4);
       const float bu[H0] = {bq[10], bq[11], q3.x, q3.y, q3.z, q3.w, q4.x, q4.y, q4.z, q4.w};
       float z[H0];
-      tmem_ldn<8>(tD + kColU, z);
-      tmem_ldn<2>(tD + kColU + 8, z + 8);
-      tc_wait_ld();
+      get10(kColU, z);
 #pragma unroll
       for (int k = 0; k < H0; ++k) u[k] = sigmoid_fast(z[k] + bu[k]);
     }
@@ -321,15 +337,13 @@ __global__ void __launch_bounds__(kTile, kCtasPerSm) coord_tc_kernel(const float
       bc[0] = q5.x; bc[1] = q5.y; bc[2] = q5.z; bc[3] = q5.w; bc[4] = q6.x; bc[5] = q6.y; bc[6] = q6.z; bc[7] = q6.w;
       bc[8] = q7.x; bc[9] = q7.y;
     }
-    mbar_wait(&S.bar2, par);
-    tc_fence_after();
-    par ^= 1;
+    wg_wait<0>();
+    put_acc(d, 4, 6);   // candidate (columns 32..47)
+    __syncthreads();
     float delta = 0.f, zs = 0.f, zi = 0.f, zl = 0.f;
     {
       float z[H0];
-      tmem_ldn<8>(tD + kColC, z);
-      tmem_ldn<2>(tD + kColC + 8, z + 8);
-      tc_wait_ld();
+      get10(kColC, z);
 #pragma unroll
       for (int k = 0; k < H0; ++k) {
         const float c = tanh_fast(z[k] + bc[k]);
@@ -363,11 +377,8 @@ __global__ void __launch_bounds__(kTile, kCtasPerSm) coord_tc_kernel(const float
       vals[H0 + F] += delta * delta;
       vals[H0 + F + 1] += llr_new;
     }
-    tc_fence_before();   // this tile's TMEM reads are ordered before the next tile's MMA (issued after a barrier)
   }
   if (cur_tensor >= 0) flush(cur_tensor);
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(S.tmem_slot, kTmemCols);
 }
 
 }  // namespace tcg

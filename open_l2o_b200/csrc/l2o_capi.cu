@@ -134,7 +134,7 @@ int l2o_step(l2o_handle h, const l2o_step_args* a, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   const bool tc_can = l2o::tc_step_ok(h, *a);
   if (h->engine == L2O_ENGINE_TC) return tc_can ? l2o::tc_step(h, *a, st) : L2O_E_UNSUPPORTED;
-  // AUTO: the tensor-core path pays a fixed ~10 us (weight image + TMEM setup) per launch; use it for real sizes
+  // AUTO: the tensor-core path pays a fixed cost (weight image prep + staging) per launch; use it for real sizes
   if (h->engine == L2O_ENGINE_AUTO && tc_can && l2o::tc_auto_default() && a->n >= 16384) return l2o::tc_step(h, *a, st);
   return l2o::ffma_step(h, *a, st);
 }
@@ -211,6 +211,6 @@ const char* l2o_status_string(int s) {
 }
 
 const char* l2o_last_cuda_error(void) { return g_cuda_err; }
-const char* l2o_version(void) { return "l2o_b200 0.2 (sm_100a; engines: ffma, tcgen05)"; }
+const char* l2o_version(void) { return "l2o_b200 0.3 (sm_90a; engines: ffma, wgmma)"; }
 
 }  // extern "C"

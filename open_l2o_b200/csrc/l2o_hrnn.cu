@@ -1,4 +1,4 @@
-// L2O-Scale HierarchicalRNN update step (SURVEY.md 8(f) row 1, BASELINE config #4) — sm_100a CUDA kernels + C-ABI.
+// L2O-Scale HierarchicalRNN update step (SURVEY.md 8(f) row 1, BASELINE config #4) — sm_90a CUDA kernels + C-ABI.
 // SC/ = Model_Free_L2O/L2O-Scale/L2O-Scale-Training/ of the reference; HR = SC/optimizer/hierarchical_rnn.py.
 //
 // One optimizer step over ALL optimizee tensors is three launches, with no host synchronisation (graph-capturable):
@@ -21,7 +21,7 @@
 
 #include "l2o_internal.h"
 #include "cwlstm_ffma.cuh"   // helpers cwlstm_tc.cuh expects
-#include "cwlstm_tc.cuh"     // tcgen05 / TMEM / mbarrier wrappers, tf32 split
+#include "cwlstm_tc.cuh"     // wgmma / mbarrier wrappers, tf32 split
 
 namespace l2o {
 namespace hrnn {
@@ -40,7 +40,7 @@ constexpr int O_G2D = 5883, O_LRM = 5887, O_OFF = 5888;
 constexpr int O_WG2 = 5889, O_BG2 = 7489, O_WC2 = 7529, O_BC2 = 8329;
 constexpr int kTheta = 8349;
 constexpr int kAcc = 24;  // per-tensor fp64 sums: [h'(10) | feat(12)], delta^2, log-lr'
-constexpr int kBlock = 128;     // coordinates per block-table entry (= one tcgen05 tile)
+constexpr int kBlock = 128;     // coordinates per block-table entry (= one tensor-core tile)
 constexpr int kB0Stride = 32;   // floats per tensor in Workspace::bias0: r 0..9 | u 10..19 | c 20..29 | pad (16-byte rows)
 
 struct BlockEnt {
@@ -458,7 +458,7 @@ void free_buried() {
 
 
 // L2O_HRNN_FFMA=1 selects the exact-fp32 FFMA kernel for the per-parameter level (debugging / A-B runs); the default
-// is the tcgen05 kernel.
+// is the tensor-core (wgmma) kernel.
 static bool use_ffma_coord() {
   static const bool v = [] {
     const char* e = getenv("L2O_HRNN_FFMA");
@@ -466,11 +466,14 @@ static bool use_ffma_coord() {
   }();
   return v;
 }
+// grid of the tensor-core kernel (0: its shared-memory size could not be set)
 static int coord_tc_grid() {
   static const int v = [] {
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    cudaFuncSetAttribute(tcg::coord_tc_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    if (cudaFuncSetAttribute(tcg::coord_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(tcg::SmemG)) !=
+        cudaSuccess)
+      return 0;
     return sms * tcg::kCtasPerSm;
   }();
   return v;
@@ -600,8 +603,11 @@ int l2o_hrnn_step_local(l2o_hrnn_handle h, const l2o_hrnn_args* a, void* stream)
   if (use_ffma_coord()) {
     coord_kernel<<<h->nblocks, kBlock, 0, st>>>(a->theta, a->g, a->state, h->n, h->d_blocks, w);
   } else {
-    const int grid = h->nblocks < coord_tc_grid() ? h->nblocks : coord_tc_grid();
-    tcg::coord_tc_kernel<<<grid, tcg::kTile, 0, st>>>(a->theta, a->g, a->state, h->n, h->d_blocks, h->nblocks, w);
+    const int cap = coord_tc_grid();
+    if (cap <= 0) return l2o::set_cuda_error(cudaGetLastError(), "coord_tc_kernel shared-memory size");
+    const int grid = h->nblocks < cap ? h->nblocks : cap;
+    tcg::coord_tc_kernel<<<grid, tcg::kTile, sizeof(tcg::SmemG), st>>>(a->theta, a->g, a->state, h->n, h->d_blocks, h->nblocks,
+                                                                       w);
   }
   L2O_CUDA_TRY(cudaGetLastError());
   l2o::count_launch();
@@ -633,7 +639,7 @@ int l2o_hrnn_coord_bwd(l2o_hrnn_handle h, const l2o_hrnn_bwd_args* a, void* stre
     return L2O_E_INVALID;
   bwd::Args k{a->theta, a->state_old, a->g, a->bias0, a->zero_flag, a->mean_log_lr, a->d_state_new, a->d_upd, a->d_sums,
               a->d_state_old, a->d_theta, a->d_bias0, a->d_mean_log_lr};
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int grid = h->nblocks < 2 * sms ? h->nblocks : 2 * sms;
   bwd::coord_bwd_kernel<<<grid, bwd::kBwdBlock, 0, (cudaStream_t)stream>>>(k, h->n, h->d_blocks, h->nblocks);

@@ -22,7 +22,7 @@ struct l2o_net {
   int64_t n_theta;
   int64_t state_floats;
   l2o::NetRt rt;
-  float* tc_img;   // device-side weight image of the tcgen05 engine (owned; lazily allocated)
+  float* tc_img;   // device-side weight image of the tensor-core engine (owned; lazily allocated)
   int tc_img_dev;
   int tc_img_mode; // what the image currently holds: -1 nothing, 0 forward layout, 1 BPTT layout
 };
@@ -45,7 +45,7 @@ int tc_step(l2o_net* h, const l2o_step_args& a, cudaStream_t st);
 bool tc_auto_default();
 bool tc_bwd_auto_default();
 bool tc_bwd_ok(const l2o_net* h, const l2o_bwd_args& a);
-int tc_unroll_bwd(l2o_net* h, const l2o_bwd_args& a, cudaStream_t st);  // does ENGINE_AUTO pick the tcgen05 engine when it can?
+int tc_unroll_bwd(l2o_net* h, const l2o_bwd_args& a, cudaStream_t st);
 }  // namespace l2o
 
 #define L2O_CUDA_TRY(expr)                                              \

@@ -1,8 +1,7 @@
-// tcgen05 engine translation unit.
+// Tensor-core (wgmma) engine translation unit.
 #include "cwlstm_ffma.cuh"   // load_vec / store_vec / preprocess helpers
 #include "cwlstm_tc.cuh"
 #include "cwlstm_tc_bwd.cuh"
-#include "cwlstm_tc_bwd2.cuh"
 #include <cstdlib>
 #include <mutex>
 #include <utility>
@@ -10,26 +9,24 @@
 #include "l2o_internal.h"
 
 namespace l2o {
-// forward / step: LSTM-20x2 with identity / LogAndSign preprocessing (cfg 0, 1) and RNNProp's fc(2->20)+ELU net (cfg 2);
-// BPTT: cfg 0, 1 layer-pipelined in one kernel; cfg 2 as two single-chain passes (its K = 48 layer-1 operands do not fit next
-// to layer 2's in shared memory / TMEM, DESIGN.md) with a caller-provided hand-over buffer
+// forward / step / BPTT: LSTM-20x2 with identity / LogAndSign preprocessing (cfg 0, 1) and RNNProp's fc(2->20)+ELU net
+// (cfg 2).  The BPTT of cfg 2 runs as two passes over time (layer 2, then layer 1) with a caller-provided hand-over buffer.
 bool tc_supported(int cfg) { return cfg == 0 || cfg == 1 || cfg == 2; }
-static bool tc_bwd_supported(int cfg) { return cfg == 0 || cfg == 1 || cfg == 2; }
 bool tc_fwd_ok(const l2o_net* h, const l2o_unroll_args& a) {
   if (a.opt_kind == L2O_OPT_QUADRATIC_BATCH) return false;  // grouped optimizees exchange x: exact-fp32 engine only
   if (h->cfg == 2) return true;                             // fused Adam-feature mode (m, v) or given (m~, g~) rows
   return a.m == nullptr && a.feat_rec == nullptr;
 }
-// L2O_TC_AUTO=0: ENGINE_AUTO never picks the tcgen05 engine (A/B runs of whole tests against the exact-fp32 engine)
+// L2O_TC_AUTO=0: ENGINE_AUTO never picks the tensor-core engine (A/B runs of whole tests against the exact-fp32 engine)
 static bool tc_auto_env() {
   static const bool on = !(std::getenv("L2O_TC_AUTO") != nullptr && std::getenv("L2O_TC_AUTO")[0] == '0');
   return on;
 }
 bool tc_auto_default() { return tc_auto_env(); }
-bool tc_bwd_auto_default() { return tc_auto_env(); }  // parity-green on the B200 (tests/test_tc_gpu.py)
+bool tc_bwd_auto_default() { return tc_auto_env(); }
 
-// Weight-image buffers (2 x 97 KB each) are recycled through a process-wide free list and never cudaFree'd: a handle may
-// be destroyed (Python GC) while ANOTHER program is capturing a CUDA graph, and cudaFree during a capture invalidates it.
+// Weight-image buffers are recycled through a process-wide free list and never cudaFree'd: a handle may be destroyed
+// (Python GC) while ANOTHER program is capturing a CUDA graph, and cudaFree during a capture invalidates it.
 namespace {
 struct ImgPool {
   std::mutex mu;
@@ -64,7 +61,7 @@ static int ensure_image(l2o_net* h) {
           break;
         }
     }
-    if (h->tc_img == nullptr) L2O_CUDA_TRY(cudaMalloc(&h->tc_img, 2 * tc::kImgAllBytes));   // fc nets: one BPTT image per pass
+    if (h->tc_img == nullptr) L2O_CUDA_TRY(cudaMalloc(&h->tc_img, tc::kImgMaxFloats * sizeof(float)));
     h->tc_img_dev = dev;
     h->tc_img_mode = -1;
   }
@@ -76,7 +73,7 @@ bool tc_bwd_ok(const l2o_net* h, const l2o_bwd_args& a) {
   const bool mode_ok = a.labels ? (a.delta_seq != nullptr && a.n_total > 0) : a.g_rec != nullptr;
   if (h->cfg == 2 && a.scratch == nullptr) return false;   // fc nets: two passes with a caller-provided hand-over buffer
   if (h->rt.tanh_output && a.delta_seq == nullptr) return false;   // tanh' comes from the recorded deltas
-  return tc_bwd_supported(h->cfg) && mode_ok;
+  return tc_supported(h->cfg) && mode_ok;
 }
 
 int tc_unroll_bwd(l2o_net* h, const l2o_bwd_args& a, cudaStream_t st) {
@@ -86,17 +83,9 @@ int tc_unroll_bwd(l2o_net* h, const l2o_bwd_args& a, cudaStream_t st) {
   const int sms = device_sms();
   if (sms <= 0) return L2O_E_CUDA;
   rc = L2O_E_UNSUPPORTED;
-  // L2O_BWD_V1=1 selects the first-generation (phase-serial) kernel for A/B measurements; the layer-pipelined kernel
-  // (cwlstm_tc_bwd2.cuh) is the product path
-  static const bool v1 = std::getenv("L2O_BWD_V1") != nullptr && std::getenv("L2O_BWD_V1")[0] == '1';
-  if (v1) {
-    if (h->cfg == 0) rc = tc_launch_bwd<Cfg<L2O_PRE_IDENTITY, 1, 1, 20, 20>>(h->rt, a, h->tc_img, st, sms);
-    if (h->cfg == 1) rc = tc_launch_bwd<Cfg<L2O_PRE_LOGSIGN, 1, 2, 20, 20>>(h->rt, a, h->tc_img, st, sms);
-  } else {
-    if (h->cfg == 0) rc = tc_launch_bwd2<Cfg<L2O_PRE_IDENTITY, 1, 1, 20, 20>>(h->rt, a, h->tc_img, st, sms);
-    if (h->cfg == 1) rc = tc_launch_bwd2<Cfg<L2O_PRE_LOGSIGN, 1, 2, 20, 20>>(h->rt, a, h->tc_img, st, sms);
-    if (h->cfg == 2) rc = tc_launch_bwd2<Cfg<L2O_PRE_FC, 2, 20, 20, 20>>(h->rt, a, h->tc_img, st, sms);
-  }
+  if (h->cfg == 0) rc = tc_launch_bwd<Cfg<L2O_PRE_IDENTITY, 1, 1, 20, 20>>(h->rt, a, h->tc_img, st, sms);
+  if (h->cfg == 1) rc = tc_launch_bwd<Cfg<L2O_PRE_LOGSIGN, 1, 2, 20, 20>>(h->rt, a, h->tc_img, st, sms);
+  if (h->cfg == 2) rc = tc_launch_bwd<Cfg<L2O_PRE_FC, 2, 20, 20, 20>>(h->rt, a, h->tc_img, st, sms);
   if (rc == L2O_OK) count_launch(h->cfg == 2 ? 3 : 2);
   h->tc_img_mode = 1;
   if (rc == L2O_E_CUDA) return set_cuda_error(cudaGetLastError(), "tc_unroll_bwd launch");
@@ -133,12 +122,10 @@ int tc_step(l2o_net* h, const l2o_step_args& s, cudaStream_t st) {
   a.feat_rec = s.feat_out;
   const tc::FwdExtra ex{s.step_ptr, s.t_offset, s.step_ptr ? 0.f : s.p};
   rc = L2O_E_UNSUPPORTED;
-  // L2O_STEP_STAGE=0 disables the TMA-staged state loads (A/B measurements)
-  static const bool stage = !(std::getenv("L2O_STEP_STAGE") != nullptr && std::getenv("L2O_STEP_STAGE")[0] == '0');
   const bool prep = !(s.reuse_weights && h->tc_img_mode == 0);   // forward image of this theta already in place
-  if (h->cfg == 0) rc = tc_launch_fwd<Cfg<L2O_PRE_IDENTITY, 1, 1, 20, 20>>(h->rt, a, h->tc_img, st, sms, s.state_out, stage, ex, prep);
-  if (h->cfg == 1) rc = tc_launch_fwd<Cfg<L2O_PRE_LOGSIGN, 1, 2, 20, 20>>(h->rt, a, h->tc_img, st, sms, s.state_out, stage, ex, prep);
-  if (h->cfg == 2) rc = tc_launch_fwd<Cfg<L2O_PRE_FC, 2, 20, 20, 20>>(h->rt, a, h->tc_img, st, sms, s.state_out, stage, ex, prep);
+  if (h->cfg == 0) rc = tc_launch_fwd<Cfg<L2O_PRE_IDENTITY, 1, 1, 20, 20>>(h->rt, a, h->tc_img, st, sms, s.state_out, ex, prep);
+  if (h->cfg == 1) rc = tc_launch_fwd<Cfg<L2O_PRE_LOGSIGN, 1, 2, 20, 20>>(h->rt, a, h->tc_img, st, sms, s.state_out, ex, prep);
+  if (h->cfg == 2) rc = tc_launch_fwd<Cfg<L2O_PRE_FC, 2, 20, 20, 20>>(h->rt, a, h->tc_img, st, sms, s.state_out, ex, prep);
   if (rc == L2O_OK) count_launch(prep ? 2 : 1);
   h->tc_img_mode = 0;
   if (rc == L2O_E_CUDA) return set_cuda_error(cudaGetLastError(), "tc_step launch");

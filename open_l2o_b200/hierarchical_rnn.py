@@ -1,4 +1,4 @@
-"""L2O-Scale ``HierarchicalRNN`` learned optimizer — the update step (inference path) on the B200 engine.
+"""L2O-Scale ``HierarchicalRNN`` learned optimizer — the update step (inference path) on the H100 engine.
 
 Mirrors the reference class ``optimizer.hierarchical_rnn.HierarchicalRNN`` (SC/optimizer/hierarchical_rnn.py:62-218;
 SC/ = Model_Free_L2O/L2O-Scale/L2O-Scale-Training/): same constructor arguments, ``apply_gradients`` as the

@@ -7,7 +7,7 @@ Model_Free_L2O/L2O-Scale/L2O-Scale-Training/), ``scale_objective`` (:586-609) an
 the meta-gradient (``tf.stop_gradient``, trainable_optimizer.py:332-338).
 
 Where the arithmetic runs.  Everything that touches the N optimizee coordinates is CUDA in ``libl2o_b200.so``: the forward
-step of the per-parameter level is the tcgen05 kernel of the inference path (``l2o_hrnn_step_local``), its backward is
+step of the per-parameter level is the tensor-core kernel of the inference path (``l2o_hrnn_step_local``), its backward is
 ``l2o_hrnn_coord_bwd`` (csrc/hrnn_bwd.cuh).  The cross-coordinate pieces — per-tensor / global BiasGRU(20), the
 1/RMS(delta) normalisation, the problem-wide mean log learning rate, the objective scaling — are ``[n_tensors x 20]``-sized
 and are written as torch ops, so ``torch.autograd`` stitches the two CUDA entry points into the BPTT graph.  No CPU path.

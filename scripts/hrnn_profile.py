@@ -1,4 +1,4 @@
-"""Profiling driver (run under ncu): a few l2o_hrnn_step calls on a state larger than L2 (16 tensors x 2M)."""
+"""Profiling driver (run under a profiler): a few l2o_hrnn_step calls on a state larger than L2 (16 tensors x 2M)."""
 import os
 import sys
 

@@ -1,4 +1,4 @@
-"""Accuracy report of the tcgen05 engine against the fp64 oracle (test infrastructure; run on the GPU box):
+"""Accuracy report of the tensor-core engine against the fp64 oracle (test infrastructure; run on the GPU box):
 pre-recorded-gradient unroll (state / deltas) and fused Rastrigin forward + BPTT (x_T, fx, dtheta), next to the
 error the fp32 oracle itself has against fp64 on the same inputs.  Used to A/B numerics-affecting kernel variants
 (L2O_LIB=<variant .so> python scripts/tc_accuracy.py)."""

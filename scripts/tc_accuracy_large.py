@@ -1,8 +1,8 @@
 """d-theta accuracy of the BPTT kernels at a size where the per-CTA accumulation is long (test infrastructure; GPU box).
 Reference = the exact-fp32 engine run over 1024-coordinate chunks whose results are summed in fp64 (each chunk: one tile
 per CTA, T steps in fp32, then fp64 atomics), i.e. no long fp32 accumulation anywhere.  Reports the max-norm relative
-error of (a) the tensor-core BPTT (layer-pipelined by default, first generation with L2O_BWD_V1=1) and (b) the exact-fp32
-engine in ONE launch, both on the same checkpoints / recorded gradients.
+error of (a) the tensor-core BPTT and (b) the exact-fp32 engine in ONE launch, both on the same checkpoints / recorded
+gradients.
 
     python scripts/tc_accuracy_large.py [n] [T]"""
 import os
@@ -50,9 +50,8 @@ def main():
     for lo in range(0, n, C):
         hi = min(n, lo + C)
         ref += bwd(ENGINE_FFMA, g_rec[:, lo:hi].contiguous(), ck4[:, :, lo:hi, :].contiguous().view(-1), hi - lo)
-    which = "first-generation (L2O_BWD_V1=1)" if os.environ.get("L2O_BWD_V1") == "1" else "layer-pipelined"
-    print("n=%d T=%d  tensor-core BPTT [%s] vs chunked-fp64 reference: %.3e   exact-fp32 engine, one launch: %.3e   "
-          "(tc vs ffma: %.3e)" % (n, T, which, rel_err(d_tc, ref), rel_err(d_ff, ref), rel_err(d_tc, d_ff)), flush=True)
+    print("n=%d T=%d  tensor-core BPTT vs chunked-fp64 reference: %.3e   exact-fp32 engine, one launch: %.3e   "
+          "(tc vs ffma: %.3e)" % (n, T, rel_err(d_tc, ref), rel_err(d_ff, ref), rel_err(d_tc, d_ff)), flush=True)
 
 
 if __name__ == "__main__":

@@ -1,4 +1,4 @@
-"""Debug helper (not a test): prints tcgen05-engine error statistics against the oracle."""
+"""Debug helper (not a test): prints tensor-core-engine error statistics against the oracle."""
 import sys, torch
 sys.path.insert(0, ".")
 from oracle import l2o_oracle as orc

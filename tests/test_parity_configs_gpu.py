@@ -49,7 +49,7 @@ def test_lasso_m250_n500_T100_training_trajectory():
 def test_lasso_full_size_B128_unrolls():
     """BASELINE config #2 at its FULL size (B=128 -> 64,000 coordinates, T=100), two training unrolls.  The oracle's
     autograd graph does not fit at this size, so: x_T and every f(x_t) against the oracle's no-grad unroll driven by
-    the engine's own theta; d-theta of the tcgen05 BPTT against the exact-fp32 engine on the same checkpoints
+    the engine's own theta; d-theta of the tensor-core BPTT against the exact-fp32 engine on the same checkpoints
     (that engine is checked against the oracle's autograd at B=8 above and in test_kernels_gpu); theta against
     TF-Adam applied by the oracle to that d-theta."""
     from open_l2o_b200 import meta, problems

@@ -1,4 +1,4 @@
-"""tcgen05 engine parity: 3xTF32 tensor-core unroll vs the CPU oracle and vs the exact-fp32 FFMA engine."""
+"""Tensor-core (wgmma) engine parity: 3xTF32 unroll vs the CPU oracle and vs the exact-fp32 FFMA engine."""
 import pytest
 import torch
 
@@ -29,7 +29,7 @@ def test_tc_unroll_fwd_prerecorded(name, n, T):
 
 @pytest.mark.parametrize("T", [20, 100])
 def test_tc_fused_rastrigin_forward_then_bptt(T):
-    """BASELINE config #5 shape at reduced d: tcgen05 forward unroll (T=100: error growth over the full unroll)
+    """BASELINE config #5 shape at reduced d: tensor-core forward unroll (T=100: error growth over the full unroll)
     feeding the BPTT kernel; both against the fp64 oracle."""
     from open_l2o_b200.engine import ENGINE_TC, OPT_KINDS
     spec = SPECS["dm_identity"]
@@ -64,10 +64,10 @@ def test_tc_fused_rastrigin_forward_then_bptt(T):
 
 
 def test_tc_matches_ffma_engine_large():
-    """Many tiles per CTA (persistent loop) + ragged tail: tcgen05 engine vs exact-fp32 engine."""
+    """Many tiles per CTA (persistent loop) + ragged tail: tensor-core engine vs exact-fp32 engine."""
     from open_l2o_b200.engine import ENGINE_FFMA, ENGINE_TC, OPT_KINDS
     spec = SPECS["dm_identity"]
-    n, T = 148 * 256 * 2 + 333, 6
+    n, T = 76_109, 6
     gen = torch.Generator().manual_seed(8)
     theta = _theta(spec, gain=0.05).to(DEV)
     a, b, x0 = (torch.randn(n, generator=gen).to(DEV) for _ in range(3))
@@ -92,7 +92,7 @@ def test_tc_bwd_matches_ffma_bwd(name):
     """Same checkpoints / recorded gradients through both BPTT kernels (multi-tile, ragged tail)."""
     from open_l2o_b200.engine import ENGINE_FFMA, ENGINE_TC
     spec = SPECS[name]
-    n, T = 148 * 128 + 77, 5
+    n, T = 19_021, 5
     gen = torch.Generator().manual_seed(21)
     theta = _theta(spec, gain=0.05).to(DEV)
     from tests.helpers import wild_gradients
@@ -118,7 +118,7 @@ def test_tc_bwd_matches_ffma_bwd(name):
 
 @pytest.mark.parametrize("name", ["dm_identity", "dm_logsign"])
 def test_tc_step_operator(name):
-    """l2o_step on the tcgen05 engine (state in HBM, out-of-place) vs the oracle; chained over 3 steps."""
+    """l2o_step on the tensor-core engine (state in HBM, out-of-place) vs the oracle; chained over 3 steps."""
     from open_l2o_b200.engine import ENGINE_TC
     from tests.helpers import random_state, state_to_arena, wild_gradients
     spec = SPECS[name]
@@ -149,11 +149,11 @@ def test_tc_step_operator(name):
 
 @pytest.mark.parametrize("name", ["dm_identity", "dm_logsign"])
 def test_tc_imitation_bptt(name):
-    """Imitation ("mt") unroll on the tcgen05 engine (DM/meta_dm_train.py:463-480): forward over pre-recorded inputs
+    """Imitation ("mt") unroll on the tensor-core engine (DM/meta_dm_train.py:463-480): forward over pre-recorded inputs
     records delta_seq; the tensor-core BPTT forms dDelta_t = (delta_t - label_t)/N from it."""
     from open_l2o_b200.engine import ENGINE_TC
     spec = SPECS[name]
-    n, T = 148 * 128 + 19, 7
+    n, T = 18_963, 7
     gen = torch.Generator().manual_seed(13)
     theta = _theta(spec, gain=1.0)
     inputs = torch.randn(T, n, generator=gen)
@@ -185,7 +185,7 @@ def test_tc_imitation_bptt(name):
 
 
 def test_tc_rnnprop_step_fused_adam_features():
-    """RNNProp (DM/networks.py:279-300 + DM/meta_rnnprop_train.py:383-388) on the tcgen05 engine: l2o_step with the
+    """RNNProp (DM/networks.py:279-300 + DM/meta_rnnprop_train.py:383-388) on the tensor-core engine: l2o_step with the
     fused Adam-feature mode (m, v in/out, p from a DEVICE scalar as the captured graphs use it), fc(2->20)+ELU in the
     epilogue, tanh output; three chained steps against the oracle, incl. the recorded (m~, g~) rows."""
     from open_l2o_b200.engine import ENGINE_TC
@@ -227,10 +227,10 @@ def test_tc_rnnprop_step_fused_adam_features():
 
 def test_tc_rnnprop_fused_unroll_matches_ffma():
     """RNNProp fused unroll (in-kernel separable optimizee, Adam moments carried in registers, checkpoints and
-    (m~, g~) rows recorded) on the tcgen05 engine vs the exact-fp32 engine, multi-tile with a ragged tail."""
+    (m~, g~) rows recorded) on the tensor-core engine vs the exact-fp32 engine, multi-tile with a ragged tail."""
     from open_l2o_b200.engine import ENGINE_FFMA, ENGINE_TC, OPT_KINDS
     spec = SPECS["rnnprop"]
-    n, T = 148 * 256 + 91, 6
+    n, T = 37_979, 6
     gen = torch.Generator().manual_seed(9)
     theta = _theta(spec).to(DEV)
     a, b, x0 = (torch.randn(n, generator=gen).to(DEV) for _ in range(3))
@@ -255,9 +255,9 @@ def test_tc_rnnprop_fused_unroll_matches_ffma():
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("n,T", [(148 * 128 + 77, 5), (2 * 148 * 128 + 300, 20), (100, 3)])
+@pytest.mark.parametrize("n,T", [(19021, 5), (38188, 20), (100, 3)])
 def test_tc_rnnprop_bptt_two_pass_matches_ffma(n, T):
-    """RNNProp (fc(20) + ELU, tanh output) BPTT on the tcgen05 engine — layer-2 pass, hand-over buffer, layer-1 pass
+    """RNNProp (fc(20) + ELU, tanh output) BPTT on the tensor-core engine — layer-2 pass, hand-over buffer, layer-1 pass
     with the fc layer's own gradient — against the exact-fp32 engine on the same checkpoints, features and deltas
     (DM/networks.py:279-300, DM/meta.py:319-376).  Several tiles per CTA and a ragged tail."""
     from open_l2o_b200.engine import ENGINE_FFMA, ENGINE_TC, OPT_KINDS
@@ -296,19 +296,19 @@ def test_tc_rnnprop_bptt_two_pass_matches_ffma(n, T):
         assert rel_err(u, w) <= 2e-5, (name, rel_err(u, w))
         off += cnt
     assert off == h.n_theta
-    with pytest.raises(Exception):   # without the hand-over buffer the tcgen05 engine refuses an fc net
+    with pytest.raises(Exception):   # without the hand-over buffer the tensor-core engine refuses an fc net
         h.unroll_bwd(theta, n, T, feat, ckpt, torch.zeros_like(ref), g_rec=g_rec, delta_seq=dseq)
 
 
 @pytest.mark.gpu
 def test_tc_bptt_tanh_output_net_uses_recorded_deltas():
-    """A tanh-output DM net (DM/networks.py:227-232) on the layer-pipelined tensor-core BPTT: tanh' of the output layer comes
+    """A tanh-output DM net (DM/networks.py:227-232) on the tensor-core BPTT: tanh' of the output layer comes
     from the deltas the forward pass recorded; against the exact-fp32 engine (which recomputes y) on the same checkpoints.
-    Without the recorded deltas the tcgen05 engine refuses such a net."""
+    Without the recorded deltas the tensor-core engine refuses such a net."""
     import dataclasses
     from open_l2o_b200.engine import ENGINE_FFMA, ENGINE_TC
     spec = dataclasses.replace(SPECS["dm_logsign"], tanh_output=True, scale=0.5)
-    n, T = 148 * 128 + 61, 6
+    n, T = 19_005, 6
     gen = torch.Generator().manual_seed(17)
     theta = _theta(spec, gain=0.6).to(DEV)
     from tests.helpers import wild_gradients
