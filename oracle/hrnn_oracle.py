@@ -205,7 +205,9 @@ def step(theta: torch.Tensor, params: List[torch.Tensor], grads: List[torch.Tens
         inp = torch.sigmoid(h_new @ P["inp_decay_weights"] + P["inp_decay_bias"])
         # ---- _compute_new_learning_rate (:663-693)
         lr_change = h_new @ P["learning_rate_weights"] + P["learning_rate_bias"]
-        step_log_lr = torch.clamp(st["log_learning_rate"] + lr_change, -33.0, 33.0)
+        # straight-through clip (:674-686): the value is clamped to [-33, max_log_lr], the gradient passes as if unclipped
+        pre_log_lr = st["log_learning_rate"] + lr_change
+        step_log_lr = pre_log_lr + (torch.clamp(pre_log_lr, -33.0, 33.0) - pre_log_lr).detach()
         lrm = torch.sigmoid(P["PerTensor/learning_rate_momentum_logit"])
         new_log_lr = lrm * st["log_learning_rate"] + (1.0 - lrm) * step_log_lr
         lr_param = torch.exp(step_log_lr + P["PerTensor/param_stepsize_offset"])

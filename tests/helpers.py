@@ -70,6 +70,63 @@ def wild_gradients(n, gen):
     return g.float()
 
 
+HRNN_CONVNET = ((3, 32, 32), 10, [(3, 3, 32), (5, 5, 32)])   # optimizee of BASELINE config #4: 354,218 coordinates
+HRNN_TILE = 128   # coordinates per tile of the HierarchicalRNN coordinate kernels (l2o_hrnn.cu kBlock)
+
+
+def hrnn_ragged_shapes(n_small=300, big=20011, seed=0):
+    """n_small tensors at the sizes around a 128-coordinate tile (a lone coordinate, one short, exactly full, one over,
+    two tiles, two tiles plus one) in a seeded order, plus one tensor of 157 tiles in the middle.  More than 16
+    tensors make the HierarchicalRNN tensor_kernel's strided loops wrap."""
+    sizes = [1, 37, 127, 128, 129, 200, 255, 257]
+    perm = torch.randperm(n_small, generator=torch.Generator().manual_seed(seed))
+    shapes = [(sizes[int(k) % len(sizes)],) for k in perm]
+    shapes.insert(n_small // 2, (big,))
+    return shapes
+
+
+def hrnn_generic_theta(seed, dtype=torch.float32):
+    """HierarchicalRNN weights with no symmetry left to hide an indexing slip.  The reference's initial distribution
+    (oracle/hrnn_oracle.init_theta) zeroes whole paths and repeats constants, so a kernel that drops a term or permutes
+    entries of a constant vector computes the same numbers there.  Starting from init_theta(seed), every such block is
+    redrawn at about init scale:
+      - learning_rate_weights N(0, 0.3), and learning_rate_bias = -(init vector . Wl) + N(0, 0.05): lr_change =
+        h' . Wl + bl starts near zero and drifts by O(0.1 - 0.4) as h' moves away from the shared init vector, with a
+        sign that differs between coordinates for suitable seeds (seed 5: -0.3 .. +0.2 within 4 steps, checked in
+        tests/test_hrnn_oracle.py).  So the log-lr path is live, and a log-lr at -33 is pushed below the clip for
+        some coordinates and stays inside it for others;
+      - every gate bias 2.2 + N(0, 0.5): distinct entries, so a permuted or misplaced gate-bias row shows;
+      - candidate biases and the Param / Global / Layer1 affine biases N(0, 0.3): they are zero at init;
+      - scl / inp decay biases and the param stepsize offset shifted by N(0, 0.3);
+      - the lr-momentum logit at 2.0 + N(0, 0.3) instead of 3.2: (1 - lrm) grows from 0.04 to about 0.12, so the
+        step log-lr (and its clip) weighs more in the new log-lr.
+    The affine matrices, readouts, GradsToDelta and init vectors are already distinct random draws and are kept."""
+    from oracle import hrnn_oracle as H
+    base = H.init_theta(seed, dtype=torch.float64)
+    g = torch.Generator().manual_seed(1000 + int(seed))
+    P = H.unpack_theta(base)
+    out = []
+    for name, shape in H.theta_spec():
+        v = P[name].reshape(-1).clone()
+        n = v.numel()
+        noise = lambda s: torch.randn(n, generator=g, dtype=torch.float64) * s
+        if name == "learning_rate_weights":
+            v = noise(0.3)
+            wl = v
+        elif name == "learning_rate_bias":   # centres lr_change at the initial hidden state (see the docstring)
+            v = -(P["Level0_RNN/init_vector"].reshape(-1) @ wl).reshape(1) + noise(0.05)
+        elif name.endswith("gates/Affine/Bias"):
+            v = 2.2 + noise(0.5)
+        elif name.endswith("Bias"):   # candidate and affine biases (the gate biases are matched above)
+            v = noise(0.3)
+        elif name in ("scl_decay_bias", "inp_decay_bias") or name.endswith("param_stepsize_offset"):
+            v = v + noise(0.3)
+        elif name.endswith("learning_rate_momentum_logit"):
+            v = 2.0 + noise(0.3)
+        out.append(v)
+    return torch.cat(out).to(dtype)
+
+
 def assert_theta_close(theta_gpu, trainer, tag=None, tol=REL_TOL, tol_all=5e-5):
     """theta after TF-Adam against the oracle trainer.  Adam's update is ~ lr * sign(g) in its first steps, so entries
     whose meta-gradient sits at round-off level (|g| <= 1e-5 max|g|) may legitimately differ by a fraction of lr; every

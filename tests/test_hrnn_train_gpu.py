@@ -7,6 +7,7 @@ import pytest
 import torch
 
 from oracle import hrnn_oracle as orc   # checker only
+from tests.helpers import HRNN_CONVNET, HRNN_TILE, hrnn_generic_theta, hrnn_ragged_shapes
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -27,19 +28,22 @@ def _problem(seed=0, dtype=torch.float64, device="cpu"):
     return objective, shapes, init
 
 
-def _oracle_meta_gradient(theta, objective, init, llr, T, carry=None, initial_obj=None, want_carry=False):
-    th = theta.double().clone().requires_grad_(True)
+def _oracle_meta_gradient(theta, objective, init, llr, T, carry=None, initial_obj=None, want_carry=False,
+                          dtype=torch.float64):
+    """Autograd through the oracle's unrolled step in `dtype` (fp64: the reference; fp32: the size of round-off an
+    exact fp32 evaluation of the same computation makes).  `objective` must compute in `dtype` too."""
+    th = theta.to(dtype).clone().requires_grad_(True)
     P = orc.unpack_theta(th)
     gen = torch.Generator().manual_seed(0)
     if carry is None:
-        params = [p.double() for p in init]
+        params = [p.to(dtype) for p in init]
         states, off = [], 0
         for p in params:
             st = orc.initial_state(P, p, gen)
-            st["log_learning_rate"] = llr[off:off + p.numel()].double().reshape(-1, 1)
+            st["log_learning_rate"] = llr[off:off + p.numel()].to(dtype).reshape(-1, 1)
             off += p.numel()
             states.append(st)
-        glob = orc.initial_global_state(P, torch.float64)
+        glob = orc.initial_global_state(P, dtype)
     else:   # truncated BPTT: everything handed over from the previous unroll is a constant
         params = [p.detach() for p in carry[0]]
         states = [{k: v.detach() for k, v in st.items()} for st in carry[1]]
@@ -69,14 +73,55 @@ def _groups():
     return out
 
 
-@pytest.mark.parametrize("T", [1, 2, 5])
-def test_hrnn_meta_gradient_matches_oracle_autograd(T):
+def _separable_problem(shapes, seed=1, dtype=torch.float64, device="cpu"):
+    """sum over tensors of mean((p - target)^2) + 0.05 mean(cos 2p) (scripts/hrnn_train_check.py): every tensor's
+    gradient depends on its own coordinates only, so the oracle's autograd stays cheap at 354 K coordinates."""
+    gen = torch.Generator().manual_seed(seed)
+    tgt = [torch.randn(s, generator=gen, dtype=torch.float64).to(device=device, dtype=dtype) for s in shapes]
+
+    def objective(params):
+        return sum(((p - t) ** 2).mean() + 0.05 * torch.cos(2.0 * p).mean() for p, t in zip(params, tgt))
+    init = [torch.randn(s, generator=gen, dtype=torch.float64) * 0.5 for s in shapes]
+    return objective, init
+
+
+def _meta_problem(problem, dtype, device):
+    if problem == "toy":
+        return _problem(dtype=dtype, device=device)
+    if problem == "convnet":
+        from open_l2o_b200.scale_problems import ConvNet
+        shapes = [tuple(s) for s in ConvNet(*HRNN_CONVNET).param_shapes]
+    else:
+        shapes = hrnn_ragged_shapes()
+    objective, init = _separable_problem(shapes, dtype=dtype, device=device)
+    return objective, shapes, init
+
+
+META_CASES = ([pytest.param("toy", T, "init", False, id=str(T)) for T in (1, 2, 5)]
+              + [pytest.param("toy", 5, "generic", False, id="toy-generic-5")]
+              + [pytest.param(p, 3, th, clip, id="%s-%s" % (p, "clip" if clip else th))
+                 for p in ("convnet", "ragged") for th, clip in (("init", False), ("generic", False), ("generic", True))])
+
+
+@pytest.mark.parametrize("problem,T,theta_kind,clip", META_CASES)
+def test_hrnn_meta_gradient_matches_oracle_autograd(problem, T, theta_kind, clip):
+    """The engine's meta-gradient against autograd through the fp64 oracle.  "convnet" (BASELINE #4 shapes, 2,770
+    tiles) and "ragged" (> 300 tensors) give coord_bwd_kernel more tiles than CTAs, so its persistent loop walks
+    tensors and flushes the per-tensor adjoints on each change; "generic" theta (tests/helpers.hrnn_generic_theta)
+    makes every block of theta live and distinct; clip starts a third of the log-lrs at -33 so that the step log-lr is
+    clipped, where the gradient passes straight through (HR:674-686)."""
     from open_l2o_b200 import hrnn_train as ht
-    obj64, shapes, init = _problem(dtype=torch.float64, device="cpu")
-    obj32, _, _ = _problem(dtype=torch.float32, device=DEV)
-    theta = orc.init_theta(seed=3)
+    obj64, shapes, init = _meta_problem(problem, torch.float64, "cpu")
+    obj32, _, _ = _meta_problem(problem, torch.float32, DEV)
+    if problem != "toy":   # every backward CTA must walk >= 2 tiles (the grid is min(tiles, 2 x SMs))
+        tiles = sum(math.ceil(math.prod(s) / HRNN_TILE) for s in shapes)
+        sms = torch.cuda.get_device_properties(0).multi_processor_count
+        assert tiles >= 4 * sms, (tiles, sms)
+    theta = orc.init_theta(seed=3) if theta_kind == "init" else hrnn_generic_theta(5)
     n = sum(int(math.prod(s)) for s in shapes)
     llr = (torch.rand(n, generator=torch.Generator().manual_seed(5), dtype=torch.float64) * 3.0 - 6.0).float()
+    if clip:
+        llr[::3] = -33.0
     meta_ref, g_ref, objs_ref, x_ref = _oracle_meta_gradient(theta, obj64, init, llr, T)
     tr = ht.MetaTrainer(shapes, theta=theta, device=DEV)
     meta, g, objs, final = tr.meta_gradient(obj32, [p.float().to(DEV) for p in init], T, log_learning_rate=llr)
@@ -101,6 +146,20 @@ def test_hrnn_meta_gradient_matches_oracle_autograd(T):
     for name, lo, hi in _groups():
         ref_nz, got_nz = bool((g_ref[lo:hi] != 0).any()), bool((g[lo:hi] != 0).any())
         assert ref_nz == got_nz, (name, ref_nz, got_nz)
+    # each block against its own largest entry: 1e-5, or 3x the distance of an exact fp32 evaluation (the fp32 oracle)
+    # from fp64 on that block where round-off alone is larger
+    obj32c, _, _ = _meta_problem(problem, torch.float32, "cpu")
+    g32 = _oracle_meta_gradient(theta, obj32c, init, llr, T, dtype=torch.float32)[1].double()
+    bad = []
+    for name, lo, hi in _groups():
+        own = float(g_ref[lo:hi].abs().max())
+        if own == 0.0:
+            continue
+        e = float((g[lo:hi] - g_ref[lo:hi]).abs().max()) / own
+        tol = max(1e-5, 3.0 * float((g32[lo:hi] - g_ref[lo:hi]).abs().max()) / own)
+        if e > tol:
+            bad.append((name, e, tol, own / scale))
+    assert not bad, bad
 
 
 def test_hrnn_meta_training_rmsprop_step_and_descent():
