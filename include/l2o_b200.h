@@ -130,7 +130,7 @@ typedef struct {
   int32_t T;
   const float* theta;
   const float* in_seq;  /* [T][n_in][n] what the net was fed (g_rec rows 0..T-1, feat_rec, or the imitation inputs) */
-  const float* ckpt;    /* [T+1] arenas (slots 0..T-1 read) */
+  const float* ckpt;    /* [T+1] arenas (slots 0..T-1 read), 16-byte aligned (L2O_E_INVALID otherwise) */
   const float* g_rec;   /* [T+1][n] raw gradients -> dDelta_t = sum_{tau>t} g_tau ; NULL in imitation mode */
   const float* labels;  /* imitation mode: dDelta_t = (delta_t - label_t)/n_total */
   int64_t n_total;

@@ -10,6 +10,7 @@
 //             of layer 1 (h1p 41..60 | features 61.. | 1) are disjoint, and each layer's staged X^T keeps the other
 //             layer's rows at zero, so the two K = 64 contractions add into disjoint accumulator rows.  The accumulators
 //             are drained into the fp64 dtheta after every tile (bounded fp32 accumulation length).
+// DM nets take the checkpoint rows from a shared-memory ring that TMA bulk copies fill one layer phase ahead (CkRing).
 // fc(20) nets (RNNProp) run the two layers as two passes over time (MODE 1: layer 2, exporting dX2[h1n] to the
 // caller's hand-over buffer; MODE 2: layer 1 with the fc layer's own gradient), DM nets both layers in one pass (MODE 0).
 // Semantics: SURVEY.md Appendix B (derived from DM/meta.py:319-376, second_derivatives=False); imitation mode
@@ -69,6 +70,11 @@ __device__ __forceinline__ void mma_ss_bf16_n80(float* d, uint64_t a, uint64_t b
 }
 // named barrier over the 128 threads of warpgroup wg
 __device__ __forceinline__ void wg_bar(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
+// L2 prefetch of `bytes` (multiple of 16, 16-byte aligned) with the TMA engine / of one element
+__device__ __forceinline__ void prefetch_l2_bulk(const void* p, uint32_t bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
 // LSTM pointwise backward for one unit from the pre-activations (i, j, f, o) -> overwritten with dz; c: previous cell
 // state; dh: gradient of h'; dc: carry in (gradient of c') / out (gradient of c).  hn: h' (the output layer needs it).
@@ -116,9 +122,18 @@ template <class C, int MODE>
 __host__ __device__ constexpr uint32_t stage_bytes() {   // per warpgroup: Xa (layer 2) [| Xa (layer 1)] | Xb, hi + lo each
   return (MODE == 0 ? 4 : 2) * kXaBytes + 2 * kXbBytes;
 }
+// Checkpoint ring of one warpgroup (MODE 0): the tile's checkpoint rows the next phase reads, copied in by TMA bulk
+// copies.  The arena is [slot][h1 | c1 | h2 | c2][n][20] floats, so one block of a tile is 64 contiguous rows of 80 B,
+// 16-byte aligned for every n.  `h` holds h2(t) for layer 2, then h1(t) for layer 1 (h2 is dead once it is in the
+// operand row), so its barrier completes twice per step: parity 0 = h2, 1 = h1.
+struct alignas(16) CkRing {   // 16: the bulk-copy destinations of the next warpgroup's ring
+  float h[tc::kTile * kH], c2[tc::kTile * kH], c1[tc::kTile * kH];
+  uint64_t barh, bar2, bar1;   // h | c2 | c1 landed
+};
 template <class C, int MODE>
 __host__ __device__ constexpr size_t bwd_smem_bytes() {
-  return ((sizeof(SmemB<C, MODE>) + 1023) & ~(size_t)1023) + (size_t)kBwdWG * stage_bytes<C, MODE>();
+  return ((sizeof(SmemB<C, MODE>) + 1023) & ~(size_t)1023) +
+         (size_t)kBwdWG * (stage_bytes<C, MODE>() + (MODE == 0 ? sizeof(CkRing) : 0));
 }
 
 // MODE 0: both layers (DM nets); 1: layer 2 only, dX2[h1n] exported to a.scratch [T][n][20]; 2: layer 1 of an fc net,
@@ -137,6 +152,11 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
   constexpr uint32_t kXa2 = 0, kXa1 = 2 * kXaBytes;                          // MODE 0 only has kXa1
   constexpr uint32_t kXb = (MODE == 0 ? 4 : 2) * kXaBytes;
   constexpr bool kL2 = MODE != 2, kL1 = MODE != 1;
+  // DM nets read the checkpoint rows from the ring, and h1n(t) from the operand row, which holds h1p(t + 1)
+  constexpr bool kRing = MODE == 0;
+  CkRing& R = *reinterpret_cast<CkRing*>(smem_raw + ((sizeof(SmemB<C, MODE>) + 1023) & ~(size_t)1023) +
+                                         (size_t)kBwdWG * stage_bytes<C, MODE>() + (size_t)wg * sizeof(CkRing));
+  const bool elected = (threadIdx.x & 127) == 0;
 
   // zero the staging (rows of the other layer stay zero for the whole kernel)
   for (uint32_t o = threadIdx.x * 4; o < kBwdWG * stage_bytes<C, MODE>(); o += blockDim.x * 4)
@@ -147,6 +167,12 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
   }
   if (threadIdx.x == 0) {
     mbar_init(&S.wbar, 1);
+    if (!kRing) fence_barrier_init();
+  }
+  if (kRing && elected) {
+    mbar_init(&R.barh, 1);
+    mbar_init(&R.bar2, 1);
+    mbar_init(&R.bar1, 1);
     fence_barrier_init();
   }
   fence_proxy_async();
@@ -177,6 +203,37 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
 #pragma unroll
   for (int k = 0; k < kN / 2; ++k) dw[k] = 0.f;
   const int kx = warp * 16 + g;   // staged coordinate index of row rh = kx + 8 rh
+  const int64_t tstride = (int64_t)gridDim.x * kBwdWG;
+
+  // ---- checkpoint ring (kRing): each buffer is loaded one layer phase ahead of its reader.  The elected thread
+  // re-arms a buffer once a warpgroup barrier has seen every thread's reads of it.  bar2 and bar1 complete once per
+  // step, so both are waited with the parity `ph` of the step count; barh twice (CkRing).
+  auto ck_block = [&](int64_t tl, int t, int blk) {   // blk 0 h1 | 1 c1 | 2 h2 | 3 c2: the tile's rows of slot t
+    return a.ckpt + (int64_t)t * slot + (blk * n + tl * tc::kTile) * kH;
+  };
+  auto tile_bytes = [&](int64_t tl) {   // the ragged last tile copies its n - 64 tl rows (a multiple of 16 bytes)
+    const int64_t r = n - tl * tc::kTile;
+    return (uint32_t)((r < tc::kTile ? r : tc::kTile) * kH * 4);
+  };
+  auto arm = [&](uint64_t* bar, float* dst, int64_t tl, int t, int blk) {
+    const uint32_t b = tile_bytes(tl);
+    mbar_expect_tx(bar, b);
+    tma_bulk_g2s(dst, ck_block(tl, t, blk), b, bar);
+  };
+  auto ring5 = [&](const float* buf, int rh, bool on, float* v) {   // this thread's 5 units of row rh of a ring buffer
+    const float* p = buf + (kx + 8 * rh) * kH + 5 * q;
+#pragma unroll
+    for (int s = 0; s < kU; ++s) v[s] = on ? p[s] : 0.f;
+  };
+  if constexpr (kRing) {
+    const int64_t tile0 = (int64_t)blockIdx.x * kBwdWG + wg;
+    if (elected && tile0 < ntiles) {
+      arm(&R.barh, R.h, tile0, T - 1, 2);
+      arm(&R.bar2, R.c2, tile0, T - 1, 3);
+      arm(&R.bar1, R.c1, tile0, T - 1, 1);
+    }
+  }
+  uint32_t ph = 0;
 
   Frag<G::KB> A;
   // X^T rows of this thread's units of the 20-vector at operand column `col`: row base + 5q + s, coordinate kx + 8 rh
@@ -237,7 +294,7 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
         }
   };
 
-  for (int64_t tile = (int64_t)blockIdx.x * kBwdWG + wg; tile < ntiles; tile += (int64_t)gridDim.x * kBwdWG) {
+  for (int64_t tile = (int64_t)blockIdx.x * kBwdWG + wg; tile < ntiles; tile += tstride) {
     const int64_t r0 = tile * tc::kTile + warp * 16 + g;
     const int64_t row[2] = {r0, r0 + 8};
     const bool act[2] = {row[0] < n, row[1] < n};
@@ -255,11 +312,15 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
 
     for (int t = T - 1; t >= 0; --t) {
       const float* ck = a.ckpt + (int64_t)t * slot;
+      // the slot the ring loads next: t - 1 of this tile, or T - 1 of the warpgroup's next tile
+      const int64_t tl_next = t > 0 ? tile : tile + tstride;
+      const int t_next = t > 0 ? t - 1 : T - 1;
       float z[kN / 2];
       float dh1n[2][kU];
       // ================================= layer 2 =================================
       if constexpr (kL2) {
         float c2p[2][kU], dy[2];
+        if constexpr (kRing) mbar_wait(&R.barh, 0);
 #pragma unroll
         for (int rh = 0; rh < 2; ++rh) {
           float h1n[kU] = {0.f, 0.f, 0.f, 0.f, 0.f}, h2p[kU] = {0.f, 0.f, 0.f, 0.f, 0.f};
@@ -268,9 +329,14 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
           float dtanh = 1.0f;
           if (act[rh]) {
             const int64_t i = row[rh];
-            load5(ck + slot + i * kH, q, h1n);   // h1n(t) IS the checkpointed h1 of slot t+1
-            load5(ck + 2 * n * kH + i * kH, q, h2p);
-            load5(ck + 2 * n * kH + (n + i) * kH, q, c2p[rh]);
+            if constexpr (kRing) {
+              if (t == T - 1) load5(ck + slot + i * kH, q, h1n);
+              ring5(R.h, rh, true, h2p);
+            } else {
+              load5(ck + slot + i * kH, q, h1n);   // h1n(t) IS the checkpointed h1 of slot t+1
+              load5(ck + 2 * n * kH + i * kH, q, h2p);
+              load5(ck + 2 * n * kH + (n + i) * kH, q, c2p[rh]);
+            }
             if (imit) lam[rh] = (a.delta_seq[(int64_t)t * n + i] - a.labels[(int64_t)t * n + i]) * inv_nt;
             if (rt.tanh_output) {   // delta = scale tanh(y): the recorded delta gives tanh' without y
               const float th = a.delta_seq[(int64_t)t * n + i] / rt.scale;
@@ -278,13 +344,19 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
             }
           }
           dy[rh] = rt.scale * lam[rh] * dtanh;
-          A.template put_vec<G::ColH1>(rh, h1n);
+          // with the ring, layer 1 of step t + 1 left h1p(t + 1) = h1n(t) in the operand row (0 on inactive rows)
+          if (!kRing || t == T - 1) A.template put_vec<G::ColH1>(rh, h1n);
           A.template put_vec<G::ColH2>(rh, h2p);
         }
         wg_fence();
         mma3<kN, G::KB, G::L2Lo, G::L2Hi>(z, A, b2h, b2l);
         wg_commit();
         wg_wait<0>();   // also retires every earlier dW batch of this warp
+        if constexpr (kRing) {   // c2 is read only now, so it is not held in registers across the MMA
+          mbar_wait(&R.bar2, ph);
+#pragma unroll
+          for (int rh = 0; rh < 2; ++rh) ring5(R.c2, rh, act[rh], c2p[rh]);
+        }
         if (q == 0) acc_bo += dy[0] + dy[1];
 #pragma unroll
         for (int rh = 0; rh < 2; ++rh)
@@ -296,6 +368,10 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
             acc_wo[s] = fmaf(hn, dy[rh], acc_wo[s]);
           }
         wg_bar(wg);   // every warp has retired the previous dW batch: the staging may be overwritten
+        if (kRing && elected) {   // and every read of h2 / c2 is done: h1(t) for layer 1, c2 of the next slot
+          arm(&R.barh, R.h, tile, t, 0);
+          if (tl_next < ntiles) arm(&R.bar2, R.c2, tl_next, t_next, 3);
+        }
 #pragma unroll
         for (int rh = 0; rh < 2; ++rh) {
           stage_vec(stage + kXa2, kRowH1N, rh, G::ColH1);
@@ -329,6 +405,7 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
         float c1p[2][kU];
         float r0v[2] = {0.f, 0.f}, r1v[2] = {0.f, 0.f};
         float ep[2][kU];   // fc nets: elu'(a) of the thread's fc outputs
+        if constexpr (kRing) mbar_wait(&R.barh, 1);
 #pragma unroll
         for (int rh = 0; rh < 2; ++rh) {
           float h1p[kU] = {0.f, 0.f, 0.f, 0.f, 0.f};
@@ -336,8 +413,12 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
           for (int s = 0; s < kU; ++s) c1p[rh][s] = 0.f;
           if (act[rh]) {
             const int64_t i = row[rh];
-            load5(ck + i * kH, q, h1p);
-            load5(ck + (n + i) * kH, q, c1p[rh]);
+            if constexpr (kRing) {
+              ring5(R.h, rh, true, h1p);
+            } else {
+              load5(ck + i * kH, q, h1p);
+              load5(ck + (n + i) * kH, q, c1p[rh]);
+            }
             if constexpr (MODE == 2) {
               load5(a.scratch + ((int64_t)t * n + i) * kH, q, dh1n[rh]);
               r0v[rh] = a.in_seq[((int64_t)t * 2) * n + i];
@@ -375,6 +456,11 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
         mma3<kN, G::KB, G::L1Lo, G::L1Hi>(z, A, b1h, b1l);
         wg_commit();
         wg_wait<0>();
+        if constexpr (kRing) {
+          mbar_wait(&R.bar1, ph);
+#pragma unroll
+          for (int rh = 0; rh < 2; ++rh) ring5(R.c1, rh, act[rh], c1p[rh]);
+        }
 #pragma unroll
         for (int rh = 0; rh < 2; ++rh)
 #pragma unroll
@@ -384,6 +470,19 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
                      dh1c[rh][s] + dh1n[rh][s], dc1[rh][s], hn);
           }
         wg_bar(wg);
+        if constexpr (kRing) {   // every read of h1 / c1 is done: h2 and c1 of the next slot, its h1 and in_seq into L2
+          if (elected && tl_next < ntiles) {
+            arm(&R.barh, R.h, tl_next, t_next, 2);
+            arm(&R.bar1, R.c1, tl_next, t_next, 1);
+            prefetch_l2_bulk(ck_block(tl_next, t_next, 0), tile_bytes(tl_next));
+          }
+#pragma unroll
+          for (int rh = 0; rh < 2; ++rh) {
+            const int64_t r = tl_next * tc::kTile + kx + 8 * rh;
+            if (q == 0 && r < n) prefetch_l2(a.in_seq + (int64_t)t_next * n + r);
+          }
+          ph ^= 1u;
+        }
 #pragma unroll
         for (int rh = 0; rh < 2; ++rh) {
           if constexpr (MODE == 2) {
@@ -454,6 +553,7 @@ int tc_launch_bwd(const NetRt& rt, const l2o_bwd_args& a, float* img, cudaStream
   const int64_t ctas = (ntiles + tcb::kBwdWG - 1) / tcb::kBwdWG;
   const int grid = (int)(ctas < sms ? ctas : sms);
   auto launch = [&](auto kern, size_t smem) {
+    if (smem > 227 * 1024) return L2O_E_INVALID;
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return L2O_E_CUDA;
     kern<<<grid, tcb::kBwdThreads, smem, st>>>(a, rt, img);
     return cudaGetLastError() == cudaSuccess ? L2O_OK : L2O_E_CUDA;

@@ -163,6 +163,8 @@ int l2o_unroll_bwd(l2o_handle h, const l2o_bwd_args* a, void* stream) {
   if (!h || !a || a->n < 0 || a->T < 0 || !a->theta || !a->dtheta) return L2O_E_INVALID;
   if (a->T > 0 && !a->in_seq) return L2O_E_INVALID;
   if (h->state_floats > 0 && !a->ckpt) return L2O_E_INVALID;
+  // both engines read checkpoint rows 16 bytes at a time (FFMA: float4 loads; tensor cores: TMA bulk copies)
+  if (reinterpret_cast<uintptr_t>(a->ckpt) % 16 != 0) return L2O_E_INVALID;
   if (!a->g_rec && (!a->labels || a->n_total <= 0)) return L2O_E_INVALID;
   if (a->n == 0 || a->T == 0) return L2O_OK;
   cudaStream_t st = (cudaStream_t)stream;
