@@ -312,6 +312,45 @@ int l2o_hrnn_coord_bwd(l2o_hrnn_handle h, const l2o_hrnn_bwd_args* a, void* stre
  * [6] raw update (fp32 [N]) */
 int l2o_hrnn_workspace_layout(l2o_hrnn_handle h, int64_t offsets[7]);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * L2O-Scale CoordinatewiseRNN (CR = SC/optimizer/coordinatewise_rnn.py): a 3-layer TF LSTMCell stack [10, 20, 20] run
+ * on every coordinate independently, with learnable RMS decay and dynamic output scale.  No handle: the update has no
+ * cross-coordinate term, so one step over all optimizee tensors is one launch over their concatenated coordinates.
+ *
+ *   l2o_crnn_theta_count   the variables of CoordinatewiseRNN.__init__ + the cells' first call        CR:80-102,206
+ *   l2o_crnn_state_floats  _initialize_state: rnn [100] | rms | decay | learning_rate                  CR:151-173
+ *   l2o_crnn_step          _compute_update: rms_scaling, MultiRNNCell, readouts, x - lr'*delta       CR:175-250,
+ *                                                                              SC/optimizer/utils.py:108-160
+ *   l2o_crnn_bwd           tf.gradients of that step (TrainableOptimizer.train BPTT; the optimizee gradient g is a
+ *                          constant, SC/optimizer/trainable_optimizer.py:330-338)
+ *
+ * theta: fp32 [6402] in TF variable creation order (open_l2o_b200/coordinatewise_rnn.py THETA_SPEC).  state: 103 fp32
+ * planes of [n]: 0..99 the rnn slot packed c1 h1 c2 h2 c3 h3 (c before h, CR:306-315), 100 rms, 101 decay,
+ * 102 learning_rate.  Every float pointer must be 4-byte aligned and d_theta 8-byte aligned (L2O_E_INVALID otherwise). */
+typedef struct {
+  int64_t n;               /* coordinates (> 0) */
+  const float* theta;
+  const float* g;          /* [n] gradients */
+  const float* state_in;   /* [103][n] */
+  float* state_out;        /* [103][n]; may alias state_in */
+  float* x;                /* optional [n]: x -= lr' * delta */
+  float* update;           /* optional [n]: lr' * delta */
+} l2o_crnn_step_args;
+typedef struct {
+  int64_t n;
+  const float* theta;
+  const float* g;            /* [n] the gradients the step was fed */
+  const float* state_old;    /* [103][n] planes before the step */
+  const float* d_state_new;  /* [103][n] adjoints of the planes after the step */
+  const float* d_update;     /* [n] adjoint of lr' * delta */
+  float* d_state_old;        /* [103][n] out; must not overlap any input */
+  double* d_theta;           /* [6402] += (the init_vector block is not touched: it only enters the initial state) */
+} l2o_crnn_bwd_args;
+int64_t l2o_crnn_theta_count(void);
+int64_t l2o_crnn_state_floats(void);
+int l2o_crnn_step(const l2o_crnn_step_args* a, void* stream);
+int l2o_crnn_bwd(const l2o_crnn_bwd_args* a, void* stream);
+
 /* Number of this library's kernels launched so far in this process (bench.py's gpu_launches). */
 int64_t l2o_launch_count(void);
 const char* l2o_status_string(int status);

@@ -32,6 +32,7 @@ EXPORTS = [
     "l2o_hrnn_workspace_bytes", "l2o_hrnn_init_state", "l2o_hrnn_prepare", "l2o_hrnn_step",
     "l2o_hrnn_set_global_sizes", "l2o_hrnn_reduce_layout", "l2o_hrnn_prepare_local", "l2o_hrnn_prepare_finish",
     "l2o_hrnn_step_local", "l2o_hrnn_step_finish", "l2o_hrnn_coord_bwd", "l2o_hrnn_workspace_layout",
+    "l2o_crnn_theta_count", "l2o_crnn_state_floats", "l2o_crnn_step", "l2o_crnn_bwd",
 ]
 
 
@@ -93,6 +94,16 @@ class HrnnBwdArgs(C.Structure):
     _fields_ = [("theta", _fp), ("state_old", _fp), ("g", _fp), ("bias0", _fp), ("zero_flag", _fp), ("mean_log_lr", _fp),
                 ("d_state_new", _fp), ("d_upd", _fp), ("d_sums", _fp), ("d_state_old", _fp), ("d_theta", _fp),
                 ("d_bias0", _fp), ("d_mean_log_lr", _fp)]
+
+
+class CrnnStepArgs(C.Structure):
+    _fields_ = [("n", C.c_int64), ("theta", _fp), ("g", _fp), ("state_in", _fp), ("state_out", _fp), ("x", _fp),
+                ("update", _fp)]
+
+
+class CrnnBwdArgs(C.Structure):
+    _fields_ = [("n", C.c_int64), ("theta", _fp), ("g", _fp), ("state_old", _fp), ("d_state_new", _fp),
+                ("d_update", _fp), ("d_state_old", _fp), ("d_theta", _fp)]
 
 
 class L2OError(RuntimeError):
@@ -223,6 +234,13 @@ def lib():
                  "l2o_hrnn_prepare_finish", "l2o_hrnn_step_local", "l2o_hrnn_step_finish"):
         getattr(L, name).argtypes = [C.c_void_p, C.POINTER(HrnnArgs), C.c_void_p]
         getattr(L, name).restype = C.c_int
+    for name in ("l2o_crnn_theta_count", "l2o_crnn_state_floats"):
+        getattr(L, name).argtypes = []
+        getattr(L, name).restype = C.c_int64
+    L.l2o_crnn_step.argtypes = [C.POINTER(CrnnStepArgs), C.c_void_p]
+    L.l2o_crnn_step.restype = C.c_int
+    L.l2o_crnn_bwd.argtypes = [C.POINTER(CrnnBwdArgs), C.c_void_p]
+    L.l2o_crnn_bwd.restype = C.c_int
     for name in ("l2o_status_string", "l2o_last_cuda_error", "l2o_version"):
         getattr(L, name).restype = C.c_char_p
     L.l2o_status_string.argtypes = [C.c_int]

@@ -279,3 +279,47 @@ def note_graph_replay(kernels_in_graph: int):
 def launch_count() -> int:
     """Kernels of this library launched so far: direct C-ABI launches + kernels replayed inside captured graphs."""
     return int(_lib.lib().l2o_launch_count()) + _graph_replayed
+
+
+def replay_loop(owner, body, objective, var_list, num_steps: int, cuda_graph: bool, kernels_per_step: int, what: str):
+    """The ``minimize`` loop of the learned optimizers: ``num_steps`` calls of ``body()`` (objective, gradients, one
+    optimizer step; returns the detached objective).  Returns the objective values as floats (one device->host read).
+
+    With ``cuda_graph`` and at least 4 steps, two eager iterations (slot creation, library warm-up) are followed by one
+    iteration captured into a CUDA graph and replayed; the graph is cached on ``owner`` for the same objective and
+    variables.  A failed capture falls back to the same kernels, eagerly, with a warning."""
+    objs = []
+    n_eager = num_steps if (not cuda_graph or num_steps < 4) else 2
+    for _ in range(n_eager):
+        objs.append(body())
+    remaining = num_steps - n_eager
+    if remaining > 0:
+        # The cache holds STRONG references to the objective and the variables and compares by identity: an id()
+        # recycled by the allocator after the old closure died can never alias a new objective.  Tensors the
+        # objective closes over are baked into the graph by address - update them in place between calls.
+        key = (objective, tuple(var_list))
+        old = getattr(owner, "_graph_key", None)
+        same = (old is not None and old[0] is objective and len(old[1]) == len(var_list)
+                and all(a is b for a, b in zip(old[1], var_list)))
+        if not same:
+            try:
+                import gc
+                gc.collect()   # no finaliser (old CUDAGraph pools, handles) may run inside the capture
+                torch.cuda.synchronize()
+                graph = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(graph):
+                    static_loss = body()
+                owner._graph, owner._graph_loss, owner._graph_key = graph, static_loss, key
+            except Exception as e:   # capture not possible for this objective: same kernels, eagerly
+                import warnings
+                warnings.warn("CUDA-graph capture of the %s step failed (%r); staying eager" % (what, e))
+                torch.cuda.synchronize()
+                owner._graph_key = None
+                for _ in range(remaining):
+                    objs.append(body())
+                remaining = 0
+        for _ in range(remaining):
+            owner._graph.replay()
+            note_graph_replay(kernels_per_step)
+            objs.append(owner._graph_loss.clone())
+    return [float(o) for o in torch.stack(objs).cpu()]

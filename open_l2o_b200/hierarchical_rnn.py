@@ -399,39 +399,6 @@ class HierarchicalRNN(object):
             cuda_graph = os.environ.get("L2O_CUDA_GRAPH", "1") != "0"
         if self.distributed:
             cuda_graph = False   # the per-step collectives stay outside graph capture
-        objs = []
-        n_eager = num_steps if (not cuda_graph or num_steps < 4) else 2
-        for _ in range(n_eager):
-            objs.append(body())
-        remaining = num_steps - n_eager
-        if remaining > 0:
-            # The cache holds STRONG references to the objective and the variables and compares by identity: an id()
-            # recycled by the allocator after the old closure died can never alias a new objective.  Tensors the
-            # objective closes over are baked into the graph by address - update them in place between calls.
-            key = (objective, tuple(var_list))
-            old = getattr(self, "_graph_key", None)
-            same = (old is not None and old[0] is objective and len(old[1]) == len(var_list)
-                    and all(a is b for a, b in zip(old[1], var_list)))
-            if not same:
-                try:
-                    import gc
-                    gc.collect()   # no finaliser (old CUDAGraph pools, handles) may run inside the capture
-                    torch.cuda.synchronize()
-                    graph = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(graph):
-                        static_loss = body()
-                    self._graph, self._graph_loss, self._graph_key = graph, static_loss, key
-                except Exception as e:   # capture not possible for this objective: same kernels, eagerly
-                    import warnings
-                    warnings.warn("CUDA-graph capture of the HierarchicalRNN step failed (%r); staying eager" % (e,))
-                    torch.cuda.synchronize()
-                    self._graph_key = None
-                    for _ in range(remaining):
-                        objs.append(body())
-                    remaining = 0
-            from . import engine as _engine
-            for _ in range(remaining):
-                self._graph.replay()
-                _engine.note_graph_replay(3)   # the three l2o_hrnn_step kernels inside the graph
-                objs.append(self._graph_loss.clone())
-        return [float(o) for o in torch.stack(objs).cpu()]
+        from . import engine as _engine
+        # 3: the three l2o_hrnn_step kernels inside the graph
+        return _engine.replay_loop(self, body, objective, var_list, num_steps, cuda_graph, 3, "HierarchicalRNN")

@@ -164,23 +164,22 @@ class OptimizerState(object):
         self.planes, self.layer, self.global_state, self.zero_flag, self.x = planes, layer, global_state, zero_flag, x
 
 
-class MetaTrainer(object):
-    """``TrainableOptimizer.train`` + the RMSProp block of ``metaopt.train_optimizer`` for the HierarchicalRNN.
+class MetaTrainerBase(object):
+    """``TrainableOptimizer.train`` + the RMSProp block of ``metaopt.train_optimizer``, for any learned optimizer whose
+    subclass provides ``initial_state(params, theta, lr_init)`` and ``unroll(objective, state, num_steps, theta=None,
+    obj_weights=None, initial_obj=None)`` -> (meta objective with its graph, objective values, final state).
 
-    objective(list of tensors shaped like ``shapes``) -> scalar.  ``theta`` is the optimizer's flat weight vector
-    (``HierarchicalRNN.theta`` layout); it is updated in place by ``train_step``.
-    """
+    ``theta`` is the optimizer's flat weight vector; it is updated in place by ``train_step``.  A state is any object
+    whose tensor attributes carry the optimizer and optimizee state between unrolls."""
 
-    def __init__(self, shapes: Sequence[Sequence[int]], theta: Optional[torch.Tensor] = None, device="cuda:0",
-                 learning_rate=1e-6, rms_decay=0.9, rms_epsilon=1e-20, gradient_clip=1e4, l2_reg=0.0,
-                 use_log_objective=True, use_numerator_epsilon=False, init_lr_range=(1e-6, 1e-2), random_seed=None):
-        if not torch.cuda.is_available():
-            raise L2OError("HierarchicalRNN meta-training needs a CUDA device (no CPU path)")
+    def _setup(self, shapes, device):
         self.device = torch.device(device)
         self.shapes = [tuple(int(d) for d in s) for s in shapes]
         self.sizes = [int(math.prod(s)) if len(s) else 1 for s in self.shapes]
-        self.engine = _Engine(self.sizes, self.device)
-        self.theta = (_init_theta(random_seed) if theta is None else theta.detach().clone().float()).to(self.device)
+
+    def _setup_meta(self, theta, learning_rate, rms_decay, rms_epsilon, gradient_clip, l2_reg, use_log_objective,
+                    use_numerator_epsilon, init_lr_range, random_seed):
+        self.theta = theta.to(self.device)
         self.theta.requires_grad_(True)
         self.learning_rate, self.rms_decay, self.rms_epsilon = learning_rate, rms_decay, rms_epsilon
         self.gradient_clip, self.l2_reg = gradient_clip, l2_reg
@@ -192,7 +191,6 @@ class MetaTrainer(object):
         if random_seed is not None:
             self._gen.manual_seed(int(random_seed))
 
-    # ---- state ---------------------------------------------------------------------------------------------------
     def _split(self, flat):
         out, off = [], 0
         for s, n in zip(self.shapes, self.sizes):
@@ -200,6 +198,100 @@ class MetaTrainer(object):
             off += n
         return out
 
+    def scale_objective(self, total_obj, all_objs, initial_obj, obj_scale_eps=1e-6):
+        """trainable_optimizer.py:586-609."""
+        if self.use_log_objective:
+            if self.use_numerator_epsilon:
+                return torch.log((all_objs + obj_scale_eps) / (initial_obj + obj_scale_eps)).mean()
+            return torch.log(all_objs / (initial_obj + obj_scale_eps) + obj_scale_eps).mean()
+        return total_obj / (initial_obj + obj_scale_eps)
+
+    # ---- meta step -------------------------------------------------------------------------------------------------
+    def meta_gradient(self, objective: Callable, params: Sequence[torch.Tensor], num_steps: int,
+                      log_learning_rate: Optional[torch.Tensor] = None, state=None,
+                      initial_obj: Optional[torch.Tensor] = None):
+        """(meta objective, d meta / d theta, objective values, final state) of one unroll — from ``params`` with a fresh
+        optimizer state, or continuing from ``state`` (a detached state: truncated BPTT over partial unrolls).
+        ``log_learning_rate``: the initial learning-rate state handed to ``initial_state`` (drawn when None)."""
+        if self.theta.grad is not None:
+            self.theta.grad = None
+        st = state if state is not None else self.initial_state(params, self.theta, log_learning_rate)
+        meta, objs, final = self.unroll(objective, st, num_steps, initial_obj=initial_obj)
+        loss = meta + self.l2_reg * (self.theta ** 2).sum() if self.l2_reg else meta
+        # (a one-step unroll scores only f(x_0): constant, no meta-gradient)
+        grad = torch.autograd.grad(loss, self.theta)[0] if loss.requires_grad else torch.zeros_like(self.theta)
+        return meta.detach(), grad, [float(o.detach()) for o in objs], final
+
+    def apply_meta_gradient(self, grad: torch.Tensor):
+        """make_finite -> clip -> tf.train.RMSPropOptimizer(lr, decay, epsilon) (SC/metaopt.py:255-289)."""
+        g = torch.where(torch.isfinite(grad), grad, torch.zeros_like(grad)).clamp(-self.gradient_clip, self.gradient_clip)
+        with torch.no_grad():
+            self.rms.mul_(self.rms_decay).addcmul_(g, g, value=1.0 - self.rms_decay)
+            self.theta.sub_(self.learning_rate * g / torch.sqrt(self.rms + self.rms_epsilon))
+        self.global_step += 1
+        return g
+
+    @staticmethod
+    def detach_state(st):
+        """The state handed from one partial unroll to the next is a constant of the next unroll's meta-gradient
+        (``init_loop_vars_to_override`` assigned from ``final_loop_vals``, SC/metaopt.py:304,546-563)."""
+        out = type(st).__new__(type(st))
+        out.__dict__.update({k: v.detach() if torch.is_tensor(v) else v for k, v in vars(st).items()})
+        return out
+
+    def train_problem(self, objective: Callable, params: Sequence[torch.Tensor], num_unrolls: int, unroll_len: int,
+                      log_learning_rate: Optional[torch.Tensor] = None, obj_train_max_multiplier: float = -1.0):
+        """One training problem of ``metaopt.train_optimizer`` (SC/metaopt.py:458-613): ``num_unrolls`` partial unrolls of
+        ``unroll_len`` steps, a clipped RMSProp meta-step after each, optimizer and optimizee state carried (detached)
+        from unroll to unroll, objectives normalised by the first unroll's initial objective.  Stops early when the
+        objective is no longer finite or (``obj_train_max_multiplier`` > 0) has grown past that multiple of the initial
+        objective (the reference's loop_cond).  Returns (meta objectives, all objective values,
+        final optimizee tensors)."""
+        state, initial, metas, values = None, None, [], []
+        for u in range(num_unrolls):
+            meta, grad, objs, final = self.meta_gradient(objective, params, unroll_len, log_learning_rate, state=state,
+                                                         initial_obj=initial)
+            if not all(math.isfinite(o) for o in objs):
+                break
+            if initial is None:
+                initial = torch.tensor(objs[0], device=self.device)
+            if obj_train_max_multiplier > 0:   # loop_cond's third clause (trainable_optimizer.py:411-418): the run ends
+                f0 = float(initial)            # once the objective has grown past a multiple of the initial one
+                if max(objs) >= f0 + (obj_train_max_multiplier - 1.0) * abs(f0):
+                    break
+            self.apply_meta_gradient(grad)
+            metas.append(float(meta))
+            values.extend(objs)
+            state = self.detach_state(final)
+        out = self._split(state.x) if state is not None else [p.detach() for p in params]
+        return metas, values, out
+
+    def train_step(self, objective: Callable, params: Sequence[torch.Tensor], num_steps: int,
+                   log_learning_rate: Optional[torch.Tensor] = None):
+        meta, grad, objs, final = self.meta_gradient(objective, params, num_steps, log_learning_rate)
+        self.apply_meta_gradient(grad)
+        return float(meta), objs, self._split(final.x.detach())
+
+
+class MetaTrainer(MetaTrainerBase):
+    """``TrainableOptimizer.train`` + the RMSProp block of ``metaopt.train_optimizer`` for the HierarchicalRNN.
+
+    objective(list of tensors shaped like ``shapes``) -> scalar.  ``theta`` is the optimizer's flat weight vector
+    (``HierarchicalRNN.theta`` layout); it is updated in place by ``train_step``.
+    """
+
+    def __init__(self, shapes: Sequence[Sequence[int]], theta: Optional[torch.Tensor] = None, device="cuda:0",
+                 learning_rate=1e-6, rms_decay=0.9, rms_epsilon=1e-20, gradient_clip=1e4, l2_reg=0.0,
+                 use_log_objective=True, use_numerator_epsilon=False, init_lr_range=(1e-6, 1e-2), random_seed=None):
+        if not torch.cuda.is_available():
+            raise L2OError("HierarchicalRNN meta-training needs a CUDA device (no CPU path)")
+        self._setup(shapes, device)
+        self.engine = _Engine(self.sizes, self.device)
+        self._setup_meta(_init_theta(random_seed) if theta is None else theta.detach().clone().float(), learning_rate,
+                         rms_decay, rms_epsilon, gradient_clip, l2_reg, use_log_objective, use_numerator_epsilon,
+                         init_lr_range, random_seed)
+
+    # ---- state ---------------------------------------------------------------------------------------------------
     def initial_state(self, params: Sequence[torch.Tensor], theta: torch.Tensor,
                       log_learning_rate: Optional[torch.Tensor] = None):
         """_initialize_state / _initialize_global_state (HR:303-350); the learnable init vectors keep their graph."""
@@ -276,77 +368,6 @@ class MetaTrainer(object):
         initial = objs[0].detach() if initial_obj is None else initial_obj
         meta = self.scale_objective(total, torch.stack([o.reshape(()) for o in objs]), initial)
         return meta, objs, OptimizerState(planes, layer, glob, zero_flag, x)
-
-    def scale_objective(self, total_obj, all_objs, initial_obj, obj_scale_eps=1e-6):
-        """trainable_optimizer.py:586-609."""
-        if self.use_log_objective:
-            if self.use_numerator_epsilon:
-                return torch.log((all_objs + obj_scale_eps) / (initial_obj + obj_scale_eps)).mean()
-            return torch.log(all_objs / (initial_obj + obj_scale_eps) + obj_scale_eps).mean()
-        return total_obj / (initial_obj + obj_scale_eps)
-
-    # ---- meta step -------------------------------------------------------------------------------------------------
-    def meta_gradient(self, objective: Callable, params: Sequence[torch.Tensor], num_steps: int,
-                      log_learning_rate: Optional[torch.Tensor] = None, state: Optional[OptimizerState] = None,
-                      initial_obj: Optional[torch.Tensor] = None):
-        """(meta objective, d meta / d theta, objective values, final state) of one unroll — from ``params`` with a fresh
-        optimizer state, or continuing from ``state`` (a detached OptimizerState: truncated BPTT over partial unrolls)."""
-        if self.theta.grad is not None:
-            self.theta.grad = None
-        st = state if state is not None else self.initial_state(params, self.theta, log_learning_rate)
-        meta, objs, final = self.unroll(objective, st, num_steps, initial_obj=initial_obj)
-        loss = meta + self.l2_reg * (self.theta ** 2).sum() if self.l2_reg else meta
-        # (a one-step unroll scores only f(x_0): constant, no meta-gradient)
-        grad = torch.autograd.grad(loss, self.theta)[0] if loss.requires_grad else torch.zeros_like(self.theta)
-        return meta.detach(), grad, [float(o.detach()) for o in objs], final
-
-    def apply_meta_gradient(self, grad: torch.Tensor):
-        """make_finite -> clip -> tf.train.RMSPropOptimizer(lr, decay, epsilon) (SC/metaopt.py:255-289)."""
-        g = torch.where(torch.isfinite(grad), grad, torch.zeros_like(grad)).clamp(-self.gradient_clip, self.gradient_clip)
-        with torch.no_grad():
-            self.rms.mul_(self.rms_decay).addcmul_(g, g, value=1.0 - self.rms_decay)
-            self.theta.sub_(self.learning_rate * g / torch.sqrt(self.rms + self.rms_epsilon))
-        self.global_step += 1
-        return g
-
-    @staticmethod
-    def detach_state(st: OptimizerState) -> OptimizerState:
-        """The state handed from one partial unroll to the next is a constant of the next unroll's meta-gradient
-        (``init_loop_vars_to_override`` assigned from ``final_loop_vals``, SC/metaopt.py:304,546-563)."""
-        return OptimizerState(st.planes.detach(), st.layer.detach(), st.global_state.detach(), st.zero_flag, st.x.detach())
-
-    def train_problem(self, objective: Callable, params: Sequence[torch.Tensor], num_unrolls: int, unroll_len: int,
-                      log_learning_rate: Optional[torch.Tensor] = None, obj_train_max_multiplier: float = -1.0):
-        """One training problem of ``metaopt.train_optimizer`` (SC/metaopt.py:458-613): ``num_unrolls`` partial unrolls of
-        ``unroll_len`` steps, a clipped RMSProp meta-step after each, optimizer and optimizee state carried (detached)
-        from unroll to unroll, objectives normalised by the first unroll's initial objective.  Stops early when the
-        objective is no longer finite or (``obj_train_max_multiplier`` > 0) has grown past that multiple of the initial
-        objective (the reference's loop_cond).  Returns (meta objectives, all objective values,
-        final optimizee tensors)."""
-        state, initial, metas, values = None, None, [], []
-        for u in range(num_unrolls):
-            meta, grad, objs, final = self.meta_gradient(objective, params, unroll_len, log_learning_rate, state=state,
-                                                         initial_obj=initial)
-            if not all(math.isfinite(o) for o in objs):
-                break
-            if initial is None:
-                initial = torch.tensor(objs[0], device=self.device)
-            if obj_train_max_multiplier > 0:   # loop_cond's third clause (trainable_optimizer.py:411-418): the run ends
-                f0 = float(initial)            # once the objective has grown past a multiple of the initial one
-                if max(objs) >= f0 + (obj_train_max_multiplier - 1.0) * abs(f0):
-                    break
-            self.apply_meta_gradient(grad)
-            metas.append(float(meta))
-            values.extend(objs)
-            state = self.detach_state(final)
-        out = self._split(state.x) if state is not None else [p.detach() for p in params]
-        return metas, values, out
-
-    def train_step(self, objective: Callable, params: Sequence[torch.Tensor], num_steps: int,
-                   log_learning_rate: Optional[torch.Tensor] = None):
-        meta, grad, objs, final = self.meta_gradient(objective, params, num_steps, log_learning_rate)
-        self.apply_meta_gradient(grad)
-        return float(meta), objs, self._split(final.x.detach())
 
 
 def train_optimizer(make_trainer: Callable, problems: Sequence, num_problems: int, num_meta_iterations: int,
