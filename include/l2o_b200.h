@@ -283,7 +283,10 @@ int l2o_hrnn_step_local(l2o_hrnn_handle h, const l2o_hrnn_args* a, void* stream)
 int l2o_hrnn_step_finish(l2o_hrnn_handle h, const l2o_hrnn_args* a, void* stream);
 
 /* Meta-training of the HierarchicalRNN (SC/optimizer/trainable_optimizer.py:200-470: BPTT through the unrolled
- * optimizer; the optimizee's gradients are stop_gradient'ed, :332-338).  The per-parameter level — everything that
+ * optimizer).  The reference's default, use_second_derivatives=True, differentiates through the optimizee's gradients
+ * g as well; it stop_gradient's them only when the flag is off (:330-338).  g is a constant of this backward when d_g
+ * is null; otherwise d_g receives the adjoint of g, which the caller carries on to x through the optimizee's
+ * Hessian-vector product.  The per-parameter level — everything that
  * touches N coordinates — is differentiated by l2o_hrnn_coord_bwd; the per-tensor / global GRUs, the 1/RMS(delta)
  * normalisation, the problem-wide mean log-lr and the objective are [n_tensors x 20]-sized and are differentiated by the
  * host (open_l2o_b200/hrnn_train.py builds them as torch autograd around these two entry points).
@@ -305,6 +308,7 @@ typedef struct {
   double* d_theta;           /* [theta_count] += (the 739 per-parameter-level weights) */
   double* d_bias0;           /* [n_tensors][32] += */
   double* d_mean_log_lr;     /* [1] += */
+  float* d_g;                /* optional [N] out: adjoint of g; 4-byte aligned, overlapping no other buffer (else L2O_E_INVALID) */
 } l2o_hrnn_bwd_args;
 int l2o_hrnn_coord_bwd(l2o_hrnn_handle h, const l2o_hrnn_bwd_args* a, void* stream);
 /* byte offsets inside the workspace: [0] sums (fp64 [n_tensors][24]) [1] any_nz (int32 [n_tensors][4]) [2] zero_flag
@@ -321,8 +325,10 @@ int l2o_hrnn_workspace_layout(l2o_hrnn_handle h, int64_t offsets[7]);
  *   l2o_crnn_state_floats  _initialize_state: rnn [100] | rms | decay | learning_rate                  CR:151-173
  *   l2o_crnn_step          _compute_update: rms_scaling, MultiRNNCell, readouts, x - lr'*delta       CR:175-250,
  *                                                                              SC/optimizer/utils.py:108-160
- *   l2o_crnn_bwd           tf.gradients of that step (TrainableOptimizer.train BPTT; the optimizee gradient g is a
- *                          constant, SC/optimizer/trainable_optimizer.py:330-338)
+ *   l2o_crnn_bwd           tf.gradients of that step (TrainableOptimizer.train BPTT).  The optimizee gradient g is a
+ *                          constant when d_g is null, as in the reference with use_second_derivatives off
+ *                          (SC/optimizer/trainable_optimizer.py:330-338); the reference's default differentiates
+ *                          through g, and d_g then receives its adjoint
  *
  * theta: fp32 [6402] in TF variable creation order (open_l2o_b200/coordinatewise_rnn.py THETA_SPEC).  state: 103 fp32
  * planes of [n]: 0..99 the rnn slot packed c1 h1 c2 h2 c3 h3 (c before h, CR:306-315), 100 rms, 101 decay,
@@ -345,6 +351,7 @@ typedef struct {
   const float* d_update;     /* [n] adjoint of lr' * delta */
   float* d_state_old;        /* [103][n] out; must not overlap any input */
   double* d_theta;           /* [6402] += (the init_vector block is not touched: it only enters the initial state) */
+  float* d_g;                /* optional [n] out: adjoint of g; 4-byte aligned, overlapping no other buffer (else L2O_E_INVALID) */
 } l2o_crnn_bwd_args;
 int64_t l2o_crnn_theta_count(void);
 int64_t l2o_crnn_state_floats(void);

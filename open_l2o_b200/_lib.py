@@ -93,7 +93,7 @@ class HrnnArgs(C.Structure):
 class HrnnBwdArgs(C.Structure):
     _fields_ = [("theta", _fp), ("state_old", _fp), ("g", _fp), ("bias0", _fp), ("zero_flag", _fp), ("mean_log_lr", _fp),
                 ("d_state_new", _fp), ("d_upd", _fp), ("d_sums", _fp), ("d_state_old", _fp), ("d_theta", _fp),
-                ("d_bias0", _fp), ("d_mean_log_lr", _fp)]
+                ("d_bias0", _fp), ("d_mean_log_lr", _fp), ("d_g", _fp)]
 
 
 class CrnnStepArgs(C.Structure):
@@ -103,7 +103,7 @@ class CrnnStepArgs(C.Structure):
 
 class CrnnBwdArgs(C.Structure):
     _fields_ = [("n", C.c_int64), ("theta", _fp), ("g", _fp), ("state_old", _fp), ("d_state_new", _fp),
-                ("d_update", _fp), ("d_state_old", _fp), ("d_theta", _fp)]
+                ("d_update", _fp), ("d_state_old", _fp), ("d_theta", _fp), ("d_g", _fp)]
 
 
 class L2OError(RuntimeError):

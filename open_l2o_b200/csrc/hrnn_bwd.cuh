@@ -1,13 +1,17 @@
 // HierarchicalRNN per-parameter level, BACKWARD (meta-training: BPTT through l2o_hrnn_step; included by l2o_hrnn.cu
 // inside namespace l2o::hrnn).  Reference: the TF autodiff of HR:444-540 (features), rnn_cells.py:46-68 (BiasGRU),
-// HR:606-706 (readouts) as driven by SC/optimizer/trainable_optimizer.py:200-470 (gradients of the optimizee are
-// stop_gradient'ed, :332-338, so g is a constant here).
+// HR:606-706 (readouts) as driven by SC/optimizer/trainable_optimizer.py:200-470.  The reference stop_gradient's the
+// optimizee's gradients only when use_second_derivatives is off (:330-338; its default is on): with a null d_g, g is a
+// constant here; otherwise the kernel also writes d g, the per-coordinate part of the second-order term (the optimizee's
+// Hessian-vector product that carries it on to x belongs to the caller).
 //
 // One thread = one coordinate: recompute the forward step from the planes BEFORE the step (exact-fp32 FFMA, the same
 // MUFU forms as the forward kernels), then walk it backwards.  Inputs: adjoints of the 21 new planes, of the raw update
 // lr*delta (w.upd, before the per-tensor 1/RMS) and of the 24 per-tensor sums (broadcast to the tensor's coordinates).
 // Outputs: adjoints of the 21 old planes; d theta of the 739 per-parameter-level weights; per-tensor d bias0 (the
-// injected gate bias) and d mean_log_lr.  The cross-coordinate pieces (per-tensor / global GRUs, 1/RMS(delta), the
+// injected gate bias) and d mean_log_lr; optionally d g.  g enters only through the four accumulators
+// acc'_s = g (1 - d_s) + acc_s d_s, so d g = sum_s d acc'_s (1 - d_s); the tensor-wide ALL(ms == 0) first-step predicate
+// is piecewise constant and has no derivative.  The cross-coordinate pieces (per-tensor / global GRUs, 1/RMS(delta), the
 // problem-wide mean log-lr, the objective) are tiny and live on the host side as torch autograd (hrnn_train.py).
 //
 // Reductions: every per-coordinate contribution is summed over the warp with a shuffle butterfly and added to a
@@ -38,6 +42,7 @@ struct Args {
   double* d_theta;          // [kTheta] +=
   double* d_bias0;          // [nt][kB0Stride] +=
   double* d_mean_log_lr;    // [1] +=
+  float* d_g;               // [n] or null
 };
 
 __device__ __forceinline__ float warp_sum(float v) {
@@ -292,7 +297,8 @@ __global__ void __launch_bounds__(kBwdBlock) coord_bwd_kernel(Args a, int64_t n,
       if (s < NS - 1) dsc[s] += din[NS + s] * sc[s + 1];
       if (s > 0) dsc[s] += din[NS + s - 1] * sc[s - 1];
     }
-    float dsd = 0.f, ddec[NS], dacc_old[NS], dms_old[NS];
+    const bool want_dg = a.d_g != nullptr;
+    float dsd = 0.f, ddec[NS], dacc_old[NS], dms_old[NS], dg = 0.f;
 #pragma unroll
     for (int s = 0; s < NS; ++s) {
       const float dr = dsc[s] / tt[s];
@@ -305,6 +311,7 @@ __global__ void __launch_bounds__(kBwdBlock) coord_bwd_kernel(Args a, int64_t n,
       if (!zf[s]) dsd += dms * (ms_old[s] - q[s]);
       dacc_old[s] = dacc * dec[s];
       ddec[s] = dacc * (acc_old[s] - gi);
+      if (want_dg) dg += dacc * (1.0f - dec[s]);
     }
 #pragma unroll
     for (int s = NS - 1; s > 0; --s) ddec[s - 1] += dec[s] > 0.f ? ddec[s] * 0.5f / dec[s] : 0.f;
@@ -319,6 +326,7 @@ __global__ void __launch_bounds__(kBwdBlock) coord_bwd_kernel(Args a, int64_t n,
         a.d_state_old[(int64_t)(P_ACC + s) * n + i] = dacc_old[s];
         a.d_state_old[(int64_t)(P_MS + s) * n + i] = dms_old[s];
       }
+      if (want_dg) a.d_g[i] = dg;
     }
   }
   if (cur_tensor >= 0) flush_ten(cur_tensor);

@@ -68,6 +68,7 @@ struct BwdArgs {
   const float* d_update;
   float* d_state_old;
   double* d_theta;
+  float* d_g;   // [n] or null
 };
 
 __device__ __forceinline__ float dsig(float s) { return s * (1.0f - s); }
@@ -192,7 +193,8 @@ __global__ void __launch_bounds__(kFwdBlock) step_kernel(StepArgs a) {
 
 // ------------------------------------------------------------------------------------------------------------------
 // backward: recompute the step from the old planes and g, then walk it backwards (readouts, LSTM 3 -> 1, asinh and the
-// ms chain).  d theta of each cell is the tile contraction X^T dZ over the CTA's 128 coordinates (X = [inp | h | 1] rows,
+// ms chain).  g enters through ms' and v = g / sqrt(ms' + 1e-16) only, so with a non-null d_g the kernel also writes
+// d g = dv / sqrt(ms' + 1e-16) + dms' (1 - d) 2g (second-order meta-gradients).  d theta of each cell is the tile contraction X^T dZ over the CTA's 128 coordinates (X = [inp | h | 1] rows,
 // dZ = gate adjoints), done from shared memory into a per-CTA image of d theta that is flushed once per CTA with fp64
 // atomics; the readout weights go through warp sums into the same image.
 struct BwdSmem {
@@ -414,13 +416,14 @@ __global__ void __launch_bounds__(kBwdBlock, 1) bwd_kernel(BwdArgs a) {
     __syncthreads();
     contract<1 + H1 + 1, H1, 2>(S, S.img + O_K1);
     __syncthreads();
-    // ---------------------------------------------------------------- asinh and the ms chain (g is a constant)
+    // ---------------------------------------------------------------- asinh and the ms chain (and d g when asked)
     const float dv = dr[0] * rsqrtf(fmaf(v, v, 1.0f));
     const float dmsn = (act ? a.d_state_new[P_RMS * n + i] : 0.f) - 0.5f * dv * v / (msn + 1e-16f);
     if (act) {
       a.d_state_old[P_RMS * n + i] = dmsn * d;
       a.d_state_old[P_DECAY * n + i] = dmsn * (ms - q);
       a.d_state_old[P_LR * n + i] = dlr;
+      if (a.d_g) a.d_g[i] = dv / sqrtf(msn + 1e-16f) + dmsn * (1.0f - d) * 2.0f * g;
     }
   }
   __syncthreads();
@@ -492,10 +495,18 @@ int l2o_crnn_bwd(const l2o_crnn_bwd_args* a, void* stream) {
   for (const void* p : fp)
     if (misaligned(p, alignof(float))) return L2O_E_INVALID;
   if (misaligned(a->d_theta, alignof(double))) return L2O_E_INVALID;
+  if (a->d_g) {
+    if (misaligned(a->d_g, alignof(float))) return L2O_E_INVALID;
+    const size_t n = (size_t)a->n, f = sizeof(float);
+    const void* other[] = {a->theta, a->g, a->state_old, a->d_state_new, a->d_update, a->d_state_old, a->d_theta};
+    const size_t bytes[] = {kTheta * f, n * f, kPlanes * n * f, kPlanes * n * f, n * f, kPlanes * n * f,
+                            kTheta * sizeof(double)};
+    if (l2o::overlaps_any(a->d_g, n * f, other, bytes, 7)) return L2O_E_INVALID;
+  }
   const int cap = bwd_grid();
   if (cap <= 0) return l2o::set_cuda_error(cudaGetLastError(), "l2o_crnn_bwd shared-memory size");
   const int64_t tiles = (a->n + kBwdBlock - 1) / kBwdBlock;
-  BwdArgs k{a->n, a->theta, a->g, a->state_old, a->d_state_new, a->d_update, a->d_state_old, a->d_theta};
+  BwdArgs k{a->n, a->theta, a->g, a->state_old, a->d_state_new, a->d_update, a->d_state_old, a->d_theta, a->d_g};
   bwd_kernel<<<(unsigned)(tiles < cap ? tiles : cap), kBwdBlock, sizeof(BwdSmem), (cudaStream_t)stream>>>(k);
   L2O_CUDA_TRY(cudaGetLastError());
   l2o::count_launch();

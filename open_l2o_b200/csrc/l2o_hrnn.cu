@@ -637,8 +637,17 @@ int l2o_hrnn_coord_bwd(l2o_hrnn_handle h, const l2o_hrnn_bwd_args* a, void* stre
   if (!h || !a || !a->theta || !a->state_old || !a->g || !a->bias0 || !a->zero_flag || !a->mean_log_lr ||
       !a->d_state_new || !a->d_upd || !a->d_sums || !a->d_state_old || !a->d_theta || !a->d_bias0 || !a->d_mean_log_lr)
     return L2O_E_INVALID;
+  if (a->d_g) {
+    if ((uintptr_t)a->d_g & (alignof(float) - 1)) return L2O_E_INVALID;
+    const size_t n = (size_t)h->n, nt = (size_t)h->nt, f = sizeof(float), d = sizeof(double);
+    const void* other[] = {a->theta, a->state_old, a->g, a->bias0, a->zero_flag, a->mean_log_lr, a->d_state_new,
+                           a->d_upd, a->d_sums, a->d_state_old, a->d_theta, a->d_bias0, a->d_mean_log_lr};
+    const size_t bytes[] = {kTheta * f, kPlanes * n * f, n * f, nt * kB0Stride * f, nt * NS * sizeof(int32_t), f,
+                            kPlanes * n * f, n * f, nt * kAcc * f, kPlanes * n * f, kTheta * d, nt * kB0Stride * d, d};
+    if (l2o::overlaps_any(a->d_g, n * f, other, bytes, 13)) return L2O_E_INVALID;
+  }
   bwd::Args k{a->theta, a->state_old, a->g, a->bias0, a->zero_flag, a->mean_log_lr, a->d_state_new, a->d_upd, a->d_sums,
-              a->d_state_old, a->d_theta, a->d_bias0, a->d_mean_log_lr};
+              a->d_state_old, a->d_theta, a->d_bias0, a->d_mean_log_lr, a->d_g};
   int dev = 0, sms = 132;
   if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int grid = h->nblocks < 2 * sms ? h->nblocks : 2 * sms;

@@ -32,6 +32,16 @@ int set_cuda_error(cudaError_t e, const char* where);  // records the message, r
 void count_launch(int n = 1);
 int device_sms();  // SM count of the current device (cached), 0 on failure
 
+// Does the byte range [p, p + bytes) share a byte with any of the ranges (q[k], qbytes[k])?  Null q[k] are skipped.
+inline bool overlaps_any(const void* p, size_t bytes, const void* const* q, const size_t* qbytes, int nq) {
+  const uintptr_t a = (uintptr_t)p;
+  for (int k = 0; k < nq; ++k) {
+    const uintptr_t b = (uintptr_t)q[k];
+    if (b && a < b + qbytes[k] && b < a + bytes) return true;
+  }
+  return false;
+}
+
 int ffma_step(const l2o_net* h, const l2o_step_args& a, cudaStream_t st);
 int ffma_unroll_fwd(const l2o_net* h, const l2o_unroll_args& a, cudaStream_t st);
 int ffma_unroll_bwd(const l2o_net* h, const l2o_bwd_args& a, cudaStream_t st);

@@ -3,8 +3,14 @@ the clipped RMSProp meta-step.
 
 Mirrors ``TrainableOptimizer.train`` (SC/optimizer/trainable_optimizer.py:200-470; SC/ =
 Model_Free_L2O/L2O-Scale/L2O-Scale-Training/), ``scale_objective`` (:586-609) and the meta-optimizer block of
-``metaopt.train_optimizer`` (SC/metaopt.py:255-289).  As in the reference the optimizee's gradients are constants of
-the meta-gradient (``tf.stop_gradient``, trainable_optimizer.py:332-338).
+``metaopt.train_optimizer`` (SC/metaopt.py:255-289).
+
+Second derivatives.  The reference differentiates through the optimizee's gradients g by default
+(``use_second_derivatives=True``, trainable_optimizer.py:61-84) and wraps them in ``tf.stop_gradient`` only when the flag
+is off (:330-338).  ``MetaTrainer(use_second_derivatives=True)`` does the same: ``l2o_hrnn_coord_bwd`` then also returns
+the adjoint of g, and torch autograd carries it on to x through the optimizee's Hessian-vector product (the gradient is
+taken with ``create_graph=True``).  The trainers' default stays ``False`` (g a constant: the cheaper, first-order
+meta-gradient) so that existing training runs keep their meta-gradients.
 
 Where the arithmetic runs.  Everything that touches the N optimizee coordinates is CUDA in ``libl2o_b200.so``: the forward
 step of the per-parameter level is the tensor-core kernel of the inference path (``l2o_hrnn_step_local``), its backward is
@@ -111,10 +117,12 @@ class _Engine(object):
         _lib.check(_lib.lib().l2o_hrnn_step_local(self._h, C.byref(a), st), "l2o_hrnn_step_local")
         return state, self.w_upd.clone(), self.w_sums.to(torch.float32), self.w_any.clone()
 
-    def coord_backward(self, theta, planes_old, bias0, mean_llr, g, zero_flag, d_planes, d_upd, d_sums):
+    def coord_backward(self, theta, planes_old, bias0, mean_llr, g, zero_flag, d_planes, d_upd, d_sums, want_dg=False):
+        """Adjoints of (theta, old planes, bias0, mean log-lr) and, with ``want_dg``, of g (else None)."""
         st = torch.cuda.current_stream().cuda_stream
         dev = self.device
         d_old = torch.empty_like(planes_old)
+        d_g = torch.empty(self.N, dtype=torch.float32, device=dev) if want_dg else None
         d_theta = torch.zeros(theta.numel(), dtype=torch.float64, device=dev)
         d_bias0 = torch.zeros(self.nt, B0_STRIDE, dtype=torch.float64, device=dev)
         d_mean = torch.zeros(1, dtype=torch.float64, device=dev)
@@ -130,12 +138,14 @@ class _Engine(object):
                                             self._f32(keep[7], "d_sums"))
         a.d_state_old = d_old.data_ptr()
         a.d_theta, a.d_bias0, a.d_mean_log_lr = d_theta.data_ptr(), d_bias0.data_ptr(), d_mean.data_ptr()
+        a.d_g = None if d_g is None else d_g.data_ptr()
         _lib.check(_lib.lib().l2o_hrnn_coord_bwd(self._h, C.byref(a), st), "l2o_hrnn_coord_bwd")
-        return d_theta.to(torch.float32), d_old, d_bias0.to(torch.float32), d_mean.to(torch.float32)
+        return d_theta.to(torch.float32), d_old, d_bias0.to(torch.float32), d_mean.to(torch.float32), d_g
 
 
 class _CoordStep(torch.autograd.Function):
-    """The per-parameter level of one optimizer step as an autograd node around the two CUDA entry points."""
+    """The per-parameter level of one optimizer step as an autograd node around the two CUDA entry points.  The adjoint
+    of g is computed only when autograd asks for it (g carries a graph: second-order meta-gradients)."""
 
     @staticmethod
     def forward(ctx, eng, theta, planes, bias0, mean_llr, g, zero_flag):
@@ -150,10 +160,10 @@ class _CoordStep(torch.autograd.Function):
         theta, planes, bias0, mean_llr, g, zero_flag = ctx.saved_tensors
         eng = ctx.eng
         z = lambda t, like: torch.zeros_like(like) if t is None else t.contiguous()
-        d_theta, d_old, d_bias0, d_mean = eng.coord_backward(
+        d_theta, d_old, d_bias0, d_mean, d_g = eng.coord_backward(
             theta, planes, bias0, mean_llr, g, zero_flag, z(d_planes, planes),
-            z(d_upd, g), z(d_sums, torch.empty(eng.nt, N_SUMS, device=planes.device)))
-        return None, d_theta, d_old, d_bias0, d_mean.reshape(mean_llr.shape), None, None
+            z(d_upd, g), z(d_sums, torch.empty(eng.nt, N_SUMS, device=planes.device)), want_dg=ctx.needs_input_grad[5])
+        return None, d_theta, d_old, d_bias0, d_mean.reshape(mean_llr.shape), d_g, None
 
 
 class OptimizerState(object):
@@ -178,12 +188,13 @@ class MetaTrainerBase(object):
         self.sizes = [int(math.prod(s)) if len(s) else 1 for s in self.shapes]
 
     def _setup_meta(self, theta, learning_rate, rms_decay, rms_epsilon, gradient_clip, l2_reg, use_log_objective,
-                    use_numerator_epsilon, init_lr_range, random_seed):
+                    use_numerator_epsilon, init_lr_range, random_seed, use_second_derivatives=False):
         self.theta = theta.to(self.device)
         self.theta.requires_grad_(True)
         self.learning_rate, self.rms_decay, self.rms_epsilon = learning_rate, rms_decay, rms_epsilon
         self.gradient_clip, self.l2_reg = gradient_clip, l2_reg
         self.use_log_objective, self.use_numerator_epsilon = use_log_objective, use_numerator_epsilon
+        self.use_second_derivatives = bool(use_second_derivatives)
         self.init_lr_range = init_lr_range
         self.rms = torch.ones_like(self.theta)     # tf.train.RMSPropOptimizer initialises its accumulator to one
         self.global_step = 0
@@ -272,24 +283,43 @@ class MetaTrainerBase(object):
         self.apply_meta_gradient(grad)
         return float(meta), objs, self._split(final.x.detach())
 
+    def _objective_and_gradient(self, objective: Callable, x: torch.Tensor):
+        """f(x_t) and g_t = df/dx_t in one evaluation.  g_t is handed to the step detached (a constant of the
+        meta-gradient) unless ``use_second_derivatives`` is on and x_t depends on theta; then it keeps its graph, so
+        that the meta-gradient includes the optimizee's Hessian-vector product."""
+        second = self.use_second_derivatives and x.requires_grad
+        with torch.enable_grad():
+            xg = x if x.requires_grad else x.detach().requires_grad_(True)
+            obj = objective(self._split(xg))
+            (g,) = torch.autograd.grad(obj, xg, retain_graph=x.requires_grad, create_graph=second)
+        if not x.requires_grad:
+            obj = obj.detach()
+        return obj, (g if second else g.detach()).contiguous()
+
 
 class MetaTrainer(MetaTrainerBase):
     """``TrainableOptimizer.train`` + the RMSProp block of ``metaopt.train_optimizer`` for the HierarchicalRNN.
 
     objective(list of tensors shaped like ``shapes``) -> scalar.  ``theta`` is the optimizer's flat weight vector
     (``HierarchicalRNN.theta`` layout); it is updated in place by ``train_step``.
+
+    ``use_second_derivatives``: differentiate through the optimizee's gradients (the reference's
+    ``TrainableOptimizer`` argument, default ``True`` there).  The default here is ``False``, the first-order
+    meta-gradient this trainer has always computed; the second-order one keeps the optimizee's double-backward graph of
+    every step of an unroll alive until the meta-gradient is taken.
     """
 
     def __init__(self, shapes: Sequence[Sequence[int]], theta: Optional[torch.Tensor] = None, device="cuda:0",
                  learning_rate=1e-6, rms_decay=0.9, rms_epsilon=1e-20, gradient_clip=1e4, l2_reg=0.0,
-                 use_log_objective=True, use_numerator_epsilon=False, init_lr_range=(1e-6, 1e-2), random_seed=None):
+                 use_log_objective=True, use_numerator_epsilon=False, init_lr_range=(1e-6, 1e-2), random_seed=None,
+                 use_second_derivatives=False):
         if not torch.cuda.is_available():
             raise L2OError("HierarchicalRNN meta-training needs a CUDA device (no CPU path)")
         self._setup(shapes, device)
         self.engine = _Engine(self.sizes, self.device)
         self._setup_meta(_init_theta(random_seed) if theta is None else theta.detach().clone().float(), learning_rate,
                          rms_decay, rms_epsilon, gradient_clip, l2_reg, use_log_objective, use_numerator_epsilon,
-                         init_lr_range, random_seed)
+                         init_lr_range, random_seed, use_second_derivatives)
 
     # ---- state ---------------------------------------------------------------------------------------------------
     def initial_state(self, params: Sequence[torch.Tensor], theta: torch.Tensor,
@@ -330,14 +360,9 @@ class MetaTrainer(MetaTrainerBase):
         objs, total = [], 0.0
         w = [1.0] * num_steps if obj_weights is None else list(obj_weights)
         for t in range(num_steps):
-            # objective at x_t, and its gradient as a CONSTANT of the meta-gradient (stop_gradient,
-            # trainable_optimizer.py:332-338): one evaluation serves both
-            with torch.enable_grad():
-                xg = x if x.requires_grad else x.detach().requires_grad_(True)
-                obj = objective(self._split(xg))
-                (g,) = torch.autograd.grad(obj, xg, retain_graph=x.requires_grad)
-            if not x.requires_grad:
-                obj = obj.detach()
+            # objective at x_t and its gradient: a constant of the meta-gradient (stop_gradient,
+            # trainable_optimizer.py:330-338) unless use_second_derivatives
+            obj, g = self._objective_and_gradient(objective, x)
             objs.append(obj)
             total = total + w[t] * obj
             # per-tensor gate bias and the problem-wide mean log-lr of the PREVIOUS state (HR:561-575, 432-442)
@@ -345,8 +370,7 @@ class MetaTrainer(MetaTrainerBase):
                      + glob @ P["PerTensor/Layer0_RNN/Global/Affine/Matrix"] + P["PerTensor/Layer0_RNN/Global/Affine/Bias"])
             bias0 = torch.cat([bias0, torch.zeros(eng.nt, B0_STRIDE - 3 * H0, device=self.device)], 1)
             mean_llr = planes[P_LLR].mean().reshape(1)
-            planes, upd, sums, any_nz = _CoordStep.apply(eng, theta, planes, bias0, mean_llr, g.detach().contiguous(),
-                                                         zero_flag)
+            planes, upd, sums, any_nz = _CoordStep.apply(eng, theta, planes, bias0, mean_llr, g, zero_flag)
             means = sums[:, :H0 + NF] / cnt[:, None]                        # mean_coords([h' | feat])  (HR:582-587)
             inv = torch.rsqrt(sums[:, H0 + NF] / cnt + 1e-16)               # 1 / RMS(delta)            (HR:621-626)
             # (per-tensor scalar broadcast as expand + cat: its backward is a handful of segment sums, where the backward

@@ -93,6 +93,7 @@ def main():
     def bwd():
         ctx = type("Ctx", (), {})()
         ctx.saved_tensors = (th, planes, g)
+        ctx.needs_input_grad = (True, True, False)
         ct._Step.backward(ctx, d_new, d_upd)
     f_ms, b_ms = time_ms(fwd, args.reps), time_ms(bwd, args.reps)
     res["train_step_convnet"] = dict(n=n, fwd_ms=f_ms, bwd_ms=b_ms, bwd_achieved_TBps=n * BWD_BYTES / b_ms / 1e9)
