@@ -358,6 +358,69 @@ int64_t l2o_crnn_state_floats(void);
 int l2o_crnn_step(const l2o_crnn_step_args* a, void* stream);
 int l2o_crnn_bwd(const l2o_crnn_bwd_args* a, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * L2O-Scale's meta-trained hand-designed baselines (SC/optimizer/): TrainableAdam (TA = trainable_adam.py),
+ * LearningRateSchedule (LRS = learning_rate_schedule.py) and GlobalLearningRate (GLR = global_learning_rate.py).  No
+ * handle; one launch per step and one per backward step over the concatenated coordinates of all optimizee tensors.
+ *
+ *   l2o_tadam_theta_count   log_learning_rate, beta1_logit, beta2_logit, log_epsilon (creation order)   TA:63-82
+ *   l2o_tadam_state_floats  _initialize_state: m | t | v, zeros, in sorted key order                  TA:89-93
+ *   l2o_tadam_step          _compute_update, with the reference's v' = v / (1 - pow(g^2, b2))           TA:95-175
+ *   l2o_tadam_bwd           tf.gradients of that step; where v == 0 the v-chain terms are exactly 0
+ *   l2o_lrsgd_step          LRS _compute_update: x - rates[min(itr, n_steps-1)] g, itr + 1             LRS:48-60
+ *                           GlobalLearningRate: a one-entry table and a null itr                        GLR:38-39
+ *   l2o_lrsgd_bwd           tf.gradients of that step
+ * In both backward entries g is a constant when d_g is null (use_second_derivatives off,
+ * SC/optimizer/trainable_optimizer.py:330-338); with d_g set it receives g's adjoint and nothing else changes.
+ * theta, the schedule and the counter stay in device memory (a CUDA-graph replay needs no host synchronisation).
+ * Float pointers must be 4-byte aligned, double pointers 8-byte aligned (L2O_E_INVALID otherwise). */
+typedef struct {
+  int64_t n;               /* coordinates (> 0) */
+  const float* theta;      /* [4] */
+  const float* g;          /* [n] */
+  const float* state_in;   /* [3][n] m | t | v */
+  float* state_out;        /* [3][n]; may alias state_in */
+  float* x;                /* optional [n]: x -= update */
+  float* update;           /* optional [n]: lr m^ / (sqrt(v^ + 1e-10) + eps) */
+} l2o_tadam_step_args;
+typedef struct {
+  int64_t n;
+  const float* theta;        /* [4] */
+  const float* g;            /* [n] the gradients the step was fed */
+  const float* state_old;    /* [3][n] planes before the step */
+  const float* d_state_new;  /* [3][n] adjoints of the planes after the step (the t plane's is ignored) */
+  const float* d_update;     /* [n] */
+  float* d_state_old;        /* [3][n] out (the t plane gets 0); must not overlap any input */
+  double* d_theta;           /* [4] += */
+  float* d_g;                /* optional [n] out: adjoint of g; 4-byte aligned, overlapping no other buffer (else L2O_E_INVALID) */
+} l2o_tadam_bwd_args;
+typedef struct {
+  int64_t n;               /* coordinates (> 0) */
+  const float* rates;      /* [n_steps] the schedule (GlobalLearningRate: its one rate) */
+  int32_t n_steps;         /* > 0 */
+  int32_t* itr;            /* optional int32 [2]: step index, then an arrival count that is 0 between launches.  The
+                              step uses rates[min(itr[0], n_steps-1)] and advances itr[0] by one in place.  Null: index 0 */
+  const float* g;          /* [n] */
+  float* x;                /* optional [n]: x -= update */
+  float* update;           /* optional [n]: rate * g */
+} l2o_lrsgd_step_args;
+typedef struct {
+  int64_t n;
+  const float* rates;      /* [n_steps] */
+  int32_t n_steps;
+  const int32_t* itr;      /* optional [2]: the counter as the step saw it (before it advanced); null: index 0 */
+  const float* g;          /* [n] */
+  const float* d_update;   /* [n] */
+  double* d_rates;         /* [n_steps] += (only the entry the step used) */
+  float* d_g;              /* optional [n] out: rate * d_update; 4-byte aligned, overlapping no other buffer */
+} l2o_lrsgd_bwd_args;
+int64_t l2o_tadam_theta_count(void);
+int64_t l2o_tadam_state_floats(void);
+int l2o_tadam_step(const l2o_tadam_step_args* a, void* stream);
+int l2o_tadam_bwd(const l2o_tadam_bwd_args* a, void* stream);
+int l2o_lrsgd_step(const l2o_lrsgd_step_args* a, void* stream);
+int l2o_lrsgd_bwd(const l2o_lrsgd_bwd_args* a, void* stream);
+
 /* Number of this library's kernels launched so far in this process (bench.py's gpu_launches). */
 int64_t l2o_launch_count(void);
 const char* l2o_status_string(int status);

@@ -33,6 +33,8 @@ EXPORTS = [
     "l2o_hrnn_set_global_sizes", "l2o_hrnn_reduce_layout", "l2o_hrnn_prepare_local", "l2o_hrnn_prepare_finish",
     "l2o_hrnn_step_local", "l2o_hrnn_step_finish", "l2o_hrnn_coord_bwd", "l2o_hrnn_workspace_layout",
     "l2o_crnn_theta_count", "l2o_crnn_state_floats", "l2o_crnn_step", "l2o_crnn_bwd",
+    "l2o_tadam_theta_count", "l2o_tadam_state_floats", "l2o_tadam_step", "l2o_tadam_bwd", "l2o_lrsgd_step",
+    "l2o_lrsgd_bwd",
 ]
 
 
@@ -104,6 +106,26 @@ class CrnnStepArgs(C.Structure):
 class CrnnBwdArgs(C.Structure):
     _fields_ = [("n", C.c_int64), ("theta", _fp), ("g", _fp), ("state_old", _fp), ("d_state_new", _fp),
                 ("d_update", _fp), ("d_state_old", _fp), ("d_theta", _fp), ("d_g", _fp)]
+
+
+class TadamStepArgs(C.Structure):
+    _fields_ = [("n", C.c_int64), ("theta", _fp), ("g", _fp), ("state_in", _fp), ("state_out", _fp), ("x", _fp),
+                ("update", _fp)]
+
+
+class TadamBwdArgs(C.Structure):
+    _fields_ = [("n", C.c_int64), ("theta", _fp), ("g", _fp), ("state_old", _fp), ("d_state_new", _fp),
+                ("d_update", _fp), ("d_state_old", _fp), ("d_theta", _fp), ("d_g", _fp)]
+
+
+class LrsgdStepArgs(C.Structure):
+    _fields_ = [("n", C.c_int64), ("rates", _fp), ("n_steps", C.c_int32), ("itr", _fp), ("g", _fp), ("x", _fp),
+                ("update", _fp)]
+
+
+class LrsgdBwdArgs(C.Structure):
+    _fields_ = [("n", C.c_int64), ("rates", _fp), ("n_steps", C.c_int32), ("itr", _fp), ("g", _fp),
+                ("d_update", _fp), ("d_rates", _fp), ("d_g", _fp)]
 
 
 class L2OError(RuntimeError):
@@ -241,6 +263,13 @@ def lib():
     L.l2o_crnn_step.restype = C.c_int
     L.l2o_crnn_bwd.argtypes = [C.POINTER(CrnnBwdArgs), C.c_void_p]
     L.l2o_crnn_bwd.restype = C.c_int
+    for name in ("l2o_tadam_theta_count", "l2o_tadam_state_floats"):
+        getattr(L, name).argtypes = []
+        getattr(L, name).restype = C.c_int64
+    for name, args in (("l2o_tadam_step", TadamStepArgs), ("l2o_tadam_bwd", TadamBwdArgs),
+                       ("l2o_lrsgd_step", LrsgdStepArgs), ("l2o_lrsgd_bwd", LrsgdBwdArgs)):
+        getattr(L, name).argtypes = [C.POINTER(args), C.c_void_p]
+        getattr(L, name).restype = C.c_int
     for name in ("l2o_status_string", "l2o_last_cuda_error", "l2o_version"):
         getattr(L, name).restype = C.c_char_p
     L.l2o_status_string.argtypes = [C.c_int]
