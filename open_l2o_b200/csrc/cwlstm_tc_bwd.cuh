@@ -6,18 +6,17 @@
 //   layer 1:  Z1 = [u, 1 | h1p] . B1 -> LSTM backward with dh1 = carry + dh1n(t) -> dZ1;  dX1 = dZ1 . W1^T -> dh1p carry
 //   dW:       dW^T rows += X^T . dZ over the tile's coordinates, on the bf16 tensor cores from shared-memory staging
 //             (x = hi + lo, hi = bf16_rn(x), lo = bf16_rn(x - hi); products hi.hi + hi.lo + lo.hi, fp32 accumulate).
-//             Both layers share ONE 64 x 80 accumulator: the operand rows of layer 2 (h1n 0..19 | h2p 20..39 | 1 40) and
-//             of layer 1 (h1p 41..60 | features 61.. | 1) are disjoint, and each layer's staged X^T keeps the other
-//             layer's rows at zero, so the two K = 64 contractions add into disjoint accumulator rows.  The accumulators
-//             are drained into the fp64 dtheta after every tile (bounded fp32 accumulation length).
+//             Both layers share ONE 64 x 80 accumulator: the operand rows of layer 2 ([h1n | h2p] in rows 0..39, 1 in
+//             row 63) and of layer 1 ([h1p | feature chunk] in rows 40..62) are disjoint (dw_row), and each layer's
+//             staged X^T keeps the other layer's rows at zero, so the two K = 64 contractions add into disjoint
+//             accumulator rows.  The accumulators are drained into the fp64 dtheta after every tile (bounded fp32
+//             accumulation length).  Both operands are staged as packed bf16 pairs with stmatrix (stage_x, stage_dz).
 // DM nets take the checkpoint rows from a shared-memory ring that TMA bulk copies fill one layer phase ahead (CkRing).
 // fc(20) nets (RNNProp) run the two layers as two passes over time (MODE 1: layer 2, exporting dX2[h1n] to the
 // caller's hand-over buffer; MODE 2: layer 1 with the fc layer's own gradient), DM nets both layers in one pass (MODE 0).
 // Semantics: SURVEY.md Appendix B (derived from DM/meta.py:319-376, second_derivatives=False); imitation mode
 // DM/meta_dm_train.py:472-475.
 #pragma once
-#include <cuda_bf16.h>
-
 #include "cwlstm_tc.cuh"
 
 namespace l2o {
@@ -32,30 +31,22 @@ constexpr uint32_t kXaLBO = 8 * 128;            // X^T: 64 rows (8 core-matrix g
 constexpr uint32_t kXbLBO = 10 * 128;           // dZ^T: 80 rows
 constexpr uint32_t kXaBytes = 8 * kXaLBO;       // per hi / lo
 constexpr uint32_t kXbBytes = 8 * kXbLBO;
-// dW accumulator rows
-constexpr int kRowH1N = 0, kRowH2P = 20, kRowOne2 = 40;                 // layer 2 (and MODE 2: h1p | e | 1)
-constexpr int kRowH1P = 41, kRowFeat = 61;                              // layer 1 of DM nets (MODE 0)
+// dW accumulator rows: 8-row blocks 0..4 hold layer 2 (MODE 2: layer 1's [h1p | e]), 5..7 layer 1 of DM nets (MODE 0),
+// row 63 the constant 1 of the blocks 0..4 operand (dw_row)
+constexpr int kBlkL1 = 5, kRowOne2 = 63;
 
-__device__ __forceinline__ uint32_t xa_off(int m, int k) {
-  return (uint32_t)((m >> 3) * 128 + (k >> 3) * (int)kXaLBO + (m & 7) * 16 + (k & 7) * 2);
+// x = hi + lo for a pair of values (v0 in the low half): hi = bf16_rn(x), lo = bf16_rn(x - hi)
+__device__ __forceinline__ void split_bf16x2(float v0, float v1, uint32_t& hi, uint32_t& lo) {
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(v1), "f"(v0));
+  const float r0 = v0 - __uint_as_float(hi << 16), r1 = v1 - __uint_as_float(hi & 0xFFFF0000u);
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(r1), "f"(r0));
 }
-__device__ __forceinline__ uint32_t xb_off(int nn, int k) {
-  return (uint32_t)((nn >> 3) * 128 + (k >> 3) * (int)kXbLBO + (nn & 7) * 16 + (k & 7) * 2);
-}
-__device__ __forceinline__ void split_bf16(float x, uint16_t& hi, uint16_t& lo) {
-  const __nv_bfloat16 h = __float2bfloat16_rn(x);
-  hi = __bfloat16_as_ushort(h);
-  lo = __bfloat16_as_ushort(__float2bfloat16_rn(x - __bfloat162float(h)));
-}
-__device__ __forceinline__ void sts16(uint32_t sa, uint16_t v) {
-  asm volatile("st.shared.u16 [%0], %1;" ::"r"(sa), "h"(v) : "memory");
-}
-// value v at (row, coordinate) of a staged hi / lo pair (lo at +lo_off bytes)
-__device__ __forceinline__ void stage_bf16(uint32_t base, uint32_t off, uint32_t lo_off, float v) {
-  uint16_t h, l;
-  split_bf16(v, h, l);
-  sts16(base + off, h);
-  sts16(base + lo_off + off, l);
+// four 8x8 b16 blocks, transposed: register i of lane l holds (row l / 4, columns 2 (l % 4) + {0, 1}) of block i, which
+// land in the 16-byte rows 2 (l % 4) + {0, 1} at 2-byte slot l / 4; lane l gives the address of row l % 8 of block l / 8
+__device__ __forceinline__ void stsm_x4_trans(uint32_t sa, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(sa), "r"(r0), "r"(r1),
+               "r"(r2), "r"(r3)
+               : "memory");
 }
 // D[64 x 80] += A[64 x 16] (shared, bf16, K-major) . B[16 x 80] (shared, bf16, K-major)
 __device__ __forceinline__ void mma_ss_bf16_n80(float* d, uint64_t a, uint64_t b) {
@@ -92,21 +83,25 @@ __device__ __forceinline__ void unit_bwd(float& zi, float& zj, float& zf, float&
   dc = dcv * f;
 }
 
-// theta index of dW accumulator row m, gate column n (-1: padding row)
+// theta index of dW accumulator row m at reference gate column 0 (-1: padding row).  Row 8b + 2p + e holds slot 2b + e
+// of quad thread p (stage_x): in blocks 0..4, slots 0..4 are units 5p + s of the first 20-vector, 5..9 of the second;
+// in the layer-1 blocks 5..7 (MODE 0), slots 10..14 are units of h1p and slot 15 is column p of the feature chunk
+// (feature p for p < F, the constant 1 at p = F).
 template <class C, int MODE>
-__device__ __forceinline__ int dw_index(int m, int n) {
-  const int col = gate_ref_col(n);
-  if (MODE == 2) {   // fc nets, layer 1: h1p | e | 1  (lstm_1/w_gates rows: the 20 fc outputs first, then h1)
-    if (m < kRowH2P) return C::O_W1 + (C::F + m) * C::G1 + col;
-    if (m < kRowOne2) return C::O_W1 + (m - kRowH2P) * C::G1 + col;
-    return m == kRowOne2 ? C::O_B1 + col : -1;
+__device__ __forceinline__ int dw_row(int m) {
+  const int p = (m & 7) >> 1, slot = 2 * (m >> 3) + (m & 1);
+  if (m == kRowOne2) return MODE == 2 ? C::O_B1 : C::O_B2;
+  if (slot < 2 * kBlkL1) {
+    const int u = 5 * p + slot % kU;
+    // MODE 2: fc nets, layer 1: h1p | e  (lstm_1/w_gates rows: the 20 fc outputs first, then h1)
+    if (MODE == 2) return C::O_W1 + (slot < kU ? C::F + u : u) * C::G1;
+    return C::O_W2 + (slot < kU ? u : kH + u) * C::G2;   // h1n | h2p rows of lstm_2/w_gates
   }
-  if (m < kRowOne2) return C::O_W2 + m * C::G2 + col;   // h1n rows 0..19, h2p rows 20..39 of lstm_2/w_gates
-  if (m == kRowOne2) return C::O_B2 + col;
   if (MODE == 0) {
-    if (m < kRowFeat) return C::O_W1 + (C::F + m - kRowH1P) * C::G1 + col;
-    if (m < kRowFeat + C::F) return C::O_W1 + (m - kRowFeat) * C::G1 + col;
-    if (m == kRowFeat + C::F) return C::O_B1 + col;
+    const int s = slot - 2 * kBlkL1;
+    if (s < kU) return C::O_W1 + (C::F + 5 * p + s) * C::G1;
+    if (p < C::F) return C::O_W1 + p * C::G1;
+    if (p == C::F) return C::O_B1;
   }
   return -1;
 }
@@ -142,7 +137,7 @@ template <class C, int MODE>
 __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args a, NetRt rt, const float* __restrict__ img) {
   using G = Geo<C>;
   static_assert(MODE == 0 ? !C::FC : C::FC, "DM nets: one pass; fc nets: two passes");
-  static_assert(MODE != 0 || kRowFeat + C::F < 64, "dW rows of both layers fit one 64-row accumulator");
+  static_assert(MODE != 0 || C::F < 3, "the feature chunk leaves quad thread 3's slot of row 63 to layer 2's 1");
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   SmemB<C, MODE>& S = *reinterpret_cast<SmemB<C, MODE>*>(smem_raw);
   const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
@@ -158,9 +153,13 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
                                          (size_t)kBwdWG * stage_bytes<C, MODE>() + (size_t)wg * sizeof(CkRing));
   const bool elected = (threadIdx.x & 127) == 0;
 
-  // zero the staging (rows of the other layer stay zero for the whole kernel)
-  for (uint32_t o = threadIdx.x * 4; o < kBwdWG * stage_bytes<C, MODE>(); o += blockDim.x * 4)
-    asm volatile("st.shared.u32 [%0], 0;" ::"r"(stage - (uint32_t)wg * stage_bytes<C, MODE>() + o) : "memory");
+  // zero the staging (rows of the other layer stay zero for the whole kernel) but for the constant 1 of the blocks 0..4
+  // operand: row kRowOne2 of its hi part, which no per-step store touches (bf16 1.0 = 0x3F80)
+  for (uint32_t o = threadIdx.x * 4; o < kBwdWG * stage_bytes<C, MODE>(); o += blockDim.x * 4) {
+    const uint32_t ow = o % stage_bytes<C, MODE>();
+    const uint32_t v = (ow < kXaBytes && (ow % kXaLBO) >> 4 == (uint32_t)kRowOne2) ? 0x3F803F80u : 0u;
+    asm volatile("st.shared.u32 [%0], %1;" ::"r"(stage - (uint32_t)wg * stage_bytes<C, MODE>() + o), "r"(v) : "memory");
+  }
   if (threadIdx.x < kH) S.wo[threadIdx.x] = a.theta[C::O_WO + threadIdx.x];
   if constexpr (C::FC) {
     if (threadIdx.x >= 32 && threadIdx.x < 92) S.win[threadIdx.x - 32] = a.theta[C::O_WIN + threadIdx.x - 32];
@@ -236,18 +235,33 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
   uint32_t ph = 0;
 
   Frag<G::KB> A;
-  // X^T rows of this thread's units of the 20-vector at operand column `col`: row base + 5q + s, coordinate kx + 8 rh
-  auto stage_vec = [&](uint32_t xh, int base, int rh, int col) {
+  // The staged operands are K-major core matrices (8 rows of 16 B = 8 coordinates), so an 8x8 block of (coordinate,
+  // row) pairs in a thread's accumulator-style registers is one transposed stmatrix block.  Each x4 stores the blocks
+  // (hi, rh 0) (hi, rh 1) (lo, rh 0) (lo, rh 1) of one 8-row group: lane l addresses row l % 8 of block l / 8.
+  const int blk = lane >> 3;
+  const uint32_t la = stage + (uint32_t)((2 * warp + (blk & 1)) * (int)kXaLBO + (blk >> 1) * (int)kXaBytes + (lane & 7) * 16);
+  const uint32_t lb = stage + kXb + (uint32_t)((2 * warp + (blk & 1)) * (int)kXbLBO + (blk >> 1) * (int)kXbBytes + (lane & 7) * 16);
+  // X^T blocks [b0, b0 + nb) of the operand at `buf`: slot i = 2 (b - b0) + e of this thread goes to row 8b + 2q + e;
+  // slots 0..4 are its units of the 20-vector at operand column c0, slots 5.. those of the one at c1 (dw_row)
+  auto stage_x = [&](uint32_t buf, int b0, int nb, int c0, int c1) {
+    auto val = [&](int i, int rh) { return A.get_at(i < kU ? c0 + 4 * i : c1 + 4 * (i - kU), rh); };
 #pragma unroll
-    for (int s = 0; s < kU; ++s) stage_bf16(xh, xa_off(base + 5 * q + s, kx + 8 * rh), kXaBytes, A.get_at(col + 4 * s, rh));
+    for (int b = 0; b < nb; ++b) {
+      uint32_t h0, l0, h1, l1;
+      split_bf16x2(val(2 * b, 0), val(2 * b + 1, 0), h0, l0);
+      split_bf16x2(val(2 * b, 1), val(2 * b + 1, 1), h1, l1);
+      stsm_x4_trans(la + buf + (uint32_t)(b0 + b) * 128, h0, h1, l0, l1);
+    }
   };
+  // dZ^T: accumulator registers z[4j + 2rh + {0, 1}] are gate columns 8j + 2q + {0, 1} of coordinate kx + 8 rh
   auto stage_dz = [&](const float* z) {
 #pragma unroll
-    for (int j = 0; j < kN / 8; ++j)
-#pragma unroll
-      for (int rh = 0; rh < 2; ++rh)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) stage_bf16(stage + kXb, xb_off(8 * j + 2 * q + e, kx + 8 * rh), kXbBytes, z[4 * j + 2 * rh + e]);
+    for (int j = 0; j < kN / 8; ++j) {
+      uint32_t h0, l0, h1, l1;
+      split_bf16x2(z[4 * j], z[4 * j + 1], h0, l0);
+      split_bf16x2(z[4 * j + 2], z[4 * j + 3], h1, l1);
+      stsm_x4_trans(lb + (uint32_t)j * 128, h0, h1, l0, l1);
+    }
   };
   // dX_l = dZ_l . W_l^T (3xTF32; the dZ accumulators as A fragments, cwlstm_tc.cuh dx_gate_col) then the dW batch
   auto dx_dw = [&](auto ncols, float* z, float* x, uint64_t th, uint64_t tl, uint64_t xah, uint64_t xal) {
@@ -282,16 +296,17 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
   auto flush_dw = [&]() {
     wg_wait<0>();
 #pragma unroll
-    for (int j = 0; j < kN / 8; ++j)
+    for (int rh = 0; rh < 2; ++rh) {
+      const int r = dw_row<C, MODE>(kx + 8 * rh);
 #pragma unroll
-      for (int rh = 0; rh < 2; ++rh)
+      for (int j = 0; j < kN / 8; ++j)
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           float& v = dw[4 * j + 2 * rh + e];
-          const int idx = dw_index<C, MODE>(warp * 16 + g + 8 * rh, 8 * j + 2 * q + e);
-          if (idx >= 0 && v != 0.f) atomicAdd(&a.dtheta[idx], (double)v);
+          if (r >= 0 && v != 0.f) atomicAdd(&a.dtheta[r + gate_ref_col(8 * j + 2 * q + e)], (double)v);
           v = 0.f;
         }
+    }
   };
 
   for (int64_t tile = (int64_t)blockIdx.x * kBwdWG + wg; tile < ntiles; tile += tstride) {
@@ -372,12 +387,7 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
           arm(&R.barh, R.h, tile, t, 0);
           if (tl_next < ntiles) arm(&R.bar2, R.c2, tl_next, t_next, 3);
         }
-#pragma unroll
-        for (int rh = 0; rh < 2; ++rh) {
-          stage_vec(stage + kXa2, kRowH1N, rh, G::ColH1);
-          stage_vec(stage + kXa2, kRowH2P, rh, G::ColH2);
-          if (q == 0) stage_bf16(stage + kXa2, xa_off(kRowOne2, kx + 8 * rh), kXaBytes, 1.0f);
-        }
+        stage_x(kXa2, 0, kBlkL1, G::ColH1, G::ColH2);   // h1n | h2p
         stage_dz(z);
         fence_proxy_async();
         wg_bar(wg);
@@ -483,17 +493,8 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
           }
           ph ^= 1u;
         }
-#pragma unroll
-        for (int rh = 0; rh < 2; ++rh) {
-          if constexpr (MODE == 2) {
-            stage_vec(stage + kXa2, kRowH1N, rh, G::ColH1);   // h1p
-            stage_vec(stage + kXa2, kRowH2P, rh, 0);          // e
-            if (q == 0) stage_bf16(stage + kXa2, xa_off(kRowOne2, kx + 8 * rh), kXaBytes, 1.0f);
-          } else {
-            stage_vec(stage + kXa1, kRowH1P, rh, G::ColH1);
-            if (q <= C::F) stage_bf16(stage + kXa1, xa_off(kRowFeat + q, kx + 8 * rh), kXaBytes, A.get_at(0, rh));
-          }
-        }
+        if constexpr (MODE == 2) stage_x(kXa2, 0, kBlkL1, G::ColH1, 0);   // h1p | e
+        else stage_x(kXa1, kBlkL1, 3, G::ColH1, 0);                     // h1p | column q of the feature chunk
         stage_dz(z);
         fence_proxy_async();
         wg_bar(wg);
