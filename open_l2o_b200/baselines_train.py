@@ -1,6 +1,6 @@
 """Meta-training of L2O-Scale's baselines (``TrainableAdam``, ``LearningRateSchedule``, ``GlobalLearningRate``): BPTT
 through the unrolled optimizer, with the meta-objective, the clipped RMSProp meta-step and the training loops of
-``hrnn_train`` (``MetaTrainerBase``, ``train_optimizer``).
+``scale_base`` (``MetaTrainerBase``, ``train_optimizer``).
 
 The loop these classes run in the reference is the Evaluation copy's ``TrainableOptimizer.train``
 (SCE/optimizer/trainable_optimizer.py:283-310; the Training copy calls ``_compute_updates`` with six arguments, and the
@@ -14,42 +14,18 @@ one ``torch.autograd.Function`` around two CUDA entry points (``l2o_tadam_step``
 from __future__ import annotations
 
 import ctypes as C
-from typing import Callable, Optional, Sequence
+from typing import Optional, Sequence
 
 import torch
 
 from . import _lib
-from ._lib import L2OError, LrsgdBwdArgs, TadamBwdArgs
-from .hrnn_train import MetaTrainerBase, train_optimizer  # noqa: F401  (train_optimizer serves every trainer)
-from .trainable_baselines import _p, _stream, _tadam_theta, lrsgd_step_launch, tadam_step_launch
+from ._lib import LrsgdBwdArgs, TadamBwdArgs
+from .engine import _ptr, _stream
+from .scale_base import MetaTrainerBase, planes_step, train_optimizer  # noqa: F401  (public names)
+from .trainable_baselines import _tadam_theta, lrsgd_step_launch, tadam_step_launch
 
-
-class _TadamStep(torch.autograd.Function):
-    """(theta [4], planes [3, N], g) -> (planes', update).  The adjoint of g is computed only when autograd asks."""
-
-    @staticmethod
-    def forward(ctx, theta, planes, g):
-        theta, planes = theta.detach().contiguous(), planes.detach().contiguous()
-        new, upd = torch.empty_like(planes), torch.empty_like(g)
-        tadam_step_launch(theta, g, planes, new, update=upd)
-        ctx.save_for_backward(theta, planes, g)
-        return new, upd
-
-    @staticmethod
-    def backward(ctx, d_new, d_upd):
-        theta, planes, g = ctx.saved_tensors
-        d_new = torch.zeros_like(planes) if d_new is None else d_new.contiguous()
-        d_upd = torch.zeros_like(g) if d_upd is None else d_upd.contiguous()
-        d_old = torch.empty_like(planes)
-        d_theta = torch.zeros(theta.numel(), dtype=torch.float64, device=theta.device)
-        d_g = torch.empty_like(g) if ctx.needs_input_grad[2] else None
-        a = TadamBwdArgs()
-        a.n = int(g.numel())
-        a.theta, a.g, a.state_old = _p(theta), _p(g), _p(planes)
-        a.d_state_new, a.d_update, a.d_state_old = _p(d_new), _p(d_upd), _p(d_old)
-        a.d_theta, a.d_g = d_theta.data_ptr(), _p(d_g)
-        _lib.check(_lib.lib().l2o_tadam_bwd(C.byref(a), _stream()), "l2o_tadam_bwd")
-        return d_theta.to(torch.float32), d_old, d_g
+# (theta [4], planes [3, N], g) -> (planes', update)
+_TadamStep = planes_step(tadam_step_launch, TadamBwdArgs, "l2o_tadam_bwd")
 
 
 class _LrsStep(torch.autograd.Function):
@@ -72,8 +48,8 @@ class _LrsStep(torch.autograd.Function):
         d_g = torch.empty_like(g) if ctx.needs_input_grad[1] else None
         a = LrsgdBwdArgs()
         a.n, a.n_steps = int(g.numel()), int(rates.numel())
-        a.rates, a.itr, a.g, a.d_update = _p(rates), _p(ctx.itr), _p(g), _p(d_upd.contiguous())
-        a.d_rates, a.d_g = d_rates.data_ptr(), _p(d_g)
+        a.rates, a.itr, a.g, a.d_update = _ptr(rates), _ptr(ctx.itr, torch.int32), _ptr(g), _ptr(d_upd.contiguous())
+        a.d_rates, a.d_g = d_rates.data_ptr(), _ptr(d_g)
         _lib.check(_lib.lib().l2o_lrsgd_bwd(C.byref(a), _stream()), "l2o_lrsgd_bwd")
         return d_rates.to(torch.float32), d_g, None, None
 
@@ -89,47 +65,14 @@ class OptimizerState(object):
 class _BaselineTrainer(MetaTrainerBase):
     """``TrainableOptimizer.train`` + the RMSProp block of ``metaopt.train_optimizer`` for one of the baselines.
 
-    objective(list of tensors shaped like ``shapes``) -> scalar.  ``theta`` is the optimizer's flat variable vector; it
-    is updated in place by ``train_step``.  ``use_second_derivatives``: differentiate through the optimizee's gradients
-    (the reference's default is ``True``; the default here stays ``False``).  See ``hrnn_train.MetaTrainer``."""
-    what = ""
+    ``theta`` is the optimizer's flat variable vector.  ``use_second_derivatives`` (default ``False``, the first-order
+    meta-gradient): see ``MetaTrainerBase``."""
 
     def __init__(self, shapes: Sequence[Sequence[int]], theta: torch.Tensor, device="cuda:0", learning_rate=1e-6,
                  rms_decay=0.9, rms_epsilon=1e-20, gradient_clip=1e4, l2_reg=0.0, use_log_objective=True,
                  use_numerator_epsilon=False, random_seed=None, use_second_derivatives=False):
-        if not torch.cuda.is_available():
-            raise L2OError("%s meta-training needs a CUDA device (no CPU path)" % self.what)
-        self._setup(shapes, device)
-        self._setup_meta(theta.detach().clone().float(), learning_rate, rms_decay, rms_epsilon, gradient_clip, l2_reg,
+        super().__init__(shapes, theta, device, learning_rate, rms_decay, rms_epsilon, gradient_clip, l2_reg,
                          use_log_objective, use_numerator_epsilon, None, random_seed, use_second_derivatives)
-
-    def _x0(self, params):
-        return torch.cat([p.detach().reshape(-1).float() for p in params]).to(self.device)
-
-    def _step(self, theta, state: OptimizerState, g):
-        """(update, the state after the step without x)."""
-        raise NotImplementedError
-
-    def unroll(self, objective: Callable, state: OptimizerState, num_steps: int, theta: Optional[torch.Tensor] = None,
-               obj_weights: Optional[Sequence[float]] = None, initial_obj: Optional[torch.Tensor] = None):
-        """``loop_body`` x num_steps.  Returns (meta objective with its graph, the list of objective values, the final
-        OptimizerState with its graph)."""
-        if num_steps < 1:
-            raise ValueError("an unroll needs at least one step")
-        theta = self.theta if theta is None else theta
-        x = state.x
-        objs, total = [], 0.0
-        w = [1.0] * num_steps if obj_weights is None else list(obj_weights)
-        for t in range(num_steps):
-            obj, g = self._objective_and_gradient(objective, x)   # g keeps its graph only for second derivatives
-            objs.append(obj)
-            total = total + w[t] * obj
-            upd, state = self._step(theta, state, g)
-            x = x - upd
-        initial = objs[0].detach() if initial_obj is None else initial_obj
-        meta = self.scale_objective(total, torch.stack([o.reshape(()) for o in objs]), initial)
-        state.x = x
-        return meta, objs, state
 
 
 class TrainableAdamTrainer(_BaselineTrainer):
@@ -143,9 +86,11 @@ class TrainableAdamTrainer(_BaselineTrainer):
         x = self._x0(params)
         return OptimizerState(x, planes=torch.zeros(3, x.numel(), device=self.device))   # TA:89-93
 
-    def _step(self, theta, state, g):
-        planes, upd = _TadamStep.apply(theta, state.planes, g)
-        return upd, OptimizerState(None, planes=planes)
+    def _stepper(self, theta):
+        def step(state, g):
+            planes, upd = _TadamStep.apply(theta, state.planes, g)
+            return upd, OptimizerState(None, planes=planes)
+        return step
 
 
 class LearningRateScheduleTrainer(_BaselineTrainer):
@@ -160,10 +105,11 @@ class LearningRateScheduleTrainer(_BaselineTrainer):
         itr = torch.zeros(2, dtype=torch.int32, device=self.device) if self.counter else None   # LRS:42-46
         return OptimizerState(self._x0(params), itr=itr)
 
-    def _step(self, theta, state, g):
-        itr_new = None if state.itr is None else state.itr.clone()
-        upd = _LrsStep.apply(theta, g, state.itr, itr_new)
-        return upd, OptimizerState(None, itr=itr_new)
+    def _stepper(self, theta):
+        def step(state, g):
+            itr_new = None if state.itr is None else state.itr.clone()
+            return _LrsStep.apply(theta, g, state.itr, itr_new), OptimizerState(None, itr=itr_new)
+        return step
 
 
 class GlobalLearningRateTrainer(LearningRateScheduleTrainer):

@@ -11,13 +11,14 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-import os
-from typing import Dict, Iterable, List, Optional, Sequence, Tuple
+from typing import List, Optional, Tuple
 
 import torch
 
 from . import _lib
-from ._lib import CrnnStepArgs, L2OError
+from ._lib import CrnnStepArgs
+from .engine import _ptr, _stream
+from .scale_base import ScaleOptimizer
 
 CELL_SIZES = (10, 20, 20)
 RNN_FLOATS = 2 * sum(CELL_SIZES)                      # the "rnn" slot: c1 h1 c2 h2 c3 h3 (CR:306-315)
@@ -92,25 +93,18 @@ def _cell_name(cell_cls) -> str:
     return name
 
 
-def _p(t: Optional[torch.Tensor]):
-    if t is None:
-        return None
-    if not t.is_cuda or t.dtype != torch.float32 or not t.is_contiguous():
-        raise L2OError("expected a contiguous fp32 CUDA tensor (this engine has no CPU path)")
-    return t.data_ptr()
-
-
 def step_launch(theta, g, state_in, state_out, x=None, update=None):
     """One ``l2o_crnn_step`` launch on the current stream (all tensors fp32, contiguous, on the GPU)."""
     a = CrnnStepArgs()
     a.n = int(g.numel())
-    a.theta, a.g, a.state_in, a.state_out = _p(theta), _p(g), _p(state_in), _p(state_out)
-    a.x, a.update = _p(x), _p(update)
-    _lib.check(_lib.lib().l2o_crnn_step(C.byref(a), torch.cuda.current_stream().cuda_stream), "l2o_crnn_step")
+    a.theta, a.g, a.state_in, a.state_out = _ptr(theta), _ptr(g), _ptr(state_in), _ptr(state_out)
+    a.x, a.update = _ptr(x), _ptr(update)
+    _lib.check(_lib.lib().l2o_crnn_step(C.byref(a), _stream()), "l2o_crnn_step")
 
 
-class CoordinatewiseRNN(object):
+class CoordinatewiseRNN(ScaleOptimizer):
     """Per-coordinate 3-layer LSTM optimizer (cells 10, 20, 20) with learnable RMS decay and dynamic output scale."""
+    trainer = "crnn_train.MetaTrainer"
 
     def __init__(self, cell_sizes, cell_cls, init_lr_range=(1., 1.), dynamic_output_scale=True, learnable_decay=True,
                  zero_init_lr_weights=False, random_seed=None, device="cuda", **kwargs):
@@ -121,6 +115,7 @@ class CoordinatewiseRNN(object):
         if init_lr_range[0] > init_lr_range[1]:
             raise ValueError("Initial LR range min is greater than max.")
         self.cell_cls = _cell_name(cell_cls)
+        self.theta_spec = theta_spec(self.cell_cls)
         built = dict(cell_sizes=CELL_SIZES, learnable_decay=True, dynamic_output_scale=True)
         asked = dict(cell_sizes=tuple(cell_sizes), learnable_decay=learnable_decay,
                      dynamic_output_scale=dynamic_output_scale)
@@ -132,59 +127,15 @@ class CoordinatewiseRNN(object):
         self.init_lr_range = tuple(init_lr_range)
         self.zero_init_lr_weights = bool(zero_init_lr_weights)
         self.random_seed = random_seed
-        self.device = torch.device(device)
         self.n_theta = int(_lib.lib().l2o_crnn_theta_count())
         seed = int(torch.seed() % (2 ** 31)) if random_seed is None else random_seed
         theta = _init_theta(seed, self.zero_init_lr_weights)
         assert theta.numel() == self.n_theta
-        self.theta = theta.to(self.device)
-        self.state = None
-        self._vars: List[torch.Tensor] = []
+        super().__init__(theta, device)
 
-    # ---- variables (the TF variable collection of OPTIMIZER_SCOPE) ---------------------------------------------------
-    def get_variables(self) -> Dict[str, torch.Tensor]:
-        out, off = {}, 0
-        for name, shape in theta_spec(self.cell_cls):
-            n = int(math.prod(shape))
-            out[name] = self.theta[off:off + n].view(shape)
-            off += n
-        return out
-
-    def load_variables(self, values: Dict[str, torch.Tensor]):
-        for name, view in self.get_variables().items():
-            if name in values:
-                view.copy_(torch.as_tensor(values[name], dtype=torch.float32).reshape(view.shape))
-
-    # ---- meta-training ---------------------------------------------------------------------------------------------
-    def meta_trainer(self, var_list: Sequence[torch.Tensor], **kwargs):
-        """A ``crnn_train.MetaTrainer`` for optimizees shaped like ``var_list`` that starts from this optimizer's
-        weights.  ``adopt(trainer)`` copies the trained weights back."""
-        from .crnn_train import MetaTrainer
-        kwargs.setdefault("init_lr_range", self.init_lr_range)
-        return MetaTrainer([tuple(v.shape) for v in var_list], theta=self.theta, device=str(self.device), **kwargs)
-
-    def adopt(self, trainer):
-        self.theta.copy_(trainer.theta.detach())
-
-    # ---- slots ---------------------------------------------------------------------------------------------------------
-    def _create_slots(self, var_list: Sequence[torch.Tensor]):
-        """One slot set per optimizee tensor (trainable_optimizer.py:94-105), laid out as 103 planes over the
-        concatenation of all tensors; the optimizee tensors become views of one flat arena."""
-        sizes = [int(v.numel()) for v in var_list]
-        if any(s <= 0 for s in sizes):
-            raise ValueError("empty optimizee variable")
-        self.sizes, self.N = sizes, sum(sizes)
-        dev = self.device
-        self.x = torch.empty(self.N, device=dev)
-        self.g = torch.empty(self.N, device=dev)
-        off = 0
-        for v, n in zip(var_list, sizes):   # re-seat the variables on the arena (zero-copy flatten/unflatten afterwards)
-            self.x[off:off + n].copy_(v.detach().reshape(-1))
-            v.data = self.x[off:off + n].view(v.shape)
-            off += n
-        self._vars = list(var_list)
-        self.state = torch.empty(STATE_PLANES, self.N, device=dev)
-        self.reset_state()
+    def _new_state(self):
+        """103 planes over the arena (trainable_optimizer.py:94-105): rnn c1 h1 c2 h2 c3 h3 | rms | decay | lr."""
+        return torch.empty(STATE_PLANES, self.N, device=self.device)
 
     def reset_state(self, seed: Optional[int] = None, learning_rate: Optional[torch.Tensor] = None):
         """_initialize_state (CR:151-173): rnn = init_vector, rms = decay = 1, learning rates exp(U(log min, log max))
@@ -216,47 +167,6 @@ class CoordinatewiseRNN(object):
         planes = {"rms": P_RMS, "decay": P_DECAY, "learning_rate": P_LR}
         return self.state[planes[key], off:off + n].view(n, 1)
 
-    # ---- the step --------------------------------------------------------------------------------------------------------
-    def apply_gradients(self, grads_and_vars: Iterable[Tuple[torch.Tensor, torch.Tensor]], global_step=None, name=None):
-        """tf.train.Optimizer.apply_gradients: one CoordinatewiseRNN step over all (grad, var) pairs.  Variables are
-        updated in place; returns the list of updated variables."""
-        grads_and_vars = tuple(grads_and_vars)
-        for g, v in grads_and_vars:
-            if g is not None and not torch.is_tensor(g):
-                raise TypeError("Gradient must be a Tensor or None: %s" % (g,))
-            if not torch.is_tensor(v):
-                raise TypeError("Variable must be a Tensor: %s" % (v,))
-        pairs = [(g, v) for g, v in grads_and_vars if g is not None]
-        if not pairs:
-            raise ValueError("No gradients provided for any variable: %s" % (grads_and_vars,))
-        if self.state is None:
-            self._create_slots([v for _, v in pairs])
-        elif len(pairs) != len(self._vars) or any(v is not w for (_, v), w in zip(pairs, self._vars)):
-            raise ValueError("apply_gradients must be called with the variables the slots were created for")
-        off = 0
-        for (g, _), n in zip(pairs, self.sizes):
-            self.g[off:off + n].copy_(g.reshape(-1))
-            off += n
-        self.step_flat()
-        return [v for _, v in pairs]
-
     def step_flat(self):
         """One step with the gradients already in ``self.g`` (flat arena order); the state is updated in place."""
         step_launch(self.theta, self.g, self.state, self.state, x=self.x)
-
-    def minimize(self, objective, var_list: Sequence[torch.Tensor], num_steps: int, cuda_graph: Optional[bool] = None):
-        """Convenience loop of the evaluation drivers (SC/metatest.py): num_steps x (objective, gradients, step).
-        Returns the list of objective values.  After two eager iterations one iteration is captured into a CUDA graph
-        and replayed (``cuda_graph=False`` or ``L2O_CUDA_GRAPH=0`` keeps everything eager)."""
-        var_list = list(var_list)
-
-        def body():
-            loss = objective(*var_list)
-            grads = torch.autograd.grad(loss, var_list)
-            self.apply_gradients(zip(grads, var_list))
-            return loss.detach()
-
-        if cuda_graph is None:
-            cuda_graph = os.environ.get("L2O_CUDA_GRAPH", "1") != "0"
-        from . import engine as _engine
-        return _engine.replay_loop(self, body, objective, var_list, num_steps, cuda_graph, 1, "CoordinatewiseRNN")

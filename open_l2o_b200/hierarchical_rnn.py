@@ -14,12 +14,14 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-from typing import Dict, Iterable, List, Optional, Sequence, Tuple
+from typing import Iterable, List, Optional, Sequence, Tuple
 
 import torch
 
 from . import _lib
-from ._lib import HrnnArgs, L2OError
+from ._lib import HrnnArgs
+from .engine import _ptr, _stream
+from .scale_base import ScaleOptimizer
 
 NUM_GRADIENT_SCALES = 4
 N_FEATURES = 12
@@ -109,16 +111,38 @@ def _init_theta(seed: Optional[int]) -> torch.Tensor:
     return torch.cat(out)
 
 
-def _p(t: Optional[torch.Tensor]):
-    if t is None:
-        return None
-    if not t.is_cuda or t.dtype != torch.float32 or not t.is_contiguous():
-        raise L2OError("expected a contiguous fp32 CUDA tensor (this engine has no CPU path)")
-    return t.data_ptr()
+class HrnnHandle(object):
+    """An ``l2o_hrnn`` handle (``_h``) for optimizee tensors of ``sizes`` coordinates and the workspace it needs,
+    aligned to the 256 B the library requires (``ptr``; ``ws`` is the aligned workspace as bytes).  The handle is
+    destroyed with this object."""
+
+    def __init__(self, sizes: Sequence[int], device):
+        L = _lib.lib()
+        self._h = C.c_void_p()
+        _lib.check(L.l2o_hrnn_create(C.byref(self._h), (C.c_int64 * len(sizes))(*sizes), len(sizes)), "l2o_hrnn_create")
+        nbytes = int(L.l2o_hrnn_workspace_bytes(self._h))
+        self._buf = torch.zeros((nbytes + 255) // 4 + 64, dtype=torch.float32, device=device)
+        self.ptr = (self._buf.data_ptr() + 255) // 256 * 256
+        self.ws = self._buf.view(torch.uint8)[self.ptr - self._buf.data_ptr():]
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None):
+                _lib.lib().l2o_hrnn_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
 
 
-class HierarchicalRNN(object):
-    """3-level hierarchical RNN optimizer (per-parameter GRU 10, per-tensor GRU 20, global GRU 20)."""
+class HierarchicalRNN(ScaleOptimizer):
+    """3-level hierarchical RNN optimizer (per-parameter GRU 10, per-tensor GRU 20, global GRU 20).
+
+    ``distributed=True``: every rank holds a contiguous slice of every optimizee tensor's coordinates (the optimizee
+    itself stays replicated); one small all-reduce of the per-tensor sums per step + an all-gather of the updated
+    parameters (SURVEY.md 8(e)).  Needs an initialised torch.distributed process group."""
+    theta_spec = THETA_SPEC
+    trainer = "hrnn_train.MetaTrainer"
+    kernels_per_step = 3
 
     def __init__(self, level_sizes=(10, 20, 20), init_lr_range=(1e-6, 1e-2), learnable_decay=True,
                  dynamic_output_scale=True, use_attention=False, use_log_objective=True, num_gradient_scales=4,
@@ -160,126 +184,58 @@ class HierarchicalRNN(object):
         self.init_lr_range = tuple(init_lr_range)
         self.random_seed = random_seed
         self.device = torch.device(device)
-        L = _lib.lib()
-        self.n_theta = int(L.l2o_hrnn_theta_count())
+        self.n_theta = int(_lib.lib().l2o_hrnn_theta_count())
         self.distributed = bool(distributed)
-        if random_seed is None:   # unseeded like the reference; the ranks of a sharded optimizer must draw the same theta
-            theta_seed = int(torch.seed() % (2 ** 31))
-            if self.distributed:
-                import torch.distributed as tdist
-                box = torch.tensor([theta_seed], dtype=torch.int64, device=self.device)
-                tdist.broadcast(box, src=0)
-                theta_seed = int(box.item())
-        else:
-            theta_seed = random_seed
-        theta = _init_theta(theta_seed)
+        # unseeded like the reference; the ranks of a sharded optimizer must draw the same theta
+        theta = _init_theta(self._fresh_seed() if random_seed is None else random_seed)
         assert theta.numel() == self.n_theta
-        self.theta = theta.to(self.device)
-        self._h = None
-        self._vars: List[torch.Tensor] = []
-        # distributed=True: every rank holds a contiguous slice of every optimizee tensor's coordinates (the optimizee
-        # itself stays replicated); one small all-reduce of the per-tensor sums per step + an all-gather of the
-        # updated parameters (SURVEY.md 8(e)).  Needs an initialised torch.distributed process group.
-        self.distributed = bool(distributed)
+        super().__init__(theta, device)
 
-    # ---- variables (the TF variable collection of OPTIMIZER_SCOPE) ---------------------------------------------------
-    def get_variables(self) -> Dict[str, torch.Tensor]:
-        out, off = {}, 0
-        for name, shape in THETA_SPEC:
-            n = int(math.prod(shape))
-            out[name] = self.theta[off:off + n].view(shape)
-            off += n
-        return out
-
-    def load_variables(self, values: Dict[str, torch.Tensor]):
-        for name, view in self.get_variables().items():
-            if name in values:
-                view.copy_(torch.as_tensor(values[name], dtype=torch.float32).reshape(view.shape))
-        if self._h is not None:
-            self._prepare()
-
-    # ---- meta-training ---------------------------------------------------------------------------------------------
-    def meta_trainer(self, var_list: Sequence[torch.Tensor], **kwargs):
-        """A ``hrnn_train.MetaTrainer`` for optimizees shaped like ``var_list`` that starts from this optimizer's
-        weights (``TrainableOptimizer.train``, SC/optimizer/trainable_optimizer.py:200-470).  ``adopt(trainer)`` copies the
-        trained weights back."""
-        from .hrnn_train import MetaTrainer
-        kwargs.setdefault("init_lr_range", self.init_lr_range)
-        return MetaTrainer([tuple(v.shape) for v in var_list], theta=self.theta, device=str(self.device), **kwargs)
-
-    def adopt(self, trainer):
-        self.theta.copy_(trainer.theta.detach())
-        if self._h is not None:
-            self._prepare()
-
-    # ---- slots ---------------------------------------------------------------------------------------------------------
-    def _create_slots(self, var_list: Sequence[torch.Tensor]):
-        """One slot set per optimizee tensor (trainable_optimizer.py:94-105), laid out as 21 planes over the
-        concatenation of all tensors; the optimizee tensors become views of one flat arena."""
-        gsizes = [int(v.numel()) for v in var_list]
-        if any(s <= 0 for s in gsizes):
-            raise ValueError("empty optimizee variable")
-        self.global_sizes = gsizes
+    def _fresh_seed(self) -> int:
+        """A fresh seed for an unseeded draw, the same on every rank of a sharded optimizer."""
+        s = int(torch.seed() % (2 ** 31))
         if self.distributed:
             import torch.distributed as tdist
-            from .dist import shard_range
-            self._rank, self._world = tdist.get_rank(), tdist.get_world_size()
-            self._ranges = [shard_range(n, self._rank, self._world) for n in gsizes]
-        else:
-            self._rank, self._world = 0, 1
-            self._ranges = [(0, n) for n in gsizes]
-        sizes = [hi - lo for lo, hi in self._ranges]
-        if sum(sizes) <= 0:
-            raise ValueError("this rank holds no coordinate (more ranks than coordinates)")
-        arr = (C.c_int64 * len(sizes))(*sizes)
-        h = C.c_void_p()
-        _lib.check(_lib.lib().l2o_hrnn_create(C.byref(h), arr, len(sizes)), "l2o_hrnn_create")
-        self._h, self.sizes, self.N = h, sizes, sum(sizes)
-        if self.distributed:
-            garr = (C.c_int64 * len(gsizes))(*gsizes)
-            _lib.check(_lib.lib().l2o_hrnn_set_global_sizes(h, garr), "l2o_hrnn_set_global_sizes")
-        dev = self.device
-        self.x = torch.empty(self.N, device=dev)
-        self.g = torch.empty(self.N, device=dev)
-        off = 0
-        for v, (lo, hi) in zip(var_list, self._ranges):
-            n = hi - lo
-            self.x[off:off + n].copy_(v.detach().reshape(-1)[lo:hi])
-            if not self.distributed:   # re-seat the variables on the arena (zero-copy flatten/unflatten afterwards)
-                v.data = self.x[off:off + n].view(v.shape)
-            off += n
-        self._vars = list(var_list)
-        self.state = torch.zeros(int(_lib.lib().l2o_hrnn_state_floats()), self.N, device=dev)
-        self.layer = torch.zeros(len(sizes), self.level_sizes[1], device=dev)
-        self.global_state = torch.zeros(self.level_sizes[2], device=dev)
-        nbytes = int(_lib.lib().l2o_hrnn_workspace_bytes(h))
-        self.workspace = torch.zeros((nbytes + 255) // 4 + 64, dtype=torch.float32, device=dev)
-        self.update = torch.empty(self.N, device=dev)
-        if self.distributed:   # views of the workspace head that the ranks all-reduce between the two step phases
-            nd, fo, nf = C.c_int64(), C.c_int64(), C.c_int64()
-            _lib.check(_lib.lib().l2o_hrnn_reduce_layout(h, C.byref(nd), C.byref(fo), C.byref(nf)), "l2o_hrnn_reduce_layout")
-            base = (self.workspace.data_ptr() + 255) // 256 * 256 - self.workspace.data_ptr()
-            raw = self.workspace.view(torch.uint8)
-            self._red_sums = raw[base:base + 8 * nd.value].view(torch.float64)
-            self._red_flags = raw[base + fo.value:base + fo.value + 4 * nf.value].view(torch.int32)
-        self.reset_state()
+            box = torch.tensor([s], dtype=torch.int64, device=self.device)
+            tdist.broadcast(box, src=0)
+            s = int(box.item())
+        return s
 
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None):
-                _lib.lib().l2o_hrnn_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
+    # ---- slots ---------------------------------------------------------------------------------------------------------
+    def _shard_ranges(self, sizes):
+        if not self.distributed:
+            return super()._shard_ranges(sizes)
+        import torch.distributed as tdist
+        from .dist import shard_range
+        rank, world = tdist.get_rank(), tdist.get_world_size()
+        return [shard_range(n, rank, world) for n in sizes]
+
+    def _new_state(self):
+        """21 planes over the arena (trainable_optimizer.py:94-105), the per-tensor and global GRU states, the handle
+        and its workspace."""
+        dev = self.device
+        self._hrnn = HrnnHandle(self.sizes, dev)
+        if self.distributed:
+            garr = (C.c_int64 * len(self.global_sizes))(*self.global_sizes)
+            _lib.check(_lib.lib().l2o_hrnn_set_global_sizes(self._hrnn._h, garr), "l2o_hrnn_set_global_sizes")
+            # views of the workspace head that the ranks all-reduce between the two step phases
+            nd, fo, nf = C.c_int64(), C.c_int64(), C.c_int64()
+            _lib.check(_lib.lib().l2o_hrnn_reduce_layout(self._hrnn._h, C.byref(nd), C.byref(fo), C.byref(nf)),
+                       "l2o_hrnn_reduce_layout")
+            self._red_sums = self._hrnn.ws[:8 * nd.value].view(torch.float64)
+            self._red_flags = self._hrnn.ws[fo.value:fo.value + 4 * nf.value].view(torch.int32)
+        self.layer = torch.zeros(len(self.sizes), self.level_sizes[1], device=dev)
+        self.global_state = torch.zeros(self.level_sizes[2], device=dev)
+        self.update = torch.empty(self.N, device=dev)
+        return torch.zeros(int(_lib.lib().l2o_hrnn_state_floats()), self.N, device=dev)
 
     def _args(self, with_xg=True) -> HrnnArgs:
         a = HrnnArgs()
-        a.theta = _p(self.theta)
-        a.x, a.g = (_p(self.x), _p(self.g)) if with_xg else (None, None)
-        a.state, a.layer, a.global_ = _p(self.state), _p(self.layer), _p(self.global_state)
-        ws = self.workspace.data_ptr()
-        a.workspace = (ws + 255) // 256 * 256
-        a.update = _p(self.update)
+        a.theta = _ptr(self.theta)
+        a.x, a.g = (_ptr(self.x), _ptr(self.g)) if with_xg else (None, None)
+        a.state, a.layer, a.global_ = _ptr(self.state), _ptr(self.layer), _ptr(self.global_state)
+        a.workspace = self._hrnn.ptr
+        a.update = _ptr(self.update)
         return a
 
     def _allreduce_sums(self):
@@ -288,31 +244,24 @@ class HierarchicalRNN(object):
         tdist.all_reduce(self._red_flags, op=tdist.ReduceOp.MAX)
 
     def _prepare(self):
-        L, st, a = _lib.lib(), torch.cuda.current_stream().cuda_stream, self._args(False)
+        L, h, a = _lib.lib(), self._hrnn._h, self._args(False)
         if not self.distributed:
-            _lib.check(L.l2o_hrnn_prepare(self._h, C.byref(a), st), "l2o_hrnn_prepare")
+            _lib.check(L.l2o_hrnn_prepare(h, C.byref(a), _stream()), "l2o_hrnn_prepare")
             return
-        _lib.check(L.l2o_hrnn_prepare_local(self._h, C.byref(a), st), "l2o_hrnn_prepare_local")
+        _lib.check(L.l2o_hrnn_prepare_local(h, C.byref(a), _stream()), "l2o_hrnn_prepare_local")
         self._allreduce_sums()
-        _lib.check(L.l2o_hrnn_prepare_finish(self._h, C.byref(a), st), "l2o_hrnn_prepare_finish")
+        _lib.check(L.l2o_hrnn_prepare_finish(h, C.byref(a), _stream()), "l2o_hrnn_prepare_finish")
 
     def reset_state(self, seed: Optional[int] = None, log_learning_rate: Optional[torch.Tensor] = None):
         """_initialize_state / _initialize_global_state (HR:303-350).  The log learning rates are drawn as in the
         reference (per-coordinate U(log(min)/2, log(max)/2) plus one per-tensor offset from the same range, clipped
         to [-33, max_log_lr]) unless given."""
-        st = torch.cuda.current_stream().cuda_stream
-        _lib.check(_lib.lib().l2o_hrnn_init_state(self._h, C.byref(self._args(False)), st), "l2o_hrnn_init_state")
+        _lib.check(_lib.lib().l2o_hrnn_init_state(self._hrnn._h, C.byref(self._args(False)), _stream()),
+                   "l2o_hrnn_init_state")
         if log_learning_rate is None:
             gen = torch.Generator()
             s = self.random_seed if seed is None else seed
-            if s is None:   # unseeded like the reference (a fresh draw per call); ranks must agree on it when sharded
-                s = int(torch.seed() % (2 ** 31))
-                if self.distributed:
-                    import torch.distributed as tdist
-                    box = torch.tensor([s], dtype=torch.int64, device=self.device)
-                    tdist.broadcast(box, src=0)
-                    s = int(box.item())
-            gen.manual_seed(int(s))
+            gen.manual_seed(int(self._fresh_seed() if s is None else s))   # unseeded: a fresh draw per call
             lo, hi = math.log(self.init_lr_range[0]) / 2.0, math.log(self.init_lr_range[1]) / 2.0
             parts = []
             for n, (slo, shi) in zip(self.global_sizes, self._ranges):   # drawn for the whole tensor, sliced per rank
@@ -341,64 +290,21 @@ class HierarchicalRNN(object):
     def apply_gradients(self, grads_and_vars: Iterable[Tuple[torch.Tensor, torch.Tensor]], global_step=None, name=None):
         """tf.train.Optimizer.apply_gradients (HR:730-805): one HierarchicalRNN step over all (grad, var) pairs.
         Variables are updated in place; returns the list of updated variables ("real_params")."""
-        grads_and_vars = tuple(grads_and_vars)
-        for g, v in grads_and_vars:
-            if g is not None and not torch.is_tensor(g):
-                raise TypeError("Gradient must be a Tensor or None: %s" % (g,))
-            if not torch.is_tensor(v):
-                raise TypeError("Variable must be a Tensor: %s" % (v,))
-        pairs = [(g, v) for g, v in grads_and_vars if g is not None]
-        if not pairs:
-            raise ValueError("No gradients provided for any variable: %s" % (grads_and_vars,))
-        if self._h is None:
-            self._create_slots([v for _, v in pairs])
-        elif len(pairs) != len(self._vars) or any(v is not w for (_, v), w in zip(pairs, self._vars)):
-            raise ValueError("apply_gradients must be called with the variables the slots were created for")
-        off = 0
-        for (g, v), (lo, hi) in zip(pairs, self._ranges):
-            n = hi - lo
-            self.g[off:off + n].copy_(g.reshape(-1)[lo:hi])
-            off += n
-        self.step_flat()
+        updated = super().apply_gradients(grads_and_vars, global_step, name)
         if self.distributed:   # republish the updated parameters to the replicated optimizee
             from .dist import allgather_shards
             off = 0
-            for (_, v), (lo, hi), n in zip(pairs, self._ranges, self.global_sizes):
+            for v, (lo, hi), n in zip(updated, self._ranges, self.global_sizes):
                 v.data.copy_(allgather_shards(self.x[off:off + hi - lo], n).view(v.shape))
                 off += hi - lo
-        return [v for _, v in pairs]
+        return updated
 
     def step_flat(self):
         """One step with the gradients already in ``self.g`` (flat arena order)."""
-        L, st, a = _lib.lib(), torch.cuda.current_stream().cuda_stream, self._args(True)
+        L, h, a = _lib.lib(), self._hrnn._h, self._args(True)
         if not self.distributed:
-            _lib.check(L.l2o_hrnn_step(self._h, C.byref(a), st), "l2o_hrnn_step")
+            _lib.check(L.l2o_hrnn_step(h, C.byref(a), _stream()), "l2o_hrnn_step")
             return
-        _lib.check(L.l2o_hrnn_step_local(self._h, C.byref(a), st), "l2o_hrnn_step_local")
+        _lib.check(L.l2o_hrnn_step_local(h, C.byref(a), _stream()), "l2o_hrnn_step_local")
         self._allreduce_sums()
-        _lib.check(L.l2o_hrnn_step_finish(self._h, C.byref(a), st), "l2o_hrnn_step_finish")
-
-    def minimize(self, objective, var_list: Sequence[torch.Tensor], num_steps: int, cuda_graph: Optional[bool] = None):
-        """Convenience loop of the evaluation drivers (SC/metatest.py): num_steps x (objective, gradients, step).
-        Returns the list of objective values (one device->host read at the end).
-
-        One iteration is ~50 tiny launches (the optimizee's forward/backward, the gradient copies, the three step
-        kernels) and nothing in it needs the host, so after two eager iterations (slot creation, library warm-up) one
-        iteration is captured into a CUDA graph and replayed (``cuda_graph=False`` or ``L2O_CUDA_GRAPH=0`` keeps
-        everything eager; a failed capture falls back to the same eager kernels with a warning)."""
-        import os
-        var_list = list(var_list)
-
-        def body():
-            loss = objective(*var_list)
-            grads = torch.autograd.grad(loss, var_list)
-            self.apply_gradients(zip(grads, var_list))
-            return loss.detach()
-
-        if cuda_graph is None:
-            cuda_graph = os.environ.get("L2O_CUDA_GRAPH", "1") != "0"
-        if self.distributed:
-            cuda_graph = False   # the per-step collectives stay outside graph capture
-        from . import engine as _engine
-        # 3: the three l2o_hrnn_step kernels inside the graph
-        return _engine.replay_loop(self, body, objective, var_list, num_steps, cuda_graph, 3, "HierarchicalRNN")
+        _lib.check(L.l2o_hrnn_step_finish(h, C.byref(a), _stream()), "l2o_hrnn_step_finish")

@@ -18,39 +18,27 @@ on.  See DESIGN §3.10.
 from __future__ import annotations
 
 import ctypes as C
-import math
-import os
-from typing import Dict, Iterable, List, Optional, Sequence, Tuple
+from typing import Dict
 
 import numpy as np
 import torch
 
 from . import _lib
-from ._lib import L2OError, LrsgdStepArgs, TadamStepArgs
+from ._lib import LrsgdStepArgs, TadamStepArgs
+from .engine import _ptr, _stream
+from .scale_base import ScaleOptimizer
 
 TADAM_THETA_SPEC = [("LOL/log_learning_rate", ()), ("LOL/beta1_logit", ()), ("LOL/beta2_logit", ()),
                     ("LOL/log_epsilon", ())]                           # TA:63-82, creation order
 TADAM_KEYS = ("m", "t", "v")                                           # TA:86, in sorted order (the planes' order)
 
 
-def _p(t: Optional[torch.Tensor]):
-    if t is None:
-        return None
-    if not t.is_cuda or t.dtype not in (torch.float32, torch.int32) or not t.is_contiguous():
-        raise L2OError("expected a contiguous fp32 (or int32 counter) CUDA tensor (this engine has no CPU path)")
-    return t.data_ptr()
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
 def tadam_step_launch(theta, g, state_in, state_out, x=None, update=None):
     """One ``l2o_tadam_step`` launch on the current stream."""
     a = TadamStepArgs()
     a.n = int(g.numel())
-    a.theta, a.g, a.state_in, a.state_out = _p(theta), _p(g), _p(state_in), _p(state_out)
-    a.x, a.update = _p(x), _p(update)
+    a.theta, a.g, a.state_in, a.state_out = _ptr(theta), _ptr(g), _ptr(state_in), _ptr(state_out)
+    a.x, a.update = _ptr(x), _ptr(update)
     _lib.check(_lib.lib().l2o_tadam_step(C.byref(a), _stream()), "l2o_tadam_step")
 
 
@@ -59,117 +47,8 @@ def lrsgd_step_launch(rates, g, itr=None, x=None, update=None):
     counter (int32 [2]) is advanced in place on the device."""
     a = LrsgdStepArgs()
     a.n, a.n_steps = int(g.numel()), int(rates.numel())
-    a.rates, a.g, a.itr, a.x, a.update = _p(rates), _p(g), _p(itr), _p(x), _p(update)
+    a.rates, a.g, a.itr, a.x, a.update = _ptr(rates), _ptr(g), _ptr(itr, torch.int32), _ptr(x), _ptr(update)
     _lib.check(_lib.lib().l2o_lrsgd_step(C.byref(a), _stream()), "l2o_lrsgd_step")
-
-
-class _Baseline(object):
-    """What the three optimizers share: the flat theta with TF names, the flat optimizee arena, ``apply_gradients``,
-    graph-replayed ``minimize``, ``meta_trainer`` / ``adopt``."""
-    theta_spec: List[Tuple[str, Tuple[int, ...]]]
-    name = ""
-
-    def __init__(self, theta: torch.Tensor, device):
-        self.device = torch.device(device)
-        self.theta = theta.to(self.device)
-        self.state = None
-        self._vars: List[torch.Tensor] = []
-
-    # ---- variables (the TF variable collection of OPTIMIZER_SCOPE) ---------------------------------------------------
-    def get_variables(self) -> Dict[str, torch.Tensor]:
-        out, off = {}, 0
-        for name, shape in self.theta_spec:
-            n = int(math.prod(shape))
-            out[name] = self.theta[off:off + n].view(shape)
-            off += n
-        return out
-
-    def load_variables(self, values: Dict[str, torch.Tensor]):
-        for name, view in self.get_variables().items():
-            if name in values:
-                view.copy_(torch.as_tensor(values[name], dtype=torch.float32).reshape(view.shape))
-
-    # ---- meta-training ---------------------------------------------------------------------------------------------
-    def meta_trainer(self, var_list: Sequence[torch.Tensor], **kwargs):
-        """A ``baselines_train`` trainer for optimizees shaped like ``var_list`` that starts from this optimizer's
-        variables.  ``adopt(trainer)`` copies the trained variables back."""
-        from . import baselines_train
-        cls = getattr(baselines_train, self.name + "Trainer")
-        return cls([tuple(v.shape) for v in var_list], theta=self.theta, device=str(self.device), **kwargs)
-
-    def adopt(self, trainer):
-        self.theta.copy_(trainer.theta.detach())
-
-    # ---- slots ---------------------------------------------------------------------------------------------------------
-    def _create_slots(self, var_list: Sequence[torch.Tensor]):
-        """One slot set per optimizee tensor (trainable_optimizer.py:94-105) over the concatenation of all tensors; the
-        optimizee tensors become views of one flat arena."""
-        sizes = [int(v.numel()) for v in var_list]
-        if any(s <= 0 for s in sizes):
-            raise ValueError("empty optimizee variable")
-        self.sizes, self.N = sizes, sum(sizes)
-        self.x = torch.empty(self.N, device=self.device)
-        self.g = torch.empty(self.N, device=self.device)
-        off = 0
-        for v, n in zip(var_list, sizes):
-            self.x[off:off + n].copy_(v.detach().reshape(-1))
-            v.data = self.x[off:off + n].view(v.shape)
-            off += n
-        self._vars = list(var_list)
-        self.state = self._new_state()
-
-    def _new_state(self):
-        raise NotImplementedError
-
-    def reset_state(self):
-        """_initialize_state: the optimizer's state as before its first step.  In place (every state is zeros at the
-        start): a CUDA graph that ``minimize`` captured keeps the state buffer's address."""
-        if self.state is not None:
-            self.state.zero_()
-
-    # ---- the step --------------------------------------------------------------------------------------------------------
-    def apply_gradients(self, grads_and_vars: Iterable[Tuple[torch.Tensor, torch.Tensor]], global_step=None, name=None):
-        """tf.train.Optimizer.apply_gradients: one step over all (grad, var) pairs.  Variables are updated in place;
-        returns the list of updated variables."""
-        grads_and_vars = tuple(grads_and_vars)
-        for g, v in grads_and_vars:
-            if g is not None and not torch.is_tensor(g):
-                raise TypeError("Gradient must be a Tensor or None: %s" % (g,))
-            if not torch.is_tensor(v):
-                raise TypeError("Variable must be a Tensor: %s" % (v,))
-        pairs = [(g, v) for g, v in grads_and_vars if g is not None]
-        if not pairs:
-            raise ValueError("No gradients provided for any variable: %s" % (grads_and_vars,))
-        if self.state is None:
-            self._create_slots([v for _, v in pairs])
-        elif len(pairs) != len(self._vars) or any(v is not w for (_, v), w in zip(pairs, self._vars)):
-            raise ValueError("apply_gradients must be called with the variables the slots were created for")
-        off = 0
-        for (g, _), n in zip(pairs, self.sizes):
-            self.g[off:off + n].copy_(g.reshape(-1))
-            off += n
-        self.step_flat()
-        return [v for _, v in pairs]
-
-    def step_flat(self):
-        raise NotImplementedError
-
-    def minimize(self, objective, var_list: Sequence[torch.Tensor], num_steps: int, cuda_graph: Optional[bool] = None):
-        """num_steps x (objective, gradients, step); returns the objective values.  After two eager iterations one
-        iteration is captured into a CUDA graph and replayed (``cuda_graph=False`` or ``L2O_CUDA_GRAPH=0`` keeps
-        everything eager)."""
-        var_list = list(var_list)
-
-        def body():
-            loss = objective(*var_list)
-            grads = torch.autograd.grad(loss, var_list)
-            self.apply_gradients(zip(grads, var_list))
-            return loss.detach()
-
-        if cuda_graph is None:
-            cuda_graph = os.environ.get("L2O_CUDA_GRAPH", "1") != "0"
-        from . import engine as _engine
-        return _engine.replay_loop(self, body, objective, var_list, num_steps, cuda_graph, 1, self.name)
 
 
 def _tadam_theta(learning_rate, beta1, beta2, epsilon) -> torch.Tensor:
@@ -180,10 +59,10 @@ def _tadam_theta(learning_rate, beta1, beta2, epsilon) -> torch.Tensor:
     return torch.from_numpy(v).float()
 
 
-class TrainableAdam(_Baseline):
+class TrainableAdam(ScaleOptimizer):
     """Adam with learnable scalar parameters (TA:29-175), including the reference's second-moment expression."""
     theta_spec = TADAM_THETA_SPEC
-    name = "TrainableAdam"
+    trainer = "baselines_train.TrainableAdamTrainer"
 
     def __init__(self, learning_rate=1e-3, beta1=0.9, beta2=0.999, epsilon=1e-8, device="cuda", **kwargs):
         # TA:54-59; **kwargs go to TrainableOptimizer, whose training flags the meta-trainer takes
@@ -198,7 +77,7 @@ class TrainableAdam(_Baseline):
         super().__init__(_tadam_theta(learning_rate, beta1, beta2, epsilon), device)
 
     def _new_state(self):
-        return torch.zeros(self.n_planes, self.N, device=self.device)   # m | t | v, zeros (TA:89-93)
+        return torch.empty(self.n_planes, self.N, device=self.device)   # m | t | v, zeroed by reset_state (TA:89-93)
 
     def get_slot(self, var_index: int, key: str) -> torch.Tensor:
         """Slot ``key`` (``m``, ``v`` or ``t``, TA:86) of optimizee tensor ``var_index``, shape [n, 1]."""
@@ -209,9 +88,9 @@ class TrainableAdam(_Baseline):
         tadam_step_launch(self.theta, self.g, self.state, self.state, x=self.x)
 
 
-class LearningRateSchedule(_Baseline):
+class LearningRateSchedule(ScaleOptimizer):
     """Learns one learning rate per step of a fixed-length schedule (LRS:27-60); steps past the end keep the last."""
-    name = "LearningRateSchedule"
+    trainer = "baselines_train.LearningRateScheduleTrainer"
 
     def __init__(self, initial_rate=0.0, n_steps=1000, device="cuda", **kwargs):
         self.n_steps = int(n_steps)
@@ -220,7 +99,7 @@ class LearningRateSchedule(_Baseline):
 
     def _new_state(self):
         # one counter for all optimizee tensors (they step together): index, then the kernel's arrival count
-        return torch.zeros(2, dtype=torch.int32, device=self.device)
+        return torch.empty(2, dtype=torch.int32, device=self.device)
 
     def get_slot(self, var_index: int, key: str) -> torch.Tensor:
         """The ``itr`` slot (LRS:42-46): the number of steps taken, an int32 scalar shared by all tensors."""
@@ -234,16 +113,16 @@ class LearningRateSchedule(_Baseline):
         lrsgd_step_launch(self.theta, self.g, itr=self.state, x=self.x)
 
 
-class GlobalLearningRate(_Baseline):
+class GlobalLearningRate(ScaleOptimizer):
     """Learns one global learning rate (GLR:27-39): x' = x - lr g, no state."""
     theta_spec = [("LOL/global_learning_rate", ())]
-    name = "GlobalLearningRate"
+    trainer = "baselines_train.GlobalLearningRateTrainer"
 
     def __init__(self, initial_rate=1e-3, device="cuda", **kwargs):
         super().__init__(torch.tensor([float(initial_rate)], dtype=torch.float32), device)
 
     def _new_state(self):
-        return torch.zeros(0, device=self.device)   # stateless (GLR:36): a placeholder that marks the slots created
+        return torch.empty(0, device=self.device)   # stateless (GLR:36): a placeholder that marks the slots created
 
     def get_slot(self, var_index: int, key: str) -> torch.Tensor:
         raise KeyError("GlobalLearningRate has no slots (GLR:36): %r" % (key,))

@@ -83,7 +83,8 @@ def main():
         raise SystemExit("baselines_profile.py measures the GPU kernels and needs a CUDA device")
     from open_l2o_b200 import baselines_train as bt
     from open_l2o_b200.scale_problems import ConvNet
-    from open_l2o_b200.trainable_baselines import lrsgd_step_launch, tadam_step_launch, _p, _stream
+    from open_l2o_b200.engine import _ptr as _p, _stream
+    from open_l2o_b200.trainable_baselines import lrsgd_step_launch, tadam_step_launch
     from open_l2o_b200 import _lib
     from tests.helpers import HRNN_CONVNET
     import ctypes as C
@@ -120,7 +121,7 @@ def main():
         rates, itr = torch.full((1000,), 1e-3, device=dev), torch.zeros(2, dtype=torch.int32, device=dev)
         ls_ms = graph_ms(lambda: lrsgd_step_launch(rates, g, itr=itr, x=xa), args.reps)
         d_rates = torch.zeros(1000, dtype=torch.float64, device=dev)
-        la = _lib.LrsgdBwdArgs(n=n, rates=_p(rates), n_steps=1000, itr=_p(itr), g=_p(g), d_update=_p(d_upd),
+        la = _lib.LrsgdBwdArgs(n=n, rates=_p(rates), n_steps=1000, itr=_p(itr, torch.int32), g=_p(g), d_update=_p(d_upd),
                                d_rates=d_rates.data_ptr(), d_g=_p(d_g))
         lb_ms = graph_ms(lambda: L.l2o_lrsgd_bwd(C.byref(la), _stream()), args.reps)
         tb = lambda b, ms: n * b / ms / 1e9

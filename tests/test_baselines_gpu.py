@@ -188,7 +188,7 @@ def test_tadam_bwd_with_nonzero_v_matches_oracle():
     within 1e-5 max-norm relative, or 3x the fp32 oracle's distance from fp64 where that is larger; the t plane's
     adjoint is exactly 0 and beta2_logit's gradient is nonzero."""
     from open_l2o_b200 import _lib
-    from open_l2o_b200.trainable_baselines import _p
+    from open_l2o_b200.engine import _ptr as _p
     gen = torch.Generator().manual_seed(31)
     n = 4096
     theta = tadam_theta(lr=1e-3, b1=0.85, b2=0.9, eps=1e-7, dtype=torch.float32)
@@ -301,7 +301,7 @@ def test_bwd_outputs_do_not_depend_on_d_g():
     """At the ConvNet size: d_state_old bit-identical with and without d_g, d_theta equal up to the fp64 atomics'
     order; the same for the schedule's backward."""
     from open_l2o_b200 import _lib
-    from open_l2o_b200.trainable_baselines import _p
+    from open_l2o_b200.engine import _ptr as _p
     L = _lib.lib()
     gen = torch.Generator().manual_seed(24)
     n = 354218
@@ -325,7 +325,7 @@ def test_bwd_outputs_do_not_depend_on_d_g():
 
     def lrs(dg):
         d_rates = torch.zeros(2, dtype=torch.float64, device=DEV)
-        a = _lib.LrsgdBwdArgs(n=n, rates=_p(rates), n_steps=2, itr=_p(itr), g=_p(g), d_update=_p(d_upd),
+        a = _lib.LrsgdBwdArgs(n=n, rates=_p(rates), n_steps=2, itr=_p(itr, torch.int32), g=_p(g), d_update=_p(d_upd),
                               d_rates=d_rates.data_ptr(), d_g=_p(dg))
         _lib.check(L.l2o_lrsgd_bwd(ctypes.byref(a), torch.cuda.current_stream().cuda_stream), "l2o_lrsgd_bwd")
         return d_rates

@@ -9,9 +9,10 @@ from oracle import hrnn_oracle as orc   # checker only
 
 
 def test_theta_views_match_oracle_layout():
-    from open_l2o_b200 import hrnn_train as ht
+    from open_l2o_b200.hierarchical_rnn import THETA_SPEC
+    from open_l2o_b200.scale_base import theta_views
     theta = orc.init_theta(seed=2)
-    mine, ref = ht.unpack_theta(theta), orc.unpack_theta(theta)
+    mine, ref = theta_views(theta, THETA_SPEC), orc.unpack_theta(theta)
     assert list(mine) == list(ref)
     for k in ref:
         assert mine[k].shape == ref[k].shape and torch.equal(mine[k], ref[k]), k

@@ -206,7 +206,7 @@ def test_hrnn_coord_bwd_outputs_do_not_depend_on_d_g():
 
 def _crnn_bwd(theta, planes, g, d_new, d_upd, d_g):
     from open_l2o_b200 import _lib
-    from open_l2o_b200.coordinatewise_rnn import _p
+    from open_l2o_b200.engine import _ptr as _p
     d_old = torch.empty_like(planes)
     d_theta = torch.zeros(theta.numel(), dtype=torch.float64, device=DEV)
     a = _lib.CrnnBwdArgs()
