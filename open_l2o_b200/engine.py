@@ -32,22 +32,74 @@ def _stream():
     return torch.cuda.current_stream().cuda_stream
 
 
-class NetHandle:
+class _Handle:
+    """What the coordinate-wise and the dense net handles share, and the surface the meta-optimizer uses on either:
+    ``n_in``, ``layers``, ``n_theta``, the state arena (``state_size`` / ``new_state`` / ``state_views``), ``step`` and
+    ``unroll_bwd``.  The state is kept per row: a row is one coordinate here, K elements for a dense net."""
+
+    n_in = 1
+    _destroy = None   # name of the C destructor
+
+    @staticmethod
+    def _layers(layers):
+        layers = tuple(int(h) for h in layers)
+        if len(layers) > 2:
+            raise L2OError("at most two LSTM layers are supported")
+        return layers
+
+    def _open(self, desc, create, theta_count, state_floats, what):
+        """Fill the descriptor's layers, create the C handle and read its sizes."""
+        desc.n_layers = len(self.layers)
+        desc.hidden[0], desc.hidden[1] = (self.layers + (0, 0))[:2]
+        self._h = C.c_void_p()
+        _lib.check(create(C.byref(self._h), C.byref(desc)), what)
+        self.n_theta = int(theta_count(self._h))
+        self.state_floats = int(state_floats(self._h))   # per row
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None):
+                getattr(_lib.lib(), self._destroy)(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+    def rows(self, n: int) -> int:
+        return n
+
+    def state_size(self, n: int) -> int:
+        """Floats of one state arena for n elements."""
+        return self.state_floats * self.rows(n)
+
+    def new_state(self, n: int, device) -> torch.Tensor:
+        return torch.zeros(max(self.state_size(n), 1), dtype=torch.float32, device=device)
+
+    def state_views(self, arena: torch.Tensor, n: int):
+        """Arena -> tuple over layers of (hidden, cell) views [rows, H] (the reference's state structure)."""
+        out, off, r = [], 0, self.rows(n)
+        for h in self.layers:
+            out.append((arena[off:off + r * h].view(r, h), arena[off + r * h:off + 2 * r * h].view(r, h)))
+            off += 2 * r * h
+        return tuple(out)
+
+    def _check_theta(self, theta):
+        if theta.numel() != self.n_theta:
+            raise L2OError(f"theta has {theta.numel()} elements, net needs {self.n_theta}")
+
+
+class NetHandle(_Handle):
     """One optimizer net: shape + run-time scalars (DM/networks.py:157-205)."""
+
+    _destroy = "l2o_net_destroy"
 
     def __init__(self, layers: Sequence[int] = (20, 20), preprocess_name: str = "identity",
                  preprocess_options: Optional[dict] = None, scale: float = 1.0, tanh_output: bool = False,
                  n_in: int = 1):
-        layers = tuple(int(h) for h in layers)
-        if len(layers) > 2:
-            raise L2OError("at most two LSTM layers are supported")
+        self.layers = self._layers(layers)
         if preprocess_name not in _PRE:
             raise L2OError(f"unsupported preprocess_name {preprocess_name!r}")
         opts = dict(preprocess_options or {})
         d = NetDesc()
-        d.n_layers = len(layers)
-        d.hidden[0] = layers[0] if len(layers) > 0 else 0
-        d.hidden[1] = layers[1] if len(layers) > 1 else 0
         d.preprocess = _PRE[preprocess_name]
         d.n_in = n_in
         d.fc_dim = int(opts.get("dim", 0))
@@ -55,26 +107,10 @@ class NetHandle:
         d.scale = float(scale)
         d.tanh_output = 1 if tanh_output else 0
         self.desc = d
-        self.layers = layers
         self.n_in = n_in
-        self._h = C.c_void_p()
         L = _lib.lib()
-        _lib.check(L.l2o_net_create(C.byref(self._h), C.byref(d)),
-                   f"l2o_net_create(layers={layers}, preprocess={preprocess_name}, n_in={n_in})")
-        self.n_theta = int(L.l2o_theta_count(self._h))
-        self.state_floats = int(L.l2o_state_floats(self._h))
-
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None):
-                _lib.lib().l2o_net_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
-
-    def state_size(self, n: int) -> int:
-        """Floats of one state arena for n coordinates."""
-        return self.state_floats * n
+        self._open(d, L.l2o_net_create, L.l2o_theta_count, L.l2o_state_floats,
+                   f"l2o_net_create(layers={self.layers}, preprocess={preprocess_name}, n_in={n_in})")
 
     def workspace_bytes(self, n: int, T: int):
         """(forward, backward) caller-owned buffer bytes for n coordinates and a T-step unroll."""
@@ -84,20 +120,6 @@ class NetHandle:
 
     def set_engine(self, engine: int):
         _lib.check(_lib.lib().l2o_net_set_engine(self._h, engine), "l2o_net_set_engine")
-
-    # ---- state arena helpers -------------------------------------------------------------
-    def new_state(self, n: int, device) -> torch.Tensor:
-        return torch.zeros(max(self.state_floats * n, 1), dtype=torch.float32, device=device)
-
-    def state_views(self, arena: torch.Tensor, n: int):
-        """Arena -> tuple over layers of (hidden, cell) views [n, H] (the reference's state structure)."""
-        out, off = [], 0
-        for h in self.layers:
-            hh = arena[off:off + n * h].view(n, h)
-            cc = arena[off + n * h:off + 2 * n * h].view(n, h)
-            out.append((hh, cc))
-            off += 2 * n * h
-        return tuple(out)
 
     # ---- kernels -------------------------------------------------------------------------
     def step(self, theta, in0, state_in, state_out, *, in1=None, m=None, v=None, beta1=0.95, beta2=0.95, p=1.0,
@@ -112,8 +134,7 @@ class NetHandle:
         a.state_in, a.state_out = _ptr(state_in, name="state_in"), _ptr(state_out, name="state_out")
         a.x, a.delta, a.feat_out = _ptr(x, name="x"), _ptr(delta, name="delta"), _ptr(feat_out, name="feat_out")
         a.step_ptr, a.t_offset = _ptr(step_ptr, torch.int32, "step_ptr"), t_offset
-        if theta.numel() != self.n_theta:
-            raise L2OError(f"theta has {theta.numel()} elements, net needs {self.n_theta}")
+        self._check_theta(theta)
         _lib.check(_lib.lib().l2o_step(self._h, C.byref(a), _stream()), "l2o_step")
 
     def unroll_fwd(self, theta, n, T, state, *, in_seq=None, opt_kind=OPT_NONE, opt_a=None, opt_b=None,
@@ -157,62 +178,32 @@ class NetHandle:
         _lib.check(_lib.lib().l2o_unroll_bwd(self._h, C.byref(a), _stream()), "l2o_unroll_bwd")
 
 
-class DenseNetHandle:
+class DenseNetHandle(_Handle):
     """Row-wise dense LSTM net with run-time shapes (StandardDeepLSTM with output_size > 1 = the reference's
     KernelDeepLSTM, DM/networks.py:154-236,303-351).  A variable of n = K * R elements in [kw, kh, cin, cout] order is
-    R rows of K inputs (element (k, r) at k * R + r); state per ROW.  Same method surface as NetHandle where the
-    meta-optimizer needs it (step / unroll_bwd / new_state / state_size)."""
+    R rows of K inputs (element (k, r) at k * R + r); state per ROW."""
 
-    n_in = 1   # one gradient input per element (the RNNProp branches of the executor key on n_in == 2)
+    _destroy = "l2o_dense_destroy"
 
     def __init__(self, layers: Sequence[int], k_in: int, k_out: int, preprocess_name: str = "identity",
                  preprocess_options: Optional[dict] = None, scale: float = 1.0, tanh_output: bool = False):
-        layers = tuple(int(h) for h in layers)
-        if len(layers) > 2:
-            raise L2OError("at most two LSTM layers are supported")
+        self.layers = self._layers(layers)
         if preprocess_name not in ("identity", "LogAndSign"):
             raise L2OError(f"unsupported preprocess_name {preprocess_name!r} for a dense net")
         d = _lib.DenseDesc()
-        d.n_layers = len(layers)
-        d.hidden[0] = layers[0] if len(layers) > 0 else 0
-        d.hidden[1] = layers[1] if len(layers) > 1 else 0
         d.n_in, d.n_out = int(k_in), int(k_out)
         d.preprocess = _PRE[preprocess_name]
         d.logsign_k = float((preprocess_options or {}).get("k", 0.0))
         d.scale, d.tanh_output = float(scale), 1 if tanh_output else 0
-        self.layers, self.k_in, self.k_out = layers, int(k_in), int(k_out)
-        self._h = C.c_void_p()
+        self.k_in, self.k_out = int(k_in), int(k_out)
         L = _lib.lib()
-        _lib.check(L.l2o_dense_create(C.byref(self._h), C.byref(d)),
-                   f"l2o_dense_create(layers={layers}, k_in={k_in}, k_out={k_out}, preprocess={preprocess_name})")
-        self.n_theta = int(L.l2o_dense_theta_count(self._h))
-        self.state_floats = int(L.l2o_dense_state_floats(self._h))   # per ROW
-
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None):
-                _lib.lib().l2o_dense_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
+        self._open(d, L.l2o_dense_create, L.l2o_dense_theta_count, L.l2o_dense_state_floats,
+                   f"l2o_dense_create(layers={self.layers}, k_in={k_in}, k_out={k_out}, preprocess={preprocess_name})")
 
     def rows(self, n: int) -> int:
         if n % self.k_in:
             raise L2OError(f"{n} elements are not a whole number of rows of {self.k_in}")
         return n // self.k_in
-
-    def state_size(self, n: int) -> int:
-        return self.state_floats * self.rows(n)
-
-    def new_state(self, n: int, device) -> torch.Tensor:
-        return torch.zeros(max(self.state_size(n), 1), dtype=torch.float32, device=device)
-
-    def state_views(self, arena: torch.Tensor, n: int):
-        out, off, r = [], 0, self.rows(n)
-        for h in self.layers:
-            out.append((arena[off:off + r * h].view(r, h), arena[off + r * h:off + 2 * r * h].view(r, h)))
-            off += 2 * r * h
-        return tuple(out)
 
     def set_engine(self, engine: int):
         if engine == ENGINE_TC:
@@ -224,8 +215,7 @@ class DenseNetHandle:
         a.theta, a.in_ = _ptr(theta, name="theta"), _ptr(in0, name="in0")
         a.state_in, a.state_out = _ptr(state_in, name="state_in"), _ptr(state_out, name="state_out")
         a.x, a.delta = _ptr(x, name="x"), _ptr(delta, name="delta")
-        if theta.numel() != self.n_theta:
-            raise L2OError(f"theta has {theta.numel()} elements, net needs {self.n_theta}")
+        self._check_theta(theta)
         _lib.check(_lib.lib().l2o_dense_step(self._h, C.byref(a), _stream()), "l2o_dense_step")
 
     def unroll_bwd(self, theta, n, T, in_seq, ckpt, dtheta, *, g_rec=None, labels=None, n_total=0, delta_seq=None):

@@ -128,6 +128,39 @@ class _Run(object):
         self.key, self.net, self.off, self.n = key, net, off, n
 
 
+def plan_arena(variables, subsets, net_keys, nets):
+    """Lay out the flat coordinate arena: variables in the order the subsets name them (so that each net's subset is
+    contiguous where possible), unassigned ones last.  Each subset is then cut into maximal contiguous runs; a
+    ``per_variable`` net gets one run per variable.  Returns ([slice of variable j in creation order], N, runs)."""
+    sizes = [int(np.prod(v["shape"])) for v in variables]
+    order = dict.fromkeys([j for subset in subsets for j in subset] + list(range(len(variables))))
+    off, N = {}, 0
+    for j in order:
+        off[j], N = N, N + sizes[j]
+    runs = []
+    for key, subset in zip(net_keys, subsets):
+        cur = None
+        for j in subset:
+            if cur is not None and cur.off + cur.n == off[j] and not getattr(nets[key], "per_variable", False):
+                cur.n += sizes[j]
+            else:
+                cur = _Run(key, nets[key], off[j], sizes[j])
+                runs.append(cur)
+    return [slice(off[j], off[j] + sizes[j]) for j in range(len(variables))], N, runs
+
+
+def _adam_slots(nets):
+    return {k: dict(m=torch.zeros_like(net.theta), v=torch.zeros_like(net.theta), k=0) for k, net in nets.items()}
+
+
+def _adam_step(nets, dtheta, slots, lr):
+    """TF-Adam on every net's theta from its meta-gradient, with the Adam slots ``slots`` (DM/meta.py:411-413)."""
+    for k, net in nets.items():
+        ad = slots[k]
+        ad["k"] += 1
+        _engine.adam_step(net.theta, dtheta[k], ad["m"], ad["v"], ad["k"], lr=lr)
+
+
 class _Program(object):
     """One meta_loss graph: variables, nets, state, workspaces and the unroll executor."""
 
@@ -151,32 +184,7 @@ class _Program(object):
         print([c["name"] for c in self.constants])
         self.nets, self.net_keys, self.subsets = _make_nets(self.variables, optimizer._config, net_assignments)
         optimizer._nets = self.nets
-
-        # flat arena: variables ordered so that each net's subset is contiguous where possible
-        order = []
-        for subset in self.subsets:
-            for j in subset:
-                if j not in order:
-                    order.append(j)
-        for j in range(len(self.variables)):
-            if j not in order:
-                order.append(j)
-        self.var_off, off = {}, 0
-        for j in order:
-            self.var_off[j] = off
-            off += int(np.prod(self.variables[j]["shape"])) if self.variables[j]["shape"] else 1
-        self.N = off
-        self.runs = []
-        for key, subset in zip(self.net_keys, self.subsets):
-            cur = None
-            for j in subset:
-                n = int(np.prod(self.variables[j]["shape"])) if self.variables[j]["shape"] else 1
-                o = self.var_off[j]
-                if cur is not None and cur.off + cur.n == o and not getattr(self.nets[key], "per_variable", False):
-                    cur.n += n
-                else:
-                    cur = _Run(key, self.nets[key], o, n)
-                    self.runs.append(cur)
+        self.var_slices, self.N, self.runs = plan_arena(self.variables, self.subsets, self.net_keys, self.nets)
         self.X = torch.zeros(self.N, device=self.device)
         self.const_vals = {}
         self.fused = getattr(make_loss, "fused", None) if os.environ.get("L2O_DISABLE_FUSED") != "1" else None
@@ -189,8 +197,7 @@ class _Program(object):
         self.producer = None
         if self.fused is not None and self.fused.kind in _PRODUCER_KINDS:
             self.producer, self.fused = self.fused, None
-        self.adam = {k: dict(m=torch.zeros_like(net.theta), v=torch.zeros_like(net.theta), k=0)
-                     for k, net in self.nets.items()}
+        self.adam = _adam_slots(self.nets)
         self.dtheta = {k: torch.zeros(net.theta.numel(), dtype=torch.float64, device=self.device)
                        for k, net in self.nets.items()}
         self.step_placeholder = Placeholder("step")
@@ -209,11 +216,12 @@ class _Program(object):
     def _alloc_workspaces(self):
         T = self.T
         for r in self.runs:
-            r.state = r.net.handle.new_state(r.n, self.device)
-            r.ckpt = torch.zeros((T + 1) * max(r.net.handle.state_size(r.n), 1), device=self.device)
+            h = r.net.handle
+            r.slot = max(h.state_size(r.n), 1)   # floats of one checkpoint slot
+            r.state = h.new_state(r.n, self.device)
+            r.ckpt = torch.zeros((T + 1) * r.slot, device=self.device)
             r.g_rec = torch.zeros(T + 1, r.n, device=self.device)
-            r.x_work = torch.zeros(r.n, device=self.device)
-            if r.net.handle.n_in == 2:
+            if h.n_in == 2:
                 r.m = torch.zeros(r.n, device=self.device)
                 r.v = torch.zeros(r.n, device=self.device)
                 r.m_work, r.v_work = torch.zeros_like(r.m), torch.zeros_like(r.v)
@@ -221,20 +229,18 @@ class _Program(object):
             # what the tensor-core BPTT of a tanh-output / fc(20) net (RNNProp) needs on top: the recorded deltas
             # (tanh' of the output layer) and the hand-over buffer between its layer-2 and layer-1 pass
             r.delta_rec = r.bwd_scratch = None
-            h = r.net.handle
             if getattr(r.net, "tanh_output", False) and isinstance(h, _engine.NetHandle):
                 r.delta_rec = torch.zeros(T, r.n, device=self.device)
             if h.n_in == 2 and isinstance(h, _engine.NetHandle) and tuple(h.layers) == (20, 20):
                 r.bwd_scratch = torch.zeros(T, r.n, 20, device=self.device)
+        self._Xw = torch.zeros(self.N, device=self.device)   # x after the last unroll, committed by `update`
         self.fx_buf = torch.zeros(T + 1, dtype=torch.float64, device=self.device)
 
     def reset_x(self):
         """Re-run the initializers of x + constants only (``reset_x`` of DM/data_generator.py:50,80).  The tensors are
         refilled IN PLACE: captured CUDA graphs and views handed out earlier keep pointing at live, current data."""
-        for v, j in zip(self.variables, range(len(self.variables))):
-            n = int(np.prod(v["shape"])) if v["shape"] else 1
-            o = self.var_off[j]
-            self.X[o:o + n].copy_(v["init"](v["shape"], self.gen).reshape(-1).to(self.device))
+        for v, xv in zip(self.variables, self._var_views(self.X)):
+            xv.view(-1).copy_(v["init"](v["shape"], self.gen).reshape(-1).to(self.device))
         for c in self.constants:
             new = c["init"](c["shape"], self.gen).to(torch.float32).contiguous()
             cur = self.const_vals.get(c["name"])
@@ -254,14 +260,19 @@ class _Program(object):
         self.unroll_idx = 0
 
     # ---- optimizee evaluation --------------------------------------------------------------------
+    @property
+    def var_off(self):
+        """Offset of each variable in the flat arena (creation order)."""
+        return [s.start for s in self.var_slices]
+
     def _var_views(self, Xflat):
         """The optimizee variables as views of the flat arena (creation order)."""
-        out = []
-        for j, v in enumerate(self.variables):
-            n = int(np.prod(v["shape"])) if v["shape"] else 1
-            o = self.var_off[j]
-            out.append(Xflat[o:o + n].view(v["shape"]))
-        return out
+        return [Xflat[s].view(v["shape"]) for s, v in zip(self.var_slices, self.variables)]
+
+    @staticmethod
+    def _fill(view, value):
+        """Copy a host array (any shape with the view's element count) into a variable's view of the arena."""
+        view.view(-1).copy_(torch.as_tensor(np.asarray(value, dtype=np.float32)).reshape(-1))
 
     def _loss_from_vars(self, var_list):
         """_make_with_custom_variables (DM/meta.py:131-155): trainables popped in creation order."""
@@ -288,23 +299,19 @@ class _Program(object):
                 self.scale_active = False
             return
         self.scale_flat.fill_(1.0)
-        for j, p in enumerate(self.scale_placeholders):
+        for p, sv in zip(self.scale_placeholders, self._var_views(self.scale_flat)):
             if p in feed:
-                n = int(np.prod(self.variables[j]["shape"])) if self.variables[j]["shape"] else 1
-                o = self.var_off[j]
-                self.scale_flat[o:o + n].copy_(torch.as_tensor(np.asarray(feed[p], dtype=np.float32)).reshape(-1))
+                self._fill(sv, feed[p])
         self.scale_active = True
 
     def assign_x(self, values):
         """assign_func of DM/train_dm.py:101-113: overwrite the optimizee variables (list in creation order)."""
-        for j, val in enumerate(values):
-            n = int(np.prod(self.variables[j]["shape"])) if self.variables[j]["shape"] else 1
-            o = self.var_off[j]
-            self.X[o:o + n].copy_(torch.as_tensor(np.asarray(val, dtype=np.float32)).reshape(-1))
+        for xv, val in zip(self._var_views(self.X), values):
+            self._fill(xv, val)
 
-    def x_values(self):
-        return [self.X[self.var_off[j]:self.var_off[j] + (int(np.prod(v["shape"])) if v["shape"] else 1)]
-                .reshape(v["shape"]).cpu().numpy() for j, v in enumerate(self.variables)]
+    def x_values(self, Xflat=None):
+        """The optimizee variables of ``Xflat`` (default: the committed x) as host arrays in creation order."""
+        return [v.cpu().numpy() for v in self._var_views(self.X if Xflat is None else Xflat)]
 
     def _produce(self, Xflat):
         """f(x) and df/dx from the fused producer kernel (one launch)."""
@@ -349,49 +356,49 @@ class _Program(object):
             return int(feed[self.step_placeholder])
         return self.unroll_idx * self.T + 1
 
+    def _moments(self, m, v, **kw):
+        """RNNProp's Adam-moment arguments: the net's (m~, g~) input is formed in-kernel from (m, v)."""
+        return dict(m=m, v=v, beta1=self.opt.beta1, beta2=self.opt.beta2, **kw)
+
+    def _load_moments(self, r):
+        """RNNProp: the unroll advances copies of the committed moments (committed by `update`)."""
+        if r.net.handle.n_in == 2:
+            r.m_work.copy_(r.m)
+            r.v_work.copy_(r.v)
+
     def _forward_fused(self, train, step0):
         r, T, f = self.runs[0], self.T, self.fused
         h = r.net.handle
-        r.x_work.copy_(self.X)
-        state = r.ckpt[:max(h.state_size(r.n), 1)]
+        self._Xw.copy_(self.X)
         work_state = r.state.clone()
         self.fx_buf.zero_()
-        kw = {}
-        if h.n_in == 2:
-            r.m_work.copy_(r.m)
-            r.v_work.copy_(r.v)
-            kw = dict(m=r.m_work, v=r.v_work, beta1=self.opt.beta1, beta2=self.opt.beta2, step0=step0,
-                      feat_rec=r.feat_rec)
+        self._load_moments(r)
+        kw = self._moments(r.m_work, r.v_work, step0=step0, feat_rec=r.feat_rec) if h.n_in == 2 else {}
         if train and r.delta_rec is not None:
             kw["delta_seq"] = r.delta_rec
         h.unroll_fwd(r.net.theta, r.n, T, work_state, opt_kind=_engine.OPT_KINDS[f.kind],
                      opt_a=self.const_vals[f.a].reshape(-1), opt_b=self.const_vals[f.b].reshape(-1),
-                     opt_alpha=f.alpha, opt_fscale=f.fscale, x=r.x_work, ckpt=r.ckpt if train else None,
+                     opt_alpha=f.alpha, opt_fscale=f.fscale, x=self._Xw, ckpt=r.ckpt if train else None,
                      g_rec=r.g_rec, fx=self.fx_buf, opt_group=getattr(f, "group", 0), **kw)
-        del state
         r.state_final = work_state
         return self.fx_buf
 
     def _forward_external(self, train, step0):
-        T = self.T
-        Xw = self.X.clone()
+        T, Xw = self.T, self._Xw
+        Xw.copy_(self.X)
         fxs = []
         for r in self.runs:
-            r.ckpt[:max(r.net.handle.state_size(r.n), 1)].copy_(r.state)
-            if r.net.handle.n_in == 2:
-                r.m_work.copy_(r.m)
-                r.v_work.copy_(r.v)
+            r.ckpt[:r.slot].copy_(r.state)
+            self._load_moments(r)
         for t in range(T):
             fx, g = self._value_and_grad(Xw)
             fxs.append(fx)
             for r in self.runs:
-                h = r.net.handle
-                slot = max(h.state_size(r.n), 1)
+                h, slot = r.net.handle, r.slot
                 r.g_rec[t].copy_(g[r.off:r.off + r.n])
                 kw = {}
                 if h.n_in == 2:
-                    kw = dict(m=r.m_work, v=r.v_work, beta1=self.opt.beta1, beta2=self.opt.beta2,
-                              step_ptr=self.step_dev, t_offset=t, feat_out=r.feat_rec[t])
+                    kw = self._moments(r.m_work, r.v_work, step_ptr=self.step_dev, t_offset=t, feat_out=r.feat_rec[t])
                 if train and r.delta_rec is not None:
                     kw["delta"] = r.delta_rec[t]
                 # theta is constant inside an unroll: the weight image built at t = 0 serves every later step (runs that
@@ -410,10 +417,7 @@ class _Program(object):
                     fx = self._loss_at(Xw)
         fxs.append(fx)
         for r in self.runs:
-            slot = max(r.net.handle.state_size(r.n), 1)
-            r.state_final = r.ckpt[T * slot:(T + 1) * slot]
-            r.x_work = Xw[r.off:r.off + r.n]
-        self._Xw = Xw
+            r.state_final = r.ckpt[T * r.slot:(T + 1) * r.slot]
         return torch.stack([f.reshape(()).double() for f in fxs])
 
     # ---- CUDA-graph path of the external-gradient regime ------------------------------------------------
@@ -421,14 +425,18 @@ class _Program(object):
         """Everything of one unroll that is launch-bound and shape-static: T x (autograd + step kernel) [+ BPTT]."""
         fx = self._forward_external(train, step0)
         if train:
-            for d in self.dtheta.values():
-                d.zero_()
-            for r in self.runs:
-                h = r.net.handle
-                in_seq = r.feat_rec if h.n_in == 2 else r.g_rec
-                h.unroll_bwd(r.net.theta, r.n, self.T, in_seq, r.ckpt, self.dtheta[r.key], g_rec=r.g_rec,
-                             **self._bwd_extra(r))
+            self._bptt()
         return fx
+
+    def _bptt(self):
+        """The meta-gradient of the unroll just run: dtheta zeroed, then one BPTT launch per run."""
+        for d in self.dtheta.values():
+            d.zero_()
+        for r in self.runs:
+            h = r.net.handle
+            in_seq = r.feat_rec if h.n_in == 2 else r.g_rec
+            h.unroll_bwd(r.net.theta, r.n, self.T, in_seq, r.ckpt, self.dtheta[r.key], g_rec=r.g_rec,
+                         **self._bwd_extra(r))
 
     @staticmethod
     def _bwd_extra(r):
@@ -466,19 +474,18 @@ class _Program(object):
                 with torch.cuda.graph(g):
                     fx = self._graph_body(train, step0)
                 self._graph_kernels[key] = _engine.launch_count() - n0   # library kernels recorded in this graph
-                self._graphs[key] = (g, fx, self._Xw, [r.state_final for r in self.runs], [r.x_work for r in self.runs])
+                self._graphs[key] = (g, fx, [r.state_final for r in self.runs])
             except Exception as e:  # capture not possible for this optimizee: keep running the same kernels eagerly
                 import warnings
                 warnings.warn("CUDA-graph capture of the unroll failed (%r); staying eager" % (e,))
                 self._graph_failed = True
                 torch.cuda.synchronize()
                 return self._graph_body(train, step0)
-        g, fx, xw, finals, xworks = self._graphs[key]
+        g, fx, finals = self._graphs[key]
         g.replay()
         _engine.note_graph_replay(self._graph_kernels[key])
-        self._Xw = xw
-        for r, f, xk in zip(self.runs, finals, xworks):
-            r.state_final, r.x_work = f, xk
+        for r, f in zip(self.runs, finals):
+            r.state_final = f
         return fx
 
     def execute(self, kinds, feed):
@@ -487,32 +494,23 @@ class _Program(object):
             return {}
         if "reset" in kinds:
             raise ValueError("fetch `reset` on its own (the reference runs it separately, DM/util.py:37)")
-        mt_kinds = set(k for k in kinds if ":" in k)
-        if mt_kinds:
-            out = {}
-            for ti in sorted(set(int(k.split(":")[1]) for k in mt_kinds)):
-                out.update(self.mt_tasks[ti].execute(set(k.split(":")[0] for k in mt_kinds if int(k.split(":")[1]) == ti), feed))
-            kinds = kinds - mt_kinds
-            if not kinds:
-                return out
-            out.update(self.execute(kinds, feed))
+        out, mt = {}, collections.defaultdict(set)   # imitation fetches are "<kind>:<task index>"
+        for k in kinds:
+            if ":" in k:
+                kind, ti = k.split(":")
+                mt[int(ti)].add(kind)
+        for ti in sorted(mt):
+            out.update(self.mt_tasks[ti].execute(mt[ti], feed))
+        kinds = set(k for k in kinds if ":" not in k)
+        if mt and not kinds:
             return out
         train = "step" in kinds
-        commit = "update" in kinds
         step0 = self._step0(feed)
-        T = self.T
-        out = {}
         self._apply_scale_feed(feed)
         if self.fused is not None and not self.scale_active:
             fx = self._forward_fused(train, step0)
             if train:
-                for d in self.dtheta.values():
-                    d.zero_()
-                for r in self.runs:
-                    h = r.net.handle
-                    in_seq = r.feat_rec if h.n_in == 2 else r.g_rec
-                    h.unroll_bwd(r.net.theta, r.n, T, in_seq, r.ckpt, self.dtheta[r.key], g_rec=r.g_rec,
-                                 **self._bwd_extra(r))
+                self._bptt()
         else:
             fx = self._run_external(train, step0)
         if train:
@@ -526,24 +524,15 @@ class _Program(object):
         if "loss" in kinds:
             out["loss"] = float(fx.sum().item())
         if "fx" in kinds:
-            out["fx"] = float(fx[T].item())
-        used_fused = self.fused is not None and not self.scale_active
+            out["fx"] = float(fx[self.T].item())
         if "x" in kinds:
-            xf = self.runs[0].x_work if used_fused else self._Xw
-            out["x"] = [xf[self.var_off[j]:self.var_off[j] + (int(np.prod(v["shape"])) if v["shape"] else 1)]
-                        .reshape(v["shape"]).cpu().numpy() for j, v in enumerate(self.variables)]
+            out["x"] = self.x_values(self._Xw)
         self.last_fx = fx
         if train:
-            for k, net in self.nets.items():
-                ad = self.adam[k]
-                ad["k"] += 1
-                _engine.adam_step(net.theta, self.dtheta[k], ad["m"], ad["v"], ad["k"], lr=self.learning_rate)
+            _adam_step(self.nets, self.dtheta, self.adam, self.learning_rate)
             out["step"] = None
-        if commit:
-            if used_fused:
-                self.X.copy_(self.runs[0].x_work)
-            else:
-                self.X.copy_(self._Xw)
+        if "update" in kinds:
+            self.X.copy_(self._Xw)
             for r in self.runs:
                 r.state.copy_(r.state_final)
                 if r.net.handle.n_in == 2:
@@ -552,7 +541,6 @@ class _Program(object):
             self.unroll_idx += 1
             out["update"] = None
         return out
-
 
 
 class _MtTask(object):
@@ -574,18 +562,16 @@ class _MtTask(object):
             if getattr(r.net, "per_variable", False):
                 raise NotImplementedError("imitation tasks are implemented for the coordinate-wise nets")
             sb = dict(run=r, n=r.n, state=h.new_state(r.n, prog.device),
-                      ckpt=torch.zeros((T + 1) * max(h.state_size(r.n), 1), device=prog.device),
+                      ckpt=torch.zeros((T + 1) * r.slot, device=prog.device),
                       dseq=torch.zeros(T * r.n, device=prog.device),
                       inp=Placeholder("mt{}_input_subset{}".format(index, len(self.subsets))),
                       lab=Placeholder("mt{}_label_subset{}".format(index, len(self.subsets))))
             if h.n_in == 2:   # RNNProp: the task carries its own Adam moments (DM/meta_rnnprop_train.py:469-486)
                 sb.update(m=torch.zeros(r.n, device=prog.device), v=torch.zeros(r.n, device=prog.device),
-                          feat=torch.zeros(T, 2, r.n, device=prog.device),
-                          scratch=r.bwd_scratch)   # hand-over buffer of the two-pass tensor-core BPTT (shared with the run)
+                          feat=torch.zeros(T, 2, r.n, device=prog.device))
             self.subsets.append(sb)
         self.n_total = sum(sb["n"] for sb in self.subsets)
-        self.adam = {k: dict(m=torch.zeros_like(net.theta), v=torch.zeros_like(net.theta), k=0)
-                     for k, net in prog.nets.items()}
+        self.adam = _adam_slots(prog.nets)
         self.il = torch.zeros(1, dtype=torch.float64, device=prog.device)
 
     def _dev(self, arr, T, n):
@@ -612,43 +598,33 @@ class _MtTask(object):
             r, n = sb["run"], sb["n"]
             h = r.net.handle
             inp, lab = self._dev(feed[sb["inp"]], T, n), self._dev(feed[sb["lab"]], T, n)
-            work = sb["state"].clone()
+            work, moments, kw, in_seq = sb["state"].clone(), None, {}, inp
             if h.n_in == 2:
                 # RNNProp imitation unroll (DM/meta_rnnprop_train.py:505-534): raw gradients in, Adam features formed
-                # in-kernel from the task's own (m, v) with p = float(step + t), recorded for the backward sweep
-                mw, vw = sb["m"].clone(), sb["v"].clone()
-                h.unroll_fwd(r.net.theta, n, T, work, in_seq=inp, ckpt=sb["ckpt"] if train else None, labels=lab,
-                             imit_loss=self.il, n_total=self.n_total, m=mw, v=vw, beta1=prog.opt.beta1,
-                             beta2=prog.opt.beta2, step0=step0, feat_rec=sb["feat"],
-                             delta_seq=sb["dseq"] if train else None)
-                if train:
-                    h.unroll_bwd(r.net.theta, n, T, sb["feat"], sb["ckpt"], prog.dtheta[r.key], labels=lab,
-                                 n_total=self.n_total, delta_seq=sb["dseq"], scratch=sb["scratch"])
-                finals.append((work, mw, vw))
-                continue
+                # in-kernel from the task's own (m, v) with p = float(step + t), recorded for the BPTT to read
+                moments = (sb["m"].clone(), sb["v"].clone())
+                kw, in_seq = prog._moments(*moments, step0=step0, feat_rec=sb["feat"]), sb["feat"]
             h.unroll_fwd(r.net.theta, n, T, work, in_seq=inp, ckpt=sb["ckpt"] if train else None, labels=lab,
-                         imit_loss=self.il, n_total=self.n_total, delta_seq=sb["dseq"] if train else None)
+                         imit_loss=self.il, n_total=self.n_total, delta_seq=sb["dseq"] if train else None, **kw)
             if train:  # the recorded deltas let the tensor-core BPTT run in imitation mode too
-                h.unroll_bwd(r.net.theta, n, T, inp, sb["ckpt"], prog.dtheta[r.key], labels=lab, n_total=self.n_total,
-                             delta_seq=sb["dseq"])
-            finals.append((work, None, None))
+                h.unroll_bwd(r.net.theta, n, T, in_seq, sb["ckpt"], prog.dtheta[r.key], labels=lab, n_total=self.n_total,
+                             **dict(prog._bwd_extra(r), delta_seq=sb["dseq"]))
+            finals.append((work, moments))
         out = {}
         if "loss_mt" in kinds:
             out["loss_mt:%d" % self.index] = float(self.il.item())
         if train:
-            for k, net in prog.nets.items():
-                ad = self.adam[k]
-                ad["k"] += 1
-                _engine.adam_step(net.theta, prog.dtheta[k], ad["m"], ad["v"], ad["k"], lr=prog.learning_rate)
+            _adam_step(prog.nets, prog.dtheta, self.adam, prog.learning_rate)
             out["step_mt:%d" % self.index] = None
         if commit:
-            for sb, (w, mw, vw) in zip(self.subsets, finals):
+            for sb, (w, moments) in zip(self.subsets, finals):
                 sb["state"].copy_(w)
-                if mw is not None:
-                    sb["m"].copy_(mw)
-                    sb["v"].copy_(vw)
+                if moments is not None:
+                    sb["m"].copy_(moments[0])
+                    sb["v"].copy_(moments[1])
             out["update_mt:%d" % self.index] = None
         return out
+
 
 class MetaOptimizer(object):
     """Learning to learn (meta) optimizer (DM/meta.py:219-414)."""

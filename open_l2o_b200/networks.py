@@ -89,7 +89,83 @@ class Network(object):
         raise NotImplementedError
 
 
-class StandardDeepLSTM(Network):
+class _LSTMNet(Network):
+    """What StandardDeepLSTM and KernelDeepLSTM share: theta in Sonnet creation order, the state arena, and one step
+    call.  Subclasses create ``_handle`` and define ``variable_shapes`` before they call ``_init_theta``."""
+
+    def _init_theta(self, initializer, seed, device):
+        self.device = torch.device(device) if device is not None else (
+            torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu"))
+        gen = torch.Generator().manual_seed(seed)
+        parts = []
+        for mod, var, shp in self.variable_shapes():
+            init = _lookup_initializer(initializer, mod, var)
+            if init is not None:
+                t = _convert_initializer(init, shp, gen)
+            elif mod.startswith("lstm"):     # Sonnet 1.x LSTM default: TruncatedNormal(1/sqrt(fan_in)) for w and b
+                fan_in = [s for m, v, s in self.variable_shapes() if m == mod and v == "w_gates"][0][0]
+                t = _trunc_normal(shp, 1.0 / math.sqrt(fan_in), gen)
+            elif var == "w":                 # Sonnet Linear default
+                t = _trunc_normal(shp, 1.0 / math.sqrt(shp[0]), gen)
+            else:
+                t = torch.zeros(shp)
+            parts.append(t.reshape(-1))
+        self.theta = torch.cat(parts).to(self.device).contiguous()
+        assert self.theta.numel() == self._handle.n_theta
+
+    @property
+    def handle(self):
+        return self._handle
+
+    def get_variables(self):
+        th = self.theta.detach().cpu().numpy()
+        out, off = [], 0
+        for _, _, shp in self.variable_shapes():
+            n = int(np.prod(shp))
+            out.append(th[off:off + n].reshape(shp).copy())
+            off += n
+        return out
+
+    def set_variables(self, data):
+        """``data``: {module: {var: ndarray}} (the .l2l format)."""
+        parts = [torch.as_tensor(np.asarray(data[m][v]), dtype=torch.float32).reshape(-1)
+                 for m, v, _ in self.variable_shapes()]
+        self.theta.copy_(torch.cat(parts).to(self.theta.device))
+
+    # ---- operator surface --------------------------------------------------------------------
+    def _state_arena(self, prev_state):
+        arena = getattr(prev_state, "arena", None)
+        if arena is not None:
+            return arena
+        parts = []
+        for h, c in prev_state:
+            parts += [h.reshape(-1), c.reshape(-1)]
+        return torch.cat(parts).contiguous() if parts else torch.zeros(1, device=self.theta.device)
+
+    def _wrap_state(self, arena, n):
+        st = State(self._handle.state_views(arena, n))
+        st.arena = arena
+        return st
+
+    def _step(self, g, prev_state, m=None):
+        """delta, next_state for the gradients ``g`` (RNNProp: and the moments ``m``, stacked as (m~, g~)).  Elements
+        are taken in memory order; delta has the shape of ``g``."""
+        gf = g.reshape(-1).contiguous()
+        n = gf.numel()
+        in0, in1 = (gf, None) if m is None else (m.reshape(-1).contiguous(), gf)
+        arena_in = self._state_arena(prev_state)
+        arena_out = torch.empty_like(arena_in)
+        delta = torch.empty(n, dtype=torch.float32, device=gf.device)
+        self._handle.step(self.theta, in0, arena_in, arena_out, in1=in1, delta=delta)
+        return delta.reshape(g.shape), self._wrap_state(arena_out, n)
+
+    def initial_state_for_inputs(self, inputs, **kwargs):
+        """Zero (hidden, cell) per layer, one state row per coordinate (DM/networks.py:234-236, 273-276)."""
+        n = int(np.prod(inputs.shape))
+        return self._wrap_state(self._handle.new_state(n, self.theta.device), n)
+
+
+class StandardDeepLSTM(_LSTMNet):
     """LSTM layers with a Linear layer on top (DM/networks.py:154-236).  Only the coordinate-wise uses
     (output_size == 1) are on the accelerated path."""
 
@@ -108,26 +184,8 @@ class StandardDeepLSTM(Network):
         self._handle = _engine.NetHandle(layers=self._layers, preprocess_name=preprocess_name,
                                          preprocess_options=self._preprocess_options, scale=scale,
                                          tanh_output=tanh_output, n_in=self._n_in)
-        self.device = torch.device(device) if device is not None else (
-            torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu"))
-        gen = torch.Generator().manual_seed(seed)
-        parts = []
-        for mod, var, shp in self.variable_shapes():
-            init = _lookup_initializer(initializer, mod, var)
-            if init is not None:
-                t = _convert_initializer(init, shp, gen)
-            elif mod.startswith("lstm"):
-                fan_in = [s for m, v, s in self.variable_shapes() if m == mod and v == "w_gates"][0][0]
-                t = _trunc_normal(shp, 1.0 / math.sqrt(fan_in), gen)      # Sonnet 1.x LSTM default
-            elif var == "w":
-                t = _trunc_normal(shp, 1.0 / math.sqrt(shp[0]), gen)      # Sonnet Linear default
-            else:
-                t = torch.zeros(shp)
-            parts.append(t.reshape(-1))
-        self.theta = torch.cat(parts).to(self.device).contiguous()
-        assert self.theta.numel() == self._handle.n_theta
+        self._init_theta(initializer, seed, device)
 
-    # ---- variables ---------------------------------------------------------------------------
     @property
     def feat(self):
         if self._preprocess_name == "fc":
@@ -148,57 +206,9 @@ class StandardDeepLSTM(Network):
         out += [("linear", "w", (k, 1)), ("linear", "b", (1,))]
         return out
 
-    def get_variables(self):
-        th = self.theta.detach().cpu().numpy()
-        out, off = [], 0
-        for _, _, shp in self.variable_shapes():
-            n = int(np.prod(shp))
-            out.append(th[off:off + n].reshape(shp).copy())
-            off += n
-        return out
-
-    def set_variables(self, data):
-        """``data``: {module: {var: ndarray}} (the .l2l format)."""
-        parts = [torch.as_tensor(np.asarray(data[m][v]), dtype=torch.float32).reshape(-1)
-                 for m, v, _ in self.variable_shapes()]
-        self.theta.copy_(torch.cat(parts).to(self.theta.device))
-
-    @property
-    def handle(self):
-        return self._handle
-
-    # ---- operator surface --------------------------------------------------------------------
-    def _reshape_inputs(self, inputs):
-        return inputs.reshape(-1)
-
-    def _state_arena(self, prev_state, n):
-        arena = getattr(prev_state, "arena", None)
-        if arena is not None:
-            return arena
-        parts = []
-        for h, c in prev_state:
-            parts += [h.reshape(-1), c.reshape(-1)]
-        return torch.cat(parts).contiguous() if parts else torch.zeros(1, device=self.theta.device)
-
-    def _wrap_state(self, arena, n):
-        st = State(self._handle.state_views(arena, n))
-        st.arena = arena
-        return st
-
     def __call__(self, inputs, prev_state):
         """delta, next_state = net(gradients, prev_state) (DM/networks.py:207-232, 254-271)."""
-        flat = self._reshape_inputs(inputs).contiguous()
-        n = flat.numel()
-        arena_in = self._state_arena(prev_state, n)
-        arena_out = torch.empty_like(arena_in)
-        delta = torch.empty(n, dtype=torch.float32, device=flat.device)
-        self._handle.step(self.theta, flat, arena_in, arena_out, delta=delta)
-        return delta.reshape(inputs.shape), self._wrap_state(arena_out, n)
-
-    def initial_state_for_inputs(self, inputs, **kwargs):
-        """Zero (hidden, cell) per layer, batch = number of coordinates (DM/networks.py:234-236, 273-276)."""
-        n = int(np.prod(inputs.shape)) if len(inputs.shape) else 1
-        return self._wrap_state(self._handle.new_state(n, self.theta.device), n)
+        return self._step(inputs, prev_state)
 
 
 class CoordinateWiseDeepLSTM(StandardDeepLSTM):
@@ -217,16 +227,10 @@ class RNNprop(StandardDeepLSTM):
         super(RNNprop, self).__init__(1, name=name, **kwargs)
 
     def __call__(self, m, g, prev_state):
-        mf, gf = m.reshape(-1).contiguous(), g.reshape(-1).contiguous()
-        n = gf.numel()
-        arena_in = self._state_arena(prev_state, n)
-        arena_out = torch.empty_like(arena_in)
-        delta = torch.empty(n, dtype=torch.float32, device=gf.device)
-        self._handle.step(self.theta, mf, arena_in, arena_out, in1=gf, delta=delta)
-        return delta.reshape(g.shape), self._wrap_state(arena_out, n)
+        return self._step(g, prev_state, m)
 
 
-class KernelDeepLSTM(Network):
+class KernelDeepLSTM(_LSTMNet):
     """``DeepLSTM`` for convolutional filters (DM/networks.py:303-351): the input is a filter bank
     [kernel_w, kernel_h, n_input_channels, n_output_channels]; every (input, output) channel pair is one ROW whose
     kernel_w*kernel_h entries are the LSTM's inputs, and the output Linear produces the row's kernel_w*kernel_h updates.
@@ -245,28 +249,7 @@ class KernelDeepLSTM(Network):
         self._handle = _engine.DenseNetHandle(self._layers, self._k, self._k, preprocess_name=preprocess_name,
                                               preprocess_options=self._preprocess_options, scale=scale,
                                               tanh_output=tanh_output)
-        self.device = torch.device(device) if device is not None else (
-            torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu"))
-        gen = torch.Generator().manual_seed(seed)
-        parts = []
-        for mod, var, shp in self.variable_shapes():
-            init = _lookup_initializer(initializer, mod, var)
-            if init is not None:
-                t = _convert_initializer(init, shp, gen)
-            elif mod.startswith("lstm"):     # Sonnet 1.x LSTM default: TruncatedNormal(1/sqrt(fan_in)) for w and b
-                fan_in = [s_ for m, v, s_ in self.variable_shapes() if m == mod and v == "w_gates"][0][0]
-                t = _trunc_normal(shp, 1.0 / math.sqrt(fan_in), gen)
-            elif var == "w":                 # Sonnet Linear default
-                t = _trunc_normal(shp, 1.0 / math.sqrt(shp[0]), gen)
-            else:
-                t = torch.zeros(shp)
-            parts.append(t.reshape(-1))
-        self.theta = torch.cat(parts).to(self.device).contiguous()
-        assert self.theta.numel() == self._handle.n_theta
-
-    @property
-    def handle(self):
-        return self._handle
+        self._init_theta(initializer, seed, device)
 
     @property
     def feat(self):
@@ -280,9 +263,6 @@ class KernelDeepLSTM(Network):
         out += [("linear", "w", (k, self._k)), ("linear", "b", (self._k,))]
         return out
 
-    get_variables = StandardDeepLSTM.get_variables
-    set_variables = StandardDeepLSTM.set_variables
-
     def _check(self, inputs):
         if inputs.dim() != 4 or list(inputs.shape[:2]) != self._kernel_shape:
             raise ValueError("KernelDeepLSTM expects a [kw, kh, cin, cout] tensor with kernel shape {}; got {}".format(
@@ -291,26 +271,13 @@ class KernelDeepLSTM(Network):
     def initial_state_for_inputs(self, inputs, **kwargs):
         """Batch size = n_input_channels * n_output_channels (DM/networks.py:347-351)."""
         self._check(inputs)
-        n = inputs.numel()
-        arena = self._handle.new_state(n, self.theta.device)
-        st = State(self._handle.state_views(arena, n))
-        st.arena = arena
-        return st
+        return super(KernelDeepLSTM, self).initial_state_for_inputs(inputs)
 
     def __call__(self, inputs, prev_state):
-        """update, next_state = net(filter_gradient, prev_state) (DM/networks.py:329-346)."""
+        """update, next_state = net(filter_gradient, prev_state) (DM/networks.py:329-346): element (k, r) of the flat
+        input is at k * R + r, so the reference's transposes are index arithmetic."""
         self._check(inputs)
-        flat = inputs.contiguous().reshape(-1)     # element (k, r) at k * R + r: the transposes are index arithmetic
-        n = flat.numel()
-        arena_in = getattr(prev_state, "arena", None)
-        if arena_in is None:
-            arena_in = torch.cat([t.reshape(-1) for hc in prev_state for t in hc]).contiguous()
-        arena_out = torch.empty_like(arena_in)
-        delta = torch.empty(n, dtype=torch.float32, device=flat.device)
-        self._handle.step(self.theta, flat, arena_in, arena_out, delta=delta)
-        st = State(self._handle.state_views(arena_out, n))
-        st.arena = arena_out
-        return delta.reshape(inputs.shape), st
+        return self._step(inputs, prev_state)
 
 
 class Sgd(Network):
