@@ -15,6 +15,8 @@
  *   l2o_unroll_fwd                      the tf.while_loop body x T                     DM/meta.py:338-376
  *                                       imitation unroll                               DM/meta_dm_train.py:463-480
  *   l2o_unroll_bwd                      tf.gradients(loss, theta) through that loop    DM/meta.py:412 (BPTT; SURVEY.md App. B)
+ *   l2o_unroll_bwd_carry                the same over one segment of the loop (recompute instead of
+ *                                       while_loop(swap_memory=True))                 DM/meta.py:364-370
  *   l2o_adam_step                       tf.train.AdamOptimizer(lr).minimize            DM/meta.py:411-413
  *   l2o_log_and_sign                    preprocess.LogAndSign                          DM/preprocess.py:52-70
  *   l2o_lasso_grad                      problems.lasso(_fixed) loss + tf.gradients     DM/problems.py:103-175, DM/meta.py:322-329
@@ -152,9 +154,22 @@ int64_t l2o_state_floats(l2o_handle h); /* per coordinate: 2*sum(H_l) */
  * The library itself allocates nothing per call (only a per-net weight image of < 100 KB at first tensor-core use). */
 int l2o_workspace_bytes(l2o_handle h, int64_t n, int32_t T, size_t* fwd_bytes, size_t* bwd_bytes);
 
+/* Boundary conditions of a BPTT sweep over one segment [t0, t1) of a longer unroll (segmented BPTT: the caller keeps
+ * the state only at segment starts and recomputes each segment's checkpoints before its backward).  The sweep starts
+ * from these buffers instead of dh = dc = 0, lambda = g_rec[T], and writes them back when it reaches t0; one thread
+ * owns each coordinate, so the update is in place.  A zero carry over a single segment is l2o_unroll_bwd. */
+typedef struct {
+  float* d_state;   /* [state arena] in: adjoint of the state after the segment; out: before it (16-byte aligned) */
+  float* lam;       /* [n] in: sum_{tau > t1} g_tau ; out: sum_{tau > t0} g_tau */
+} l2o_bwd_carry;
+
 int l2o_step(l2o_handle h, const l2o_step_args* a, void* stream);
 int l2o_unroll_fwd(l2o_handle h, const l2o_unroll_args* a, void* stream);
 int l2o_unroll_bwd(l2o_handle h, const l2o_bwd_args* a, void* stream);
+/* l2o_unroll_bwd over one segment with carried boundary conditions: a->T is the segment length, a->ckpt its T + 1
+ * slots, a->g_rec / in_seq / delta_seq / scratch its rows (g_rec rows t0..t1).  Meta-loss mode only: imitation
+ * (a->labels) returns L2O_E_UNSUPPORTED.  Same engine choice as l2o_unroll_bwd. */
+int l2o_unroll_bwd_carry(l2o_handle h, const l2o_bwd_args* a, const l2o_bwd_carry* c, void* stream);
 
 /* TF-1.14 Adam on theta: k = 1-based step count. */
 int l2o_adam_step(float* theta, const double* dtheta, float* m, float* v, int64_t n, int32_t k, float lr,

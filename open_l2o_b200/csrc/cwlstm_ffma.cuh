@@ -489,8 +489,9 @@ struct BwdGeom {
   static constexpr size_t BYTES = (size_t)S_END * sizeof(float);
 };
 
-template <class C>
-__global__ void __launch_bounds__(kTile) unroll_bwd_kernel(l2o_bwd_args a, NetRt rt) {
+// CARRY: one segment of a longer unroll (l2o_unroll_bwd_carry): the carries start from cy and are written back there
+template <class C, bool CARRY>
+__global__ void __launch_bounds__(kTile) unroll_bwd_kernel(l2o_bwd_args a, NetRt rt, l2o_bwd_carry cy) {
   using B = BwdGeom<C>;
   static_assert(!(C::FC && C::H1 == 0), "fc preprocessing needs at least one LSTM layer");
   extern __shared__ __align__(16) float smem[];
@@ -529,6 +530,19 @@ __global__ void __launch_bounds__(kTile) unroll_bwd_kernel(l2o_bwd_args a, NetRt
 #pragma unroll
     for (int k = 0; k < cmax(C::H2, 1); ++k) { dh2c[k] = 0.f; dc2c[k] = 0.f; }
     float lam = (act && a.g_rec) ? a.g_rec[(int64_t)T * n + i] : 0.f;
+    if constexpr (CARRY) {   // the adjoint of the state after the segment, and lambda = carry + g_t1 (same order)
+      if (act) {
+        if constexpr (C::H1 > 0) {
+          load_vec<C::H1>(cy.d_state + i * C::H1, dh1c);
+          load_vec<C::H1>(cy.d_state + (n + i) * C::H1, dc1c);
+        }
+        if constexpr (C::H2 > 0) {
+          load_vec<C::H2>(cy.d_state + 2 * n * C::H1 + i * C::H2, dh2c);
+          load_vec<C::H2>(cy.d_state + 2 * n * C::H1 + (n + i) * C::H2, dc2c);
+        }
+        lam = cy.lam[i] + a.g_rec[(int64_t)T * n + i];
+      }
+    }
 
     for (int t = T - 1; t >= 0; --t) {
       // ---------------- phase A: forward recompute + out layer + layer-2 backward ----------------
@@ -649,7 +663,8 @@ __global__ void __launch_bounds__(kTile) unroll_bwd_kernel(l2o_bwd_args a, NetRt
           *reinterpret_cast<float4*>(myDZO) = make_float4(dy, 0.f, 0.f, 0.f);
         }
         (void)top; (void)dtop;
-        if (a.g_rec) lam += a.g_rec[(int64_t)t * n + i];
+        // a segment hands sum_{tau > t0} on: g_t0 is the previous segment's last row
+        if (a.g_rec && (!CARRY || t > 0)) lam += a.g_rec[(int64_t)t * n + i];
       } else {
         float zrow[B::INS];
 #pragma unroll
@@ -735,6 +750,19 @@ __global__ void __launch_bounds__(kTile) unroll_bwd_kernel(l2o_bwd_args a, NetRt
         dw_pass<B::KR1, cmax(C::G1, 4), B::INS, B::DZS>(sIN, sDZ, sACC + B::ACC1 * kTile, tid);
         if constexpr (C::FC) dw_pass<B::KRF, cmax(C::F, 4), B::INF, B::DZF>(sINF, sDZF, sACC + B::ACCF * kTile, tid);
         __syncthreads();
+      }
+    }
+    if constexpr (CARRY) {
+      if (act) {
+        if constexpr (C::H1 > 0) {
+          store_vec<C::H1>(cy.d_state + i * C::H1, dh1c);
+          store_vec<C::H1>(cy.d_state + (n + i) * C::H1, dc1c);
+        }
+        if constexpr (C::H2 > 0) {
+          store_vec<C::H2>(cy.d_state + 2 * n * C::H1 + i * C::H2, dh2c);
+          store_vec<C::H2>(cy.d_state + 2 * n * C::H1 + (n + i) * C::H2, dc2c);
+        }
+        cy.lam[i] = lam;
       }
     }
   }

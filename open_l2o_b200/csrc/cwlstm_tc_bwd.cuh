@@ -132,9 +132,11 @@ __host__ __device__ constexpr size_t bwd_smem_bytes() {
 }
 
 // MODE 0: both layers (DM nets); 1: layer 2 only, dX2[h1n] exported to a.scratch [T][n][20]; 2: layer 1 of an fc net,
-// dX2[h1n] read from a.scratch.
-template <class C, int MODE>
-__global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args a, NetRt rt, const float* __restrict__ img) {
+// dX2[h1n] read from a.scratch.  CARRY: one segment of a longer unroll (l2o_unroll_bwd_carry); the pass's carries (layer 2
+// and lambda, layer 1) start from cy and are written back there.
+template <class C, int MODE, bool CARRY>
+__global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args a, NetRt rt, const float* __restrict__ img,
+                                                                    l2o_bwd_carry cy) {
   using G = Geo<C>;
   static_assert(MODE == 0 ? !C::FC : C::FC, "DM nets: one pass; fc nets: two passes");
   static_assert(MODE != 0 || C::F < 3, "the feature chunk leaves quad thread 3's slot of row 63 to layer 2's 1");
@@ -321,6 +323,22 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
     float lam[2];
 #pragma unroll
     for (int rh = 0; rh < 2; ++rh) lam[rh] = (kL2 && act[rh] && !imit) ? a.g_rec[(int64_t)T * n + row[rh]] : 0.f;
+    if constexpr (CARRY) {   // state arena [h1 | c1 | h2 | c2][n][20]; lambda = carry + g_t1 (the order of a whole sweep)
+#pragma unroll
+      for (int rh = 0; rh < 2; ++rh) {
+        if (!act[rh]) continue;
+        const int64_t i = row[rh];
+        if constexpr (kL2) {
+          load5(cy.d_state + (2 * n + i) * kH, q, dh2c[rh]);
+          load5(cy.d_state + (3 * n + i) * kH, q, dc2[rh]);
+          lam[rh] = cy.lam[i] + a.g_rec[(int64_t)T * n + i];
+        }
+        if constexpr (kL1) {
+          load5(cy.d_state + i * kH, q, dh1c[rh]);
+          load5(cy.d_state + (n + i) * kH, q, dc1[rh]);
+        }
+      }
+    }
     A.zero();
     A.template put<(G::ColOne & ~3)>(0, q == (G::ColOne & 3) ? 1.0f : 0.f);
     A.template put<(G::ColOne & ~3)>(1, q == (G::ColOne & 3) ? 1.0f : 0.f);
@@ -408,7 +426,7 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
         }
 #pragma unroll
         for (int rh = 0; rh < 2; ++rh)
-          if (!imit && act[rh]) lam[rh] += a.g_rec[(int64_t)t * n + row[rh]];
+          if (!imit && act[rh] && (!CARRY || t > 0)) lam[rh] += a.g_rec[(int64_t)t * n + row[rh]];   // g_t0: the previous segment's
       }
       // ================================= layer 1 =================================
       if constexpr (kL1) {
@@ -514,6 +532,22 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
           }
       }
     }
+    if constexpr (CARRY) {
+#pragma unroll
+      for (int rh = 0; rh < 2; ++rh) {
+        if (!act[rh]) continue;
+        const int64_t i = row[rh];
+        if constexpr (kL2) {
+          store5(cy.d_state + (2 * n + i) * kH, q, dh2c[rh]);
+          store5(cy.d_state + (3 * n + i) * kH, q, dc2[rh]);
+          if (q == 0) cy.lam[i] = lam[rh];
+        }
+        if constexpr (kL1) {
+          store5(cy.d_state + i * kH, q, dh1c[rh]);
+          store5(cy.d_state + (n + i) * kH, q, dc1[rh]);
+        }
+      }
+    }
     flush_dw();
   }
   wg_wait<0>();
@@ -547,8 +581,9 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
 
 }  // namespace tcb
 
-template <class C>
-int tc_launch_bwd(const NetRt& rt, const l2o_bwd_args& a, float* img, cudaStream_t st, int sms, bool prep = true) {
+template <class C, bool CARRY>
+int tc_launch_bwd(const NetRt& rt, const l2o_bwd_args& a, float* img, cudaStream_t st, int sms, const l2o_bwd_carry& cy,
+                  bool prep = true) {
   if (prep) tc::prep_weights_kernel<C><<<16, 256, 0, st>>>(a.theta, img, 1);
   const int64_t ntiles = (a.n + tc::kTile - 1) / tc::kTile;
   const int64_t ctas = (ntiles + tcb::kBwdWG - 1) / tcb::kBwdWG;
@@ -556,16 +591,16 @@ int tc_launch_bwd(const NetRt& rt, const l2o_bwd_args& a, float* img, cudaStream
   auto launch = [&](auto kern, size_t smem) {
     if (smem > 227 * 1024) return L2O_E_INVALID;
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return L2O_E_CUDA;
-    kern<<<grid, tcb::kBwdThreads, smem, st>>>(a, rt, img);
+    kern<<<grid, tcb::kBwdThreads, smem, st>>>(a, rt, img, cy);
     return cudaGetLastError() == cudaSuccess ? L2O_OK : L2O_E_CUDA;
   };
   if constexpr (C::FC) {
     // two passes over time: layer 2 (exporting dX2[h1n] to a.scratch), then layer 1 fed by it
-    int rc = launch(tcb::unroll_bwd_kernel<C, 1>, tcb::bwd_smem_bytes<C, 1>());
+    int rc = launch(tcb::unroll_bwd_kernel<C, 1, CARRY>, tcb::bwd_smem_bytes<C, 1>());
     if (rc != L2O_OK) return rc;
-    return launch(tcb::unroll_bwd_kernel<C, 2>, tcb::bwd_smem_bytes<C, 2>());
+    return launch(tcb::unroll_bwd_kernel<C, 2, CARRY>, tcb::bwd_smem_bytes<C, 2>());
   } else {
-    return launch(tcb::unroll_bwd_kernel<C, 0>, tcb::bwd_smem_bytes<C, 0>());
+    return launch(tcb::unroll_bwd_kernel<C, 0, CARRY>, tcb::bwd_smem_bytes<C, 0>());
   }
 }
 

@@ -174,6 +174,24 @@ int l2o_unroll_bwd(l2o_handle h, const l2o_bwd_args* a, void* stream) {
   return l2o::ffma_unroll_bwd(h, *a, st);
 }
 
+int l2o_unroll_bwd_carry(l2o_handle h, const l2o_bwd_args* a, const l2o_bwd_carry* c, void* stream) {
+  if (!h || !a || !c || a->n < 0 || a->T < 0 || !a->theta || !a->dtheta) return L2O_E_INVALID;
+  if (a->T > 0 && !a->in_seq) return L2O_E_INVALID;
+  if (h->state_floats > 0 && (!a->ckpt || !c->d_state)) return L2O_E_INVALID;
+  // the FFMA engine moves checkpoint and adjoint-state rows as float4, the tensor-core engine copies checkpoints by TMA
+  if (reinterpret_cast<uintptr_t>(a->ckpt) % 16 != 0 || reinterpret_cast<uintptr_t>(c->d_state) % 16 != 0)
+    return L2O_E_INVALID;
+  if (!c->lam) return L2O_E_INVALID;
+  if (!a->g_rec && (!a->labels || a->n_total <= 0)) return L2O_E_INVALID;
+  if (a->labels) return L2O_E_UNSUPPORTED;   // imitation losses have no lambda to carry
+  if (a->n == 0 || a->T == 0) return L2O_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool tc_can = l2o::tc_bwd_ok(h, *a);
+  if (h->engine == L2O_ENGINE_TC) return tc_can ? l2o::tc_unroll_bwd(h, *a, st, c) : L2O_E_UNSUPPORTED;
+  if (h->engine == L2O_ENGINE_AUTO && tc_can && l2o::tc_bwd_auto_default()) return l2o::tc_unroll_bwd(h, *a, st, c);
+  return l2o::ffma_unroll_bwd(h, *a, st, c);
+}
+
 int l2o_adam_step(float* theta, const double* dtheta, float* m, float* v, int64_t n, int32_t k, float lr, float beta1,
                   float beta2, float eps, void* stream) {
   if (!theta || !dtheta || !m || !v || n < 0 || k < 1) return L2O_E_INVALID;

@@ -44,7 +44,8 @@ inline bool overlaps_any(const void* p, size_t bytes, const void* const* q, cons
 
 int ffma_step(const l2o_net* h, const l2o_step_args& a, cudaStream_t st);
 int ffma_unroll_fwd(const l2o_net* h, const l2o_unroll_args& a, cudaStream_t st);
-int ffma_unroll_bwd(const l2o_net* h, const l2o_bwd_args& a, cudaStream_t st);
+// c: the boundary conditions of a segmented sweep (l2o_unroll_bwd_carry), null for a whole unroll
+int ffma_unroll_bwd(const l2o_net* h, const l2o_bwd_args& a, cudaStream_t st, const l2o_bwd_carry* c = nullptr);
 
 bool tc_supported(int cfg);
 void tc_release_image(l2o_net* h);   // hand the weight image back to the process-wide pool (never cudaFree)
@@ -55,7 +56,7 @@ int tc_step(l2o_net* h, const l2o_step_args& a, cudaStream_t st);
 bool tc_auto_default();
 bool tc_bwd_auto_default();
 bool tc_bwd_ok(const l2o_net* h, const l2o_bwd_args& a);
-int tc_unroll_bwd(l2o_net* h, const l2o_bwd_args& a, cudaStream_t st);
+int tc_unroll_bwd(l2o_net* h, const l2o_bwd_args& a, cudaStream_t st, const l2o_bwd_carry* c = nullptr);
 }  // namespace l2o
 
 #define L2O_CUDA_TRY(expr)                                              \

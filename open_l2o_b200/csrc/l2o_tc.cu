@@ -76,16 +76,22 @@ bool tc_bwd_ok(const l2o_net* h, const l2o_bwd_args& a) {
   return tc_supported(h->cfg) && mode_ok;
 }
 
-int tc_unroll_bwd(l2o_net* h, const l2o_bwd_args& a, cudaStream_t st) {
+template <class C>
+static int tc_launch_bwd_any(const l2o_net* h, const l2o_bwd_args& a, cudaStream_t st, int sms, const l2o_bwd_carry* c) {
+  return c ? tc_launch_bwd<C, true>(h->rt, a, h->tc_img, st, sms, *c)
+           : tc_launch_bwd<C, false>(h->rt, a, h->tc_img, st, sms, l2o_bwd_carry{});
+}
+
+int tc_unroll_bwd(l2o_net* h, const l2o_bwd_args& a, cudaStream_t st, const l2o_bwd_carry* c) {
   if (!tc_bwd_ok(h, a)) return L2O_E_UNSUPPORTED;
   int rc = ensure_image(h);
   if (rc) return rc;
   const int sms = device_sms();
   if (sms <= 0) return L2O_E_CUDA;
   rc = L2O_E_UNSUPPORTED;
-  if (h->cfg == 0) rc = tc_launch_bwd<Cfg<L2O_PRE_IDENTITY, 1, 1, 20, 20>>(h->rt, a, h->tc_img, st, sms);
-  if (h->cfg == 1) rc = tc_launch_bwd<Cfg<L2O_PRE_LOGSIGN, 1, 2, 20, 20>>(h->rt, a, h->tc_img, st, sms);
-  if (h->cfg == 2) rc = tc_launch_bwd<Cfg<L2O_PRE_FC, 2, 20, 20, 20>>(h->rt, a, h->tc_img, st, sms);
+  if (h->cfg == 0) rc = tc_launch_bwd_any<Cfg<L2O_PRE_IDENTITY, 1, 1, 20, 20>>(h, a, st, sms, c);
+  if (h->cfg == 1) rc = tc_launch_bwd_any<Cfg<L2O_PRE_LOGSIGN, 1, 2, 20, 20>>(h, a, st, sms, c);
+  if (h->cfg == 2) rc = tc_launch_bwd_any<Cfg<L2O_PRE_FC, 2, 20, 20, 20>>(h, a, st, sms, c);
   if (rc == L2O_OK) count_launch(h->cfg == 2 ? 3 : 2);
   h->tc_img_mode = 1;
   if (rc == L2O_E_CUDA) return set_cuda_error(cudaGetLastError(), "tc_unroll_bwd launch");

@@ -164,6 +164,21 @@ class NetHandle(_Handle):
         """BPTT over the T checkpoint slots.  ``scratch`` ([T, n, 20] floats) lets fc(20) nets (RNNProp) run on the
         tensor-core engine; ``delta_seq`` (the deltas the forward pass recorded) is what a tanh-output net's
         tensor-core BPTT differentiates the output layer with."""
+        a = self._bwd_args(theta, n, T, in_seq, ckpt, dtheta, g_rec, labels, n_total, delta_seq, scratch)
+        _lib.check(_lib.lib().l2o_unroll_bwd(self._h, C.byref(a), _stream()), "l2o_unroll_bwd")
+
+    def unroll_bwd_carry(self, theta, n, T, in_seq, ckpt, dtheta, d_state, lam, *, g_rec, delta_seq=None,
+                         scratch=None):
+        """BPTT over one T-step segment of a longer unroll: ``ckpt`` holds the segment's T + 1 slots and ``g_rec`` its
+        rows t0..t1.  ``d_state`` (a state arena, the adjoint of the state after the segment) and ``lam`` ([n],
+        sum_{tau > t1} g_tau) are updated in place to the adjoint of the state before it and sum_{tau > t0} g_tau."""
+        a = self._bwd_args(theta, n, T, in_seq, ckpt, dtheta, g_rec, None, 0, delta_seq, scratch)
+        c = _lib.BwdCarry()
+        c.d_state, c.lam = _ptr(d_state, name="d_state"), _ptr(lam, name="lam")
+        _lib.check(_lib.lib().l2o_unroll_bwd_carry(self._h, C.byref(a), C.byref(c), _stream()), "l2o_unroll_bwd_carry")
+
+    @staticmethod
+    def _bwd_args(theta, n, T, in_seq, ckpt, dtheta, g_rec, labels, n_total, delta_seq, scratch):
         a = BwdArgs()
         a.n, a.T = n, T
         a.theta = _ptr(theta, name="theta")
@@ -175,7 +190,7 @@ class NetHandle(_Handle):
         if scratch is not None and scratch.numel() < T * n * 20:
             raise L2OError(f"scratch has {scratch.numel()} floats, the fc-net BPTT needs T*n*20 = {T * n * 20}")
         a.scratch = _ptr(scratch, name="scratch")
-        _lib.check(_lib.lib().l2o_unroll_bwd(self._h, C.byref(a), _stream()), "l2o_unroll_bwd")
+        return a
 
 
 class DenseNetHandle(_Handle):

@@ -149,6 +149,70 @@ def plan_arena(variables, subsets, net_keys, nets):
     return [slice(off[j], off[j] + sizes[j]) for j in range(len(variables))], N, runs
 
 
+SegmentPlan = collections.namedtuple("SegmentPlan", "S bounds bytes")
+
+
+def plan_segments(T, slot_floats, n, free_bytes=None, *, S=None, boundary_floats=0, step_floats=0, fixed_bytes=0,
+                  headroom=0.9):
+    """How the BPTT of a T-step unroll keeps the states it differentiates through.  ``slot_floats``: one checkpoint slot
+    (every segmented run's state arena); ``n``: their coordinates (the carried lambda); ``boundary_floats``: what a
+    segment start saves besides the state (the fused regime's x, RNNProp's m and v); ``step_floats``: floats per step of
+    the buffers the backward sizes by its sweep length (RNNProp's tensor-core hand-over buffer); ``fixed_bytes``: what
+    the program allocates either way.
+
+    Full checkpoints (S = T) when they fit in ``headroom`` of ``free_bytes`` (None: always); otherwise segments of the
+    S that minimises ceil(T/S) + S, and L2OError when even those do not fit.  ``S`` forces the segment length.  Returns
+    SegmentPlan(S, bounds [0, S, 2S, ..., T], bytes per buffer): "ckpt" (S + 1 slots: the whole unroll's, or the one
+    segment the backward recomputes), "handover" (S steps), and when segmented "boundary" (the state at every bound and
+    the extras at every segment start) and "recompute" (the scratch copies a recompute runs on, and the carry)."""
+    T = int(T)
+
+    def plan(s):
+        s = min(max(int(s), 1), max(T, 1))
+        bounds = list(range(0, T, s)) + [T]
+        b = {"ckpt": 4 * (s + 1) * slot_floats, "handover": 4 * s * step_floats}
+        if s < T:
+            nseg = len(bounds) - 1
+            b["boundary"] = 4 * ((nseg + 1) * slot_floats + nseg * boundary_floats)
+            b["recompute"] = 4 * (2 * slot_floats + boundary_floats + n)
+        return SegmentPlan(s, bounds, b)
+
+    if S is not None:
+        return plan(S)
+    full = plan(T)
+    if free_bytes is None or fixed_bytes + sum(full.bytes.values()) <= headroom * free_bytes:
+        return full
+    seg = plan(min(range(1, T + 1), key=lambda s: (-(-T // s) + s, s)))
+    need = fixed_bytes + sum(seg.bytes.values())
+    if need > headroom * free_bytes:
+        raise _engine.L2OError("the unroll needs {:.3g} GB even with BPTT segments of {} steps ({}), {:.3g} GB of {:.3g} GB "
+                               "free may be used".format(need / 1e9, seg.S, seg.bytes, headroom * free_bytes / 1e9,
+                                                         free_bytes / 1e9))
+    return seg
+
+
+def bptt_buffers(plan, runs, N, fused):
+    """The BPTT buffers _Program allocates for ``plan``, under the plan's byte keys: {key: [(owner, name, shape)]},
+    owner a run index or None (the program).  ``runs``: (slot floats, n, RNNProp moments, hand-over buffer) per
+    segmented run; ``N``: the arena the fused regime saves x of."""
+    S, nseg = plan.S, len(plan.bounds) - 1
+    out = collections.defaultdict(list)
+    for i, (slot, n, moments, handover) in enumerate(runs):
+        out["ckpt"].append((i, "ckpt", ((S + 1) * slot,)))
+        if handover:
+            out["handover"].append((i, "bwd_scratch", (S, n, 20)))
+        if nseg > 1:
+            out["boundary"].append((i, "bstate", (nseg + 1, slot)))
+            out["recompute"] += [(i, "rstate", (slot,)), (i, "d_state", (slot,)), (i, "lam", (n,))]
+            if moments:
+                out["boundary"].append((i, "bmv", (nseg, 2, n)))
+                out["recompute"].append((i, "mv", (2, n)))
+    if nseg > 1 and fused:
+        out["boundary"].append((None, "bx", (nseg, N)))
+        out["recompute"].append((None, "x_scr", (N,)))
+    return dict(out)
+
+
 def _adam_slots(nets):
     return {k: dict(m=torch.zeros_like(net.theta), v=torch.zeros_like(net.theta), k=0) for k, net in nets.items()}
 
@@ -209,17 +273,19 @@ class _Program(object):
         self.mt_tasks = []
         self.unroll_idx = 0
         self._graphs, self._eager_calls, self._graph_failed, self._graph_kernels = {}, {}, False, {}
-        self._alloc_workspaces()
+        self._alloc_workspaces(optimizer.bptt_segment)
         self.reset()
 
     # ---- memory ---------------------------------------------------------------------------------
-    def _alloc_workspaces(self):
+    def _alloc_workspaces(self, segment=None):
+        """``segment``: force BPTT segments of that many steps (tests); otherwise full checkpoints when they fit in the
+        free device memory, segments otherwise (plan_segments)."""
         T = self.T
+        fixed = 0
         for r in self.runs:
             h = r.net.handle
             r.slot = max(h.state_size(r.n), 1)   # floats of one checkpoint slot
             r.state = h.new_state(r.n, self.device)
-            r.ckpt = torch.zeros((T + 1) * r.slot, device=self.device)
             r.g_rec = torch.zeros(T + 1, r.n, device=self.device)
             if h.n_in == 2:
                 r.m = torch.zeros(r.n, device=self.device)
@@ -231,8 +297,29 @@ class _Program(object):
             r.delta_rec = r.bwd_scratch = None
             if getattr(r.net, "tanh_output", False) and isinstance(h, _engine.NetHandle):
                 r.delta_rec = torch.zeros(T, r.n, device=self.device)
-            if h.n_in == 2 and isinstance(h, _engine.NetHandle) and tuple(h.layers) == (20, 20):
-                r.bwd_scratch = torch.zeros(T, r.n, 20, device=self.device)
+            r.handover = h.n_in == 2 and isinstance(h, _engine.NetHandle) and tuple(h.layers) == (20, 20)
+            # the dense engine (KernelDeepLSTM) has no segmented BPTT: its runs keep full checkpoints
+            r.seg_ok = isinstance(h, _engine.NetHandle)
+            fixed += 4 * (r.state.numel() + r.g_rec.numel() + (5 * r.n + 2 * T * r.n if h.n_in == 2 else 0) +
+                          (T * r.n if r.delta_rec is not None else 0))
+            if not r.seg_ok:
+                r.ckpt = torch.zeros((T + 1) * r.slot, device=self.device)
+                fixed += 4 * r.ckpt.numel()
+        seg_runs = [r for r in self.runs if r.seg_ok]
+        fused_N = self.N if self.fused is not None else 0
+        free = None if segment is not None else torch.cuda.mem_get_info(self.device)[0]
+        self.plan = plan_segments(T, sum(r.slot for r in seg_runs), sum(r.n for r in seg_runs), free, S=segment,
+                                  boundary_floats=fused_N + sum(2 * r.n for r in seg_runs if r.net.handle.n_in == 2),
+                                  step_floats=sum(20 * r.n for r in seg_runs if r.handover),
+                                  fixed_bytes=fixed + 4 * 3 * self.N)
+        self.segmented = len(self.plan.bounds) > 2
+        self._bound_index = {t: k for k, t in enumerate(self.plan.bounds)}
+        spec = [(r.slot, r.n, r.net.handle.n_in == 2, r.handover) for r in seg_runs]
+        for bufs in bptt_buffers(self.plan, spec, self.N, self.fused is not None).values():
+            for owner, name, shape in bufs:
+                setattr(self if owner is None else seg_runs[owner], name, torch.zeros(shape, device=self.device))
+        for r in self.runs:
+            r.seg = self.segmented and r.seg_ok
         self._Xw = torch.zeros(self.N, device=self.device)   # x after the last unroll, committed by `update`
         self.fx_buf = torch.zeros(T + 1, dtype=torch.float64, device=self.device)
 
@@ -366,44 +453,100 @@ class _Program(object):
             r.m_work.copy_(r.m)
             r.v_work.copy_(r.v)
 
+    def _fused_unroll(self, r, t0, t1, state, x, m, v, ckpt, fx, train):
+        """The fused forward kernel over steps t0..t1 from (state, x, m, v), updated in place; records rows t0.. of
+        g_rec (and RNNProp's features, the deltas) and adds f(x_t) to fx[t - t0]."""
+        f, h = self.fused, r.net.handle
+        kw = self._moments(m, v, step0=self._fused_step0 + t0, feat_rec=r.feat_rec[t0:]) if h.n_in == 2 else {}
+        if train and r.delta_rec is not None:
+            kw["delta_seq"] = r.delta_rec[t0:]
+        h.unroll_fwd(r.net.theta, r.n, t1 - t0, state, opt_kind=_engine.OPT_KINDS[f.kind],
+                     opt_a=self.const_vals[f.a].reshape(-1), opt_b=self.const_vals[f.b].reshape(-1),
+                     opt_alpha=f.alpha, opt_fscale=f.fscale, x=x, ckpt=ckpt, g_rec=r.g_rec[t0:], fx=fx,
+                     opt_group=getattr(f, "group", 0), **kw)
+
     def _forward_fused(self, train, step0):
-        r, T, f = self.runs[0], self.T, self.fused
-        h = r.net.handle
+        r, T = self.runs[0], self.T
+        self._fused_regime, self._fused_step0 = True, step0
         self._Xw.copy_(self.X)
         work_state = r.state.clone()
         self.fx_buf.zero_()
         self._load_moments(r)
-        kw = self._moments(r.m_work, r.v_work, step0=step0, feat_rec=r.feat_rec) if h.n_in == 2 else {}
-        if train and r.delta_rec is not None:
-            kw["delta_seq"] = r.delta_rec
-        h.unroll_fwd(r.net.theta, r.n, T, work_state, opt_kind=_engine.OPT_KINDS[f.kind],
-                     opt_a=self.const_vals[f.a].reshape(-1), opt_b=self.const_vals[f.b].reshape(-1),
-                     opt_alpha=f.alpha, opt_fscale=f.fscale, x=self._Xw, ckpt=r.ckpt if train else None,
-                     g_rec=r.g_rec, fx=self.fx_buf, opt_group=getattr(f, "group", 0), **kw)
+        m, v = (r.m_work, r.v_work) if r.net.handle.n_in == 2 else (None, None)
+        if train and r.seg:
+            # one launch per segment, the state, x (and m, v) carried through HBM between them and saved at each
+            # segment start; f(x_t0) of a later segment replaces the earlier segment's last row
+            for k, (t0, t1) in enumerate(zip(self.plan.bounds[:-1], self.plan.bounds[1:])):
+                r.bstate[k].copy_(work_state)
+                self.bx[k].copy_(self._Xw)
+                if m is not None:
+                    r.bmv[k, 0].copy_(m)
+                    r.bmv[k, 1].copy_(v)
+                if k > 0:
+                    self.fx_buf[t0].zero_()
+                self._fused_unroll(r, t0, t1, work_state, self._Xw, m, v, None, self.fx_buf[t0:], train)
+        else:
+            self._fused_unroll(r, 0, T, work_state, self._Xw, m, v, r.ckpt if train else None, self.fx_buf, train)
         r.state_final = work_state
         return self.fx_buf
 
+    def _recompute(self, r, k):
+        """Checkpoint slots 0..t1-t0 of segment k into r.ckpt, with the kernel and mode of the forward that ran, from
+        scratch copies of what it saved at t0 (the boundary store and the committed x stay untouched)."""
+        t0, t1 = self.plan.bounds[k], self.plan.bounds[k + 1]
+        h, slot = r.net.handle, r.slot
+        m = v = None
+        if h.n_in == 2:
+            r.mv.copy_(r.bmv[k])
+            m, v = r.mv[0], r.mv[1]
+        if self._fused_regime:
+            r.rstate.copy_(r.bstate[k])
+            self.x_scr.copy_(self.bx[k])
+            self._fused_unroll(r, t0, t1, r.rstate, self.x_scr, m, v, r.ckpt, None, True)
+            return
+        r.ckpt[:slot].copy_(r.bstate[k])
+        for t in range(t0, t1):
+            kw = self._moments(m, v, step_ptr=self.step_dev, t_offset=t) if h.n_in == 2 else {}
+            j = t - t0
+            h.step(r.net.theta, r.g_rec[t], r.ckpt[j * slot:(j + 1) * slot], r.ckpt[(j + 1) * slot:(j + 2) * slot],
+                   reuse_weights=(j > 0), **kw)
+
+    def _state_slot(self, r, t):
+        """Where the external-gradient forward keeps run r's state before step t: its checkpoint slot; segmented, the
+        boundary store at a segment start and otherwise one of two rolling slots (the recompute scratch)."""
+        slot = r.slot
+        if not r.seg:
+            return r.ckpt[t * slot:(t + 1) * slot]
+        k = self._bound_index.get(t)
+        if k is not None:
+            return r.bstate[k]
+        return r.ckpt[(t % 2) * slot:(t % 2 + 1) * slot]
+
     def _forward_external(self, train, step0):
         T, Xw = self.T, self._Xw
+        self._fused_regime = False
         Xw.copy_(self.X)
         fxs = []
         for r in self.runs:
-            r.ckpt[:r.slot].copy_(r.state)
+            self._state_slot(r, 0).copy_(r.state)
             self._load_moments(r)
         for t in range(T):
             fx, g = self._value_and_grad(Xw)
             fxs.append(fx)
             for r in self.runs:
-                h, slot = r.net.handle, r.slot
+                h = r.net.handle
                 r.g_rec[t].copy_(g[r.off:r.off + r.n])
                 kw = {}
                 if h.n_in == 2:
+                    if r.seg and t in self._bound_index:   # the moments a recompute of this segment starts from
+                        r.bmv[self._bound_index[t], 0].copy_(r.m_work)
+                        r.bmv[self._bound_index[t], 1].copy_(r.v_work)
                     kw = self._moments(r.m_work, r.v_work, step_ptr=self.step_dev, t_offset=t, feat_out=r.feat_rec[t])
                 if train and r.delta_rec is not None:
                     kw["delta"] = r.delta_rec[t]
                 # theta is constant inside an unroll: the weight image built at t = 0 serves every later step (runs that
                 # share a net share its handle, so only the first run of step 0 rebuilds)
-                h.step(r.net.theta, r.g_rec[t], r.ckpt[t * slot:(t + 1) * slot], r.ckpt[(t + 1) * slot:(t + 2) * slot],
+                h.step(r.net.theta, r.g_rec[t], self._state_slot(r, t), self._state_slot(r, t + 1),
                        x=Xw[r.off:r.off + r.n], reuse_weights=(t > 0), **kw)
         if train:
             fx, g = self._value_and_grad(Xw)
@@ -417,7 +560,7 @@ class _Program(object):
                     fx = self._loss_at(Xw)
         fxs.append(fx)
         for r in self.runs:
-            r.state_final = r.ckpt[T * r.slot:(T + 1) * r.slot]
+            r.state_final = self._state_slot(r, T)
         return torch.stack([f.reshape(()).double() for f in fxs])
 
     # ---- CUDA-graph path of the external-gradient regime ------------------------------------------------
@@ -435,8 +578,20 @@ class _Program(object):
         for r in self.runs:
             h = r.net.handle
             in_seq = r.feat_rec if h.n_in == 2 else r.g_rec
-            h.unroll_bwd(r.net.theta, r.n, self.T, in_seq, r.ckpt, self.dtheta[r.key], g_rec=r.g_rec,
-                         **self._bwd_extra(r))
+            if not r.seg:
+                h.unroll_bwd(r.net.theta, r.n, self.T, in_seq, r.ckpt, self.dtheta[r.key], g_rec=r.g_rec,
+                             **self._bwd_extra(r))
+                continue
+            # last segment first: recompute its checkpoints, then BPTT over them from the carried adjoint state and
+            # lambda suffix sum (zero after the last step)
+            r.d_state.zero_()
+            r.lam.zero_()
+            for k in reversed(range(len(self.plan.bounds) - 1)):
+                t0, t1 = self.plan.bounds[k], self.plan.bounds[k + 1]
+                self._recompute(r, k)
+                kw = {} if r.delta_rec is None else {"delta_seq": r.delta_rec[t0:]}
+                h.unroll_bwd_carry(r.net.theta, r.n, t1 - t0, in_seq[t0:], r.ckpt, self.dtheta[r.key], r.d_state, r.lam,
+                                   g_rec=r.g_rec[t0:], scratch=r.bwd_scratch, **kw)
 
     @staticmethod
     def _bwd_extra(r):
@@ -569,6 +724,8 @@ class _MtTask(object):
             if h.n_in == 2:   # RNNProp: the task carries its own Adam moments (DM/meta_rnnprop_train.py:469-486)
                 sb.update(m=torch.zeros(r.n, device=prog.device), v=torch.zeros(r.n, device=prog.device),
                           feat=torch.zeros(T, 2, r.n, device=prog.device))
+            if r.bwd_scratch is not None and prog.segmented:   # imitation keeps whole-unroll BPTT: a T-step hand-over
+                sb["scratch"] = torch.zeros(T, r.n, 20, device=prog.device)
             self.subsets.append(sb)
         self.n_total = sum(sb["n"] for sb in self.subsets)
         self.adam = _adam_slots(prog.nets)
@@ -607,8 +764,11 @@ class _MtTask(object):
             h.unroll_fwd(r.net.theta, n, T, work, in_seq=inp, ckpt=sb["ckpt"] if train else None, labels=lab,
                          imit_loss=self.il, n_total=self.n_total, delta_seq=sb["dseq"] if train else None, **kw)
             if train:  # the recorded deltas let the tensor-core BPTT run in imitation mode too
+                extra = dict(prog._bwd_extra(r), delta_seq=sb["dseq"])
+                if "scratch" in sb:
+                    extra["scratch"] = sb["scratch"]
                 h.unroll_bwd(r.net.theta, n, T, in_seq, sb["ckpt"], prog.dtheta[r.key], labels=lab, n_total=self.n_total,
-                             **dict(prog._bwd_extra(r), delta_seq=sb["dseq"]))
+                             **extra)
             finals.append((work, moments))
         out = {}
         if "loss_mt" in kinds:
@@ -640,6 +800,8 @@ class MetaOptimizer(object):
         self._nets = None
         self.seed = int(kwargs.pop("_seed", 0))
         self.distributed = bool(kwargs.pop("_distributed", False))
+        # BPTT segment length (steps); None: full checkpoints whenever they fit in device memory (plan_segments)
+        self.bptt_segment = kwargs.pop("_bptt_segment", None)
         if not kwargs:
             # default coordinatewise network (DM/meta.py:244-255)
             self._config = {
