@@ -17,6 +17,7 @@
 // Semantics: SURVEY.md Appendix B (derived from DM/meta.py:319-376, second_derivatives=False); imitation mode
 // DM/meta_dm_train.py:472-475.
 #pragma once
+#include <type_traits>
 #include "cwlstm_tc.cuh"
 
 namespace l2o {
@@ -131,18 +132,30 @@ __host__ __device__ constexpr size_t bwd_smem_bytes() {
          (size_t)kBwdWG * (stage_bytes<C, MODE>() + (MODE == 0 ? sizeof(CkRing) : 0));
 }
 
+// Output-layer flags of an instantiation (FL), fixed at launch from the arguments: imitation mode (a.labels, the
+// gradient of the output comes from delta_seq - labels) and a tanh output (rt.tanh_output, tanh' from delta_seq).  The
+// plain instantiation (FL = 0) never reads delta_seq or labels.
+constexpr int kFlImit = 1, kFlTanh = 2;
+
 // MODE 0: both layers (DM nets); 1: layer 2 only, dX2[h1n] exported to a.scratch [T][n][20]; 2: layer 1 of an fc net,
 // dX2[h1n] read from a.scratch.  CARRY: one segment of a longer unroll (l2o_unroll_bwd_carry); the pass's carries (layer 2
-// and lambda, layer 1) start from cy and are written back there.
-template <class C, int MODE, bool CARRY>
+// and lambda, layer 1) start from cy and are written back there.  FULL (DM nets, n a multiple of 64): every tile is
+// full, so the body tests no rows.
+template <class C, int MODE, bool CARRY, int FL, bool FULL>
 __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args a, NetRt rt, const float* __restrict__ img,
                                                                     l2o_bwd_carry cy) {
   using G = Geo<C>;
   static_assert(MODE == 0 ? !C::FC : C::FC, "DM nets: one pass; fc nets: two passes");
   static_assert(MODE != 0 || C::F < 3, "the feature chunk leaves quad thread 3's slot of row 63 to layer 2's 1");
+  static_assert(MODE != 2 || FL == 0, "the output-layer flags belong to the layer-2 passes");
+  static_assert(MODE == 0 || !FULL, "the full-tile body is the DM nets'");
+  constexpr bool kImit = (FL & kFlImit) != 0, kTanh = (FL & kFlTanh) != 0;
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   SmemB<C, MODE>& S = *reinterpret_cast<SmemB<C, MODE>*>(smem_raw);
-  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  // wg through a shuffle from lane 0: provably warp-uniform, so the staging descriptors built from it live in uniform
+  // registers and feed the wgmma without a per-use copy
+  const int wg = __shfl_sync(0xffffffffu, threadIdx.x >> 7, 0);
+  const int warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
   const int g = lane >> 2, q = lane & 3;
   const uint32_t stage = smem_u32(smem_raw) + (uint32_t)((sizeof(SmemB<C, MODE>) + 1023) & ~(size_t)1023) +
                          (uint32_t)wg * stage_bytes<C, MODE>();
@@ -193,8 +206,7 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
   const int T = a.T;
   const int64_t n = a.n, slot = n * C::SF;
   const int64_t ntiles = (n + tc::kTile - 1) / tc::kTile;
-  const bool imit = a.labels != nullptr;
-  const float inv_nt = imit ? 1.0f / (float)a.n_total : 0.f;
+  const float inv_nt = kImit ? 1.0f / (float)a.n_total : 0.f;
   float wo[kU];
 #pragma unroll
   for (int s = 0; s < kU; ++s) wo[s] = S.wo[5 * q + s];
@@ -205,21 +217,24 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
   for (int k = 0; k < kN / 2; ++k) dw[k] = 0.f;
   const int kx = warp * 16 + g;   // staged coordinate index of row rh = kx + 8 rh
   const int64_t tstride = (int64_t)gridDim.x * kBwdWG;
+  // The time loop steps a pointer to the tile's block-0 checkpoint rows of slot t (a.ckpt + t slot + 64 tile kH) back
+  // by one slot per step; from slot 0 of a tile, slot T - 1 of the warpgroup's next tile is ck_wrap ahead.
+  const int64_t nkh = n * kH;
+  const int64_t ck_wrap = (int64_t)(T - 1) * slot + tstride * tc::kTile * kH;
 
   // ---- checkpoint ring (kRing): each buffer is loaded one layer phase ahead of its reader.  The elected thread
   // re-arms a buffer once a warpgroup barrier has seen every thread's reads of it.  bar2 and bar1 complete once per
   // step, so both are waited with the parity `ph` of the step count; barh twice (CkRing).
-  auto ck_block = [&](int64_t tl, int t, int blk) {   // blk 0 h1 | 1 c1 | 2 h2 | 3 c2: the tile's rows of slot t
-    return a.ckpt + (int64_t)t * slot + (blk * n + tl * tc::kTile) * kH;
+  auto ck_block = [&](const float* ckt, int blk) {   // blk 0 h1 | 1 c1 | 2 h2 | 3 c2 of the tile's slot at ckt
+    return ckt + blk * nkh;
   };
   auto tile_bytes = [&](int64_t tl) {   // the ragged last tile copies its n - 64 tl rows (a multiple of 16 bytes)
     const int64_t r = n - tl * tc::kTile;
     return (uint32_t)((r < tc::kTile ? r : tc::kTile) * kH * 4);
   };
-  auto arm = [&](uint64_t* bar, float* dst, int64_t tl, int t, int blk) {
-    const uint32_t b = tile_bytes(tl);
+  auto arm = [&](uint64_t* bar, float* dst, const float* ckt, int blk, uint32_t b) {
     mbar_expect_tx(bar, b);
-    tma_bulk_g2s(dst, ck_block(tl, t, blk), b, bar);
+    tma_bulk_g2s(dst, ck_block(ckt, blk), b, bar);
   };
   auto ring5 = [&](const float* buf, int rh, bool on, float* v) {   // this thread's 5 units of row rh of a ring buffer
     const float* p = buf + (kx + 8 * rh) * kH + 5 * q;
@@ -229,9 +244,11 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
   if constexpr (kRing) {
     const int64_t tile0 = (int64_t)blockIdx.x * kBwdWG + wg;
     if (elected && tile0 < ntiles) {
-      arm(&R.barh, R.h, tile0, T - 1, 2);
-      arm(&R.bar2, R.c2, tile0, T - 1, 3);
-      arm(&R.bar1, R.c1, tile0, T - 1, 1);
+      const float* ck0 = a.ckpt + (int64_t)(T - 1) * slot + tile0 * tc::kTile * kH;
+      const uint32_t b = tile_bytes(tile0);
+      arm(&R.barh, R.h, ck0, 2, b);
+      arm(&R.bar2, R.c2, ck0, 3, b);
+      arm(&R.bar1, R.c1, ck0, 1, b);
     }
   }
   uint32_t ph = 0;
@@ -312,9 +329,13 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
   };
 
   for (int64_t tile = (int64_t)blockIdx.x * kBwdWG + wg; tile < ntiles; tile += tstride) {
-    const int64_t r0 = tile * tc::kTile + warp * 16 + g;
+    const int64_t r0 = tile * tc::kTile + kx;
     const int64_t row[2] = {r0, r0 + 8};
-    const bool act[2] = {row[0] < n, row[1] < n};
+    const bool act[2] = {FULL || row[0] < n, FULL || row[1] < n};
+    // slot t, walked back one slot per step (see ck_wrap above): the tile's checkpoint rows and t n, the offset of
+    // step t in the [T (+1)][n] per-coordinate sequences (both warp-uniform)
+    const float* ckt = a.ckpt + (int64_t)(T - 1) * slot + tile * tc::kTile * kH;
+    int64_t tn = (int64_t)(T - 1) * n;
     float dc2[2][kU], dh2c[2][kU], dc1[2][kU], dh1c[2][kU];
 #pragma unroll
     for (int rh = 0; rh < 2; ++rh)
@@ -322,7 +343,7 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
       for (int s = 0; s < kU; ++s) { dc2[rh][s] = 0.f; dh2c[rh][s] = 0.f; dc1[rh][s] = 0.f; dh1c[rh][s] = 0.f; }
     float lam[2];
 #pragma unroll
-    for (int rh = 0; rh < 2; ++rh) lam[rh] = (kL2 && act[rh] && !imit) ? a.g_rec[(int64_t)T * n + row[rh]] : 0.f;
+    for (int rh = 0; rh < 2; ++rh) lam[rh] = (kL2 && act[rh] && !kImit) ? a.g_rec[tn + n + row[rh]] : 0.f;
     if constexpr (CARRY) {   // state arena [h1 | c1 | h2 | c2][n][20]; lambda = carry + g_t1 (the order of a whole sweep)
 #pragma unroll
       for (int rh = 0; rh < 2; ++rh) {
@@ -331,7 +352,7 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
         if constexpr (kL2) {
           load5(cy.d_state + (2 * n + i) * kH, q, dh2c[rh]);
           load5(cy.d_state + (3 * n + i) * kH, q, dc2[rh]);
-          lam[rh] = cy.lam[i] + a.g_rec[(int64_t)T * n + i];
+          lam[rh] = cy.lam[i] + a.g_rec[tn + n + i];
         }
         if constexpr (kL1) {
           load5(cy.d_state + i * kH, q, dh1c[rh]);
@@ -344,10 +365,7 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
     A.template put<(G::ColOne & ~3)>(1, q == (G::ColOne & 3) ? 1.0f : 0.f);
 
     for (int t = T - 1; t >= 0; --t) {
-      const float* ck = a.ckpt + (int64_t)t * slot;
-      // the slot the ring loads next: t - 1 of this tile, or T - 1 of the warpgroup's next tile
-      const int64_t tl_next = t > 0 ? tile : tile + tstride;
-      const int t_next = t > 0 ? t - 1 : T - 1;
+      const float* ckr = ckt + kx * kH;   // this thread's row r0 of slot t (row r0 + 8 at + 8 kH)
       float z[kN / 2];
       float dh1n[2][kU];
       // ================================= layer 2 =================================
@@ -361,18 +379,18 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
           for (int s = 0; s < kU; ++s) c2p[rh][s] = 0.f;
           float dtanh = 1.0f;
           if (act[rh]) {
-            const int64_t i = row[rh];
+            const float* cr = ckr + 8 * kH * rh;
             if constexpr (kRing) {
-              if (t == T - 1) load5(ck + slot + i * kH, q, h1n);
+              if (t == T - 1) load5(cr + slot, q, h1n);
               ring5(R.h, rh, true, h2p);
             } else {
-              load5(ck + slot + i * kH, q, h1n);   // h1n(t) IS the checkpointed h1 of slot t+1
-              load5(ck + 2 * n * kH + i * kH, q, h2p);
-              load5(ck + 2 * n * kH + (n + i) * kH, q, c2p[rh]);
+              load5(cr + slot, q, h1n);   // h1n(t) IS the checkpointed h1 of slot t+1
+              load5(cr + 2 * nkh, q, h2p);
+              load5(cr + 3 * nkh, q, c2p[rh]);
             }
-            if (imit) lam[rh] = (a.delta_seq[(int64_t)t * n + i] - a.labels[(int64_t)t * n + i]) * inv_nt;
-            if (rt.tanh_output) {   // delta = scale tanh(y): the recorded delta gives tanh' without y
-              const float th = a.delta_seq[(int64_t)t * n + i] / rt.scale;
+            if constexpr (kImit) lam[rh] = (a.delta_seq[tn + row[rh]] - a.labels[tn + row[rh]]) * inv_nt;
+            if constexpr (kTanh) {   // delta = scale tanh(y): the recorded delta gives tanh' without y
+              const float th = a.delta_seq[tn + row[rh]] / rt.scale;
               dtanh = fmaf(-th, th, 1.0f);
             }
           }
@@ -401,9 +419,13 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
             acc_wo[s] = fmaf(hn, dy[rh], acc_wo[s]);
           }
         wg_bar(wg);   // every warp has retired the previous dW batch: the staging may be overwritten
-        if (kRing && elected) {   // and every read of h2 / c2 is done: h1(t) for layer 1, c2 of the next slot
-          arm(&R.barh, R.h, tile, t, 0);
-          if (tl_next < ntiles) arm(&R.bar2, R.c2, tl_next, t_next, 3);
+        if constexpr (kRing) {   // and every read of h2 / c2 is done: h1(t) for layer 1, c2 of the next slot
+          if (elected) {
+            // the slot the ring loads next: t - 1 of this tile, or T - 1 of the warpgroup's next tile
+            const int64_t tl_next = t > 0 ? tile : tile + tstride;
+            arm(&R.barh, R.h, ckt, 0, tile_bytes(tile));
+            if (tl_next < ntiles) arm(&R.bar2, R.c2, t > 0 ? ckt - slot : ckt + ck_wrap, 3, tile_bytes(tl_next));
+          }
         }
         stage_x(kXa2, 0, kBlkL1, G::ColH1, G::ColH2);   // h1n | h2p
         stage_dz(z);
@@ -422,17 +444,18 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
         if constexpr (MODE == 1) {
 #pragma unroll
           for (int rh = 0; rh < 2; ++rh)
-            if (act[rh]) store5(a.scratch + ((int64_t)t * n + row[rh]) * kH, q, dh1n[rh]);
+            if (act[rh]) store5(a.scratch + (tn + row[rh]) * kH, q, dh1n[rh]);
         }
 #pragma unroll
         for (int rh = 0; rh < 2; ++rh)
-          if (!imit && act[rh] && (!CARRY || t > 0)) lam[rh] += a.g_rec[(int64_t)t * n + row[rh]];   // g_t0: the previous segment's
+          if (!kImit && act[rh] && (!CARRY || t > 0)) lam[rh] += a.g_rec[tn + row[rh]];   // g_t0: the previous segment's
       }
       // ================================= layer 1 =================================
       if constexpr (kL1) {
         float c1p[2][kU];
-        float r0v[2] = {0.f, 0.f}, r1v[2] = {0.f, 0.f};
-        float ep[2][kU];   // fc nets: elu'(a) of the thread's fc outputs
+        float r0v[2] = {0.f, 0.f};
+        [[maybe_unused]] float r1v[2] = {0.f, 0.f};   // fc nets: the second input row
+        [[maybe_unused]] float ep[2][kU];             // fc nets: elu'(a) of the thread's fc outputs
         if constexpr (kRing) mbar_wait(&R.barh, 1);
 #pragma unroll
         for (int rh = 0; rh < 2; ++rh) {
@@ -440,19 +463,18 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
 #pragma unroll
           for (int s = 0; s < kU; ++s) c1p[rh][s] = 0.f;
           if (act[rh]) {
-            const int64_t i = row[rh];
             if constexpr (kRing) {
               ring5(R.h, rh, true, h1p);
             } else {
-              load5(ck + i * kH, q, h1p);
-              load5(ck + (n + i) * kH, q, c1p[rh]);
+              load5(ckr + 8 * kH * rh, q, h1p);
+              load5(ckr + nkh + 8 * kH * rh, q, c1p[rh]);
             }
             if constexpr (MODE == 2) {
-              load5(a.scratch + ((int64_t)t * n + i) * kH, q, dh1n[rh]);
-              r0v[rh] = a.in_seq[((int64_t)t * 2) * n + i];
-              r1v[rh] = a.in_seq[((int64_t)t * 2 + 1) * n + i];
+              load5(a.scratch + (tn + row[rh]) * kH, q, dh1n[rh]);
+              r0v[rh] = a.in_seq[2 * tn + row[rh]];
+              r1v[rh] = a.in_seq[2 * tn + n + row[rh]];
             } else {
-              r0v[rh] = a.in_seq[(int64_t)t * n + i];
+              r0v[rh] = a.in_seq[tn + row[rh]];
             }
           } else if constexpr (MODE == 2) {
 #pragma unroll
@@ -499,16 +521,20 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
           }
         wg_bar(wg);
         if constexpr (kRing) {   // every read of h1 / c1 is done: h2 and c1 of the next slot, its h1 and in_seq into L2
+          const int64_t tl_next = t > 0 ? tile : tile + tstride;
           if (elected && tl_next < ntiles) {
-            arm(&R.barh, R.h, tl_next, t_next, 2);
-            arm(&R.bar1, R.c1, tl_next, t_next, 1);
-            prefetch_l2_bulk(ck_block(tl_next, t_next, 0), tile_bytes(tl_next));
+            const float* ckn = t > 0 ? ckt - slot : ckt + ck_wrap;
+            const uint32_t b = tile_bytes(tl_next);
+            arm(&R.barh, R.h, ckn, 2, b);
+            arm(&R.bar1, R.c1, ckn, 1, b);
+            prefetch_l2_bulk(ck_block(ckn, 0), b);
           }
+          // in_seq rows of the next slot: t - 1 of this tile, or T - 1 of the next tile
+          const int64_t rn = t > 0 ? r0 : r0 + tstride * tc::kTile;
+          const float* in_next = a.in_seq + (t > 0 ? tn - n : (int64_t)(T - 1) * n) + rn;
 #pragma unroll
-          for (int rh = 0; rh < 2; ++rh) {
-            const int64_t r = tl_next * tc::kTile + kx + 8 * rh;
-            if (q == 0 && r < n) prefetch_l2(a.in_seq + (int64_t)t_next * n + r);
-          }
+          for (int rh = 0; rh < 2; ++rh)
+            if (q == 0 && ((FULL && t > 0) || rn + 8 * rh < n)) prefetch_l2(in_next + 8 * rh);
           ph ^= 1u;
         }
         if constexpr (MODE == 2) stage_x(kXa2, 0, kBlkL1, G::ColH1, 0);   // h1p | e
@@ -531,6 +557,8 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
             }
           }
       }
+      ckt -= slot;
+      tn -= n;
     }
     if constexpr (CARRY) {
 #pragma unroll
@@ -594,13 +622,28 @@ int tc_launch_bwd(const NetRt& rt, const l2o_bwd_args& a, float* img, cudaStream
     kern<<<grid, tcb::kBwdThreads, smem, st>>>(a, rt, img, cy);
     return cudaGetLastError() == cudaSuccess ? L2O_OK : L2O_E_CUDA;
   };
+  // the layer-2 pass's instantiation for the output-layer flags of these arguments
+  const int fl = (a.labels != nullptr ? tcb::kFlImit : 0) | (rt.tanh_output ? tcb::kFlTanh : 0);
+  // the layer-2 pass's instantiation for these flags, and for DM nets whether every tile is full
+  auto launch_l2 = [&](auto mode, auto full) {
+    constexpr int M = decltype(mode)::value;
+    constexpr bool F = decltype(full)::value;
+    constexpr size_t smem = tcb::bwd_smem_bytes<C, M>();
+    switch (fl) {
+      case 0: return launch(tcb::unroll_bwd_kernel<C, M, CARRY, 0, F>, smem);
+      case tcb::kFlImit: return launch(tcb::unroll_bwd_kernel<C, M, CARRY, tcb::kFlImit, F>, smem);
+      case tcb::kFlTanh: return launch(tcb::unroll_bwd_kernel<C, M, CARRY, tcb::kFlTanh, F>, smem);
+      default: return launch(tcb::unroll_bwd_kernel<C, M, CARRY, tcb::kFlImit | tcb::kFlTanh, F>, smem);
+    }
+  };
   if constexpr (C::FC) {
     // two passes over time: layer 2 (exporting dX2[h1n] to a.scratch), then layer 1 fed by it
-    int rc = launch(tcb::unroll_bwd_kernel<C, 1, CARRY>, tcb::bwd_smem_bytes<C, 1>());
+    int rc = launch_l2(tc::IC<1>{}, std::false_type{});
     if (rc != L2O_OK) return rc;
-    return launch(tcb::unroll_bwd_kernel<C, 2, CARRY>, tcb::bwd_smem_bytes<C, 2>());
+    return launch(tcb::unroll_bwd_kernel<C, 2, CARRY, 0, false>, tcb::bwd_smem_bytes<C, 2>());
   } else {
-    return launch(tcb::unroll_bwd_kernel<C, 0, CARRY>, tcb::bwd_smem_bytes<C, 0>());
+    if (a.n % tc::kTile == 0) return launch_l2(tc::IC<0>{}, std::true_type{});
+    return launch_l2(tc::IC<0>{}, std::false_type{});
   }
 }
 
