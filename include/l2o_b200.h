@@ -170,6 +170,10 @@ int l2o_unroll_bwd(l2o_handle h, const l2o_bwd_args* a, void* stream);
  * slots, a->g_rec / in_seq / delta_seq / scratch its rows (g_rec rows t0..t1).  Meta-loss mode only: imitation
  * (a->labels) returns L2O_E_UNSUPPORTED.  Same engine choice as l2o_unroll_bwd. */
 int l2o_unroll_bwd_carry(l2o_handle h, const l2o_bwd_args* a, const l2o_bwd_carry* c, void* stream);
+/* Which tensor-core forward kernel l2o_unroll_fwd would run *a on, without launching anything: 1 = the full-tile
+ * instantiation (DM net, in-kernel Rastrigin or diagonal quadratic, n % 64 == 0, T >= 1, plain output layer, ckpt and
+ * g_rec both set or both NULL), 0 = the general one, L2O_E_UNSUPPORTED = not the tensor-core engine's call. */
+int l2o_tc_fwd_variant(l2o_handle h, const l2o_unroll_args* a);
 
 /* TF-1.14 Adam on theta: k = 1-based step count. */
 int l2o_adam_step(float* theta, const double* dtheta, float* m, float* v, int64_t n, int32_t k, float lr,

@@ -362,17 +362,23 @@ struct SmemF {
   float wo[kH + 4];               // linear/w, linear/b
   float win[64];                  // fc nets: input_projection/w [2][20] then /b [20]
   uint64_t wbar;
-  uint64_t pad;
-  double fx[1];                   // [T+1], dynamic tail
 };
-// dynamic tail after SmemF<C>: fx [T+1] doubles | (fc nets) Adam bias corrections [T][2] floats
+// dynamic tail after SmemF<C>: (fc nets) Adam bias corrections [T][2] floats
 template <class C>
-__host__ __device__ constexpr size_t adamc_offset(int T) {
-  return (sizeof(SmemF<C>) + (size_t)(T + 1) * sizeof(double) + 15) & ~(size_t)15;
+__host__ __device__ constexpr size_t adamc_offset() {
+  return (sizeof(SmemF<C>) + 15) & ~(size_t)15;
 }
 template <class C>
 __host__ __device__ constexpr size_t fwd_smem_bytes(int T) {
-  return adamc_offset<C>(T) + (C::FC ? (size_t)T * 2 * sizeof(float) : 0);
+  return adamc_offset<C>() + (C::FC ? (size_t)T * 2 * sizeof(float) : 0);
+}
+// fx partial sum of a warp whose lanes q = 2, 3 of every quad hold 0: warp_sum_d without its xor-2 level, which would
+// only add those zeros
+__device__ __forceinline__ double warp_sum_pairs_d(double v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 16);
+  v += __shfl_xor_sync(0xffffffffu, v, 8);
+  v += __shfl_xor_sync(0xffffffffu, v, 4);
+  return v + __shfl_xor_sync(0xffffffffu, v, 1);
 }
 
 // ------------------------------------------------------------------ forward kernel
@@ -380,21 +386,31 @@ __host__ __device__ constexpr size_t fwd_smem_bytes(int T) {
 // rows in, then per step  features -> layer-1 MMAs -> layer-1 epilogue -> layer-2 MMAs -> layer-2 epilogue + output
 // layer + parameter add.  The three warpgroups of a CTA run independent tiles, so one warpgroup's MMA round trip
 // overlaps the others' epilogues.
-template <class C>
+//
+// FAST (tc_fwd_fast: DM nets, n a multiple of 64, in-kernel optimizee, plain output layer, T >= 1, state in place) is
+// the full-tile instantiation: no row tests, the optimizee kind OPT is a compile-time constant, CKPT says whether the
+// checkpoints and g_rec are written (both or neither), and the tanh output, recorded deltas, imitation labels and Adam
+// features are compiled out.  Its arithmetic is the general instantiation's, operation for operation.
+template <class C, bool FAST = false, int OPT = L2O_OPT_NONE, bool CKPT = false>
 __global__ void __launch_bounds__(kFwdThreads, 1) unroll_fwd_kernel(l2o_unroll_args a, NetRt rt, const float* __restrict__ img,
                                                                      float* __restrict__ state_out, FwdExtra ex) {
+  static_assert(!FAST || (!C::FC && OPT != L2O_OPT_NONE), "the full-tile forward is the DM nets' with an optimizee");
   using G = Geo<C>;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   SmemF<C>& S = *reinterpret_cast<SmemF<C>*>(smem_raw);
   const int T = a.T;
   const int64_t n = a.n;
-  const bool in_kernel_opt = a.opt_kind != L2O_OPT_NONE;
+  const bool in_kernel_opt = FAST || a.opt_kind != L2O_OPT_NONE;
+  const int opt_kind = FAST ? OPT : a.opt_kind;
   const bool want_fx = in_kernel_opt && a.fx != nullptr;
   const bool adam_mode = C::NIN == 2 && a.m != nullptr;   // fused RNNProp features (DM/meta_rnnprop_train.py:383-388)
-  float* adamc = reinterpret_cast<float*>(smem_raw + adamc_offset<C>(T));
+  const bool has_ckpt = FAST ? CKPT : a.ckpt != nullptr;
+  const bool has_grec = FAST ? CKPT : a.g_rec != nullptr;
+  const bool tanh_out = !FAST && rt.tanh_output;
+  const bool has_delta = !FAST && a.delta_seq != nullptr;
+  const bool has_labels = !FAST && a.labels != nullptr;
+  float* adamc = reinterpret_cast<float*>(smem_raw + adamc_offset<C>());
 
-  if (want_fx)
-    for (int t = threadIdx.x; t <= T; t += blockDim.x) S.fx[t] = 0.0;
   if (threadIdx.x < kH) S.wo[threadIdx.x] = a.theta[C::O_WO + threadIdx.x];
   if (threadIdx.x == kH) S.wo[kH] = a.theta[C::O_BO];
   if constexpr (C::FC) {
@@ -416,12 +432,14 @@ __global__ void __launch_bounds__(kFwdThreads, 1) unroll_fwd_kernel(l2o_unroll_a
   __syncthreads();
   stage_image(S.img, img, G::FwdFloats * 4, &S.wbar);
 
-  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  // the warpgroup index through lane 0, so the compiler can prove the tile indices warp-uniform
+  const int wg = __shfl_sync(0xffffffffu, threadIdx.x >> 7, 0), warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
   const int g = lane >> 2, q = lane & 3, own = q & 1;
   const uint64_t b1h = img_desc(S.img, kN), b1l = img_desc(S.img + G::B1Floats, kN);
   const uint64_t b2h = img_desc(S.img + 2 * G::B1Floats, kN), b2l = img_desc(S.img + 2 * G::B1Floats + G::B2Floats, kN);
   const int64_t ntiles = (n + kTile - 1) / kTile;
   const int64_t slot = n * C::SF;
+  const int64_t nk = n * kH;   // one [n][20] block of the state arena
   const float bo = S.wo[kH];
   float wo[kU];
 #pragma unroll
@@ -434,10 +452,14 @@ __global__ void __launch_bounds__(kFwdThreads, 1) unroll_fwd_kernel(l2o_unroll_a
   for (int64_t tile = (int64_t)blockIdx.x * kFwdWG + wg; tile < ntiles; tile += (int64_t)gridDim.x * kFwdWG) {
     const int64_t r0 = tile * kTile + warp * 16 + g;
     const int64_t row[2] = {r0, r0 + 8};
-    const bool act[2] = {row[0] < n, row[1] < n};
+    const bool act[2] = {FAST || row[0] < n, FAST || row[1] < n};
     const int64_t io = own ? row[1] : row[0];   // the row whose per-coordinate scalars this thread computes
-    const bool oact = io < n;
+    const bool oact = FAST || io < n;
     const bool writer = q < 2 && oact;
+    // checkpoint rows of the thread's first coordinate (the second is 8 rows on) and its g_rec entry, stepped by one
+    // slot / one row per step
+    float* ck = has_ckpt ? a.ckpt + r0 * kH : nullptr;
+    float* gr = has_grec ? a.g_rec + io : nullptr;
     Frag<G::KB> A;
     A.zero();
     float c1[2][kU], c2[2][kU];
@@ -452,13 +474,14 @@ __global__ void __launch_bounds__(kFwdThreads, 1) unroll_fwd_kernel(l2o_unroll_a
         load5(a.state + (n + i) * kH, q, c1[rh]);
         load5(a.state + 2 * n * kH + i * kH, q, h2);
         load5(a.state + 2 * n * kH + (n + i) * kH, q, c2[rh]);
-        if (a.ckpt) {
-          store5(a.ckpt + i * kH, q, h1);
-          store5(a.ckpt + (n + i) * kH, q, c1[rh]);
-          store5(a.ckpt + 2 * n * kH + i * kH, q, h2);
-          store5(a.ckpt + 2 * n * kH + (n + i) * kH, q, c2[rh]);
+        if (has_ckpt) {
+          float* p = ck + rh * 8 * kH;
+          store5(p, q, h1);
+          store5(p + nk, q, c1[rh]);
+          store5(p + 2 * nk, q, h2);
+          store5(p + 3 * nk, q, c2[rh]);
         }
-        if (T == 0 && state_out != a.state) {
+        if (!FAST && T == 0 && state_out != a.state) {
           store5(state_out + i * kH, q, h1);
           store5(state_out + (n + i) * kH, q, c1[rh]);
           store5(state_out + 2 * n * kH + i * kH, q, h2);
@@ -474,18 +497,22 @@ __global__ void __launch_bounds__(kFwdThreads, 1) unroll_fwd_kernel(l2o_unroll_a
     }
     float x = 0.f, oa = 0.f, ob = 0.f, am = 0.f, av = 0.f;
     if (oact) {
-      if (a.x) x = a.x[io];
+      if (FAST || a.x) x = a.x[io];
       if (in_kernel_opt) { oa = a.opt_a[io]; ob = a.opt_b[io]; }
       if (adam_mode) { am = a.m[io]; av = a.v[io]; }
     }
 
     for (int t = 0; t < T; ++t) {
+      if (has_ckpt) ck += slot;   // slot t + 1
       // ---- gradient + preprocessing of the own row, then the feature columns of both rows -------------------------
       float fval = 0.f, raw0 = 0.f, raw1 = 0.f;
       if (oact) {
         if (in_kernel_opt) {
-          optimizee_eval(a.opt_kind, x, oa, ob, a.opt_alpha, a.opt_fscale, fval, raw0);
-          if (a.g_rec && q < 2) a.g_rec[(int64_t)t * n + io] = raw0;
+          optimizee_eval(opt_kind, x, oa, ob, a.opt_alpha, a.opt_fscale, fval, raw0);
+          if (has_grec) {
+            if (q < 2) *gr = raw0;
+            gr += n;
+          }
         } else if (C::NIN == 2 && !adam_mode) {   // operator surface: (m~, g~) given
           raw0 = a.in_seq[((int64_t)t * 2) * n + io];
           raw1 = a.in_seq[((int64_t)t * 2 + 1) * n + io];
@@ -534,8 +561,10 @@ __global__ void __launch_bounds__(kFwdThreads, 1) unroll_fwd_kernel(l2o_unroll_a
         }
       }
       if (want_fx) {
-        const double ws = warp_sum_d(q < 2 ? (double)fval : 0.0);
-        if (lane == 0) atomicAdd(&S.fx[t], ws);
+        // straight to global memory: a fire-and-forget reduction, where a shared-memory fp64 atomicAdd is a
+        // compare-and-swap loop that the warps of the CTA contend for every step
+        const double ws = warp_sum_pairs_d(q < 2 ? (double)fval : 0.0);
+        if (lane == 0) atomicAdd(&a.fx[t], ws);
       }
       // ---- layer 1 ---------------------------------------------------------------------------------------------------
       wg_fence();
@@ -549,18 +578,14 @@ __global__ void __launch_bounds__(kFwdThreads, 1) unroll_fwd_kernel(l2o_unroll_a
         for (int s = 0; s < kU; ++s)
           lstm_point_fwd(d[acc_idx(s, 0, rh)], d[acc_idx(s, 1, rh)], d[acc_idx(s, 2, rh)], d[acc_idx(s, 3, rh)], c1[rh][s], h[s]);
         A.template put_vec<G::ColH1>(rh, h);
-        if (act[rh]) {
-          const int64_t i = row[rh];
-          if (a.ckpt) {
-            float* ck = a.ckpt + (int64_t)(t + 1) * slot;
-            store5(ck + i * kH, q, h);
-            store5(ck + (n + i) * kH, q, c1[rh]);
-          }
-          if (t == T - 1) {
-            store5(state_out + i * kH, q, h);
-            store5(state_out + (n + i) * kH, q, c1[rh]);
-          }
+        if (act[rh] && has_ckpt) {
+          store5(ck + rh * 8 * kH, q, h);
+          store5(ck + nk + rh * 8 * kH, q, c1[rh]);
         }
+        // without a branch around them, ptxas would sink the stores behind the layer-2 MMAs and issue all 40 of the
+        // step at its end; the warp barrier keeps them where the epilogue produced their values.  It sits outside the
+        // row test, so every lane reaches it on a ragged tile too.
+        if (has_ckpt) __syncwarp();
       }
       // ---- layer 2 + output layer + parameter add --------------------------------------------------------------------
       wg_fence();
@@ -579,63 +604,79 @@ __global__ void __launch_bounds__(kFwdThreads, 1) unroll_fwd_kernel(l2o_unroll_a
         }
         A.template put_vec<G::ColH2>(rh, h);
         y[rh] = quad_sum(yp) + bo;
-        if (act[rh]) {
-          const int64_t i = row[rh];
-          if (a.ckpt) {
-            float* ck = a.ckpt + (int64_t)(t + 1) * slot + 2 * n * kH;
-            store5(ck + i * kH, q, h);
-            store5(ck + (n + i) * kH, q, c2[rh]);
-          }
-          if (t == T - 1) {
-            store5(state_out + 2 * n * kH + i * kH, q, h);
-            store5(state_out + 2 * n * kH + (n + i) * kH, q, c2[rh]);
-          }
+        if (act[rh] && has_ckpt) {
+          store5(ck + 2 * nk + rh * 8 * kH, q, h);
+          store5(ck + 3 * nk + rh * 8 * kH, q, c2[rh]);
         }
+        if (has_ckpt) __syncwarp();
       }
       const float yo = own ? y[1] : y[0];
-      const float dl = rt.tanh_output ? tanh_acc(yo) * rt.scale : yo * rt.scale;
+      // __fmul_rn: Delta is rounded before x += Delta in every instantiation (an fma here would change x)
+      const float dl = tanh_out ? tanh_acc(yo) * rt.scale : __fmul_rn(yo, rt.scale);
       x += dl;
       if (writer) {
-        if (a.delta_seq) a.delta_seq[(int64_t)t * n + io] = dl;
-        if (a.labels) {
+        if (has_delta) a.delta_seq[(int64_t)t * n + io] = dl;
+        if (has_labels) {
           const float r = a.labels[(int64_t)t * n + io] - dl;
           imit += 0.5 * (double)r * (double)r;
         }
       }
     }
-    // ---- tile epilogue: x, f(x_T), g_T, Adam moments ---------------------------------------------------------------
+    // ---- tile epilogue: final state (h exactly as hi + lo of its fragment), x, f(x_T), g_T, Adam moments ----------
+    if (FAST || T > 0) {
+#pragma unroll
+      for (int rh = 0; rh < 2; ++rh) {
+        if (!act[rh]) continue;
+        float h1[kU], h2[kU];
+#pragma unroll
+        for (int s = 0; s < kU; ++s) {
+          h1[s] = A.get_at(G::ColH1 + 4 * s, rh);
+          h2[s] = A.get_at(G::ColH2 + 4 * s, rh);
+        }
+        float* p = state_out + row[rh] * kH;
+        store5(p, q, h1);
+        store5(p + nk, q, c1[rh]);
+        store5(p + 2 * nk, q, h2);
+        store5(p + 3 * nk, q, c2[rh]);
+      }
+    }
     float fval = 0.f;
     if (writer) {
       if (in_kernel_opt) {
         float gT;
-        optimizee_eval(a.opt_kind, x, oa, ob, a.opt_alpha, a.opt_fscale, fval, gT);
-        if (a.g_rec) a.g_rec[(int64_t)T * n + io] = gT;
+        optimizee_eval(opt_kind, x, oa, ob, a.opt_alpha, a.opt_fscale, fval, gT);
+        if (has_grec) *gr = gT;
       }
-      if (a.x) a.x[io] = x;
+      if (FAST || a.x) a.x[io] = x;
       if (adam_mode) { a.m[io] = am; a.v[io] = av; }
     }
     if (want_fx) {
-      const double ws = warp_sum_d((double)fval);
-      if (lane == 0) atomicAdd(&S.fx[T], ws);
+      const double ws = warp_sum_pairs_d((double)fval);
+      if (lane == 0) atomicAdd(&a.fx[T], ws);
     }
   }
-  if (a.labels && a.imit_loss) {
+  if (has_labels && a.imit_loss) {
     const double ws = warp_sum_d(imit);
     if (lane == 0) atomicAdd(a.imit_loss, ws / (double)a.n_total);
   }
-  __syncthreads();
-  if (want_fx)
-    for (int t = threadIdx.x; t <= T; t += blockDim.x) atomicAdd(&a.fx[t], S.fx[t]);
 }
 
 }  // namespace tc
 
 // ------------------------------------------------------------------ host side (called from l2o_tc.cu)
-template <class C>
-int tc_launch_fwd(const NetRt& rt, const l2o_unroll_args& a, float* img, cudaStream_t st, int sms, float* state_out = nullptr,
-                  tc::FwdExtra ex = tc::FwdExtra{nullptr, 0, 0.f}, bool prep = true) {
-  if (prep) tc::prep_weights_kernel<C><<<16, 256, 0, st>>>(a.theta, img, 0);
-  auto k = tc::unroll_fwd_kernel<C>;
+// Whether a forward call runs the full-tile instantiation of unroll_fwd_kernel (FAST): a DM net (not fc) on an in-kernel
+// Rastrigin or diagonal quadratic, n a multiple of 64, T >= 1, the state updated in place, checkpoints and g_rec both
+// recorded or neither, and a plain output layer (no tanh, recorded deltas or imitation labels).
+inline bool tc_fwd_fast(bool fc, const NetRt& rt, const l2o_unroll_args& a, const float* state_out) {
+  return !fc && (a.opt_kind == L2O_OPT_RASTRIGIN_SEP || a.opt_kind == L2O_OPT_QUADRATIC_DIAG) && a.n > 0 &&
+         a.n % tc::kTile == 0 && a.T > 0 && (state_out == nullptr || state_out == a.state) && a.x != nullptr &&
+         (a.ckpt == nullptr) == (a.g_rec == nullptr) && !rt.tanh_output && a.delta_seq == nullptr && a.labels == nullptr;
+}
+
+template <class C, bool FAST, int OPT, bool CKPT>
+int tc_run_fwd(const NetRt& rt, const l2o_unroll_args& a, float* img, cudaStream_t st, int sms, float* state_out,
+               tc::FwdExtra ex) {
+  auto k = tc::unroll_fwd_kernel<C, FAST, OPT, CKPT>;
   const size_t smem = tc::fwd_smem_bytes<C>(a.T);
   if (smem > 227 * 1024) return L2O_E_INVALID;
   if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return L2O_E_CUDA;
@@ -644,6 +685,23 @@ int tc_launch_fwd(const NetRt& rt, const l2o_unroll_args& a, float* img, cudaStr
   const int grid = (int)(ctas < sms ? ctas : sms);
   k<<<grid, tc::kFwdThreads, smem, st>>>(a, rt, img, state_out ? state_out : a.state, ex);
   return cudaGetLastError() == cudaSuccess ? L2O_OK : L2O_E_CUDA;
+}
+
+template <class C>
+int tc_launch_fwd(const NetRt& rt, const l2o_unroll_args& a, float* img, cudaStream_t st, int sms, float* state_out = nullptr,
+                  tc::FwdExtra ex = tc::FwdExtra{nullptr, 0, 0.f}, bool prep = true) {
+  if (prep) tc::prep_weights_kernel<C><<<16, 256, 0, st>>>(a.theta, img, 0);
+  if constexpr (!C::FC) {
+    if (tc_fwd_fast(false, rt, a, state_out)) {
+      constexpr int R = L2O_OPT_RASTRIGIN_SEP, Q = L2O_OPT_QUADRATIC_DIAG;
+      if (a.opt_kind == R)
+        return a.ckpt ? tc_run_fwd<C, true, R, true>(rt, a, img, st, sms, state_out, ex)
+                      : tc_run_fwd<C, true, R, false>(rt, a, img, st, sms, state_out, ex);
+      return a.ckpt ? tc_run_fwd<C, true, Q, true>(rt, a, img, st, sms, state_out, ex)
+                    : tc_run_fwd<C, true, Q, false>(rt, a, img, st, sms, state_out, ex);
+    }
+  }
+  return tc_run_fwd<C, false, L2O_OPT_NONE, false>(rt, a, img, st, sms, state_out, ex);
 }
 
 }  // namespace l2o

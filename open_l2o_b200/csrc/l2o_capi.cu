@@ -159,6 +159,11 @@ int l2o_unroll_fwd(l2o_handle h, const l2o_unroll_args* a, void* stream) {
   return l2o::ffma_unroll_fwd(h, *a, st);
 }
 
+int l2o_tc_fwd_variant(l2o_handle h, const l2o_unroll_args* a) {
+  if (!h || !a) return L2O_E_INVALID;
+  return l2o::tc_fwd_variant(h, *a);
+}
+
 int l2o_unroll_bwd(l2o_handle h, const l2o_bwd_args* a, void* stream) {
   if (!h || !a || a->n < 0 || a->T < 0 || !a->theta || !a->dtheta) return L2O_E_INVALID;
   if (a->T > 0 && !a->in_seq) return L2O_E_INVALID;

@@ -51,6 +51,7 @@ bool tc_supported(int cfg);
 void tc_release_image(l2o_net* h);   // hand the weight image back to the process-wide pool (never cudaFree)
 bool tc_fwd_ok(const l2o_net* h, const l2o_unroll_args& a);
 int tc_unroll_fwd(l2o_net* h, const l2o_unroll_args& a, cudaStream_t st);
+int tc_fwd_variant(const l2o_net* h, const l2o_unroll_args& a);   // l2o_tc_fwd_variant
 bool tc_step_ok(const l2o_net* h, const l2o_step_args& a);
 int tc_step(l2o_net* h, const l2o_step_args& a, cudaStream_t st);
 bool tc_auto_default();

@@ -155,4 +155,9 @@ int tc_unroll_fwd(l2o_net* h, const l2o_unroll_args& a, cudaStream_t st) {
   if (rc == L2O_E_CUDA) return set_cuda_error(cudaGetLastError(), "tc_unroll_fwd launch");
   return rc;
 }
+
+int tc_fwd_variant(const l2o_net* h, const l2o_unroll_args& a) {
+  if (!tc_supported(h->cfg) || !tc_fwd_ok(h, a)) return L2O_E_UNSUPPORTED;
+  return tc_fwd_fast(h->cfg == 2, h->rt, a, nullptr) ? 1 : 0;
+}
 }  // namespace l2o
