@@ -20,6 +20,7 @@
  *   l2o_adam_step                       tf.train.AdamOptimizer(lr).minimize            DM/meta.py:411-413
  *   l2o_log_and_sign                    preprocess.LogAndSign                          DM/preprocess.py:52-70
  *   l2o_lasso_grad                      problems.lasso(_fixed) loss + tf.gradients     DM/problems.py:103-175, DM/meta.py:322-329
+ *   l2o_confocal_grad                   problems.confocal_microscopy_3d + tf.gradients DM/problems.py:701-956, DM/meta.py:322-329
  *
  * Conventions: every pointer is a DEVICE pointer owned by the caller (PyTorch allocates); no hidden
  * allocation; `stream` is a cudaStream_t passed as void*; every entry returns 0 or a negative
@@ -248,6 +249,26 @@ typedef struct {
   double* f;            /* optional scalar: += f */
 } l2o_lasso_args;
 int l2o_lasso_grad(const l2o_lasso_args* a, void* stream);
+
+/*   l2o_confocal_grad  problems.confocal_microscopy_3d (inference=False), DM/problems.py:701-956 + tf.gradients at
+ *                      DM/meta.py:322-329:  f = mean_b sum_v (sum_p psf(theta_p; v) + bg_b - t_b[v])^2 with the target
+ *                      t_b = l2_normalize_v(sum_p psf(sim_p; v) + bg_sim_b), g = df/dx.  theta = x (.) scale (optional,
+ *                      random-scaling trick as l2o_lasso_grad), mapped through tfd.Uniform(lo, hi).quantile(p) =
+ *                      lo + p (hi - lo): I0 in [0.5, 2], x0/y0/z0 in [0.5, roi - 1], sigma_xy and sigma_z in [2, 4].
+ *                      Layout of x, scale, sim and g: [6P+1][batch], rows I, x0, y0, z0, sigma_xy, sigma_z of point
+ *                      0..P-1 then bg (the reference's creation order).  One CTA per batch row holds the whole image
+ *                      in shared memory: 4 (V + 4 P (nx+ny+nz) + 2P) bytes, V = nx ny nz, at most 200 KB (32^3 fits
+ *                      for P <= 47), L2O_E_UNSUPPORTED beyond. */
+typedef struct {
+  int32_t batch, num_points;
+  int32_t roi[3];       /* image size nx, ny, nz */
+  const float* x;       /* [6P+1][batch] */
+  const float* sim;     /* [6P+1][batch] simulated parameters (and bg_sim) */
+  const float* scale;   /* optional [6P+1][batch] */
+  float* g;             /* [6P+1][batch] */
+  double* f;            /* optional scalar: += f */
+} l2o_confocal_args;
+int l2o_confocal_grad(const l2o_confocal_args* a, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * L2O-Scale HierarchicalRNN update step (SURVEY.md 8(f) row 1; BASELINE config #4).

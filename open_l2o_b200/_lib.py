@@ -25,6 +25,7 @@ ENGINE_AUTO, ENGINE_FFMA, ENGINE_TC = 0, 1, 2
 EXPORTS = [
     "l2o_net_create", "l2o_net_destroy", "l2o_net_set_engine", "l2o_theta_count", "l2o_state_floats", "l2o_workspace_bytes",
     "l2o_step", "l2o_unroll_fwd", "l2o_unroll_bwd", "l2o_unroll_bwd_carry", "l2o_tc_fwd_variant", "l2o_adam_step", "l2o_log_and_sign", "l2o_lasso_grad",
+    "l2o_confocal_grad",
     "l2o_dense_create", "l2o_dense_destroy", "l2o_dense_theta_count", "l2o_dense_state_floats", "l2o_dense_step",
     "l2o_dense_unroll_bwd",
     "l2o_launch_count", "l2o_status_string", "l2o_last_cuda_error", "l2o_version",
@@ -74,6 +75,11 @@ class BwdCarry(C.Structure):
 class LassoArgs(C.Structure):
     _fields_ = [("batch", C.c_int32), ("m", C.c_int32), ("n", C.c_int32), ("A", _fp), ("y", _fp), ("x", _fp),
                 ("scale", _fp), ("l1", C.c_float), ("g", _fp), ("f", _fp)]
+
+
+class ConfocalArgs(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("num_points", C.c_int32), ("roi", C.c_int32 * 3), ("x", _fp), ("sim", _fp),
+                ("scale", _fp), ("g", _fp), ("f", _fp)]
 
 
 class DenseDesc(C.Structure):
@@ -228,6 +234,8 @@ def lib():
     L.l2o_log_and_sign.restype = C.c_int
     L.l2o_lasso_grad.argtypes = [C.POINTER(LassoArgs), C.c_void_p]
     L.l2o_lasso_grad.restype = C.c_int
+    L.l2o_confocal_grad.argtypes = [C.POINTER(ConfocalArgs), C.c_void_p]
+    L.l2o_confocal_grad.restype = C.c_int
     L.l2o_dense_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(DenseDesc)]
     L.l2o_dense_create.restype = C.c_int
     L.l2o_dense_destroy.argtypes = [C.c_void_p]

@@ -273,6 +273,37 @@ def lasso_grad(A, y, x, l1, g, f=None, scale=None):
     _lib.check(_lib.lib().l2o_lasso_grad(C.byref(a), _stream()), "l2o_lasso_grad")
 
 
+CONFOCAL_SMEM_LIMIT = 200 * 1024   # l2o_producers.cu kConfSmemLimit
+
+
+def confocal_fits(num_points, roi) -> bool:
+    """Whether l2o_confocal_grad takes this shape: one CTA holds the image and its per-axis tables in shared memory,
+    4 (V + 4 P (nx+ny+nz) + 2P) bytes (include/l2o_b200.h)."""
+    nx, ny, nz = (int(r) for r in roi)
+    P = int(num_points)
+    return max(nx, ny, nz) <= 65536 and 4 * (nx * ny * nz + 4 * P * (nx + ny + nz) + 2 * P) <= CONFOCAL_SMEM_LIMIT
+
+
+def confocal_grad(x, sim, g, batch, num_points, roi, f=None, scale=None):
+    """f and df/dx of problems.confocal_microscopy_3d (DM/problems.py:701-956, inference=False) in one launch.  x, sim,
+    g and scale are [6P+1][batch] (rows I, x0, y0, z0, sigma_xy, sigma_z of each point, then bg); writes g and
+    accumulates the scalar loss into the fp64 tensor ``f`` (if given)."""
+    a = _lib.ConfocalArgs()
+    a.batch, a.num_points = int(batch), int(num_points)
+    if len(roi) != 3:
+        raise L2OError("confocal_grad: roi must have three sizes")
+    for k in range(3):
+        a.roi[k] = int(roi[k])
+    rows = 6 * a.num_points + 1
+    for name, t in (("x", x), ("sim", sim), ("g", g), ("scale", scale)):
+        if t is not None and t.numel() != rows * a.batch:
+            raise L2OError(f"confocal_grad: {name} has {t.numel()} elements, [6P+1][batch] = {rows * a.batch}")
+    a.x, a.sim, a.scale = _ptr(x, name="x"), _ptr(sim, name="sim"), _ptr(scale, name="scale")
+    a.g = _ptr(g, name="g")
+    a.f = _ptr(f, torch.float64, "f")
+    _lib.check(_lib.lib().l2o_confocal_grad(C.byref(a), _stream()), "l2o_confocal_grad")
+
+
 _graph_replayed = 0  # kernels of this library launched through CUDA-graph replays (not visible to the C-side counter)
 
 

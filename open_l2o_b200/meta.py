@@ -26,7 +26,7 @@ from . import engine as _engine
 from . import networks
 from .variables import variable_getter
 
-_PRODUCER_KINDS = ("lasso_batch", "mlp_xent")
+_PRODUCER_KINDS = ("lasso_batch", "mlp_xent", "confocal_psf")
 MetaLoss = collections.namedtuple("MetaLoss", "loss, update, reset, fx, x")
 MetaStep = collections.namedtuple("MetaStep", "step, update, reset, fx, x")
 
@@ -253,14 +253,25 @@ class _Program(object):
         self.const_vals = {}
         self.fused = getattr(make_loss, "fused", None) if os.environ.get("L2O_DISABLE_FUSED") != "1" else None
         one_net = len(self.runs) == 1 and self.runs[0].n == self.N
-        if self.fused is not None and not (one_net and (len(self.variables) == 1 or self.fused.kind == "mlp_xent")):
+        if self.fused is not None and not (one_net and (len(self.variables) == 1 or
+                                                        self.fused.kind in ("mlp_xent", "confocal_psf"))):
             self.fused = None
+        if self.fused is not None and self.fused.kind == "confocal_psf" and not self._confocal_layout_ok(self.fused):
+            self.fused = None   # the arena is not the kernel's [6P+1][B] row order: autograd, not a wrong layout
         # "producer" optimizees (SURVEY.md 8(f) row 4): f and df/dx come from ONE library kernel per step instead of
         # torch autograd (~15 launches); the unroll stays step-at-a-time (the gradient couples coordinates) and is
         # captured into one CUDA graph like every external-gradient unroll
         self.producer = None
         if self.fused is not None and self.fused.kind in _PRODUCER_KINDS:
             self.producer, self.fused = self.fused, None
+        if self.producer is not None and self.producer.kind == "confocal_psf":
+            # the simulated constants as row views of ONE [6P+1][B] buffer: reset_x refills them in place, so the kernel
+            # reads them with no packing launch per step and captured graphs stay valid
+            names = self.producer.extra["constants"]
+            shapes = {c["name"]: c["shape"] for c in self.constants}
+            self._confocal_sim = torch.zeros(len(names), self.variables[0]["shape"][0], device=self.device)
+            for row, name in zip(self._confocal_sim, names):
+                self.const_vals[name] = row.view(shapes[name])
         self.adam = _adam_slots(self.nets)
         self.dtheta = {k: torch.zeros(net.theta.numel(), dtype=torch.float64, device=self.device)
                        for k, net in self.nets.items()}
@@ -275,6 +286,14 @@ class _Program(object):
         self._graphs, self._eager_calls, self._graph_failed, self._graph_kernels = {}, {}, False, {}
         self._alloc_workspaces(optimizer.bptt_segment)
         self.reset()
+
+    def _confocal_layout_ok(self, spec):
+        """The arena and the constants are the [6P+1][B] rows l2o_confocal_grad reads, in its order."""
+        B = self.variables[0]["shape"][0]
+        return ([v["name"] for v in self.variables] == spec.extra["variables"] and
+                [c["name"] for c in self.constants] == spec.extra["constants"] and
+                all(tuple(r["shape"]) == (B, 1) for r in self.variables + self.constants) and
+                [s.start for s in self.var_slices] == [j * B for j in range(len(self.variables))])
 
     # ---- memory ---------------------------------------------------------------------------------
     def _alloc_workspaces(self, segment=None):
@@ -408,6 +427,9 @@ class _Program(object):
         if p.kind == "lasso_batch":
             _engine.lasso_grad(self.const_vals[p.a], self.const_vals[p.b], Xflat, p.alpha, g, f=fx,
                                scale=self.scale_flat if self.scale_active else None)
+        elif p.kind == "confocal_psf":
+            _engine.confocal_grad(Xflat, self._confocal_sim, g, self._confocal_sim.shape[1], p.extra["num_points"],
+                                  p.extra["roi"], f=fx, scale=self.scale_flat if self.scale_active else None)
         elif p.kind == "mlp_xent":
             from .problems import mlp_value_and_grad
             with torch.no_grad():

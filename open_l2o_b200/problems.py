@@ -8,8 +8,10 @@ from __future__ import annotations
 import math
 from dataclasses import dataclass
 
+import numpy as np
 import torch
 
+from .engine import confocal_fits
 from .variables import (constant_initializer, get_variable, ones_initializer, random_normal_initializer,
                         random_uniform_initializer)
 
@@ -18,13 +20,15 @@ from .variables import (constant_initializer, get_variable, ones_initializer, ra
 class FusedSpec:
     kind: str        # "rastrigin_sep" | "quadratic_diag" | "quadratic_batch" (in-kernel, include/l2o_b200.h L2O_OPT_*)
                      # | "lasso_batch" (producer kernel l2o_lasso_grad: a = A / w, b = y, alpha = l1 weight)
+                     # | "mlp_xent" (mlp_value_and_grad) | "confocal_psf" (producer kernel l2o_confocal_grad)
     var: str         # name of the trainable variable
     a: str           # constant names
     b: str
     alpha: float = 10.0
     fscale: float = 1.0
     group: int = 0   # "quadratic_batch": coordinates per dense group
-    extra: dict = None   # producer-specific structure ("mlp_xent": activation, number of layers)
+    extra: dict = None   # producer-specific structure ("mlp_xent": activation, number of layers;
+                         # "confocal_psf": points, ROI, the trainable and the simulated names in kernel row order)
 
 
 def simple():
@@ -207,3 +211,81 @@ def mlp_value_and_grad(params, data, labels, activation, grads_out):
             dh = dz @ params[2 * i].t()
             dz = dh * hs[i] * (1.0 - hs[i]) if activation == "sigmoid" else dh * (hs[i] > 0).to(dh.dtype)
     return loss
+
+
+_PSF_PARAMS = ("I", "x", "y", "z", "sigmaxy", "sigmaz")
+
+
+def _psf_3d(theta, ROI):
+    """point_spread_function_3d (DM/problems.py:899-932): theta = [I0, x0, y0, z0, sigmaxy, sigmaz] as [B, 1] quantiles
+    of their tfd.Uniform priors (quantile(p) = low + p (high - low)); returns the image [B, nx*ny*nz] on the reference's
+    tf.meshgrid ('xy' indexing) voxel order."""
+    dt, dev = theta[0].dtype, theta[0].device
+    lows = (0.5, 0.5, 0.5, 0.5, 2.0, 2.0)
+    highs = (2.0, ROI[0] - 1, ROI[1] - 1, ROI[2] - 1, 4.0, 4.0)
+    xs, ys, zs = (torch.linspace(0.0, float(n - 1), n, dtype=dt, device=dev) for n in ROI)
+    X, Y, Z = torch.meshgrid(xs, ys, zs, indexing="xy")
+    I0, x0, y0, z0, sigmaxy, sigmaz = (lo + t.reshape(t.shape[0], 1) * (hi - lo)
+                                       for t, lo, hi in zip(theta, lows, highs))
+    xk, yk, zk = X.reshape(1, -1), Y.reshape(1, -1), Z.reshape(1, -1)
+    sqrt2 = float(np.sqrt(np.float32(2.0), dtype=np.float32))   # tf.math.sqrt(2.0); a Python scalar keeps graph capture free
+                                                                # of host-to-device copies
+    return I0 * ((-torch.erf((-0.5 - x0 + xk) / (sqrt2 * sigmaxy)) + torch.erf((0.5 - x0 + xk) / (sqrt2 * sigmaxy)))
+                 * (-torch.erf((-0.5 - y0 + yk) / (sqrt2 * sigmaxy)) + torch.erf((0.5 - y0 + yk) / (sqrt2 * sigmaxy)))
+                 * (-torch.erf((-0.5 - z0 + zk) / (sqrt2 * sigmaz)) + torch.erf((0.5 - z0 + zk) / (sqrt2 * sigmaz)))) / 8.0
+
+
+def _l2_normalize(v):
+    """tf.math.l2_normalize(v, axis=1): v * rsqrt(max(sum v^2, 1e-12))."""
+    return v * torch.rsqrt(torch.clamp_min(torch.sum(v * v, dim=1, keepdim=True), 1e-12))
+
+
+def confocal_microscopy_3d(batch_size=128, num_points=5, ROI=(28, 28, 28), stddev=0.01):
+    """Fit num_points Gaussian point-spread functions and a background to a simulated confocal image (DM/problems.py:
+    701-956, the ``inference=False`` branch :799-956).  Trainables [batch, 1]: I_var_p, x_var_p, y_var_p, z_var_p,
+    sigmaxy_var_p, sigmaz_var_p per point, then bg_var; the simulated constants likewise (``y_sim%d`` has no underscore
+    in the reference, :871), then bg_sim."""
+    ROI = tuple(int(n) for n in ROI)
+
+    def build():
+        var = [[get_variable("%s_var_%d" % (name, i), shape=[batch_size, 1], initializer=random_uniform_initializer())
+                for name in _PSF_PARAMS] for i in range(num_points)]
+        sim = [[get_variable(("y_sim%d" if name == "y" else name + "_sim_%d") % i, shape=[batch_size, 1],
+                             initializer=random_uniform_initializer(), trainable=False)
+                for name in _PSF_PARAMS] for i in range(num_points)]
+        y_pred = _psf_3d(var[0], ROI)
+        for i in range(1, num_points):
+            y_pred = y_pred + _psf_3d(var[i], ROI)
+        y_sim = _psf_3d(sim[0], ROI)
+        for i in range(1, num_points):
+            y_sim = y_sim + _psf_3d(sim[i], ROI)
+        bg_var = get_variable("bg_var", shape=[batch_size, 1], initializer=random_normal_initializer(stddev=stddev))
+        bg_sim = get_variable("bg_sim", shape=[batch_size, 1], initializer=random_uniform_initializer(), trainable=False)
+        return torch.mean(torch.sum((y_pred + bg_var - _l2_normalize(y_sim + bg_sim)) ** 2, dim=1))
+    # the separable PSF lets one kernel launch produce f and df/dx without forming the [batch, voxels] image in HBM
+    if confocal_fits(num_points, ROI):
+        names = ["%s_var_%d" % (n, i) for i in range(num_points) for n in _PSF_PARAMS] + ["bg_var"]
+        sims = [("y_sim%d" if n == "y" else n + "_sim_%d") % i for i in range(num_points) for n in _PSF_PARAMS]
+        build.fused = FusedSpec("confocal_psf", "I_var_0", "I_sim_0", "bg_sim",
+                                extra=dict(num_points=num_points, roi=ROI, variables=names, constants=sims + ["bg_sim"]))
+    return build
+
+
+def square_cos(batch_size=128, num_dims=10, stddev=0.01):
+    """f = mean_b( ||W_b x_b - y_b||^2 - sum(Wcos_b 10 cos(c x_b)) + 10 num_dims ), c = fp32(2 * 3.1415926)
+    (DM/problems.py:959-995).  At the registry's 256 coordinates the graph-captured autograd step is the fast path
+    (see ``quadratic``), so it has no kernel."""
+    c = float(np.float32(2 * 3.1415926))
+
+    def build():
+        x = get_variable("x", shape=[batch_size, num_dims], initializer=random_normal_initializer(stddev=stddev))
+        w = get_variable("w", shape=[batch_size, num_dims, num_dims], initializer=random_uniform_initializer(),
+                         trainable=False)
+        y = get_variable("y", shape=[batch_size, num_dims], initializer=random_uniform_initializer(), trainable=False)
+        wcos = get_variable("wcos", shape=[batch_size, num_dims, num_dims], initializer=random_uniform_initializer(),
+                            trainable=False)
+        product = torch.bmm(w, x.unsqueeze(-1)).squeeze(-1)
+        product2 = torch.bmm(wcos, (10 * torch.cos(c * x)).unsqueeze(-1)).squeeze(-1)
+        product3 = torch.sum((product - y) ** 2, 1) - torch.sum(product2, 1) + 10 * num_dims
+        return torch.mean(product3)
+    return build

@@ -98,6 +98,12 @@ def get_config(problem_name, path=None, mode=None, num_hidden_layer=None, net_na
     elif problem_name == "lasso":
         problem = problems.lasso(batch_size=128, num_dims=2)
         net_config = _cw20(path)
+    elif problem_name == "confocal_microscopy_3d":
+        problem = problems.confocal_microscopy_3d(batch_size=32, num_points=5)
+        net_config = _cw20(path)
+    elif problem_name == "square_cos":
+        problem = problems.square_cos(batch_size=128, num_dims=2)
+        net_config = _cw20(path)
     elif problem_name == "rastrigin_separable":   # BASELINE config #5
         problem = problems.rastrigin_separable(num_dims=1000000)
         net_config = _cw20(path)
