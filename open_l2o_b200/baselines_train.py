@@ -22,7 +22,7 @@ from . import _lib
 from ._lib import LrsgdBwdArgs, TadamBwdArgs
 from .engine import _ptr, _stream
 from .scale_base import MetaTrainerBase, planes_step, train_optimizer  # noqa: F401  (public names)
-from .trainable_baselines import _tadam_theta, lrsgd_step_launch, tadam_step_launch
+from .trainable_baselines import TADAM_THETA_SPEC, _tadam_theta, lrsgd_step_launch, tadam_step_launch
 
 # (theta [4], planes [3, N], g) -> (planes', update)
 _TadamStep = planes_step(tadam_step_launch, TadamBwdArgs, "l2o_tadam_bwd")
@@ -78,6 +78,7 @@ class _BaselineTrainer(MetaTrainerBase):
 class TrainableAdamTrainer(_BaselineTrainer):
     """Meta-trains TrainableAdam's four scalars (theta = log_learning_rate, beta1_logit, beta2_logit, log_epsilon)."""
     what = "TrainableAdam"
+    theta_spec = TADAM_THETA_SPEC
 
     def __init__(self, shapes, theta: Optional[torch.Tensor] = None, device="cuda:0", **kwargs):
         super().__init__(shapes, _tadam_theta(1e-3, 0.9, 0.999, 1e-8) if theta is None else theta, device, **kwargs)

@@ -38,6 +38,7 @@ class MetaTrainer(MetaTrainerBase):
     ``theta`` is the optimizer's flat weight vector (``CoordinatewiseRNN.theta`` layout).  ``use_second_derivatives``
     (default ``False``, the first-order meta-gradient): see ``MetaTrainerBase``."""
     what = "CoordinatewiseRNN"
+    theta_spec = THETA_SPEC
 
     def __init__(self, shapes: Sequence[Sequence[int]], theta: Optional[torch.Tensor] = None, device="cuda:0",
                  learning_rate=1e-6, rms_decay=0.9, rms_epsilon=1e-20, gradient_clip=1e4, l2_reg=0.0,

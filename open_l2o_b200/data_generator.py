@@ -1,10 +1,41 @@
 """Imitation-learning data (DM/data_generator.py:35-124): roll a hand-designed optimizer (Adam / RMSProp / Nesterov
-momentum, TF-1.14 update rules, lr 0.01) on the optimizee and record, per unroll, the flattened gradients
+momentum, TF-1.14 update rules, lr 0.01: ``teacher_update``, which L2O-Scale's ``scale_base.teacher_labels`` shares) on
+the optimizee and record, per unroll, the flattened gradients
 ``inputs [T, N]`` and the parameter moves ``labels [T, N]`` for every net subset."""
 from __future__ import annotations
 
 import numpy as np
 import torch
+
+TEACHERS = ("adam", "rmsprop", "nag")
+
+
+def teacher_state(x: torch.Tensor) -> dict:
+    """Fresh slots of a teacher for the coordinates ``x``."""
+    return dict(m=torch.zeros_like(x), v=torch.zeros_like(x), k=0)
+
+
+def teacher_update(name: str, x: torch.Tensor, g: torch.Tensor, st: dict, lr: float = 0.01):
+    """One step of a hand-designed teacher with the TF-1.14 update rules, on ``x`` and the slots ``st`` in place.
+    The imitation data of L2O-DM (``data_loader.get_data``) and of L2O-Scale (``scale_base.teacher_labels``) both
+    come from here."""
+    if name == "adam":            # tf.train.AdamOptimizer(0.01)
+        st["k"] += 1
+        st["m"].mul_(0.9).add_(g, alpha=0.1)
+        st["v"].mul_(0.999).addcmul_(g, g, value=0.001)
+        lr_t = lr * np.sqrt(1 - 0.999 ** st["k"]) / (1 - 0.9 ** st["k"])
+        x.sub_(lr_t * st["m"] / (st["v"].sqrt() + 1e-8))
+    elif name == "rmsprop":       # tf.train.RMSPropOptimizer(0.01): decay 0.9, eps 1e-10, ms initialised to 1
+        if st["k"] == 0:
+            st["v"].fill_(1.0)
+        st["k"] += 1
+        st["v"].mul_(0.9).addcmul_(g, g, value=0.1)
+        x.sub_(lr * g / (st["v"] + 1e-10).sqrt())
+    elif name == "nag":           # tf.train.MomentumOptimizer(0.01, 0.9, use_nesterov=True)
+        st["m"].mul_(0.9).add_(g)
+        x.sub_(lr * (g + 0.9 * st["m"]))
+    else:
+        raise ValueError("unknown teacher %r (one of %s)" % (name, ", ".join(TEACHERS)))
 
 
 class data_loader(object):
@@ -43,27 +74,10 @@ class data_loader(object):
             prog.assign_x([xv / rs for xv, rs in zip(prog.x_values(), r_scale)])
         prog._apply_scale_feed(feed)
         X = prog.X
-        st = dict(m=torch.zeros_like(X), v=torch.zeros_like(X), k=0)
-        lr = 0.01
+        st = teacher_state(X)
 
         def update(g):
-            if name == "adam":            # tf.train.AdamOptimizer(0.01)
-                st["k"] += 1
-                st["m"].mul_(0.9).add_(g, alpha=0.1)
-                st["v"].mul_(0.999).addcmul_(g, g, value=0.001)
-                lr_t = lr * np.sqrt(1 - 0.999 ** st["k"]) / (1 - 0.9 ** st["k"])
-                X.sub_(lr_t * st["m"] / (st["v"].sqrt() + 1e-8))
-            elif name == "rmsprop":       # tf.train.RMSPropOptimizer(0.01): decay 0.9, eps 1e-10, ms initialised to 1
-                if st["k"] == 0:
-                    st["v"].fill_(1.0)
-                st["k"] += 1
-                st["v"].mul_(0.9).addcmul_(g, g, value=0.1)
-                X.sub_(lr * g / (st["v"] + 1e-10).sqrt())
-            elif name == "nag":           # tf.train.MomentumOptimizer(0.01, 0.9, use_nesterov=True)
-                st["m"].mul_(0.9).add_(g)
-                X.sub_(lr * (g + 0.9 * st["m"]))
-            else:
-                raise ValueError(name)
+            teacher_update(name, X, g, st)
 
         sl = self._subset_slices()
         data = {"inputs": [], "labels": []}

@@ -104,7 +104,9 @@ class ScaleOptimizer(object):
             kwargs.setdefault("init_lr_range", self.init_lr_range)
         module, cls = self.trainer.rsplit(".", 1)   # the trainer modules import the optimizer modules
         cls = getattr(importlib.import_module("." + module, __package__), cls)
-        return cls([tuple(v.shape) for v in var_list], theta=self.theta, device=str(self.device), **kwargs)
+        tr = cls([tuple(v.shape) for v in var_list], theta=self.theta, device=str(self.device), **kwargs)
+        tr.theta_spec = self.theta_spec      # checkpoints of the trainer carry this optimizer's variable names
+        return tr
 
     def adopt(self, trainer):
         self.theta.copy_(trainer.theta.detach())
@@ -219,6 +221,7 @@ class MetaTrainerBase(object):
     meta-gradient; the second-order one keeps the optimizee's double-backward graph of every step of an unroll alive
     until the meta-gradient is taken."""
     what = ""
+    theta_spec = None     # (name, shape) layout of theta for get_variables; None: one flat "theta"
 
     def __init__(self, shapes, theta, device, learning_rate, rms_decay, rms_epsilon, gradient_clip, l2_reg,
                  use_log_objective, use_numerator_epsilon, init_lr_range, random_seed, use_second_derivatives):
@@ -278,27 +281,48 @@ class MetaTrainerBase(object):
         return obj, (g if second else g.detach()).contiguous()
 
     def unroll(self, objective: Callable, state, num_steps: int, theta: Optional[torch.Tensor] = None,
-               obj_weights: Optional[Sequence[float]] = None, initial_obj: Optional[torch.Tensor] = None):
+               obj_weights: Optional[Sequence[float]] = None, initial_obj: Optional[torch.Tensor] = None,
+               labels: Optional[torch.Tensor] = None, grads: Optional[torch.Tensor] = None):
         """``loop_body`` x num_steps (trainable_optimizer.py:263-401).  Returns (meta objective with its graph, the list
-        of objective values, the final state with its graph)."""
+        of objective values, the final state with its graph).
+
+        With ``labels`` ([num_steps, N], a teacher's positive steps) the unroll imitates (``mode_mt``): x is
+        teacher-forced, ``x_{t+1} = x_t - labels[t]`` (hierarchical_rnn.py:398-404), while the optimizer's own update
+        still drives its state, and the meta objective is ``sum_t w_t sum_i (upd_t,i - labels_t,i)^2 / 2 / N`` with
+        ``w_t = 1 / num_steps`` by default (trainable_optimizer.py:383-389, SC/metaopt.py:407-408).  ``grads``
+        ([num_steps, N]) are the optimizee gradients at the teacher-forced points, recorded by ``teacher_labels``: given,
+        the unroll replays them and evaluates no objective; None, it evaluates ``objective`` at each forced point."""
         if num_steps < 1:
             raise ValueError("an unroll needs at least one step")
         step = self._stepper(self.theta if theta is None else theta)
         x = state.x
         objs, total = [], 0.0
-        w = [1.0] * num_steps if obj_weights is None else list(obj_weights)
+        if obj_weights is not None:
+            w = list(obj_weights)
+        else:
+            w = [1.0] * num_steps if labels is None else [1.0 / num_steps] * num_steps
         for t in range(num_steps):
-            # objective at x_t and its gradient: a constant of the meta-gradient (stop_gradient,
-            # trainable_optimizer.py:330-338) unless use_second_derivatives
-            obj, g = self._objective_and_gradient(objective, x)
-            objs.append(obj)
-            total = total + w[t] * obj
+            if grads is None:
+                # objective at x_t and its gradient: a constant of the meta-gradient (stop_gradient,
+                # trainable_optimizer.py:330-338) unless use_second_derivatives
+                obj, g = self._objective_and_gradient(objective, x)
+                objs.append(obj)
+            else:
+                g = grads[t]
             upd, state = step(state, g)
-            x = x - upd
+            if labels is None:
+                total = total + w[t] * obj
+                x = x - upd
+            else:
+                d = upd - labels[t]
+                total = total + (w[t] * 0.5 / d.numel()) * (d * d).sum()
+                x = x - labels[t]
+        state.x = x
+        if labels is not None:
+            return total, objs, state
         # normalised by the objective at the start of the SERIES of partial unrolls (trainable_optimizer.py:438-441)
         initial = objs[0].detach() if initial_obj is None else initial_obj
         meta = self.scale_objective(total, torch.stack([o.reshape(()) for o in objs]), initial)
-        state.x = x
         return meta, objs, state
 
     # ---- meta step -------------------------------------------------------------------------------------------------
@@ -308,10 +332,27 @@ class MetaTrainerBase(object):
         """(meta objective, d meta / d theta, objective values, final state) of one unroll — from ``params`` with a fresh
         optimizer state, or continuing from ``state`` (a detached state: truncated BPTT over partial unrolls).
         ``log_learning_rate``: the initial learning-rate state handed to ``initial_state`` (drawn when None)."""
+        return self._meta_gradient(objective, params, num_steps, log_learning_rate, state, initial_obj=initial_obj)
+
+    def meta_gradient_mt(self, objective: Optional[Callable], params: Sequence[torch.Tensor], labels: torch.Tensor,
+                         grads: Optional[torch.Tensor], log_learning_rate: Optional[torch.Tensor] = None, state=None):
+        """``meta_gradient`` of one imitation unroll (``metaobjmt``): ``labels.shape[0]`` steps with x teacher-forced
+        along ``labels`` and the meta objective the weighted mean-square distance of the optimizer's updates from them
+        (``unroll``).  Returns (meta objective, d meta / d theta, objective values, final state).
+
+        Replay, not re-evaluation: on a teacher-forced run x_t is a point where the teacher took its gradient, so the
+        unroll consumes the gradient rows ``grads`` that ``teacher_labels`` recorded there and evaluates no objective
+        (the objective values are then an empty list; ``objective`` may be None).  ``grads=None`` evaluates
+        ``objective`` at the forced points instead.  Either way the gradients are constants of the meta-gradient, also
+        under ``use_second_derivatives``: x_t does not depend on theta."""
+        return self._meta_gradient(objective, params, int(labels.shape[0]), log_learning_rate, state, labels=labels,
+                                   grads=grads)
+
+    def _meta_gradient(self, objective, params, num_steps, log_learning_rate, state, **unroll_kwargs):
         if self.theta.grad is not None:
             self.theta.grad = None
         st = state if state is not None else self.initial_state(params, self.theta, log_learning_rate)
-        meta, objs, final = self.unroll(objective, st, num_steps, initial_obj=initial_obj)
+        meta, objs, final = self.unroll(objective, st, num_steps, **unroll_kwargs)
         loss = meta + self.l2_reg * (self.theta ** 2).sum() if self.l2_reg else meta
         # (a one-step unroll scores only f(x_0): constant, no meta-gradient)
         grad = torch.autograd.grad(loss, self.theta)[0] if loss.requires_grad else torch.zeros_like(self.theta)
@@ -366,6 +407,56 @@ class MetaTrainerBase(object):
         out = self._split(state.x) if state is not None else [p.detach() for p in params]
         return metas, values, out
 
+    def train_problem_mt(self, objective: Optional[Callable], params: Sequence[torch.Tensor], labels: torch.Tensor,
+                         grads: Optional[torch.Tensor], unroll_lens: Sequence[int],
+                         log_learning_rate: Optional[torch.Tensor] = None):
+        """One imitation run (SC/metaopt.py:541-548): the partial unrolls of ``unroll_lens`` over consecutive rows of
+        ``labels`` / ``grads`` (``teacher_labels`` of the whole run), each ``meta_gradient_mt`` followed by the clipped
+        RMSProp meta-step on the same accumulator, optimizer state carried (detached) from unroll to unroll.  Returns
+        (meta objectives, final optimizee tensors)."""
+        unroll_lens = [int(n) for n in unroll_lens]
+        if sum(unroll_lens) != labels.shape[0] or (grads is not None and grads.shape[0] != labels.shape[0]):
+            raise ValueError("labels / grads must have one row per step of the run (%d)" % sum(unroll_lens))
+        state, metas, off = None, [], 0
+        for ln in unroll_lens:
+            rows = slice(off, off + ln)
+            meta, grad, _, final = self.meta_gradient_mt(objective, params, labels[rows],
+                                                         None if grads is None else grads[rows], log_learning_rate,
+                                                         state=state)
+            self.apply_meta_gradient(grad)
+            metas.append(float(meta))
+            state = self.detach_state(final)
+            off += ln
+        out = self._split(state.x) if state is not None else [p.detach() for p in params]
+        return metas, out
+
+    def evaluate(self, objective: Callable, params: Sequence[torch.Tensor], unroll_lens: Sequence[int]) -> float:
+        """``validate`` (SC/metaopt.py:741-780): a run of partial unrolls from ``params`` with a fresh optimizer state,
+        state carried from unroll to unroll, no meta-gradient and no meta-step.  Returns the objective at the run's
+        last step."""
+        if not unroll_lens:
+            raise ValueError("an evaluation run needs at least one unroll")
+        theta = self.theta.detach()
+        with torch.no_grad():
+            state = self.initial_state(params, theta, None)
+            for ln in unroll_lens:
+                _, objs, state = self.unroll(objective, state, int(ln), theta=theta)
+        return float(objs[-1])
+
+    def get_variables(self) -> Dict[str, torch.Tensor]:
+        """Named copies of theta (``ScaleOptimizer.get_variables`` names when ``theta_spec`` is known), for checkpoints
+        that ``ScaleOptimizer.load_variables`` and ``load_variables`` read back."""
+        return {k: v.clone() for k, v in theta_views(self.theta.detach().cpu(), self._spec()).items()}
+
+    def load_variables(self, values: Dict[str, torch.Tensor]):
+        spec = self._spec()
+        with torch.no_grad():
+            for name, view in theta_views(self.theta, spec).items():
+                view.copy_(torch.as_tensor(values[name], dtype=torch.float32).reshape(view.shape))
+
+    def _spec(self):
+        return self.theta_spec or [("theta", (self.theta.numel(),))]
+
     def train_step(self, objective: Callable, params: Sequence[torch.Tensor], num_steps: int,
                    log_learning_rate: Optional[torch.Tensor] = None):
         meta, grad, objs, final = self.meta_gradient(objective, params, num_steps, log_learning_rate)
@@ -373,25 +464,115 @@ class MetaTrainerBase(object):
         return float(meta), objs, self._split(final.x.detach())
 
 
+def teacher_labels(objective: Callable, x0: torch.Tensor, sizes: Sequence, lens: Sequence[int], name: str = "adam",
+                   k: int = 1):
+    """The imitation targets of one run (``mt_utils.get_mt_labels``, SC/mt_utils.py:55-92): a teacher (``name``:
+    "adam", "rmsprop" or "nag", the TF-1.14 rules with lr 0.01 and fresh slots, ``data_generator.teacher_update``)
+    starts at the flat coordinates ``x0`` and takes ``k`` steps per label.  ``sizes``: the optimizee tensors' shapes
+    (an int is a 1-D tensor), for ``objective(list of tensors) -> scalar``; ``lens``: the run's partial-unroll
+    lengths.
+
+    Returns ``(labels, grads)``, both ``[sum(lens), N]`` in run order.  ``labels[t] = x_prev - x_cur`` over the t-th
+    group of ``k`` steps (the positive step: ``x - labels[t]`` is the teacher's next point); ``grads[t]`` is the
+    gradient at the group's first point, the point a teacher-forced unroll visits at step t.  After each group the
+    teacher continues from ``x_prev - labels[t]``, which is what teacher forcing computes, so those points are
+    bitwise the ones ``MetaTrainerBase.meta_gradient_mt`` replays.  Both live on x0's device: 8 N bytes per step."""
+    from .data_generator import teacher_state, teacher_update
+    if k < 1:
+        raise ValueError("mt_k must be >= 1")
+    shapes = [tuple(int(d) for d in s) if isinstance(s, (tuple, list, torch.Size)) else (int(s),) for s in sizes]
+    counts = [int(math.prod(s)) for s in shapes]
+    x = x0.detach().reshape(-1).float().clone()
+    if sum(counts) != x.numel():
+        raise ValueError("sizes cover %d coordinates, x0 has %d" % (sum(counts), x.numel()))
+
+    def gradient(at):
+        with torch.enable_grad():
+            xg = at.detach().requires_grad_(True)
+            (g,) = torch.autograd.grad(objective([v.view(s) for v, s in zip(xg.split(counts), shapes)]), xg)
+        return g.detach().contiguous()
+
+    T = int(sum(int(n) for n in lens))
+    labels = torch.empty(T, x.numel(), dtype=x.dtype, device=x.device)
+    grads = torch.empty_like(labels)
+    st = teacher_state(x)
+    for t in range(T):
+        x_prev = x.clone()
+        for j in range(k):
+            g = gradient(x)
+            if j == 0:
+                grads[t] = g
+            teacher_update(name, x, g, st)
+        torch.sub(x_prev, x, out=labels[t])
+        torch.sub(x_prev, labels[t], out=x)
+    return labels, grads
+
+
+SCALE_NUM_STEPS = [100, 200, 500, 1000, 1500, 2000, 2500, 3000, 3500, 4000, 4500, 5000]   # SC/metaopt.py:172
+
+
 def train_optimizer(make_trainer: Callable, problems: Sequence, num_problems: int, num_meta_iterations: int,
                     num_unroll_func: Callable[[], int], num_partial_unroll_itrs_func: Callable[[], int],
                     select_random_problems: bool = True, callbacks: Optional[Sequence[Callable]] = None,
                     fix_unroll: bool = False, fix_unroll_length: int = 20, fix_num_steps: int = 100, seed: int = 0,
-                    out=None):
-    """The sampling loop of ``metaopt.train_optimizer`` (SC/metaopt.py:117-613) around a meta-trainer: ``num_problems``
+                    out=None, if_mt: bool = False, mt_ratio: float = 0.3, mt_k: int = 1, teacher: str = "adam",
+                    if_cl: bool = False, evaluation_period: int = 1, evaluation_epochs: int = 20,
+                    fix_num_steps_eval: int = 100, save_path: Optional[str] = None, min_num_eval: int = 3):
+    """The sampling loop of ``metaopt.train_optimizer`` (SC/metaopt.py:117-700) around a meta-trainer: ``num_problems``
     draws of a training problem; on each, ``num_meta_iterations`` optimizee runs, every run a series of partial unrolls
     (``num_unroll_func()`` unrolls of ``num_partial_unroll_itrs_func()`` steps, or ``fix_num_steps // fix_unroll_length``
     unrolls of ``fix_unroll_length`` steps with ``fix_unroll``) with a clipped RMSProp meta-step after each unroll.
 
     problems: sequence of ``(objective, init_fn)`` — ``objective(list of tensors) -> scalar``, ``init_fn() -> list of
     tensors`` (fresh optimizee parameters for a run).  make_trainer(shapes, theta) -> a ``MetaTrainerBase`` (or, when
-    every run's partial unrolls have one length, anything with ``theta`` and ``train_problem``); one trainer per problem
-    shape, theta handed on from problem to problem.  Returns (theta, log of (problem index, meta objectives)).  The
-    curriculum / evaluation / checkpoint bookkeeping of the reference driver (SC/metaopt.py:172-176, 613-700) is
-    host-side policy and stays with the caller."""
+    every run's partial unrolls have one length and the keywords below are off, anything with ``theta`` and
+    ``train_problem``); one trainer per problem shape, theta handed on from problem to problem.  Returns (theta, log of
+    (problem index, meta objectives)) with one entry per optimizee run; imitation runs are not logged.
+
+    The enhanced-training recipe (all off by default; off, the loop draws no extra random number and runs exactly the
+    plain loop):
+
+    * ``if_mt``: each run is, with probability ``mt_ratio`` (drawn from the seeded generator that also draws the
+      problems), an imitation run: ``teacher_labels(name=teacher, k=mt_k)`` from the run's initial tensors, then
+      ``train_problem_mt`` over the same partial unrolls (SC/metaopt.py:354-360, 416-431, 541-548).
+    * ``if_cl``: the curriculum (SC/metaopt.py:170-176, 613-690) — runs of ``SCALE_NUM_STEPS[idx] // fix_unroll_length``
+      unrolls of ``fix_unroll_length`` steps, evaluated at the next stage's length.  The schedule is
+      ``train_dm.Curriculum``: a new best saves ``-idx`` and ``-0``; ``min_num_eval`` evaluations after an improvement
+      restore ``-idx`` and advance (and re-evaluate); ``min_num_eval`` without one end this problem's runs.  At the
+      last stage evaluation runs at that stage's own length.
+    * Evaluation (with ``if_cl`` or ``save_path``): every ``evaluation_period`` runs of a problem, the mean over
+      ``evaluation_epochs`` fresh starts of the objective at the last step of an evaluation run
+      (``MetaTrainerBase.evaluate``); without ``if_cl`` the run has ``fix_num_steps_eval // fix_unroll_length`` unrolls
+      and a new best is saved as ``-0``.
+    * ``save_path``: checkpoints are ``torch.save`` files of the trainer's ``get_variables()`` at
+      ``"<save_path>-<idx>"``.  The restore of an advance reads the in-memory copy of the same snapshot, so the
+      curriculum also runs without ``save_path``."""
     import random
+    from .train_dm import Curriculum
     rng = random.Random(seed)
     theta, rms, log, trainers = None, None, [], {}
+    cl = Curriculum(fix_unroll_length, min_num_eval, SCALE_NUM_STEPS) if if_cl else None
+    evaluating = if_cl or save_path is not None
+    best, snapshots = float("inf"), {}
+
+    def say(msg):
+        if out is not None:
+            print(msg, file=out)
+
+    def save(tr, idx):
+        snapshots[idx] = tr.get_variables()
+        if save_path is not None:
+            torch.save(snapshots[idx], "%s-%d" % (save_path, idx))
+
+    def evaluate(tr, objective, init_fn):
+        if cl is None:
+            n = fix_num_steps_eval // fix_unroll_length
+        else:    # the next stage's length; the last stage has no next one
+            i = cl.idx if cl.idx >= 0 else len(cl.num_unrolls) - 1
+            n = cl.num_unrolls[min(i + 1, len(cl.num_unrolls) - 1)]
+        lens = [fix_unroll_length] * n
+        return sum(tr.evaluate(objective, init_fn(), lens) for _ in range(evaluation_epochs)) / evaluation_epochs
+
     for draw in range(num_problems):
         k = rng.randrange(len(problems)) if select_random_problems else draw % len(problems)
         objective, init_fn = problems[k]
@@ -404,20 +585,50 @@ def train_optimizer(make_trainer: Callable, problems: Sequence, num_problems: in
                 tr.theta.copy_(theta)
                 if rms is not None and getattr(tr, "rms", None) is not None:
                     tr.rms.copy_(rms)
-        for _ in range(num_meta_iterations):
-            if fix_unroll:
+        for it in range(num_meta_iterations):
+            mt = if_mt and rng.random() < mt_ratio
+            if cl is not None:
+                lens = [fix_unroll_length] * cl.train_unrolls()
+            elif fix_unroll:
                 lens = [fix_unroll_length] * (fix_num_steps // fix_unroll_length)
             else:
                 lens = [num_partial_unroll_itrs_func() for _ in range(num_unroll_func())]
             params = init_fn()
-            # the reference feeds one unroll length per partial unroll
-            if len(set(lens)) <= 1:
-                metas, _, _ = tr.train_problem(objective, params, len(lens), lens[0] if lens else 0)
+            if mt and lens:
+                labels, grads = teacher_labels(objective, tr._x0(params), tr.shapes, lens, teacher, mt_k)
+                metas, _ = tr.train_problem_mt(None, params, labels, grads, lens)
+                del labels, grads
+                say("problem %d: imitation (%s), %d unrolls, meta objective %s"
+                    % (k, teacher, len(metas), ["%.4g" % m for m in metas]))
             else:
-                metas, _, _ = tr._train_unrolls(objective, params, lens)
-            log.append((k, metas))
-            if out is not None:
-                print("problem %d: %d unrolls, meta objective %s" % (k, len(metas), ["%.4f" % m for m in metas]), file=out)
+                # the reference feeds one unroll length per partial unroll
+                if len(set(lens)) <= 1:
+                    metas, _, _ = tr.train_problem(objective, params, len(lens), lens[0] if lens else 0)
+                else:
+                    metas, _, _ = tr._train_unrolls(objective, params, lens)
+                log.append((k, metas))
+                say("problem %d: %d unrolls, meta objective %s" % (k, len(metas), ["%.4f" % m for m in metas]))
+            if not evaluating or (it + 1) % evaluation_period != 0:
+                continue
+            cost = evaluate(tr, objective, init_fn)
+            say("problem %d: evaluation %.6g" % (k, cost))
+            if cl is None:
+                if cost < best:
+                    best = cost
+                    save(tr, 0)
+                continue
+            action = cl.observe(cost)
+            if action[0] == "save":
+                save(tr, action[1])
+                save(tr, 0)
+            elif action[0] == "advance":
+                tr.load_variables(snapshots[action[1]])
+                cl.rebase(evaluate(tr, objective, init_fn))
+                say("curriculum %d -> %d (%d steps), evaluation %.6g" % (action[1], action[2], cl.num_steps[action[2]],
+                                                                         cl.best))
+            elif action[0] == "stop":
+                say("no improvement during curriculum %d: stop" % action[1])
+                break
         theta, rms = tr.theta, getattr(tr, "rms", None)
         for cb in callbacks or ():
             cb(draw, k, tr)
