@@ -312,11 +312,10 @@ int l2o_hrnn_step(l2o_hrnn_handle h, const l2o_hrnn_args* a, void* stream);
 /* Sharded use (SURVEY.md 8(e): the one path with an exchange per INNER step).  Every rank holds a contiguous slice of
  * every tensor's coordinates (tensor_sizes given to l2o_hrnn_create are the LOCAL counts, 0 allowed) and replicas of
  * layer / global.  l2o_hrnn_set_global_sizes gives the counts the per-tensor and problem-wide means divide by.  Per
- * step: l2o_hrnn_step_local; all-reduce SUM of the n_doubles fp64 values at the start of the workspace and all-reduce
- * MAX of the n_flags int32 values at flags_offset_bytes (l2o_hrnn_reduce_layout); l2o_hrnn_step_finish.  Same for
+ * step: l2o_hrnn_step_local; all-reduce SUM of the n_tensors x 24 fp64 sums at workspace offset [0] and all-reduce MAX
+ * of the n_tensors x 4 int32 flags at offset [1] (l2o_hrnn_workspace_layout); l2o_hrnn_step_finish.  Same for
  * prepare.  l2o_hrnn_step / l2o_hrnn_prepare are exactly local + finish. */
 int l2o_hrnn_set_global_sizes(l2o_hrnn_handle h, const int64_t* global_sizes);
-int l2o_hrnn_reduce_layout(l2o_hrnn_handle h, int64_t* n_doubles, int64_t* flags_offset_bytes, int64_t* n_flags);
 int l2o_hrnn_prepare_local(l2o_hrnn_handle h, const l2o_hrnn_args* a, void* stream);
 int l2o_hrnn_prepare_finish(l2o_hrnn_handle h, const l2o_hrnn_args* a, void* stream);
 int l2o_hrnn_step_local(l2o_hrnn_handle h, const l2o_hrnn_args* a, void* stream);

@@ -31,7 +31,7 @@ EXPORTS = [
     "l2o_launch_count", "l2o_status_string", "l2o_last_cuda_error", "l2o_version",
     "l2o_hrnn_create", "l2o_hrnn_destroy", "l2o_hrnn_theta_count", "l2o_hrnn_state_floats", "l2o_hrnn_coords",
     "l2o_hrnn_workspace_bytes", "l2o_hrnn_init_state", "l2o_hrnn_prepare", "l2o_hrnn_step",
-    "l2o_hrnn_set_global_sizes", "l2o_hrnn_reduce_layout", "l2o_hrnn_prepare_local", "l2o_hrnn_prepare_finish",
+    "l2o_hrnn_set_global_sizes", "l2o_hrnn_prepare_local", "l2o_hrnn_prepare_finish",
     "l2o_hrnn_step_local", "l2o_hrnn_step_finish", "l2o_hrnn_coord_bwd", "l2o_hrnn_workspace_layout",
     "l2o_crnn_theta_count", "l2o_crnn_state_floats", "l2o_crnn_step", "l2o_crnn_bwd",
     "l2o_tadam_theta_count", "l2o_tadam_state_floats", "l2o_tadam_step", "l2o_tadam_bwd", "l2o_lrsgd_step",
@@ -262,8 +262,6 @@ def lib():
         getattr(L, name).restype = C.c_int64
     L.l2o_hrnn_set_global_sizes.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
     L.l2o_hrnn_set_global_sizes.restype = C.c_int
-    L.l2o_hrnn_reduce_layout.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
-    L.l2o_hrnn_reduce_layout.restype = C.c_int
     L.l2o_hrnn_coord_bwd.argtypes = [C.c_void_p, C.POINTER(HrnnBwdArgs), C.c_void_p]
     L.l2o_hrnn_coord_bwd.restype = C.c_int
     L.l2o_hrnn_workspace_layout.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]

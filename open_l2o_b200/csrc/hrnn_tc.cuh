@@ -1,7 +1,8 @@
 // HierarchicalRNN per-parameter level on the sm_90a tensor cores (included by l2o_hrnn.cu, inside namespace l2o::hrnn).
 //
-// Same arithmetic as coord_kernel (HR:444-540 features, rnn_cells.py:46-68 BiasGRU(10), HR:606-706 readouts); the
-// two GRU products run as error-compensated 3xTF32 wgmma with the per-coordinate operand rows staged in shared memory:
+// The step of oracle/hrnn_oracle.py and of the exact-fp32 recompute in hrnn_bwd.cuh (HR:444-540 features,
+// rnn_cells.py:46-68 BiasGRU(10), HR:606-706 readouts); the two GRU products run as error-compensated 3xTF32 wgmma with
+// the per-coordinate operand rows staged in shared memory:
 //   MMA 1  D[128 x 48] = A1[128 x 24] . B1[24 x 48]     A1 = [feat 0..11 | h 12..21 | 1 | 0]
 //          D columns: r 0..9 | u 16..25 | candidate (feature part + bc) 32..41        (per 64-row half: 3 K-steps x 3)
 //   MMA 2  D[:, 32..47] += A2[128 x 16] . B2[16 x 16]   A2 = [r*h 0..9 | 0]           (the same accumulator registers)

@@ -135,7 +135,7 @@ int l2o_step(l2o_handle h, const l2o_step_args* a, void* stream) {
   const bool tc_can = l2o::tc_step_ok(h, *a);
   if (h->engine == L2O_ENGINE_TC) return tc_can ? l2o::tc_step(h, *a, st) : L2O_E_UNSUPPORTED;
   // AUTO: the tensor-core path pays a fixed cost (weight image prep + staging) per launch; use it for real sizes
-  if (h->engine == L2O_ENGINE_AUTO && tc_can && l2o::tc_auto_default() && a->n >= 16384) return l2o::tc_step(h, *a, st);
+  if (h->engine == L2O_ENGINE_AUTO && tc_can && a->n >= 16384) return l2o::tc_step(h, *a, st);
   return l2o::ffma_step(h, *a, st);
 }
 
@@ -155,7 +155,7 @@ int l2o_unroll_fwd(l2o_handle h, const l2o_unroll_args* a, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   const bool tc_can = l2o::tc_supported(h->cfg) && l2o::tc_fwd_ok(h, *a);
   if (h->engine == L2O_ENGINE_TC) return tc_can ? l2o::tc_unroll_fwd(h, *a, st) : L2O_E_UNSUPPORTED;
-  if (h->engine == L2O_ENGINE_AUTO && tc_can && l2o::tc_auto_default()) return l2o::tc_unroll_fwd(h, *a, st);
+  if (h->engine == L2O_ENGINE_AUTO && tc_can) return l2o::tc_unroll_fwd(h, *a, st);
   return l2o::ffma_unroll_fwd(h, *a, st);
 }
 
@@ -175,7 +175,7 @@ int l2o_unroll_bwd(l2o_handle h, const l2o_bwd_args* a, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   const bool tc_can = l2o::tc_bwd_ok(h, *a);
   if (h->engine == L2O_ENGINE_TC) return tc_can ? l2o::tc_unroll_bwd(h, *a, st) : L2O_E_UNSUPPORTED;
-  if (h->engine == L2O_ENGINE_AUTO && tc_can && l2o::tc_bwd_auto_default()) return l2o::tc_unroll_bwd(h, *a, st);
+  if (h->engine == L2O_ENGINE_AUTO && tc_can) return l2o::tc_unroll_bwd(h, *a, st);
   return l2o::ffma_unroll_bwd(h, *a, st);
 }
 
@@ -193,7 +193,7 @@ int l2o_unroll_bwd_carry(l2o_handle h, const l2o_bwd_args* a, const l2o_bwd_carr
   cudaStream_t st = (cudaStream_t)stream;
   const bool tc_can = l2o::tc_bwd_ok(h, *a);
   if (h->engine == L2O_ENGINE_TC) return tc_can ? l2o::tc_unroll_bwd(h, *a, st, c) : L2O_E_UNSUPPORTED;
-  if (h->engine == L2O_ENGINE_AUTO && tc_can && l2o::tc_bwd_auto_default()) return l2o::tc_unroll_bwd(h, *a, st, c);
+  if (h->engine == L2O_ENGINE_AUTO && tc_can) return l2o::tc_unroll_bwd(h, *a, st, c);
   return l2o::ffma_unroll_bwd(h, *a, st, c);
 }
 

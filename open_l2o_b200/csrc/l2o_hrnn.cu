@@ -2,10 +2,12 @@
 // SC/ = Model_Free_L2O/L2O-Scale/L2O-Scale-Training/ of the reference; HR = SC/optimizer/hierarchical_rnn.py.
 //
 // One optimizer step over ALL optimizee tensors is three launches, with no host synchronisation (graph-capturable):
-//   1. coord_kernel  — thread = coordinate (HBM-bound: 88 B read + 88 B written per coordinate-step): gradient
-//                      accumulators at 4 timescales, RMS scaling, the 12 input features, the per-parameter
-//                      BiasGRU(10), the readouts (update direction, decays, log learning rate), and the per-tensor
-//                      sums the upper levels need (fp64 atomics: mean of [h' | features], mean delta^2, sum log-lr).
+//   1. coord_tc_kernel (hrnn_tc.cuh) — thread = coordinate (HBM-bound: 88 B read + 88 B written per coordinate-step):
+//                      gradient accumulators at 4 timescales, RMS scaling, the 12 input features, the per-parameter
+//                      BiasGRU(10) on the tensor cores, the readouts (update direction, decays, log learning rate), and
+//                      the per-tensor sums the upper levels need (fp64 atomics: mean of [h' | features], mean delta^2,
+//                      sum log-lr).  Its reference is the fp64 oracle (oracle/hrnn_oracle.py); the backward
+//                      (hrnn_bwd.cuh) recomputes the same step in exact fp32.
 //   2. tensor_kernel — one CTA: per-tensor BiasGRU(20), the global BiasGRU(20) (fed by the LAST tensor's layer
 //                      state only, HR:426-427), 1/RMS(delta) per tensor, and the NEXT step's per-tensor gate bias,
 //                      problem-wide mean log-lr and first-step flags.
@@ -14,7 +16,6 @@
 //   0..9 parameter (BiasGRU hidden), 10 scl_decay, 11 inp_decay, 12 log_learning_rate, 13..16 grad_accum1..4,
 //   17..20 ms1..4  (HR:303-343; "true_param" duplicates x when use_attention=False and is not stored).
 #include <cstdint>
-#include <cstdlib>
 #include <new>
 #include <mutex>
 #include <vector>
@@ -96,170 +97,6 @@ __device__ __forceinline__ float sqrt_approx(float x) {
 __device__ __forceinline__ float log_fast(float x) { return 0.6931471805599453f * lg2_approx(x); }
 __device__ __forceinline__ float exp_fast(float x) { return ex2_approx(1.4426950408889634f * x); }
 
-// ---------------------------------------------------------------------------------------------------------------
-// per-parameter level (HR:444-540 features, rnn_cells.py:46-68 GRU, HR:606-706 readouts)
-__global__ void __launch_bounds__(kBlock) coord_kernel(const float* __restrict__ theta, const float* __restrict__ g,
-                                                       float* __restrict__ state, int64_t n, const BlockEnt* __restrict__ blocks,
-                                                       Workspace w) {
-  __shared__ __align__(16) float sWg[(F + H0) * 2 * H0];  // [22][20]
-  __shared__ __align__(16) float sWc[(F + H0) * H0];      // [22][10]
-  __shared__ float sSm[64];                               // bg0 20 | bc0 10 | bias0 30
-  __shared__ double sRed[kBlock / 32][kAcc];
-  const BlockEnt be = blocks[blockIdx.x];
-  const int tid = threadIdx.x;
-  for (int k = tid; k < (F + H0) * 2 * H0; k += kBlock) sWg[k] = theta[O_WG0 + k];
-  for (int k = tid; k < (F + H0) * H0; k += kBlock) sWc[k] = theta[O_WC0 + k];
-  float* sBg = sSm;            // 20
-  float* sBc = sSm + 20;       // 10
-  float* sB0 = sSm + 30;       // 30: per-tensor injected bias r|u|c
-  // (the 4x10 readout weights are read straight from theta through the read-only cache)
-  if (tid < 2 * H0) sBg[tid] = theta[O_BG0 + tid];
-  if (tid < H0) sBc[tid] = theta[O_BC0 + tid];
-  if (tid < 3 * H0) sB0[tid] = w.bias0[be.tensor * kB0Stride + tid];
-  __syncthreads();
-
-  const bool act = tid < be.count;
-  const int64_t i = be.start + (act ? tid : 0);
-  float vals[kAcc];
-#pragma unroll
-  for (int k = 0; k < kAcc; ++k) vals[k] = 0.f;
-  int nz_mask = 0;
-  if (act) {
-    float h[H0], in[F + H0];
-#pragma unroll
-    for (int k = 0; k < H0; ++k) h[k] = state[(int64_t)(P_H + k) * n + i];
-    const float sd = state[(int64_t)P_SCL * n + i];
-    const float d0 = state[(int64_t)P_INP * n + i];
-    const float llr = state[(int64_t)P_LLR * n + i];
-    const float gi = g[i];
-    const float mean_llr = *w.mean_log_lr;
-    float dec[NS];
-    dec[0] = d0;
-#pragma unroll
-    for (int s = 1; s < NS; ++s) dec[s] = sqrt_approx(dec[s - 1]);  // each accumulator on twice the timescale (HR:466-470)
-    float sc[NS], lm[NS];
-#pragma unroll
-    for (int s = 0; s < NS; ++s) {
-      const float acc_old = state[(int64_t)(P_ACC + s) * n + i];
-      const float ms_old = state[(int64_t)(P_MS + s) * n + i];
-      const float acc = gi * (1.0f - dec[s]) + acc_old * dec[s];                 // HR:483-484
-      const float dk = w.zero_flag[be.tensor * NS + s] ? 0.f : sd;               // utils.py:128-130
-      const float ms = (1.0f - dk) * (acc * acc + 1e-12f) + dk * ms_old;         // utils.py:133-134
-      const float r = acc * rsqrt_approx(ms + 1e-16f);
-      sc[s] = log_fast(r + sqrt_approx(fmaf(r, r, 1.0f)));                       // utils.asinh as written (utils.py:36-38)
-      lm[s] = log_fast(ms + 1e-16f);
-      state[(int64_t)(P_ACC + s) * n + i] = acc;
-      state[(int64_t)(P_MS + s) * n + i] = ms;
-      if (ms != 0.f) nz_mask |= 1 << s;
-    }
-    // features (HR:498-531): scaled grads, neighbouring products, centred log mean-squares, relative log-lr
-#pragma unroll
-    for (int s = 0; s < NS; ++s) in[s] = sc[s];
-#pragma unroll
-    for (int s = 0; s < NS - 1; ++s) in[NS + s] = sc[s] * sc[s + 1];
-    const float avg = (((lm[0] + lm[1]) + lm[2]) + lm[3]) / 4.0f;
-#pragma unroll
-    for (int s = 0; s < NS; ++s) in[2 * NS - 1 + s] = lm[s] - avg;
-    in[F - 1] = llr - mean_llr;
-#pragma unroll
-    for (int k = 0; k < H0; ++k) in[F + k] = h[k];
-    // BiasGRU(10) (rnn_cells.py:46-68): gates on [feat | h], candidate on [feat | r*h]
-    float pg[2 * H0];
-#pragma unroll
-    for (int o = 0; o < 2 * H0; ++o) pg[o] = 0.f;
-#pragma unroll
-    for (int k = 0; k < F + H0; ++k) {
-      const float4* row = reinterpret_cast<const float4*>(sWg + k * 2 * H0);
-#pragma unroll
-      for (int q = 0; q < 2 * H0 / 4; ++q) {
-        const float4 wv = row[q];
-        pg[4 * q + 0] = fmaf(in[k], wv.x, pg[4 * q + 0]);
-        pg[4 * q + 1] = fmaf(in[k], wv.y, pg[4 * q + 1]);
-        pg[4 * q + 2] = fmaf(in[k], wv.z, pg[4 * q + 2]);
-        pg[4 * q + 3] = fmaf(in[k], wv.w, pg[4 * q + 3]);
-      }
-    }
-    float r[H0], u[H0];
-#pragma unroll
-    for (int k = 0; k < H0; ++k) {
-      r[k] = sigmoid_fast((pg[k] + sBg[k]) + sB0[k]);
-      u[k] = sigmoid_fast((pg[H0 + k] + sBg[H0 + k]) + sB0[H0 + k]);
-    }
-#pragma unroll
-    for (int k = 0; k < H0; ++k) in[F + k] = r[k] * h[k];
-    float pc[H0];
-#pragma unroll
-    for (int o = 0; o < H0; ++o) pc[o] = 0.f;
-#pragma unroll
-    for (int k = 0; k < F + H0; ++k) {
-      const float2* row = reinterpret_cast<const float2*>(sWc + k * H0);
-#pragma unroll
-      for (int q = 0; q < H0 / 2; ++q) {
-        const float2 wv = row[q];
-        pc[2 * q + 0] = fmaf(in[k], wv.x, pc[2 * q + 0]);
-        pc[2 * q + 1] = fmaf(in[k], wv.y, pc[2 * q + 1]);
-      }
-    }
-    float hn[H0];
-    float delta = 0.f, zs = 0.f, zi = 0.f, zl = 0.f;
-#pragma unroll
-    for (int k = 0; k < H0; ++k) {
-      const float c = tanh_fast((pc[k] + sBc[k]) + sB0[2 * H0 + k]);
-      hn[k] = u[k] * h[k] + (1.0f - u[k]) * c;
-      state[(int64_t)(P_H + k) * n + i] = hn[k];
-      delta = fmaf(hn[k], __ldg(theta + O_WU + k), delta);       // update direction (HR:609-611)
-      zs = fmaf(hn[k], __ldg(theta + O_WS + k), zs);
-      zi = fmaf(hn[k], __ldg(theta + O_WI + k), zi);
-      zl = fmaf(hn[k], __ldg(theta + O_WL + k), zl);
-    }
-    float short_cut = 0.f;                                        // gradient shortcut (HR:612-620), no bias
-#pragma unroll
-    for (int s = 0; s < NS; ++s) short_cut = fmaf(sc[s], __ldg(theta + O_G2D + s), short_cut);
-    delta += short_cut;
-    const float scl_new = sigmoid_fast(zs + __ldg(theta + O_BS));    // HR:645-651
-    const float inp_new = sigmoid_fast(zi + __ldg(theta + O_BI));
-    const float step_llr = fminf(fmaxf(llr + (zl + __ldg(theta + O_BL)), -33.0f), 33.0f);   // HR:667-683
-    const float lrm = sigmoid_fast(__ldg(theta + O_LRM));
-    const float llr_new = lrm * llr + (1.0f - lrm) * step_llr;    // HR:688-689
-    const float lr_param = exp_fast(step_llr + __ldg(theta + O_OFF)); // HR:692
-    state[(int64_t)P_SCL * n + i] = scl_new;
-    state[(int64_t)P_INP * n + i] = inp_new;
-    state[(int64_t)P_LLR * n + i] = llr_new;
-    w.upd[i] = lr_param * delta;   // the per-tensor 1/RMS(delta) is applied by apply_kernel
-#pragma unroll
-    for (int k = 0; k < H0; ++k) vals[k] = hn[k];
-    // features as fed to the GRU gates (the candidate pass overwrote only the h part of `in`)
-#pragma unroll
-    for (int k = 0; k < F; ++k) vals[H0 + k] = in[k];
-    vals[H0 + F] = delta * delta;
-    vals[H0 + F + 1] = llr_new;
-  }
-  // block reduction of the 24 per-tensor sums (fp64) + the any(ms != 0) flags
-  const int lane = tid & 31, wid = tid >> 5;
-#pragma unroll
-  for (int k = 0; k < kAcc; ++k) {   // fp32 butterfly inside the warp (32 terms), fp64 across warps / blocks
-    float v = vals[k];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if (lane == 0) sRed[wid][k] = (double)v;
-  }
-  const unsigned any0 = __ballot_sync(0xffffffffu, nz_mask & 1), any1 = __ballot_sync(0xffffffffu, nz_mask & 2);
-  const unsigned any2 = __ballot_sync(0xffffffffu, nz_mask & 4), any3 = __ballot_sync(0xffffffffu, nz_mask & 8);
-  if (lane == 0) {
-    if (any0) atomicOr(&w.any_nz[be.tensor * NS + 0], 1);
-    if (any1) atomicOr(&w.any_nz[be.tensor * NS + 1], 1);
-    if (any2) atomicOr(&w.any_nz[be.tensor * NS + 2], 1);
-    if (any3) atomicOr(&w.any_nz[be.tensor * NS + 3], 1);
-  }
-  __syncthreads();
-  if (tid < kAcc) {
-    double v = 0.0;
-#pragma unroll
-    for (int q = 0; q < kBlock / 32; ++q) v += sRed[q][tid];
-    atomicAdd(&w.acc[be.tensor * kAcc + tid], v);
-  }
-}
-
 #include "hrnn_tc.cuh"
 #include "hrnn_bwd.cuh"
 
@@ -326,7 +163,7 @@ __device__ void bias_gru(const float* __restrict__ Wg, const float* __restrict__
   __syncthreads();
 }
 
-// upper levels + bookkeeping for the next step.  mode 0 = after coord_kernel (full step), 1 = prepare only.
+// upper levels + bookkeeping for the next step.  mode 0 = after coord_tc_kernel (full step), 1 = prepare only.
 __global__ void __launch_bounds__(64) tensor_kernel(const float* __restrict__ theta, float* __restrict__ layer,
                                                     float* __restrict__ global, int nt, const int64_t* __restrict__ sizes,
                                                     int64_t n_total, Workspace w, int mode) {
@@ -456,27 +293,11 @@ void free_buried() {
 }
 }  // namespace
 
-
-// L2O_HRNN_FFMA=1 selects the exact-fp32 FFMA kernel for the per-parameter level (debugging / A-B runs); the default
-// is the tensor-core (wgmma) kernel.
-static bool use_ffma_coord() {
-  static const bool v = [] {
-    const char* e = getenv("L2O_HRNN_FFMA");
-    return e && e[0] == '1';
-  }();
-  return v;
-}
-// grid of the tensor-core kernel (0: its shared-memory size could not be set)
-static int coord_tc_grid() {
-  static const int v = [] {
-    int dev = 0, sms = 132;
-    if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (cudaFuncSetAttribute(tcg::coord_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(tcg::SmemG)) !=
-        cudaSuccess)
-      return 0;
-    return sms * tcg::kCtasPerSm;
-  }();
-  return v;
+// coord_tc_kernel needs more than the default 48 KB of dynamic shared memory: raise its limit once per process
+static bool coord_tc_smem_set() {
+  static const bool ok = cudaFuncSetAttribute(tcg::coord_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              (int)sizeof(tcg::SmemG)) == cudaSuccess;
+  return ok;
 }
 
 extern "C" {
@@ -563,7 +384,7 @@ int l2o_hrnn_init_state(l2o_hrnn_handle h, const l2o_hrnn_args* a, void* stream)
 }
 
 // ---- phases.  Single-GPU: prepare = prepare_local + prepare_finish, step = step_local + step_finish.  Sharded: the
-// caller all-reduces the per-tensor sums (l2o_hrnn_reduce_layout) between the two phases.
+// caller all-reduces the per-tensor sums and flags (l2o_hrnn_workspace_layout offsets 0 and 1) between the two phases.
 int l2o_hrnn_prepare_local(l2o_hrnn_handle h, const l2o_hrnn_args* a, void* stream) {
   int rc = check_args(h, a, false);
   if (rc) return rc;
@@ -600,15 +421,13 @@ int l2o_hrnn_step_local(l2o_hrnn_handle h, const l2o_hrnn_args* a, void* stream)
   cudaStream_t st = (cudaStream_t)stream;
   Workspace w;
   carve(w, a->workspace, h->nt, h->n);
-  if (use_ffma_coord()) {
-    coord_kernel<<<h->nblocks, kBlock, 0, st>>>(a->theta, a->g, a->state, h->n, h->d_blocks, w);
-  } else {
-    const int cap = coord_tc_grid();
-    if (cap <= 0) return l2o::set_cuda_error(cudaGetLastError(), "coord_tc_kernel shared-memory size");
-    const int grid = h->nblocks < cap ? h->nblocks : cap;
-    tcg::coord_tc_kernel<<<grid, tcg::kTile, sizeof(tcg::SmemG), st>>>(a->theta, a->g, a->state, h->n, h->d_blocks, h->nblocks,
-                                                                       w);
-  }
+  if (!coord_tc_smem_set()) return l2o::set_cuda_error(cudaGetLastError(), "coord_tc_kernel shared-memory size");
+  const int sms = l2o::device_sms();
+  if (sms <= 0) return L2O_E_CUDA;
+  const int cap = sms * tcg::kCtasPerSm;   // persistent CTAs
+  const int grid = h->nblocks < cap ? h->nblocks : cap;
+  tcg::coord_tc_kernel<<<grid, tcg::kTile, sizeof(tcg::SmemG), st>>>(a->theta, a->g, a->state, h->n, h->d_blocks, h->nblocks,
+                                                                     w);
   L2O_CUDA_TRY(cudaGetLastError());
   l2o::count_launch();
   return L2O_OK;
@@ -648,8 +467,8 @@ int l2o_hrnn_coord_bwd(l2o_hrnn_handle h, const l2o_hrnn_bwd_args* a, void* stre
   }
   bwd::Args k{a->theta, a->state_old, a->g, a->bias0, a->zero_flag, a->mean_log_lr, a->d_state_new, a->d_upd, a->d_sums,
               a->d_state_old, a->d_theta, a->d_bias0, a->d_mean_log_lr, a->d_g};
-  int dev = 0, sms = 132;
-  if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = l2o::device_sms();
+  if (sms <= 0) return L2O_E_CUDA;
   const int grid = h->nblocks < 2 * sms ? h->nblocks : 2 * sms;
   bwd::coord_bwd_kernel<<<grid, bwd::kBwdBlock, 0, (cudaStream_t)stream>>>(k, h->n, h->d_blocks, h->nblocks);
   L2O_CUDA_TRY(cudaGetLastError());
@@ -681,16 +500,6 @@ int l2o_hrnn_set_global_sizes(l2o_hrnn_handle h, const int64_t* global_sizes) {
   }
   L2O_CUDA_TRY(cudaMemcpy(h->d_sizes, global_sizes, sizeof(int64_t) * h->nt, cudaMemcpyHostToDevice));
   h->n_global = tot;
-  return L2O_OK;
-}
-
-int l2o_hrnn_reduce_layout(l2o_hrnn_handle h, int64_t* n_doubles, int64_t* flags_offset_bytes, int64_t* n_flags) {
-  if (!h) return L2O_E_INVALID;
-  Workspace w;
-  carve(w, (void*)256, h->nt, h->n);   // offsets relative to a dummy non-null base
-  if (n_doubles) *n_doubles = (int64_t)h->nt * kAcc;
-  if (flags_offset_bytes) *flags_offset_bytes = (int64_t)((char*)w.any_nz - (char*)w.acc);
-  if (n_flags) *n_flags = (int64_t)h->nt * NS;
   return L2O_OK;
 }
 

@@ -54,8 +54,6 @@ int tc_unroll_fwd(l2o_net* h, const l2o_unroll_args& a, cudaStream_t st);
 int tc_fwd_variant(const l2o_net* h, const l2o_unroll_args& a);   // l2o_tc_fwd_variant
 bool tc_step_ok(const l2o_net* h, const l2o_step_args& a);
 int tc_step(l2o_net* h, const l2o_step_args& a, cudaStream_t st);
-bool tc_auto_default();
-bool tc_bwd_auto_default();
 bool tc_bwd_ok(const l2o_net* h, const l2o_bwd_args& a);
 int tc_unroll_bwd(l2o_net* h, const l2o_bwd_args& a, cudaStream_t st, const l2o_bwd_carry* c = nullptr);
 }  // namespace l2o

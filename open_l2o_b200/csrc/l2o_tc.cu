@@ -2,7 +2,6 @@
 #include "cwlstm_ffma.cuh"   // load_vec / store_vec / preprocess helpers
 #include "cwlstm_tc.cuh"
 #include "cwlstm_tc_bwd.cuh"
-#include <cstdlib>
 #include <mutex>
 #include <utility>
 #include <vector>
@@ -17,14 +16,6 @@ bool tc_fwd_ok(const l2o_net* h, const l2o_unroll_args& a) {
   if (h->cfg == 2) return true;                             // fused Adam-feature mode (m, v) or given (m~, g~) rows
   return a.m == nullptr && a.feat_rec == nullptr;
 }
-// L2O_TC_AUTO=0: ENGINE_AUTO never picks the tensor-core engine (A/B runs of whole tests against the exact-fp32 engine)
-static bool tc_auto_env() {
-  static const bool on = !(std::getenv("L2O_TC_AUTO") != nullptr && std::getenv("L2O_TC_AUTO")[0] == '0');
-  return on;
-}
-bool tc_auto_default() { return tc_auto_env(); }
-bool tc_bwd_auto_default() { return tc_auto_env(); }
-
 // Weight-image buffers are recycled through a process-wide free list and never cudaFree'd: a handle may be destroyed
 // (Python GC) while ANOTHER program is capturing a CUDA graph, and cudaFree during a capture invalidates it.
 namespace {

@@ -25,6 +25,7 @@ from .scale_base import ScaleOptimizer
 
 NUM_GRADIENT_SCALES = 4
 N_FEATURES = 12
+N_SUMS, B0_STRIDE = 24, 32   # per-tensor fp64 sums [h'(10) | features(12) | delta^2 | log-lr'], gate-bias row stride
 STATE_PLANES = ("parameter",) * 10 + ("scl_decay", "inp_decay", "log_learning_rate", "grad_accum1", "grad_accum2",
                                       "grad_accum3", "grad_accum4", "ms1", "ms2", "ms3", "ms4")
 
@@ -113,8 +114,11 @@ def _init_theta(seed: Optional[int]) -> torch.Tensor:
 
 class HrnnHandle(object):
     """An ``l2o_hrnn`` handle (``_h``) for optimizee tensors of ``sizes`` coordinates and the workspace it needs,
-    aligned to the 256 B the library requires (``ptr``; ``ws`` is the aligned workspace as bytes).  The handle is
-    destroyed with this object."""
+    aligned to the 256 B the library requires (``ptr``), with views of the workspace regions that
+    ``l2o_hrnn_workspace_layout`` places: ``w_sums`` [n_tensors, 24] fp64 per-tensor sums, ``w_any`` / ``w_zero``
+    [n_tensors, 4] int32 flags any(ms != 0) seen this step / all(ms == 0) before the next, ``w_bias0`` [n_tensors, 32]
+    per-tensor gate bias, ``w_mean`` [1] problem-wide mean log learning rate, ``w_upd`` [N] raw update lr * delta.
+    The handle is destroyed with this object."""
 
     def __init__(self, sizes: Sequence[int], device):
         L = _lib.lib()
@@ -123,7 +127,19 @@ class HrnnHandle(object):
         nbytes = int(L.l2o_hrnn_workspace_bytes(self._h))
         self._buf = torch.zeros((nbytes + 255) // 4 + 64, dtype=torch.float32, device=device)
         self.ptr = (self._buf.data_ptr() + 255) // 256 * 256
-        self.ws = self._buf.view(torch.uint8)[self.ptr - self._buf.data_ptr():]
+        ws = self._buf.view(torch.uint8)[self.ptr - self._buf.data_ptr():]
+        off = (C.c_int64 * 7)()
+        _lib.check(L.l2o_hrnn_workspace_layout(self._h, off), "l2o_hrnn_workspace_layout")
+
+        def region(k, dtype, *shape):
+            return ws[off[k]:off[k] + dtype.itemsize * math.prod(shape)].view(dtype).view(*shape)
+        nt, n = len(sizes), int(sum(sizes))
+        self.w_sums = region(0, torch.float64, nt, N_SUMS)
+        self.w_any = region(1, torch.int32, nt, NUM_GRADIENT_SCALES)
+        self.w_zero = region(2, torch.int32, nt, NUM_GRADIENT_SCALES)
+        self.w_bias0 = region(3, torch.float32, nt, B0_STRIDE)
+        self.w_mean = region(5, torch.float32, 1)
+        self.w_upd = region(6, torch.float32, n)
 
     def __del__(self):
         try:
@@ -218,12 +234,6 @@ class HierarchicalRNN(ScaleOptimizer):
         if self.distributed:
             garr = (C.c_int64 * len(self.global_sizes))(*self.global_sizes)
             _lib.check(_lib.lib().l2o_hrnn_set_global_sizes(self._hrnn._h, garr), "l2o_hrnn_set_global_sizes")
-            # views of the workspace head that the ranks all-reduce between the two step phases
-            nd, fo, nf = C.c_int64(), C.c_int64(), C.c_int64()
-            _lib.check(_lib.lib().l2o_hrnn_reduce_layout(self._hrnn._h, C.byref(nd), C.byref(fo), C.byref(nf)),
-                       "l2o_hrnn_reduce_layout")
-            self._red_sums = self._hrnn.ws[:8 * nd.value].view(torch.float64)
-            self._red_flags = self._hrnn.ws[fo.value:fo.value + 4 * nf.value].view(torch.int32)
         self.layer = torch.zeros(len(self.sizes), self.level_sizes[1], device=dev)
         self.global_state = torch.zeros(self.level_sizes[2], device=dev)
         self.update = torch.empty(self.N, device=dev)
@@ -240,8 +250,8 @@ class HierarchicalRNN(ScaleOptimizer):
 
     def _allreduce_sums(self):
         import torch.distributed as tdist
-        tdist.all_reduce(self._red_sums, op=tdist.ReduceOp.SUM)
-        tdist.all_reduce(self._red_flags, op=tdist.ReduceOp.MAX)
+        tdist.all_reduce(self._hrnn.w_sums, op=tdist.ReduceOp.SUM)
+        tdist.all_reduce(self._hrnn.w_any, op=tdist.ReduceOp.MAX)
 
     def _prepare(self):
         L, h, a = _lib.lib(), self._hrnn._h, self._args(False)

@@ -29,13 +29,12 @@ import torch
 from . import _lib
 from ._lib import HrnnArgs, HrnnBwdArgs
 from .engine import _ptr, _stream
-from .hierarchical_rnn import THETA_SPEC, HrnnHandle, _init_theta
+from .hierarchical_rnn import B0_STRIDE, N_SUMS, THETA_SPEC, HrnnHandle, _init_theta
 from .scale_base import MetaTrainerBase, theta_views, train_optimizer  # noqa: F401  (train_optimizer: public name)
 
 H0, H1, H2, NF, NS = 10, 20, 20, 12, 4
 PLANES = 21
 P_H, P_SCL, P_INP, P_LLR, P_ACC, P_MS = 0, 10, 11, 12, 13, 17
-B0_STRIDE, N_SUMS = 32, 24
 
 
 def _bias_gru(inputs, state, Wg, bg, Wc, bc, bias):
@@ -49,22 +48,14 @@ def _bias_gru(inputs, state, Wg, bg, Wc, bc, bias):
 
 
 class _Engine(HrnnHandle):
-    """The handle and workspace of one optimizee (a list of tensor sizes), with views of the workspace regions that the
-    coordinate kernels share with the torch-level pieces."""
+    """The handle and workspace of one optimizee (a list of tensor sizes); the coordinate kernels share the workspace
+    regions with the torch-level pieces through the handle's views."""
 
     def __init__(self, sizes: Sequence[int], device):
         self.sizes = [int(s) for s in sizes]
         self.nt, self.N, self.device = len(self.sizes), int(sum(self.sizes)), device
         super().__init__(self.sizes, device)
-        off = (C.c_int64 * 7)()
-        _lib.check(_lib.lib().l2o_hrnn_workspace_layout(self._h, off), "l2o_hrnn_workspace_layout")
-        ws, nt, N = self.ws, self.nt, self.N
-        self.w_sums = ws[off[0]:off[0] + 8 * nt * N_SUMS].view(torch.float64).view(nt, N_SUMS)
-        self.w_any = ws[off[1]:off[1] + 4 * nt * NS].view(torch.int32).view(nt, NS)
-        self.w_zero = ws[off[2]:off[2] + 4 * nt * NS].view(torch.int32).view(nt, NS)
-        self.w_bias0 = ws[off[3]:off[3] + 4 * nt * B0_STRIDE].view(torch.float32).view(nt, B0_STRIDE)
-        self.w_mean = ws[off[5]:off[5] + 4].view(torch.float32)
-        self.w_upd = ws[off[6]:off[6] + 4 * N].view(torch.float32)
+        nt, N = self.nt, self.N
         self._dummy_x = torch.zeros(N, device=device)
         self._dummy_layer = torch.zeros(nt, H1, device=device)
         self._dummy_global = torch.zeros(H2, device=device)

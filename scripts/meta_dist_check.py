@@ -74,7 +74,7 @@ def main():
                 "theta_all": max(rel(t, tr) for (_, t, _), (_, tr, _) in zip(trace, ref)),
                 "x_shard": rel(x_shard, x_full[lo:hi])}
         # d-theta of this problem is a sum with heavy cancellation: two runs of the EXACT-fp32 engine that differ only in
-        # how the coordinates are grouped into CTAs already differ by 1.6e-5 of max|dtheta| (measured, L2O_TC_AUTO=0),
+        # how the coordinates are grouped into CTAs already differ by 1.6e-5 of max|dtheta| (measured, set_engine(ENGINE_FFMA)),
         # so the sharded-vs-single bar for d-theta / theta is 5e-5; f(x_T) and x have no such cancellation: 1e-5
         ok = ok and errs["fx"] <= 1e-5 and errs["x_shard"] <= 1e-5 and \
             all(errs[k] <= 5e-5 for k in ("dtheta", "theta", "theta_all"))

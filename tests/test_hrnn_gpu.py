@@ -154,22 +154,6 @@ def test_hrnn_steps_match_oracle(shapes, steps, theta_kind, clip):
         assert clipped > 0 and inside > 0, (clipped, inside)
 
 
-def test_hrnn_ffma_coord_kernel_matches_oracle():
-    """L2O_HRNN_FFMA=1 swaps the tensor-core coordinate kernel for the exact-fp32 FFMA one (coord_kernel).  The switch
-    is read once per process, so the ConvNet and ragged cases of test_hrnn_steps_match_oracle run again in a child."""
-    import os
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    env = dict(os.environ, L2O_HRNN_FFMA="1")
-    py = [sys.executable] + (["-s"] if sys.flags.no_user_site else [])
-    r = subprocess.run(py + ["-m", "pytest", "-q", "-p", "no:cacheprovider", "-m", "gpu",
-                             os.path.join(root, "tests", "test_hrnn_gpu.py"),
-                             "-k", "test_hrnn_steps_match_oracle and (convnet or ragged)"],
-                       capture_output=True, text=True, timeout=1800, cwd=root, env=env)
-    assert r.returncode == 0 and "6 passed" in r.stdout, r.stdout[-3000:] + r.stderr[-2000:]
-
-
 def test_hrnn_argument_errors():
     from open_l2o_b200 import hierarchical_rnn as hr
     with pytest.raises(ValueError):
