@@ -19,6 +19,7 @@
 //    over the thread's 5 units are combined with two quad shuffles.
 #pragma once
 #include "cwlstm_common.cuh"
+#include "l2o_internal.h"
 
 namespace l2o {
 namespace tc {
@@ -674,34 +675,37 @@ inline bool tc_fwd_fast(bool fc, const NetRt& rt, const l2o_unroll_args& a, cons
 }
 
 template <class C, bool FAST, int OPT, bool CKPT>
-int tc_run_fwd(const NetRt& rt, const l2o_unroll_args& a, float* img, cudaStream_t st, int sms, float* state_out,
-               tc::FwdExtra ex) {
+int tc_run_fwd(const char* fn, const NetRt& rt, const l2o_unroll_args& a, float* img, cudaStream_t st, int sms,
+               float* state_out, tc::FwdExtra ex) {
   auto k = tc::unroll_fwd_kernel<C, FAST, OPT, CKPT>;
   const size_t smem = tc::fwd_smem_bytes<C>(a.T);
   if (smem > 227 * 1024) return L2O_E_INVALID;
-  if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return L2O_E_CUDA;
+  if (int rc = raise_smem_limit(fn, k, smem)) return rc;
   const int64_t ntiles = (a.n + tc::kTile - 1) / tc::kTile;
   const int64_t ctas = (ntiles + tc::kFwdWG - 1) / tc::kFwdWG;
   const int grid = (int)(ctas < sms ? ctas : sms);
   k<<<grid, tc::kFwdThreads, smem, st>>>(a, rt, img, state_out ? state_out : a.state, ex);
-  return cudaGetLastError() == cudaSuccess ? L2O_OK : L2O_E_CUDA;
+  return after_launch(fn);
 }
 
 template <class C>
-int tc_launch_fwd(const NetRt& rt, const l2o_unroll_args& a, float* img, cudaStream_t st, int sms, float* state_out = nullptr,
-                  tc::FwdExtra ex = tc::FwdExtra{nullptr, 0, 0.f}, bool prep = true) {
-  if (prep) tc::prep_weights_kernel<C><<<16, 256, 0, st>>>(a.theta, img, 0);
+int tc_launch_fwd(const char* fn, const NetRt& rt, const l2o_unroll_args& a, float* img, cudaStream_t st, int sms,
+                  float* state_out = nullptr, tc::FwdExtra ex = tc::FwdExtra{nullptr, 0, 0.f}, bool prep = true) {
+  if (prep) {
+    tc::prep_weights_kernel<C><<<16, 256, 0, st>>>(a.theta, img, 0);
+    if (int rc = after_launch(fn)) return rc;
+  }
   if constexpr (!C::FC) {
     if (tc_fwd_fast(false, rt, a, state_out)) {
       constexpr int R = L2O_OPT_RASTRIGIN_SEP, Q = L2O_OPT_QUADRATIC_DIAG;
       if (a.opt_kind == R)
-        return a.ckpt ? tc_run_fwd<C, true, R, true>(rt, a, img, st, sms, state_out, ex)
-                      : tc_run_fwd<C, true, R, false>(rt, a, img, st, sms, state_out, ex);
-      return a.ckpt ? tc_run_fwd<C, true, Q, true>(rt, a, img, st, sms, state_out, ex)
-                    : tc_run_fwd<C, true, Q, false>(rt, a, img, st, sms, state_out, ex);
+        return a.ckpt ? tc_run_fwd<C, true, R, true>(fn, rt, a, img, st, sms, state_out, ex)
+                      : tc_run_fwd<C, true, R, false>(fn, rt, a, img, st, sms, state_out, ex);
+      return a.ckpt ? tc_run_fwd<C, true, Q, true>(fn, rt, a, img, st, sms, state_out, ex)
+                    : tc_run_fwd<C, true, Q, false>(fn, rt, a, img, st, sms, state_out, ex);
     }
   }
-  return tc_run_fwd<C, false, L2O_OPT_NONE, false>(rt, a, img, st, sms, state_out, ex);
+  return tc_run_fwd<C, false, L2O_OPT_NONE, false>(fn, rt, a, img, st, sms, state_out, ex);
 }
 
 }  // namespace l2o

@@ -610,17 +610,18 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
 }  // namespace tcb
 
 template <class C, bool CARRY>
-int tc_launch_bwd(const NetRt& rt, const l2o_bwd_args& a, float* img, cudaStream_t st, int sms, const l2o_bwd_carry& cy,
-                  bool prep = true) {
-  if (prep) tc::prep_weights_kernel<C><<<16, 256, 0, st>>>(a.theta, img, 1);
+int tc_launch_bwd(const char* fn, const NetRt& rt, const l2o_bwd_args& a, float* img, cudaStream_t st, int sms,
+                  const l2o_bwd_carry& cy) {
+  tc::prep_weights_kernel<C><<<16, 256, 0, st>>>(a.theta, img, 1);
+  if (int rc = after_launch(fn)) return rc;
   const int64_t ntiles = (a.n + tc::kTile - 1) / tc::kTile;
   const int64_t ctas = (ntiles + tcb::kBwdWG - 1) / tcb::kBwdWG;
   const int grid = (int)(ctas < sms ? ctas : sms);
   auto launch = [&](auto kern, size_t smem) {
     if (smem > 227 * 1024) return L2O_E_INVALID;
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return L2O_E_CUDA;
+    if (int rc = raise_smem_limit(fn, kern, smem)) return rc;
     kern<<<grid, tcb::kBwdThreads, smem, st>>>(a, rt, img, cy);
-    return cudaGetLastError() == cudaSuccess ? L2O_OK : L2O_E_CUDA;
+    return after_launch(fn);
   };
   // the layer-2 pass's instantiation for the output-layer flags of these arguments
   const int fl = (a.labels != nullptr ? tcb::kFlImit : 0) | (rt.tanh_output ? tcb::kFlTanh : 0);

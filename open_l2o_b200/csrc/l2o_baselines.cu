@@ -256,28 +256,6 @@ __global__ void __launch_bounds__(kBlock) lrs_bwd_kernel(LrsBwd a) {
   block_flush<1>(acc, scale, dst);
 }
 
-// resident CTAs of `kernel` on the current device, cached per kernel and device (0 on failure)
-template <class Args>
-static int grid_cap(void (*kernel)(Args)) {
-  static thread_local int cached_dev = -1, v = 0;
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 0;
-  if (dev != cached_dev) {
-    int per = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, kernel, kBlock, 0) != cudaSuccess) return 0;
-    v = per * device_sms();
-    cached_dev = dev;
-  }
-  return v;
-}
-
-static unsigned blocks_for(int64_t n, int cap) {
-  const int64_t b = (n + kBlock - 1) / kBlock;
-  return (unsigned)(b < cap ? b : cap);
-}
-
-static bool misaligned(const void* p, uintptr_t align) { return ((uintptr_t)p & (align - 1)) != 0; }
-
 }  // namespace baselines
 }  // namespace l2o
 
@@ -293,14 +271,9 @@ int l2o_tadam_step(const l2o_tadam_step_args* a, void* stream) {
     return L2O_E_INVALID;
   const void* fp[] = {a->theta, a->g, a->state_in, a->state_out, a->x, a->update};
   for (const void* p : fp)
-    if (misaligned(p, alignof(float))) return L2O_E_INVALID;
-  const int cap = grid_cap(tadam_step_kernel);
-  if (cap <= 0) return l2o::set_cuda_error(cudaGetLastError(), "l2o_tadam_step occupancy");
+    if (l2o::misaligned(p, alignof(float))) return L2O_E_INVALID;
   TadamStep k{a->n, a->theta, a->g, a->state_in, a->state_out, a->x, a->update};
-  tadam_step_kernel<<<blocks_for(a->n, cap), kBlock, 0, (cudaStream_t)stream>>>(k);
-  L2O_CUDA_TRY(cudaGetLastError());
-  l2o::count_launch();
-  return L2O_OK;
+  return l2o::occupancy_launch("l2o_tadam_step", tadam_step_kernel, kBlock, 0, a->n, (cudaStream_t)stream, k);
 }
 
 int l2o_tadam_bwd(const l2o_tadam_bwd_args* a, void* stream) {
@@ -309,8 +282,8 @@ int l2o_tadam_bwd(const l2o_tadam_bwd_args* a, void* stream) {
     return L2O_E_INVALID;
   const void* fp[] = {a->theta, a->g, a->state_old, a->d_state_new, a->d_update, a->d_state_old, a->d_g};
   for (const void* p : fp)
-    if (misaligned(p, alignof(float))) return L2O_E_INVALID;
-  if (misaligned(a->d_theta, alignof(double))) return L2O_E_INVALID;
+    if (l2o::misaligned(p, alignof(float))) return L2O_E_INVALID;
+  if (l2o::misaligned(a->d_theta, alignof(double))) return L2O_E_INVALID;
   if (a->d_g) {
     const size_t n = (size_t)a->n, f = sizeof(float);
     const void* other[] = {a->theta, a->g, a->state_old, a->d_state_new, a->d_update, a->d_state_old, a->d_theta};
@@ -318,48 +291,33 @@ int l2o_tadam_bwd(const l2o_tadam_bwd_args* a, void* stream) {
                             kTheta * sizeof(double)};
     if (l2o::overlaps_any(a->d_g, n * f, other, bytes, 7)) return L2O_E_INVALID;
   }
-  const int cap = grid_cap(tadam_bwd_kernel);
-  if (cap <= 0) return l2o::set_cuda_error(cudaGetLastError(), "l2o_tadam_bwd occupancy");
   TadamBwd k{a->n, a->theta, a->g, a->state_old, a->d_state_new, a->d_update, a->d_state_old, a->d_theta, a->d_g};
-  tadam_bwd_kernel<<<blocks_for(a->n, cap), kBlock, 0, (cudaStream_t)stream>>>(k);
-  L2O_CUDA_TRY(cudaGetLastError());
-  l2o::count_launch();
-  return L2O_OK;
+  return l2o::occupancy_launch("l2o_tadam_bwd", tadam_bwd_kernel, kBlock, 0, a->n, (cudaStream_t)stream, k);
 }
 
 int l2o_lrsgd_step(const l2o_lrsgd_step_args* a, void* stream) {
   if (!a || a->n <= 0 || a->n_steps <= 0 || !a->rates || !a->g) return L2O_E_INVALID;
   const void* fp[] = {a->rates, a->g, a->x, a->update, a->itr};
   for (const void* p : fp)
-    if (misaligned(p, 4)) return L2O_E_INVALID;
-  const int cap = grid_cap(lrs_step_kernel);
-  if (cap <= 0) return l2o::set_cuda_error(cudaGetLastError(), "l2o_lrsgd_step occupancy");
+    if (l2o::misaligned(p, 4)) return L2O_E_INVALID;
   LrsStep k{a->n, a->rates, a->n_steps, a->itr, a->g, a->x, a->update};
-  lrs_step_kernel<<<blocks_for(a->n, cap), kBlock, 0, (cudaStream_t)stream>>>(k);
-  L2O_CUDA_TRY(cudaGetLastError());
-  l2o::count_launch();
-  return L2O_OK;
+  return l2o::occupancy_launch("l2o_lrsgd_step", lrs_step_kernel, kBlock, 0, a->n, (cudaStream_t)stream, k);
 }
 
 int l2o_lrsgd_bwd(const l2o_lrsgd_bwd_args* a, void* stream) {
   if (!a || a->n <= 0 || a->n_steps <= 0 || !a->rates || !a->g || !a->d_update || !a->d_rates) return L2O_E_INVALID;
   const void* fp[] = {a->rates, a->g, a->d_update, a->itr, a->d_g};
   for (const void* p : fp)
-    if (misaligned(p, 4)) return L2O_E_INVALID;
-  if (misaligned(a->d_rates, alignof(double))) return L2O_E_INVALID;
+    if (l2o::misaligned(p, 4)) return L2O_E_INVALID;
+  if (l2o::misaligned(a->d_rates, alignof(double))) return L2O_E_INVALID;
   if (a->d_g) {
     const size_t n = (size_t)a->n, f = sizeof(float);
     const void* other[] = {a->rates, a->g, a->d_update, a->itr, a->d_rates};
     const size_t bytes[] = {(size_t)a->n_steps * f, n * f, n * f, 2 * sizeof(int32_t), (size_t)a->n_steps * sizeof(double)};
     if (l2o::overlaps_any(a->d_g, n * f, other, bytes, 5)) return L2O_E_INVALID;
   }
-  const int cap = grid_cap(lrs_bwd_kernel);
-  if (cap <= 0) return l2o::set_cuda_error(cudaGetLastError(), "l2o_lrsgd_bwd occupancy");
   LrsBwd k{a->n, a->rates, a->n_steps, a->itr, a->g, a->d_update, a->d_rates, a->d_g};
-  lrs_bwd_kernel<<<blocks_for(a->n, cap), kBlock, 0, (cudaStream_t)stream>>>(k);
-  L2O_CUDA_TRY(cudaGetLastError());
-  l2o::count_launch();
-  return L2O_OK;
+  return l2o::occupancy_launch("l2o_lrsgd_bwd", lrs_bwd_kernel, kBlock, 0, a->n, (cudaStream_t)stream, k);
 }
 
 }  // extern "C"

@@ -4,7 +4,10 @@
 #include <atomic>
 #include <cmath>
 #include <cstdio>
+#include <map>
 #include <new>
+#include <tuple>
+#include <utility>
 
 #include "l2o_internal.h"
 
@@ -46,22 +49,73 @@ __global__ void log_and_sign_kernel(const float* __restrict__ g, float* __restri
 }  // namespace
 
 namespace l2o {
-int set_cuda_error(cudaError_t e, const char* where) {
-  snprintf(g_cuda_err, sizeof(g_cuda_err), "%s: %s", where, cudaGetErrorString(e));
+int set_cuda_error(cudaError_t e, const char* fn, const char* call) {
+  snprintf(g_cuda_err, sizeof(g_cuda_err), "%s: %s: %s", fn, call, cudaGetErrorString(e));
   return L2O_E_CUDA;
 }
-void count_launch(int n) { g_launches += n; }
-int device_sms() {
+
+static int current_device(const char* fn, int& dev) {
+  L2O_CUDA_TRY(fn, cudaGetDevice(&dev));
+  return L2O_OK;
+}
+
+int device_sms(const char* fn) {
   static thread_local int cached_dev = -1, sms = 0;
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 0;
+  if (current_device(fn, dev)) return 0;
   if (dev != cached_dev) {
     int v = 0;
-    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return 0;
+    const cudaError_t e = cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
+    if (e != cudaSuccess) {
+      set_cuda_error(e, fn, "cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev)");
+      return 0;
+    }
     sms = v;
     cached_dev = dev;
   }
   return sms;
+}
+
+static int raise_smem_limit_on(const char* fn, int dev, const void* kernel, size_t smem) {
+  static thread_local std::map<std::pair<const void*, int>, size_t> limit;
+  size_t& lim = limit[{kernel, dev}];
+  if (smem <= lim) return L2O_OK;
+  L2O_CUDA_TRY(fn, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  lim = smem;
+  return L2O_OK;
+}
+
+int raise_smem_limit(const char* fn, const void* kernel, size_t smem) {
+  int dev = 0;
+  if (int rc = current_device(fn, dev)) return rc;
+  return raise_smem_limit_on(fn, dev, kernel, smem);
+}
+
+int occupancy_grid(const char* fn, const void* kernel, int block, size_t smem, int64_t n, int& grid) {
+  static thread_local std::map<std::tuple<const void*, int, int, size_t>, int> resident;
+  int dev = 0;
+  if (int rc = current_device(fn, dev)) return rc;
+  const auto key = std::make_tuple(kernel, dev, block, smem);
+  auto it = resident.find(key);
+  if (it == resident.end()) {
+    if (int rc = raise_smem_limit_on(fn, dev, kernel, smem)) return rc;
+    int occ = 0;
+    L2O_CUDA_TRY(fn, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, block, smem));
+    if (occ < 1) return L2O_E_UNSUPPORTED;
+    const int sms = device_sms(fn);
+    if (sms <= 0) return L2O_E_CUDA;
+    it = resident.emplace(key, occ * sms).first;
+  }
+  const int64_t blocks = (n + block - 1) / block;
+  grid = (int)(blocks < it->second ? blocks : it->second);
+  return L2O_OK;
+}
+
+int after_launch(const char* fn) {
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_cuda_error(e, fn, "kernel launch");
+  ++g_launches;
+  return L2O_OK;
 }
 }  // namespace l2o
 
@@ -169,7 +223,7 @@ int l2o_unroll_bwd(l2o_handle h, const l2o_bwd_args* a, void* stream) {
   if (a->T > 0 && !a->in_seq) return L2O_E_INVALID;
   if (h->state_floats > 0 && !a->ckpt) return L2O_E_INVALID;
   // both engines read checkpoint rows 16 bytes at a time (FFMA: float4 loads; tensor cores: TMA bulk copies)
-  if (reinterpret_cast<uintptr_t>(a->ckpt) % 16 != 0) return L2O_E_INVALID;
+  if (l2o::misaligned(a->ckpt, 16)) return L2O_E_INVALID;
   if (!a->g_rec && (!a->labels || a->n_total <= 0)) return L2O_E_INVALID;
   if (a->n == 0 || a->T == 0) return L2O_OK;
   cudaStream_t st = (cudaStream_t)stream;
@@ -184,8 +238,7 @@ int l2o_unroll_bwd_carry(l2o_handle h, const l2o_bwd_args* a, const l2o_bwd_carr
   if (a->T > 0 && !a->in_seq) return L2O_E_INVALID;
   if (h->state_floats > 0 && (!a->ckpt || !c->d_state)) return L2O_E_INVALID;
   // the FFMA engine moves checkpoint and adjoint-state rows as float4, the tensor-core engine copies checkpoints by TMA
-  if (reinterpret_cast<uintptr_t>(a->ckpt) % 16 != 0 || reinterpret_cast<uintptr_t>(c->d_state) % 16 != 0)
-    return L2O_E_INVALID;
+  if (l2o::misaligned(a->ckpt, 16) || l2o::misaligned(c->d_state, 16)) return L2O_E_INVALID;
   if (!c->lam) return L2O_E_INVALID;
   if (!a->g_rec && (!a->labels || a->n_total <= 0)) return L2O_E_INVALID;
   if (a->labels) return L2O_E_UNSUPPORTED;   // imitation losses have no lambda to carry
@@ -206,9 +259,7 @@ int l2o_adam_step(float* theta, const double* dtheta, float* m, float* v, int64_
   const int block = 256;
   adam_kernel<<<(int)((n + block - 1) / block), block, 0, (cudaStream_t)stream>>>(theta, dtheta, m, v, n, (float)lr_t,
                                                                                  beta1, beta2, eps);
-  l2o::count_launch();
-  L2O_CUDA_TRY(cudaGetLastError());
-  return L2O_OK;
+  return l2o::after_launch("l2o_adam_step");
 }
 
 int l2o_log_and_sign(const float* g, float* out, int64_t n, float k, void* stream) {
@@ -217,9 +268,7 @@ int l2o_log_and_sign(const float* g, float* out, int64_t n, float k, void* strea
   const int block = 256;
   log_and_sign_kernel<<<(int)((n + block - 1) / block), block, 0, (cudaStream_t)stream>>>(g, out, n, k,
                                                                                          (float)std::exp((double)k));
-  l2o::count_launch();
-  L2O_CUDA_TRY(cudaGetLastError());
-  return L2O_OK;
+  return l2o::after_launch("l2o_log_and_sign");
 }
 
 int64_t l2o_launch_count(void) { return g_launches.load(); }

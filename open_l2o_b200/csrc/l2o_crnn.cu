@@ -431,36 +431,6 @@ __global__ void __launch_bounds__(kBwdBlock, 1) bwd_kernel(BwdArgs a) {
     if (e < O_INIT || e >= O_K1) atomicAdd(&a.d_theta[e], (double)S.img[e]);
 }
 
-static int fwd_grid() {   // resident CTAs of step_kernel on the current device (0 on failure)
-  static thread_local int cached_dev = -1, v = 0;
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 0;
-  if (dev != cached_dev) {
-    int per = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, step_kernel, kFwdBlock, 0) != cudaSuccess) return 0;
-    v = per * device_sms();
-    cached_dev = dev;
-  }
-  return v;
-}
-
-static int bwd_grid() {
-  static thread_local int cached_dev = -1, v = 0;
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 0;
-  if (dev != cached_dev) {
-    int per = 0;
-    if (cudaFuncSetAttribute(bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BwdSmem)) != cudaSuccess)
-      return 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, bwd_kernel, kBwdBlock, sizeof(BwdSmem)) != cudaSuccess) return 0;
-    v = per * device_sms();
-    cached_dev = dev;
-  }
-  return v;
-}
-
-static bool misaligned(const void* p, uintptr_t align) { return ((uintptr_t)p & (align - 1)) != 0; }
-
 }  // namespace crnn
 }  // namespace l2o
 
@@ -476,15 +446,9 @@ int l2o_crnn_step(const l2o_crnn_step_args* a, void* stream) {
     return L2O_E_INVALID;
   const void* fp[] = {a->theta, a->g, a->state_in, a->state_out, a->x, a->update};
   for (const void* p : fp)
-    if (misaligned(p, alignof(float))) return L2O_E_INVALID;
-  const int cap = fwd_grid();
-  if (cap <= 0) return l2o::set_cuda_error(cudaGetLastError(), "l2o_crnn_step occupancy");
-  const int64_t blocks = (a->n + kFwdBlock - 1) / kFwdBlock;
+    if (l2o::misaligned(p, alignof(float))) return L2O_E_INVALID;
   StepArgs k{a->n, a->theta, a->g, a->state_in, a->state_out, a->x, a->update};
-  step_kernel<<<(unsigned)(blocks < cap ? blocks : cap), kFwdBlock, 0, (cudaStream_t)stream>>>(k);
-  L2O_CUDA_TRY(cudaGetLastError());
-  l2o::count_launch();
-  return L2O_OK;
+  return l2o::occupancy_launch("l2o_crnn_step", step_kernel, kFwdBlock, 0, a->n, (cudaStream_t)stream, k);
 }
 
 int l2o_crnn_bwd(const l2o_crnn_bwd_args* a, void* stream) {
@@ -493,24 +457,18 @@ int l2o_crnn_bwd(const l2o_crnn_bwd_args* a, void* stream) {
     return L2O_E_INVALID;
   const void* fp[] = {a->theta, a->g, a->state_old, a->d_state_new, a->d_update, a->d_state_old};
   for (const void* p : fp)
-    if (misaligned(p, alignof(float))) return L2O_E_INVALID;
-  if (misaligned(a->d_theta, alignof(double))) return L2O_E_INVALID;
+    if (l2o::misaligned(p, alignof(float))) return L2O_E_INVALID;
+  if (l2o::misaligned(a->d_theta, alignof(double))) return L2O_E_INVALID;
   if (a->d_g) {
-    if (misaligned(a->d_g, alignof(float))) return L2O_E_INVALID;
+    if (l2o::misaligned(a->d_g, alignof(float))) return L2O_E_INVALID;
     const size_t n = (size_t)a->n, f = sizeof(float);
     const void* other[] = {a->theta, a->g, a->state_old, a->d_state_new, a->d_update, a->d_state_old, a->d_theta};
     const size_t bytes[] = {kTheta * f, n * f, kPlanes * n * f, kPlanes * n * f, n * f, kPlanes * n * f,
                             kTheta * sizeof(double)};
     if (l2o::overlaps_any(a->d_g, n * f, other, bytes, 7)) return L2O_E_INVALID;
   }
-  const int cap = bwd_grid();
-  if (cap <= 0) return l2o::set_cuda_error(cudaGetLastError(), "l2o_crnn_bwd shared-memory size");
-  const int64_t tiles = (a->n + kBwdBlock - 1) / kBwdBlock;
   BwdArgs k{a->n, a->theta, a->g, a->state_old, a->d_state_new, a->d_update, a->d_state_old, a->d_theta, a->d_g};
-  bwd_kernel<<<(unsigned)(tiles < cap ? tiles : cap), kBwdBlock, sizeof(BwdSmem), (cudaStream_t)stream>>>(k);
-  L2O_CUDA_TRY(cudaGetLastError());
-  l2o::count_launch();
-  return L2O_OK;
+  return l2o::occupancy_launch("l2o_crnn_bwd", bwd_kernel, kBwdBlock, sizeof(BwdSmem), a->n, (cudaStream_t)stream, k);
 }
 
 }  // extern "C"

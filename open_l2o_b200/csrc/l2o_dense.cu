@@ -235,9 +235,7 @@ int l2o_dense_step(l2o_dense_handle h, const l2o_dense_step_args* a, void* strea
   if (h->SF > 0 && (!a->state_in || !a->state_out)) return L2O_E_INVALID;
   if (a->rows == 0) return L2O_OK;
   dense_step_kernel<<<(int)((a->rows + kRows - 1) / kRows), kRows, 0, (cudaStream_t)stream>>>(make_shape(h), *a);
-  l2o::count_launch();
-  L2O_CUDA_TRY(cudaGetLastError());
-  return L2O_OK;
+  return l2o::after_launch("l2o_dense_step");
 }
 
 int l2o_dense_unroll_bwd(l2o_dense_handle h, const l2o_dense_bwd_args* a, void* stream) {
@@ -248,11 +246,9 @@ int l2o_dense_unroll_bwd(l2o_dense_handle h, const l2o_dense_bwd_args* a, void* 
   if (a->rows == 0 || a->T == 0) return L2O_OK;
   const size_t smem = (size_t)h->P * sizeof(float);
   if (smem > 200 * 1024) return L2O_E_UNSUPPORTED;
-  L2O_CUDA_TRY(cudaFuncSetAttribute(dense_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  if (int rc = l2o::raise_smem_limit("l2o_dense_unroll_bwd", dense_bwd_kernel, smem)) return rc;
   dense_bwd_kernel<<<(int)((a->rows + kRows - 1) / kRows), kRows, smem, (cudaStream_t)stream>>>(make_shape(h), *a, (int)h->P);
-  l2o::count_launch();
-  L2O_CUDA_TRY(cudaGetLastError());
-  return L2O_OK;
+  return l2o::after_launch("l2o_dense_unroll_bwd");
 }
 
 }  // extern "C"

@@ -1,23 +1,15 @@
 // FFMA engine, single-step kernel instantiations.
-#include "l2o_ffma_launch.cuh"
+#include "cwlstm_ffma.cuh"
+#include "l2o_internal.h"
 
 namespace l2o {
-template <class C>
-static int do_step(const l2o_net* h, const l2o_step_args& a, cudaStream_t st) {
-  auto k = step_kernel<C>;
-  const size_t smem = (size_t)(round4(C::P) + 4) * sizeof(float);
-  int grid = 1;
-  int rc = ffma_launch_cfg(k, smem, a.n, grid);
-  if (rc) return rc;
-  k<<<grid, kTile, smem, st>>>(a, h->rt);
-  count_launch();
-  L2O_CUDA_TRY(cudaGetLastError());
-  return L2O_OK;
-}
-
 int ffma_step(const l2o_net* h, const l2o_step_args& a, cudaStream_t st) {
-#define X(id, PRE, NIN, F, H1, H2) \
-  if (h->cfg == id) return do_step<Cfg<PRE, NIN, F, H1, H2>>(h, a, st);
+#define X(id, PRE, NIN, F, H1, H2)                                                                  \
+  if (h->cfg == id) {                                                                               \
+    using C = Cfg<PRE, NIN, F, H1, H2>;                                                             \
+    const size_t smem = (size_t)(round4(C::P) + 4) * sizeof(float);                                 \
+    return occupancy_launch("l2o_step", step_kernel<C>, kTile, smem, a.n, st, a, h->rt);            \
+  }
   L2O_FOR_EACH_CFG(X)
 #undef X
   return L2O_E_UNSUPPORTED;

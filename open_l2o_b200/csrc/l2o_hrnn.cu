@@ -293,13 +293,6 @@ void free_buried() {
 }
 }  // namespace
 
-// coord_tc_kernel needs more than the default 48 KB of dynamic shared memory: raise its limit once per process
-static bool coord_tc_smem_set() {
-  static const bool ok = cudaFuncSetAttribute(tcg::coord_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                              (int)sizeof(tcg::SmemG)) == cudaSuccess;
-  return ok;
-}
-
 extern "C" {
 
 int l2o_hrnn_create(l2o_hrnn_handle* out, const int64_t* tensor_sizes, int32_t n_tensors) {
@@ -342,7 +335,7 @@ int l2o_hrnn_create(l2o_hrnn_handle* out, const int64_t* tensor_sizes, int32_t n
     if (h->d_blocks) cudaFree(h->d_blocks);
     if (h->d_sizes) cudaFree(h->d_sizes);
     delete h;
-    return l2o::set_cuda_error(e, "l2o_hrnn_create");
+    return l2o::set_cuda_error(e, "l2o_hrnn_create", "cudaMalloc / cudaMemcpy");
   }
   *out = h;
   return L2O_OK;
@@ -368,7 +361,7 @@ int64_t l2o_hrnn_workspace_bytes(l2o_hrnn_handle h) {
 static int check_args(l2o_hrnn_handle h, const l2o_hrnn_args* a, bool need_xg) {
   if (!h || !a || !a->theta || !a->state || !a->layer || !a->global || !a->workspace) return L2O_E_INVALID;
   if (need_xg && (!a->x || !a->g)) return L2O_E_INVALID;
-  if (((uintptr_t)a->workspace & 255) != 0) return L2O_E_INVALID;
+  if (l2o::misaligned(a->workspace, 256)) return L2O_E_INVALID;
   return L2O_OK;
 }
 
@@ -378,9 +371,7 @@ int l2o_hrnn_init_state(l2o_hrnn_handle h, const l2o_hrnn_args* a, void* stream)
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t work = h->n > (int64_t)h->nt * H1 ? h->n : (int64_t)h->nt * H1;
   init_state_kernel<<<(unsigned)((work + 255) / 256), 256, 0, st>>>(a->theta, a->state, h->n, a->layer, a->global, h->nt);
-  L2O_CUDA_TRY(cudaGetLastError());
-  l2o::count_launch();
-  return L2O_OK;
+  return l2o::after_launch("l2o_hrnn_init_state");
 }
 
 // ---- phases.  Single-GPU: prepare = prepare_local + prepare_finish, step = step_local + step_finish.  Sharded: the
@@ -391,11 +382,10 @@ int l2o_hrnn_prepare_local(l2o_hrnn_handle h, const l2o_hrnn_args* a, void* stre
   cudaStream_t st = (cudaStream_t)stream;
   Workspace w;
   const size_t bytes = carve(w, a->workspace, h->nt, h->n);
-  L2O_CUDA_TRY(cudaMemsetAsync(a->workspace, 0, bytes - align_up(sizeof(float) * (size_t)h->n, 256), st));
+  L2O_CUDA_TRY("l2o_hrnn_prepare_local",
+               cudaMemsetAsync(a->workspace, 0, bytes - align_up(sizeof(float) * (size_t)h->n, 256), st));
   scan_kernel<<<h->nblocks, kBlock, 0, st>>>(a->state, h->n, h->d_blocks, w);
-  L2O_CUDA_TRY(cudaGetLastError());
-  l2o::count_launch();
-  return L2O_OK;
+  return l2o::after_launch("l2o_hrnn_prepare_local");
 }
 
 int l2o_hrnn_prepare_finish(l2o_hrnn_handle h, const l2o_hrnn_args* a, void* stream) {
@@ -405,9 +395,7 @@ int l2o_hrnn_prepare_finish(l2o_hrnn_handle h, const l2o_hrnn_args* a, void* str
   Workspace w;
   carve(w, a->workspace, h->nt, h->n);
   tensor_kernel<<<1, 64, 0, st>>>(a->theta, a->layer, a->global, h->nt, h->d_sizes, h->n_global, w, 1);
-  L2O_CUDA_TRY(cudaGetLastError());
-  l2o::count_launch();
-  return L2O_OK;
+  return l2o::after_launch("l2o_hrnn_prepare_finish");
 }
 
 int l2o_hrnn_prepare(l2o_hrnn_handle h, const l2o_hrnn_args* a, void* stream) {
@@ -421,16 +409,16 @@ int l2o_hrnn_step_local(l2o_hrnn_handle h, const l2o_hrnn_args* a, void* stream)
   cudaStream_t st = (cudaStream_t)stream;
   Workspace w;
   carve(w, a->workspace, h->nt, h->n);
-  if (!coord_tc_smem_set()) return l2o::set_cuda_error(cudaGetLastError(), "coord_tc_kernel shared-memory size");
-  const int sms = l2o::device_sms();
+  const char* fn = "l2o_hrnn_step_local";
+  rc = l2o::raise_smem_limit(fn, tcg::coord_tc_kernel, sizeof(tcg::SmemG));
+  if (rc) return rc;
+  const int sms = l2o::device_sms(fn);
   if (sms <= 0) return L2O_E_CUDA;
   const int cap = sms * tcg::kCtasPerSm;   // persistent CTAs
   const int grid = h->nblocks < cap ? h->nblocks : cap;
   tcg::coord_tc_kernel<<<grid, tcg::kTile, sizeof(tcg::SmemG), st>>>(a->theta, a->g, a->state, h->n, h->d_blocks, h->nblocks,
                                                                      w);
-  L2O_CUDA_TRY(cudaGetLastError());
-  l2o::count_launch();
-  return L2O_OK;
+  return l2o::after_launch(fn);
 }
 
 int l2o_hrnn_step_finish(l2o_hrnn_handle h, const l2o_hrnn_args* a, void* stream) {
@@ -440,11 +428,10 @@ int l2o_hrnn_step_finish(l2o_hrnn_handle h, const l2o_hrnn_args* a, void* stream
   Workspace w;
   carve(w, a->workspace, h->nt, h->n);
   tensor_kernel<<<1, 64, 0, st>>>(a->theta, a->layer, a->global, h->nt, h->d_sizes, h->n_global, w, 0);
-  L2O_CUDA_TRY(cudaGetLastError());
+  rc = l2o::after_launch("l2o_hrnn_step_finish");
+  if (rc) return rc;
   apply_kernel<<<(h->nblocks + 3) / 4, kBlock, 0, st>>>(a->x, a->update, h->d_blocks, h->nblocks, w);
-  L2O_CUDA_TRY(cudaGetLastError());
-  l2o::count_launch(2);
-  return L2O_OK;
+  return l2o::after_launch("l2o_hrnn_step_finish");
 }
 
 int l2o_hrnn_step(l2o_hrnn_handle h, const l2o_hrnn_args* a, void* stream) {
@@ -457,7 +444,7 @@ int l2o_hrnn_coord_bwd(l2o_hrnn_handle h, const l2o_hrnn_bwd_args* a, void* stre
       !a->d_state_new || !a->d_upd || !a->d_sums || !a->d_state_old || !a->d_theta || !a->d_bias0 || !a->d_mean_log_lr)
     return L2O_E_INVALID;
   if (a->d_g) {
-    if ((uintptr_t)a->d_g & (alignof(float) - 1)) return L2O_E_INVALID;
+    if (l2o::misaligned(a->d_g, alignof(float))) return L2O_E_INVALID;
     const size_t n = (size_t)h->n, nt = (size_t)h->nt, f = sizeof(float), d = sizeof(double);
     const void* other[] = {a->theta, a->state_old, a->g, a->bias0, a->zero_flag, a->mean_log_lr, a->d_state_new,
                            a->d_upd, a->d_sums, a->d_state_old, a->d_theta, a->d_bias0, a->d_mean_log_lr};
@@ -467,13 +454,11 @@ int l2o_hrnn_coord_bwd(l2o_hrnn_handle h, const l2o_hrnn_bwd_args* a, void* stre
   }
   bwd::Args k{a->theta, a->state_old, a->g, a->bias0, a->zero_flag, a->mean_log_lr, a->d_state_new, a->d_upd, a->d_sums,
               a->d_state_old, a->d_theta, a->d_bias0, a->d_mean_log_lr, a->d_g};
-  const int sms = l2o::device_sms();
+  const int sms = l2o::device_sms("l2o_hrnn_coord_bwd");
   if (sms <= 0) return L2O_E_CUDA;
   const int grid = h->nblocks < 2 * sms ? h->nblocks : 2 * sms;
   bwd::coord_bwd_kernel<<<grid, bwd::kBwdBlock, 0, (cudaStream_t)stream>>>(k, h->n, h->d_blocks, h->nblocks);
-  L2O_CUDA_TRY(cudaGetLastError());
-  l2o::count_launch();
-  return L2O_OK;
+  return l2o::after_launch("l2o_hrnn_coord_bwd");
 }
 
 int l2o_hrnn_workspace_layout(l2o_hrnn_handle h, int64_t offsets[7]) {
@@ -498,7 +483,8 @@ int l2o_hrnn_set_global_sizes(l2o_hrnn_handle h, const int64_t* global_sizes) {
     if (global_sizes[j] <= 0) return L2O_E_INVALID;
     tot += global_sizes[j];
   }
-  L2O_CUDA_TRY(cudaMemcpy(h->d_sizes, global_sizes, sizeof(int64_t) * h->nt, cudaMemcpyHostToDevice));
+  L2O_CUDA_TRY("l2o_hrnn_set_global_sizes",
+               cudaMemcpy(h->d_sizes, global_sizes, sizeof(int64_t) * h->nt, cudaMemcpyHostToDevice));
   h->n_global = tot;
   return L2O_OK;
 }

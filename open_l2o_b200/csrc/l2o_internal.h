@@ -28,9 +28,36 @@ struct l2o_net {
 };
 
 namespace l2o {
-int set_cuda_error(cudaError_t e, const char* where);  // records the message, returns L2O_E_CUDA
-void count_launch(int n = 1);
-int device_sms();  // SM count of the current device (cached), 0 on failure
+// Host side of every launch.  `fn` names the C entry point being served: a failure is recorded for
+// l2o_last_cuda_error as "<fn>: <CUDA call>: <error string>" and returns L2O_E_CUDA.
+int set_cuda_error(cudaError_t e, const char* fn, const char* call);
+int device_sms(const char* fn);   // SM count of the current device (cached), 0 on failure
+// Raises kernel's dynamic shared-memory limit on the current device to at least smem.  Each thread remembers the
+// highest limit it set per kernel and device, so the limit is only ever raised: a lower one would break the
+// launches another thread sized for a higher one.
+int raise_smem_limit(const char* fn, const void* kernel, size_t smem);
+// raise_smem_limit, then grid = min(ceil(n / block), occupancy x SMs) for (kernel, block, smem), the resident CTAs
+// cached per kernel, device, block and smem on each thread.  L2O_E_UNSUPPORTED when not one CTA fits on an SM.
+int occupancy_grid(const char* fn, const void* kernel, int block, size_t smem, int64_t n, int& grid);
+// Checks the launch just issued with one cudaGetLastError and counts it in l2o_launch_count if it succeeded.
+int after_launch(const char* fn);
+
+template <class K>
+int raise_smem_limit(const char* fn, K* kernel, size_t smem) {
+  return raise_smem_limit(fn, (const void*)kernel, smem);
+}
+
+// Launches kernel(args...) over n items, `block` per CTA, with at most as many CTAs as are resident at once (the
+// kernels loop over the remaining blocks).
+template <class K, class... Args>
+int occupancy_launch(const char* fn, K* kernel, int block, size_t smem, int64_t n, cudaStream_t st, const Args&... args) {
+  int grid = 0;
+  if (int rc = occupancy_grid(fn, (const void*)kernel, block, smem, n, grid)) return rc;
+  kernel<<<grid, block, smem, st>>>(args...);
+  return after_launch(fn);
+}
+
+inline bool misaligned(const void* p, uintptr_t align) { return ((uintptr_t)p & (align - 1)) != 0; }
 
 // Does the byte range [p, p + bytes) share a byte with any of the ranges (q[k], qbytes[k])?  Null q[k] are skipped.
 inline bool overlaps_any(const void* p, size_t bytes, const void* const* q, const size_t* qbytes, int nq) {
@@ -58,8 +85,8 @@ bool tc_bwd_ok(const l2o_net* h, const l2o_bwd_args& a);
 int tc_unroll_bwd(l2o_net* h, const l2o_bwd_args& a, cudaStream_t st, const l2o_bwd_carry* c = nullptr);
 }  // namespace l2o
 
-#define L2O_CUDA_TRY(expr)                                              \
-  do {                                                                  \
-    cudaError_t e__ = (expr);                                           \
-    if (e__ != cudaSuccess) return l2o::set_cuda_error(e__, #expr);     \
+#define L2O_CUDA_TRY(fn, expr)                                            \
+  do {                                                                    \
+    cudaError_t e__ = (expr);                                             \
+    if (e__ != cudaSuccess) return l2o::set_cuda_error(e__, fn, #expr);   \
   } while (0)

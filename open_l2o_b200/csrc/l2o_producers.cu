@@ -277,11 +277,9 @@ extern "C" int l2o_lasso_grad(const l2o_lasso_args* a, void* stream) {
   if (a->batch == 0) return L2O_OK;
   const size_t smem = (size_t)(((a->n + 3) & ~3) + a->m) * sizeof(float);
   if (smem > 200 * 1024) return L2O_E_UNSUPPORTED;
-  L2O_CUDA_TRY(cudaFuncSetAttribute(lasso_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  if (int rc = l2o::raise_smem_limit("l2o_lasso_grad", lasso_grad_kernel, smem)) return rc;
   lasso_grad_kernel<<<a->batch, kLassoThreads, smem, (cudaStream_t)stream>>>(*a);
-  l2o::count_launch();
-  L2O_CUDA_TRY(cudaGetLastError());
-  return L2O_OK;
+  return l2o::after_launch("l2o_lasso_grad");
 }
 
 extern "C" int l2o_confocal_grad(const l2o_confocal_args* a, void* stream) {
@@ -293,9 +291,7 @@ extern "C" int l2o_confocal_grad(const l2o_confocal_args* a, void* stream) {
   const size_t smem = confocal_smem_bytes(a->num_points, a->roi);
   if (smem > kConfSmemLimit) return L2O_E_UNSUPPORTED;
   if (a->batch == 0) return L2O_OK;
-  L2O_CUDA_TRY(cudaFuncSetAttribute(confocal_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  if (int rc = l2o::raise_smem_limit("l2o_confocal_grad", confocal_grad_kernel, smem)) return rc;
   confocal_grad_kernel<<<a->batch, kConfThreads, smem, (cudaStream_t)stream>>>(*a);
-  l2o::count_launch();
-  L2O_CUDA_TRY(cudaGetLastError());
-  return L2O_OK;
+  return l2o::after_launch("l2o_confocal_grad");
 }

@@ -37,9 +37,9 @@ void tc_release_image(l2o_net* h) {
   h->tc_img = nullptr;
 }
 
-static int ensure_image(l2o_net* h) {
+static int ensure_image(l2o_net* h, const char* fn) {
   int dev = 0;
-  L2O_CUDA_TRY(cudaGetDevice(&dev));
+  L2O_CUDA_TRY(fn, cudaGetDevice(&dev));
   if (h->tc_img == nullptr || h->tc_img_dev != dev) {
     tc_release_image(h);
     {
@@ -52,7 +52,7 @@ static int ensure_image(l2o_net* h) {
           break;
         }
     }
-    if (h->tc_img == nullptr) L2O_CUDA_TRY(cudaMalloc(&h->tc_img, tc::kImgMaxFloats * sizeof(float)));
+    if (h->tc_img == nullptr) L2O_CUDA_TRY(fn, cudaMalloc(&h->tc_img, tc::kImgMaxFloats * sizeof(float)));
     h->tc_img_dev = dev;
     h->tc_img_mode = -1;
   }
@@ -68,24 +68,24 @@ bool tc_bwd_ok(const l2o_net* h, const l2o_bwd_args& a) {
 }
 
 template <class C>
-static int tc_launch_bwd_any(const l2o_net* h, const l2o_bwd_args& a, cudaStream_t st, int sms, const l2o_bwd_carry* c) {
-  return c ? tc_launch_bwd<C, true>(h->rt, a, h->tc_img, st, sms, *c)
-           : tc_launch_bwd<C, false>(h->rt, a, h->tc_img, st, sms, l2o_bwd_carry{});
+static int tc_launch_bwd_any(const char* fn, const l2o_net* h, const l2o_bwd_args& a, cudaStream_t st, int sms,
+                             const l2o_bwd_carry* c) {
+  return c ? tc_launch_bwd<C, true>(fn, h->rt, a, h->tc_img, st, sms, *c)
+           : tc_launch_bwd<C, false>(fn, h->rt, a, h->tc_img, st, sms, l2o_bwd_carry{});
 }
 
 int tc_unroll_bwd(l2o_net* h, const l2o_bwd_args& a, cudaStream_t st, const l2o_bwd_carry* c) {
   if (!tc_bwd_ok(h, a)) return L2O_E_UNSUPPORTED;
-  int rc = ensure_image(h);
+  const char* fn = c ? "l2o_unroll_bwd_carry" : "l2o_unroll_bwd";
+  int rc = ensure_image(h, fn);
   if (rc) return rc;
-  const int sms = device_sms();
+  const int sms = device_sms(fn);
   if (sms <= 0) return L2O_E_CUDA;
   rc = L2O_E_UNSUPPORTED;
-  if (h->cfg == 0) rc = tc_launch_bwd_any<Cfg<L2O_PRE_IDENTITY, 1, 1, 20, 20>>(h, a, st, sms, c);
-  if (h->cfg == 1) rc = tc_launch_bwd_any<Cfg<L2O_PRE_LOGSIGN, 1, 2, 20, 20>>(h, a, st, sms, c);
-  if (h->cfg == 2) rc = tc_launch_bwd_any<Cfg<L2O_PRE_FC, 2, 20, 20, 20>>(h, a, st, sms, c);
-  if (rc == L2O_OK) count_launch(h->cfg == 2 ? 3 : 2);
-  h->tc_img_mode = 1;
-  if (rc == L2O_E_CUDA) return set_cuda_error(cudaGetLastError(), "tc_unroll_bwd launch");
+  if (h->cfg == 0) rc = tc_launch_bwd_any<Cfg<L2O_PRE_IDENTITY, 1, 1, 20, 20>>(fn, h, a, st, sms, c);
+  if (h->cfg == 1) rc = tc_launch_bwd_any<Cfg<L2O_PRE_LOGSIGN, 1, 2, 20, 20>>(fn, h, a, st, sms, c);
+  if (h->cfg == 2) rc = tc_launch_bwd_any<Cfg<L2O_PRE_FC, 2, 20, 20, 20>>(fn, h, a, st, sms, c);
+  h->tc_img_mode = rc == L2O_OK ? 1 : -1;   // after a failed call the image may hold either layout, or a partial one
   return rc;
 }
 
@@ -98,9 +98,10 @@ bool tc_step_ok(const l2o_net* h, const l2o_step_args& a) {
 // out-of-place final-state write.
 int tc_step(l2o_net* h, const l2o_step_args& s, cudaStream_t st) {
   if (!tc_step_ok(h, s)) return L2O_E_UNSUPPORTED;
-  int rc = ensure_image(h);
+  const char* fn = "l2o_step";
+  int rc = ensure_image(h, fn);
   if (rc) return rc;
-  const int sms = device_sms();
+  const int sms = device_sms(fn);
   if (sms <= 0) return L2O_E_CUDA;
   l2o_unroll_args a{};
   a.n = s.n;
@@ -120,30 +121,28 @@ int tc_step(l2o_net* h, const l2o_step_args& s, cudaStream_t st) {
   const tc::FwdExtra ex{s.step_ptr, s.t_offset, s.step_ptr ? 0.f : s.p};
   rc = L2O_E_UNSUPPORTED;
   const bool prep = !(s.reuse_weights && h->tc_img_mode == 0);   // forward image of this theta already in place
-  if (h->cfg == 0) rc = tc_launch_fwd<Cfg<L2O_PRE_IDENTITY, 1, 1, 20, 20>>(h->rt, a, h->tc_img, st, sms, s.state_out, ex, prep);
-  if (h->cfg == 1) rc = tc_launch_fwd<Cfg<L2O_PRE_LOGSIGN, 1, 2, 20, 20>>(h->rt, a, h->tc_img, st, sms, s.state_out, ex, prep);
-  if (h->cfg == 2) rc = tc_launch_fwd<Cfg<L2O_PRE_FC, 2, 20, 20, 20>>(h->rt, a, h->tc_img, st, sms, s.state_out, ex, prep);
-  if (rc == L2O_OK) count_launch(prep ? 2 : 1);
-  h->tc_img_mode = 0;
-  if (rc == L2O_E_CUDA) return set_cuda_error(cudaGetLastError(), "tc_step launch");
+  if (h->cfg == 0)
+    rc = tc_launch_fwd<Cfg<L2O_PRE_IDENTITY, 1, 1, 20, 20>>(fn, h->rt, a, h->tc_img, st, sms, s.state_out, ex, prep);
+  if (h->cfg == 1)
+    rc = tc_launch_fwd<Cfg<L2O_PRE_LOGSIGN, 1, 2, 20, 20>>(fn, h->rt, a, h->tc_img, st, sms, s.state_out, ex, prep);
+  if (h->cfg == 2)
+    rc = tc_launch_fwd<Cfg<L2O_PRE_FC, 2, 20, 20, 20>>(fn, h->rt, a, h->tc_img, st, sms, s.state_out, ex, prep);
+  h->tc_img_mode = rc == L2O_OK ? 0 : -1;
   return rc;
 }
 
 int tc_unroll_fwd(l2o_net* h, const l2o_unroll_args& a, cudaStream_t st) {
   if (!tc_supported(h->cfg) || !tc_fwd_ok(h, a)) return L2O_E_UNSUPPORTED;
-  {
-    int rc0 = ensure_image(h);
-    if (rc0) return rc0;
-  }
-  const int sms = device_sms();
+  const char* fn = "l2o_unroll_fwd";
+  int rc = ensure_image(h, fn);
+  if (rc) return rc;
+  const int sms = device_sms(fn);
   if (sms <= 0) return L2O_E_CUDA;
-  int rc = L2O_E_UNSUPPORTED;
-  if (h->cfg == 0) rc = tc_launch_fwd<Cfg<L2O_PRE_IDENTITY, 1, 1, 20, 20>>(h->rt, a, h->tc_img, st, sms);
-  if (h->cfg == 1) rc = tc_launch_fwd<Cfg<L2O_PRE_LOGSIGN, 1, 2, 20, 20>>(h->rt, a, h->tc_img, st, sms);
-  if (h->cfg == 2) rc = tc_launch_fwd<Cfg<L2O_PRE_FC, 2, 20, 20, 20>>(h->rt, a, h->tc_img, st, sms);
-  if (rc == L2O_OK) count_launch(2);
-  h->tc_img_mode = 0;
-  if (rc == L2O_E_CUDA) return set_cuda_error(cudaGetLastError(), "tc_unroll_fwd launch");
+  rc = L2O_E_UNSUPPORTED;
+  if (h->cfg == 0) rc = tc_launch_fwd<Cfg<L2O_PRE_IDENTITY, 1, 1, 20, 20>>(fn, h->rt, a, h->tc_img, st, sms);
+  if (h->cfg == 1) rc = tc_launch_fwd<Cfg<L2O_PRE_LOGSIGN, 1, 2, 20, 20>>(fn, h->rt, a, h->tc_img, st, sms);
+  if (h->cfg == 2) rc = tc_launch_fwd<Cfg<L2O_PRE_FC, 2, 20, 20, 20>>(fn, h->rt, a, h->tc_img, st, sms);
+  h->tc_img_mode = rc == L2O_OK ? 0 : -1;
   return rc;
 }
 
