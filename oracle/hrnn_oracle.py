@@ -225,5 +225,5 @@ def step(theta: torch.Tensor, params: List[torch.Tensor], grads: List[torch.Tens
                            P["Layer2_RNN/BiasGRUCell/gates/Affine/Bias"],
                            P["Layer2_RNN/BiasGRUCell/candidate/Affine/Matrix"],
                            P["Layer2_RNN/BiasGRUCell/candidate/Affine/Bias"],
-                           torch.zeros(1, 3 * levels[2], dtype=theta.dtype))  # bias=None -> zeros
+                           torch.zeros(1, 3 * levels[2], dtype=theta.dtype, device=theta.device))  # bias=None -> zeros
     return new_params, new_states, new_global, update_steps
