@@ -460,6 +460,84 @@ int l2o_tadam_bwd(const l2o_tadam_bwd_args* a, void* stream);
 int l2o_lrsgd_step(const l2o_lrsgd_step_args* a, void* stream);
 int l2o_lrsgd_bwd(const l2o_lrsgd_bwd_args* a, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * Model-based L2O's LISTA family (MB = Model_Base_L2O/): ISTA unrolled into K trained layers, starting from x_0 = 0.
+ * Row-major: y [B][M] (row stride ldy, so a data batch [y | x_true] can be passed as is), x [B][N], A [M][N].
+ *
+ *   l2o_ista_fwd              layers [k0, k1) of the Keras model's call                       MB/models/lista.py:32-45
+ *                             (one launch)                                   lista_cp.py, lista_cpss.py:29-39, alista.py:29-39
+ *                             with shrink_free / shrink_ss                                    MB/models/utils.py:11-52
+ *   l2o_ista_bwd              tf.gradients of a loss on x_{k1} w.r.t. every variable          MB/train.py:307 (model.fit)
+ *                             and x_{k0}, times utils.Adam's 0.3^age multipliers              MB/utils.py:115-135
+ *                             (two launches; apply them with l2o_adam_step, eps = 1e-7 for Keras)
+ *   l2o_ista_loss_grad        utils.MSE / utils.LassoLoss per row and their gradient          MB/utils.py:6-38
+ *   l2o_ista_workspace_bytes  the scratch l2o_ista_bwd needs (dz_k and per-CTA partial sums)
+ *
+ * Forms: L2O_ISTA_LISTA   z_k = y B1^T + s_k x_k W_k^T  (layer 0 has no W term); B1 [N][M], W slots [N][N], slot k-1
+ *                         for layer k (one slot when share_W).
+ *        L2O_ISTA_COUPLED z_k = x_k + s_k (y - x_k A^T) W_k;  W slots [M][N], slot k (one slot when share_W).
+ * x_{k+1} = sign(z) relu(|z| - theta_k); with ss_rank, entries with |z| > theta_k and |z| > t_b pass unshrunk, t_b
+ * being row b's |z| at 0-based rank ss_rank[k] in descending order (the caller maps the percentile to the rank).
+ * The backward overwrites every gradient it is given (zero for layers outside [k0, k1)); gscale[j] multiplies the
+ * gradient of every variable created with layer j (B1: layer 0; a shared W: its first layer).  L2O_E_UNSUPPORTED when
+ * M or N > 2048 or when a CTA's shared-memory plan exceeds 200 KB: 4 (8 (M + 4N) + 2048) bytes in the LISTA form,
+ * 4 (8 (2M + 3N) + 2048) in the coupled form (so the coupled form at M = 256, N = 512 needs 72 KB and at M = 1024 fits
+ * N <= 1365); l2o_ista_loss_grad: 4 (M + N) bytes > 200 KB.  Float pointers 4-byte aligned, double pointers
+ * 8-byte aligned (L2O_E_INVALID otherwise). */
+#define L2O_ISTA_LISTA 0
+#define L2O_ISTA_COUPLED 1
+#define L2O_ISTA_TASK_SC 0
+#define L2O_ISTA_TASK_LASSO 1
+typedef struct {
+  int32_t form;            /* L2O_ISTA_LISTA or L2O_ISTA_COUPLED */
+  int32_t batch, m, n;     /* > 0 */
+  int32_t num_layers;      /* K: sizes theta, step, ss_rank and the W slots */
+  int32_t k0, k1;          /* layers run: 0 <= k0 < k1 <= K */
+  int32_t share_W;         /* 0 or 1 */
+  const float* A;          /* [M][N] (coupled form) */
+  const float* B1;         /* [N][M] (LISTA form) */
+  const float* W;          /* W slots (see above) */
+  const float* theta;      /* [K] */
+  const float* step;       /* [K] s_k, or NULL: every s_k = 1 */
+  const int32_t* ss_rank;  /* [K] support-selection ranks (>= N reads as N-1, < 0 as soft shrinkage), or NULL: soft
+                              shrinkage in every layer */
+  const float* y;          /* [B] rows of stride ldy >= M */
+  int64_t ldy;
+  const float* x_in;       /* [B][N] x_{k0}, or NULL: zeros */
+  float* xs;               /* [k1-k0][B][N] out: x_{k0+1} .. x_{k1} */
+  float* zs;               /* [k1-k0][B][N] out: z_k before shrinkage, or NULL (required by the backward) */
+  float* rs;               /* [k1-k0][B][M] out: coupled r_k = y - x_k A^T, or NULL (required by the backward) */
+  uint8_t* sel;            /* [k1-k0][B][N] out: 1 where support selection passed z through, or NULL (required by the
+                              backward with ss_rank) */
+} l2o_ista_args;
+typedef struct {
+  const float* d_xk;       /* [B][N] dL/dx_{k1} */
+  float* d_x_in;           /* optional [B][N] out: dL/dx_{k0} */
+  double* dW;              /* W slots out, or NULL: W is a constant (ALISTA) */
+  double* dB1;             /* [N][M] out (LISTA form, required) */
+  double* dtheta;          /* [K] out */
+  double* dstep;           /* [K] out, or NULL */
+  const float* gscale;     /* [K] gradient multipliers by creation layer, or NULL: all 1 */
+  void* scratch;           /* l2o_ista_workspace_bytes */
+} l2o_ista_grads;
+typedef struct {
+  int32_t task;            /* L2O_ISTA_TASK_SC: 0.5 ||x - x_true||^2;  LASSO: 0.5 (0.5 ||x A^T - y||^2) + lam ||x||_1 */
+  int32_t batch, m, n;
+  const float* A;          /* [M][N] (lasso) */
+  const float* y;          /* rows of stride ldy (lasso) */
+  int64_t ldy;
+  const float* x_true;     /* rows of stride ldx (sc) */
+  int64_t ldx;
+  const float* x;          /* [B][N] x_K */
+  float lam;
+  float* d_x;              /* [B][N] out: dL/dx_K */
+  double* loss;            /* optional [B] out: the loss of each row */
+} l2o_ista_loss_args;
+int l2o_ista_workspace_bytes(const l2o_ista_args* a, size_t* bytes);
+int l2o_ista_fwd(const l2o_ista_args* a, void* stream);
+int l2o_ista_bwd(const l2o_ista_args* a, const l2o_ista_grads* g, void* stream);
+int l2o_ista_loss_grad(const l2o_ista_loss_args* a, void* stream);
+
 /* Number of this library's kernels launched so far in this process (bench.py's gpu_launches). */
 int64_t l2o_launch_count(void);
 const char* l2o_status_string(int status);

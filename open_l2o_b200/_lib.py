@@ -36,6 +36,7 @@ EXPORTS = [
     "l2o_crnn_theta_count", "l2o_crnn_state_floats", "l2o_crnn_step", "l2o_crnn_bwd",
     "l2o_tadam_theta_count", "l2o_tadam_state_floats", "l2o_tadam_step", "l2o_tadam_bwd", "l2o_lrsgd_step",
     "l2o_lrsgd_bwd",
+    "l2o_ista_workspace_bytes", "l2o_ista_fwd", "l2o_ista_bwd", "l2o_ista_loss_grad",
 ]
 
 
@@ -136,6 +137,24 @@ class LrsgdStepArgs(C.Structure):
 class LrsgdBwdArgs(C.Structure):
     _fields_ = [("n", C.c_int64), ("rates", _fp), ("n_steps", C.c_int32), ("itr", _fp), ("g", _fp),
                 ("d_update", _fp), ("d_rates", _fp), ("d_g", _fp)]
+
+
+class IstaArgs(C.Structure):
+    _fields_ = [("form", C.c_int32), ("batch", C.c_int32), ("m", C.c_int32), ("n", C.c_int32),
+                ("num_layers", C.c_int32), ("k0", C.c_int32), ("k1", C.c_int32), ("share_W", C.c_int32),
+                ("A", _fp), ("B1", _fp), ("W", _fp), ("theta", _fp), ("step", _fp), ("ss_rank", _fp), ("y", _fp),
+                ("ldy", C.c_int64), ("x_in", _fp), ("xs", _fp), ("zs", _fp), ("rs", _fp), ("sel", _fp)]
+
+
+class IstaGrads(C.Structure):
+    _fields_ = [("d_xk", _fp), ("d_x_in", _fp), ("dW", _fp), ("dB1", _fp), ("dtheta", _fp), ("dstep", _fp),
+                ("gscale", _fp), ("scratch", _fp)]
+
+
+class IstaLossArgs(C.Structure):
+    _fields_ = [("task", C.c_int32), ("batch", C.c_int32), ("m", C.c_int32), ("n", C.c_int32), ("A", _fp),
+                ("y", _fp), ("ldy", C.c_int64), ("x_true", _fp), ("ldx", C.c_int64), ("x", _fp), ("lam", C.c_float),
+                ("d_x", _fp), ("loss", _fp)]
 
 
 class L2OError(RuntimeError):
@@ -283,6 +302,12 @@ def lib():
     for name, args in (("l2o_tadam_step", TadamStepArgs), ("l2o_tadam_bwd", TadamBwdArgs),
                        ("l2o_lrsgd_step", LrsgdStepArgs), ("l2o_lrsgd_bwd", LrsgdBwdArgs)):
         getattr(L, name).argtypes = [C.POINTER(args), C.c_void_p]
+        getattr(L, name).restype = C.c_int
+    L.l2o_ista_workspace_bytes.argtypes = [C.POINTER(IstaArgs), C.POINTER(C.c_size_t)]
+    L.l2o_ista_fwd.argtypes = [C.POINTER(IstaArgs), C.c_void_p]
+    L.l2o_ista_bwd.argtypes = [C.POINTER(IstaArgs), C.POINTER(IstaGrads), C.c_void_p]
+    L.l2o_ista_loss_grad.argtypes = [C.POINTER(IstaLossArgs), C.c_void_p]
+    for name in ("l2o_ista_workspace_bytes", "l2o_ista_fwd", "l2o_ista_bwd", "l2o_ista_loss_grad"):
         getattr(L, name).restype = C.c_int
     for name in ("l2o_status_string", "l2o_last_cuda_error", "l2o_version"):
         getattr(L, name).restype = C.c_char_p

@@ -1,0 +1,643 @@
+// Model-based L2O's LISTA family (MB/ = Model_Base_L2O/ of the reference) — sm_90a kernels + C-ABI.
+//
+// Two cell forms over a batch of rows, layers k = k0 .. k1-1 (row-major: y [B,M], x [B,N], A [M,N]):
+//   LISTA   (MB/models/lista.py:32-45)        z_k = y B1^T + s_k x_k W_k^T       (layer 0: no W term)
+//   coupled (lista_cp.py, lista_cpss.py, alista.py)  r_k = y - x_k A^T,  z_k = x_k + s_k r_k W_k
+// then x_{k+1} = shrink(z_k): soft shrinkage sign(z) relu(|z| - theta_k) (MB/models/utils.py shrink_free), or support
+// selection (shrink_ss): entries with |z| > theta_k and |z| > the row's rank-q_k magnitude pass through unshrunk.
+//
+// Design.  One thread-block cluster of kCl CTAs owns kR batch rows for the whole pass, so a forward or backward over
+// any number of layers is ONE launch.  Each CTA of the cluster computes a 1/kCl column slice of every per-layer GEMM
+// for the cluster's rows and writes it into every CTA's shared memory (distributed shared memory); a cluster barrier
+// then makes the full rows visible to all of them.  The shrinkage, and the per-row rank selection of support
+// selection (a radix select, one warp per row), run redundantly in every CTA on the full rows, so the next layer
+// starts without another exchange.  The weights are read from global memory (they stay L2-resident across clusters).
+// The GEMMs are fp32 FFMA on the CUDA cores.  A CTA's slice, computed transposed, is one m64n8 wgmma tile
+// ((N / kCl) output columns x kR rows); running it on the tensor cores with the engine's 3xTF32 split and streaming the
+// weights by TMA is the next step (DESIGN §3.12), and matters most for large batches.
+//
+// The backward is the same cluster recurrence run from k1-1 down to k0; it records dz_k and per-CTA partial sums of
+// dtheta_k and ds_k.  A second launch forms the weight gradients from them (one GEMM per output, reducing over the
+// batch and, for a shared W or B1, over the layers: dB1 = sum_k dz_k^T y), and reduces the partial sums.
+#include <cooperative_groups.h>
+
+#include <algorithm>
+#include <cmath>
+#include <cstdint>
+
+#include "l2o_internal.h"
+
+namespace cg = cooperative_groups;
+
+namespace l2o {
+namespace ista {
+
+constexpr int kCl = 8;        // CTAs per cluster
+constexpr int kR = 8;         // batch rows per cluster (one warp per row in the rank selection)
+constexpr int kThreads = 256;
+constexpr int kWarps = kThreads / 32;
+constexpr int kMaxDim = kCl * kThreads;   // M, N <= 2048: a CTA's column slice is at most one thread per column
+constexpr int kTile = 64;                 // weight-gradient output tile
+constexpr int kChunk = 16;                // weight-gradient reduction chunk
+
+struct Slice {
+  int lo, hi;
+};
+__host__ __device__ inline Slice slice_of(int len, int c) {
+  const int w = (len + kCl - 1) / kCl;
+  const int lo = min(len, c * w);
+  return {lo, min(len, lo + w)};
+}
+
+__device__ __forceinline__ const float* w_slot(const l2o_ista_args& a, int k) {
+  if (a.form == L2O_ISTA_COUPLED) return a.W + (a.share_W ? 0 : (size_t)k * a.m * a.n);
+  return a.W + (a.share_W ? 0 : (size_t)(k - 1) * a.n * a.n);
+}
+__device__ __forceinline__ float step_of(const l2o_ista_args& a, int k) { return a.step ? a.step[k] : 1.f; }
+
+// out[b][j] = sum_t in[b][t] W[j][t] for j in [j0, j1): a warp per pair of outputs, lanes across t.
+template <class F>
+__device__ __forceinline__ void gemm_rows(const float* in, int ld_in, const float* __restrict__ W, int ldw, int T,
+                                          int j0, int j1, F&& epi) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  for (int j = j0 + 2 * w; j < j1; j += 2 * kWarps) {
+    const bool two = j + 1 < j1;
+    const float* w0 = W + (size_t)j * ldw;
+    const float* w1 = two ? w0 + ldw : w0;
+    float a0[kR], a1[kR];
+#pragma unroll
+    for (int b = 0; b < kR; ++b) a0[b] = a1[b] = 0.f;
+    for (int t = lane; t < T; t += 32) {
+      const float q0 = __ldg(w0 + t), q1 = __ldg(w1 + t);
+#pragma unroll
+      for (int b = 0; b < kR; ++b) {
+        const float v = in[b * ld_in + t];
+        a0[b] = fmaf(v, q0, a0[b]);
+        a1[b] = fmaf(v, q1, a1[b]);
+      }
+    }
+#pragma unroll
+    for (int b = 0; b < kR; ++b)
+#pragma unroll
+      for (int o = 16; o; o >>= 1) {
+        a0[b] += __shfl_xor_sync(0xffffffffu, a0[b], o);
+        a1[b] += __shfl_xor_sync(0xffffffffu, a1[b], o);
+      }
+#pragma unroll
+    for (int b = 0; b < kR; ++b) {
+      if (lane == b) epi(b, j, a0[b]);
+      if (two && lane == kR + b) epi(b, j + 1, a1[b]);
+    }
+  }
+}
+
+// out[b][j] = sum_t in[b][t] W[t][j] for j in [j0, j1): a thread per (column, t-group), groups summed through red.
+// Called by every thread of the CTA (it synchronises).
+template <class F>
+__device__ __forceinline__ void gemm_cols(const float* in, int ld_in, const float* __restrict__ W, int ldw, int T,
+                                          int j0, int j1, float* red, F&& epi) {
+  const int nj = j1 - j0;
+  if (nj <= 0) return;
+  const int G = kThreads / nj, jj = threadIdx.x % nj, g = threadIdx.x / nj;
+  float acc[kR];
+#pragma unroll
+  for (int b = 0; b < kR; ++b) acc[b] = 0.f;
+  if (g < G) {
+    const float* wc = W + j0 + jj;
+    for (int t = g; t < T; t += G) {
+      const float q = __ldg(wc + (size_t)t * ldw);
+#pragma unroll
+      for (int b = 0; b < kR; ++b) acc[b] = fmaf(in[b * ld_in + t], q, acc[b]);
+    }
+#pragma unroll
+    for (int b = 0; b < kR; ++b) red[(g * kR + b) * nj + jj] = acc[b];
+  }
+  __syncthreads();
+  for (int o = threadIdx.x; o < nj * kR; o += kThreads) {
+    const int b = o / nj, j = o % nj;
+    float s = 0.f;
+    for (int q = 0; q < G; ++q) s += red[(q * kR + b) * nj + j];
+    epi(b, j0 + j, s);
+  }
+  __syncthreads();
+}
+
+// |z| at 0-based rank t in descending order over one row (MSB-first radix select on the fp32 bit patterns, which
+// order like the values for |z| >= 0).  One warp; hist is the warp's 256 counters.
+__device__ float row_rank_abs(const float* z, int n, int t, unsigned* hist) {
+  const int lane = threadIdx.x & 31;
+  unsigned prefix = 0, mask = 0;
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    for (int i = lane; i < 256; i += 32) hist[i] = 0;
+    __syncwarp();
+    for (int i = lane; i < n; i += 32) {
+      const unsigned key = __float_as_uint(fabsf(z[i]));
+      if ((key & mask) == prefix) atomicAdd(&hist[(key >> shift) & 255u], 1u);
+    }
+    __syncwarp();
+    unsigned c[8], s = 0;
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      c[q] = hist[255 - 8 * lane - q];
+      s += c[q];
+    }
+    unsigned inc = s;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned v = __shfl_up_sync(0xffffffffu, inc, o);
+      if (lane >= o) inc += v;
+    }
+    const unsigned exc = inc - s;
+    const unsigned ball = __ballot_sync(0xffffffffu, exc <= (unsigned)t && (unsigned)t < inc);
+    const int src = __ffs(ball) - 1;
+    int bucket = 0;
+    unsigned before = 0;
+    if (lane == src) {
+      unsigned acc = exc;
+      bool found = false;
+#pragma unroll
+      for (int q = 0; q < 8; ++q) {
+        if (!found && (unsigned)t < acc + c[q]) {
+          bucket = 255 - 8 * lane - q;
+          before = acc;
+          found = true;
+        }
+        acc += c[q];
+      }
+    }
+    bucket = __shfl_sync(0xffffffffu, bucket, src);
+    before = __shfl_sync(0xffffffffu, before, src);
+    t -= (int)before;
+    prefix |= (unsigned)bucket << shift;
+    mask |= 255u << shift;
+    __syncwarp();
+  }
+  return __uint_as_float(prefix);
+}
+
+// Shared-memory plan of one CTA, in floats.
+struct Smem {
+  int y, x, r, z, by, red, total;
+};
+__host__ __device__ inline Smem smem_plan(const l2o_ista_args& a) {
+  Smem s;
+  s.y = 0;
+  s.x = s.y + kR * a.m;
+  s.r = s.x + kR * a.n;
+  s.z = s.r + (a.form == L2O_ISTA_COUPLED ? kR * a.m : 0);
+  s.by = s.z + 2 * kR * a.n;
+  s.red = s.by + (a.form == L2O_ISTA_LISTA ? kR * a.n : 0);
+  s.total = s.red + kThreads * kR;   // also the rank selection's 8 x 256 counters
+  return s;
+}
+
+__device__ __forceinline__ bool has_w_term(const l2o_ista_args& a, int k) {
+  return a.form == L2O_ISTA_COUPLED || k >= 1;
+}
+
+__global__ void __cluster_dims__(kCl, 1, 1) __launch_bounds__(kThreads)
+    ista_fwd_kernel(const l2o_ista_args a) {
+  extern __shared__ float4 smem_f4[];
+  float* sm = reinterpret_cast<float*>(smem_f4);
+  cg::cluster_group cl = cg::this_cluster();
+  const int c = (int)cl.block_rank();
+  const int row0 = (blockIdx.x / kCl) * kR;
+  const int M = a.m, N = a.n, tid = threadIdx.x;
+  const Smem P = smem_plan(a);
+  float *ys = sm + P.y, *xs = sm + P.x, *rb = sm + P.r, *by = sm + P.by, *red = sm + P.red;
+  unsigned* hist = reinterpret_cast<unsigned*>(red);
+  __shared__ float thr[kR];
+  const Slice sm_ = slice_of(M, c), sn = slice_of(N, c);
+
+  for (int e = tid; e < kR * M; e += kThreads) {
+    const int b = e / M, i = e % M, row = row0 + b;
+    ys[e] = row < a.batch ? a.y[(size_t)row * a.ldy + i] : 0.f;
+  }
+  for (int e = tid; e < kR * N; e += kThreads) {
+    const int b = e / N, n = e % N, row = row0 + b;
+    xs[e] = (a.x_in && row < a.batch) ? a.x_in[(size_t)row * N + n] : 0.f;
+  }
+  __syncthreads();
+  if (a.form == L2O_ISTA_LISTA) {   // y B1^T is the same in every layer of the pass: own slice only
+    gemm_rows(ys, M, a.B1, M, M, sn.lo, sn.hi, [&](int b, int n, float v) { by[b * N + n] = v; });
+  }
+  cl.sync();   // every CTA of the cluster has started (and finished its prologue) before any remote write
+
+  for (int k = a.k0; k < a.k1; ++k) {
+    const int l = k - a.k0;
+    float* zb = sm + P.z + (l & 1) * kR * N;
+    const float s = step_of(a, k), th = a.theta[k];
+    auto put_z = [&](int b, int n, float z) {
+      for (int q = 0; q < kCl; ++q) cl.map_shared_rank(zb, q)[b * N + n] = z;
+    };
+    if (a.form == L2O_ISTA_COUPLED) {
+      const float* W = w_slot(a, k);
+      gemm_rows(xs, N, a.A, N, N, sm_.lo, sm_.hi, [&](int b, int i, float v) {
+        const float r = ys[b * M + i] - v;
+        for (int q = 0; q < kCl; ++q) cl.map_shared_rank(rb, q)[b * M + i] = r;
+        if (a.rs && row0 + b < a.batch) a.rs[((size_t)l * a.batch + row0 + b) * M + i] = r;
+      });
+      cl.sync();
+      gemm_cols(rb, M, W, N, M, sn.lo, sn.hi, red, [&](int b, int n, float v) { put_z(b, n, xs[b * N + n] + s * v); });
+    } else if (has_w_term(a, k)) {
+      gemm_rows(xs, N, w_slot(a, k), N, N, sn.lo, sn.hi,
+                [&](int b, int n, float v) { put_z(b, n, by[b * N + n] + s * v); });
+    } else {
+      for (int e = tid; e < kR * (sn.hi - sn.lo); e += kThreads) {
+        const int b = e / (sn.hi - sn.lo), n = sn.lo + e % (sn.hi - sn.lo);
+        put_z(b, n, by[b * N + n]);
+      }
+    }
+    cl.sync();
+    const int rank = a.ss_rank ? min(a.ss_rank[k], N - 1) : -1;   // negative: soft shrinkage in this layer
+    if (rank >= 0) {
+      const int w = tid >> 5;
+      const float t = row_rank_abs(zb + w * N, N, rank, hist + w * 256);
+      if ((tid & 31) == 0) thr[w] = t;
+    }
+    __syncthreads();
+    for (int e = tid; e < kR * N; e += kThreads) {
+      const int b = e / N, n = e % N, row = row0 + b;
+      const float z = zb[e], az = fabsf(z);
+      const bool pick = rank >= 0 && az > th && az > thr[b];
+      const float m = fmaxf(az - th, 0.f);
+      const float x = pick ? z : (z > 0.f ? m : (z < 0.f ? -m : 0.f));
+      xs[e] = x;
+      if (n >= sn.lo && n < sn.hi && row < a.batch) {
+        const size_t o = ((size_t)l * a.batch + row) * N + n;
+        a.xs[o] = x;
+        if (a.zs) a.zs[o] = z;
+        if (a.sel) a.sel[o] = pick;
+      }
+    }
+    __syncthreads();
+  }
+  cl.sync();   // no CTA leaves while another may still write into its shared memory
+}
+
+struct Bwd {
+  l2o_ista_args a;
+  l2o_ista_grads g;
+};
+
+__device__ __forceinline__ float* dz_rec(const Bwd& p) { return reinterpret_cast<float*>(p.g.scratch); }
+__device__ __forceinline__ float* part_rec(const Bwd& p) {
+  return dz_rec(p) + (size_t)(p.a.k1 - p.a.k0) * p.a.batch * p.a.n;
+}
+__device__ __forceinline__ const float* layer_input(const l2o_ista_args& a, int l, int row) {
+  if (l == 0) return a.x_in ? a.x_in + (size_t)row * a.n : nullptr;
+  return a.xs + ((size_t)(l - 1) * a.batch + row) * a.n;
+}
+
+__device__ float block_sum(float v, float* scratch) {
+  for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) scratch[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float s = 0.f;
+  if (threadIdx.x == 0)
+    for (int w = 0; w < kWarps; ++w) s += scratch[w];
+  __syncthreads();
+  return s;
+}
+
+__global__ void __cluster_dims__(kCl, 1, 1) __launch_bounds__(kThreads) ista_bwd_kernel(const Bwd p) {
+  extern __shared__ float4 smem_f4[];
+  float* sm = reinterpret_cast<float*>(smem_f4);
+  const l2o_ista_args& a = p.a;
+  cg::cluster_group cl = cg::this_cluster();
+  const int c = (int)cl.block_rank();
+  const int row0 = (blockIdx.x / kCl) * kR;
+  const int M = a.m, N = a.n, tid = threadIdx.x;
+  const Smem P = smem_plan(a);
+  float *dx = sm + P.x, *rb = sm + P.r, *red = sm + P.red;
+  __shared__ float wsum[kWarps];
+  const Slice sm_ = slice_of(M, c), sn = slice_of(N, c);
+  const int ns = sn.hi - sn.lo;
+  float* dzr = dz_rec(p);
+  float* part = part_rec(p);
+  const int nblk = gridDim.x;
+
+  for (int e = tid; e < kR * ns; e += kThreads) {
+    const int b = e / ns, n = sn.lo + e % ns, row = row0 + b;
+    dx[b * N + n] = row < a.batch ? p.g.d_xk[(size_t)row * N + n] : 0.f;
+  }
+  cl.sync();   // every CTA of the cluster has started before any remote write
+  for (int k = a.k1 - 1; k >= a.k0; --k) {
+    const int l = k - a.k0;
+    float* zb = sm + P.z + (l & 1) * kR * N;
+    const float s = step_of(a, k), th = a.theta[k];
+    float dth = 0.f, ds = 0.f;
+    for (int e = tid; e < kR * ns; e += kThreads) {
+      const int b = e / ns, n = sn.lo + e % ns, row = row0 + b;
+      float dz = 0.f;
+      if (row < a.batch) {
+        const size_t o = ((size_t)l * a.batch + row) * N + n;
+        const float z = a.zs[o], az = fabsf(z), d = dx[b * N + n];
+        const bool pick = a.sel && a.sel[o];
+        const bool live = az > th && z != 0.f;   // relu'(0) = 0 and sign'(z) = 0
+        dz = (pick || live) ? d : 0.f;
+        if (!pick && live) dth -= (z > 0.f ? d : -d);
+        dzr[o] = dz;
+      }
+      for (int q = 0; q < kCl; ++q) cl.map_shared_rank(zb, q)[b * N + n] = dz;
+    }
+    cl.sync();
+    const bool wterm = has_w_term(a, k);
+    if (a.form == L2O_ISTA_COUPLED) {
+      const float* W = w_slot(a, k);
+      gemm_rows(zb, N, W, N, N, sm_.lo, sm_.hi, [&](int b, int i, float u) {
+        const int row = row0 + b;
+        if (row < a.batch) ds += a.rs[((size_t)l * a.batch + row) * M + i] * u;
+        for (int q = 0; q < kCl; ++q) cl.map_shared_rank(rb, q)[b * M + i] = s * u;
+      });
+      cl.sync();
+      gemm_cols(rb, M, a.A, N, M, sn.lo, sn.hi, red, [&](int b, int n, float v) { dx[b * N + n] = zb[b * N + n] - v; });
+    } else if (wterm) {
+      gemm_cols(zb, N, w_slot(a, k), N, N, sn.lo, sn.hi, red, [&](int b, int j, float u) {
+        const int row = row0 + b;
+        if (row < a.batch) {
+          const float* xin = layer_input(a, l, row);
+          if (xin) ds += xin[j] * u;
+        }
+        dx[b * N + j] = s * u;
+      });
+    } else {
+      for (int e = tid; e < kR * ns; e += kThreads) dx[(e / ns) * N + sn.lo + e % ns] = 0.f;
+      __syncthreads();
+    }
+    const float sth = block_sum(dth, wsum), sds = block_sum(ds, wsum);
+    if (tid == 0) {
+      part[((size_t)l * nblk + blockIdx.x) * 2 + 0] = sth;
+      part[((size_t)l * nblk + blockIdx.x) * 2 + 1] = sds;
+    }
+  }
+  if (p.g.d_x_in)
+    for (int e = tid; e < kR * ns; e += kThreads) {
+      const int b = e / ns, n = sn.lo + e % ns, row = row0 + b;
+      if (row < a.batch) p.g.d_x_in[(size_t)row * N + n] = dx[b * N + n];
+    }
+  cl.sync();
+}
+
+// Weight slots of the gradient launch.  Returns the creation layer of slot g (its gradient multiplier's index) and
+// the range of pass layers [la, lb) that contribute to it; la >= lb: the slot's gradient is 0 in this pass.
+struct SlotInfo {
+  int birth, la, lb;
+};
+__host__ __device__ inline int w_slots(const l2o_ista_args& a) {
+  if (a.share_W) return 1;
+  return a.form == L2O_ISTA_COUPLED ? a.num_layers : a.num_layers - 1;
+}
+__device__ inline SlotInfo slot_info(const l2o_ista_args& a, int g) {
+  const int first = a.form == L2O_ISTA_COUPLED ? 0 : 1;   // the first layer with a W term
+  SlotInfo s;
+  if (a.share_W) {
+    s.birth = first;
+    s.la = max(a.k0, first) - a.k0;
+    s.lb = a.k1 - a.k0;
+  } else {
+    const int k = g + first;
+    s.birth = k;
+    s.la = k >= a.k0 && k < a.k1 ? k - a.k0 : 0;
+    s.lb = k >= a.k0 && k < a.k1 ? s.la + 1 : 0;
+  }
+  return s;
+}
+
+// blockIdx.y < w_slots: dW slot; == w_slots (LISTA): dB1; last: dtheta and ds (blockIdx.x = layer).
+// C[p][q] = scale * sum_{l in [la, lb)} c_l sum_b P_l[b][p] Q_l[b][q] over 64 x 64 tiles (4 x 4 per thread).
+__global__ void __launch_bounds__(kThreads) ista_grad_kernel(const Bwd p, int nblk_bwd) {
+  const l2o_ista_args& a = p.a;
+  const int M = a.m, N = a.n, B = a.batch;
+  const int nw = p.g.dW ? w_slots(a) : 0;
+  const int nb1 = a.form == L2O_ISTA_LISTA && p.g.dB1 ? 1 : 0;
+  const float* dzr = dz_rec(p);
+  const int y_slot = blockIdx.y;
+  if (y_slot == nw + nb1) {   // per-layer scalars
+    const int k = blockIdx.x;
+    if (k >= a.num_layers) return;
+    const float* part = part_rec(p);
+    __shared__ double acc[2][kWarps];
+    double t = 0.0, s = 0.0;
+    if (k >= a.k0 && k < a.k1)
+      for (int i = threadIdx.x; i < nblk_bwd; i += kThreads) {
+        t += part[((size_t)(k - a.k0) * nblk_bwd + i) * 2];
+        s += part[((size_t)(k - a.k0) * nblk_bwd + i) * 2 + 1];
+      }
+    for (int o = 16; o; o >>= 1) {
+      t += __shfl_xor_sync(0xffffffffu, t, o);
+      s += __shfl_xor_sync(0xffffffffu, s, o);
+    }
+    if ((threadIdx.x & 31) == 0) acc[0][threadIdx.x >> 5] = t, acc[1][threadIdx.x >> 5] = s;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      t = s = 0.0;
+      for (int w = 0; w < kWarps; ++w) t += acc[0][w], s += acc[1][w];
+      const double sc = p.g.gscale ? (double)p.g.gscale[k] : 1.0;
+      p.g.dtheta[k] = sc * t;
+      if (p.g.dstep) p.g.dstep[k] = sc * s;
+    }
+    return;
+  }
+  int Pd, Qd, la, lb, birth;
+  double* out;
+  const bool b1 = y_slot == nw;
+  if (b1) {   // dB1 [N][M] = sum_k dz_k^T y
+    Pd = N, Qd = M, la = 0, lb = a.k1 - a.k0, birth = 0;
+    out = p.g.dB1;
+  } else {
+    const SlotInfo si = slot_info(a, y_slot);
+    la = si.la, lb = si.lb, birth = si.birth;
+    if (a.form == L2O_ISTA_COUPLED) Pd = M, Qd = N;   // dW [M][N] = s r^T dz
+    else Pd = N, Qd = N;                              // dW [N][N] = s dz^T x
+    out = p.g.dW + (size_t)y_slot * Pd * Qd;
+  }
+  const int tiles_q = (Qd + kTile - 1) / kTile, tiles = tiles_q * ((Pd + kTile - 1) / kTile);
+  if ((int)blockIdx.x >= tiles) return;
+  const int p0 = (blockIdx.x / tiles_q) * kTile, q0 = (blockIdx.x % tiles_q) * kTile;
+  __shared__ float Ps[kChunk][kTile], Qs[kChunk][kTile];
+  const int tp = threadIdx.x / 16, tq = threadIdx.x % 16;
+  double acc[4][4] = {};   // per-layer fp32 sums, added across layers in fp64 (a shared W or B1 sums K of them)
+  for (int l = la; l < lb; ++l) {
+    float lacc[4][4] = {};
+    const int k = a.k0 + l;
+    const float coef = b1 ? 1.f : step_of(a, k);
+    for (int b0 = 0; b0 < B; b0 += kChunk) {
+      for (int e = threadIdx.x; e < kChunk * kTile; e += kThreads) {
+        const int bb = e / kTile, j = e % kTile, row = b0 + bb;
+        float pv = 0.f, qv = 0.f;
+        if (row < B) {
+          const float* dz = dzr + ((size_t)l * B + row) * N;
+          if (a.form == L2O_ISTA_COUPLED) {
+            if (p0 + j < Pd) pv = a.rs[((size_t)l * B + row) * M + p0 + j];
+            if (q0 + j < Qd) qv = dz[q0 + j];
+          } else {
+            if (p0 + j < Pd) pv = dz[p0 + j];
+            if (q0 + j < Qd) {
+              if (b1) qv = a.y[(size_t)row * a.ldy + q0 + j];
+              else {
+                const float* xin = layer_input(a, l, row);
+                qv = xin ? xin[q0 + j] : 0.f;
+              }
+            }
+          }
+        }
+        Ps[bb][j] = coef * pv;
+        Qs[bb][j] = qv;
+      }
+      __syncthreads();
+#pragma unroll
+      for (int bb = 0; bb < kChunk; ++bb) {
+        float pr[4], qr[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) pr[i] = Ps[bb][tp + 16 * i], qr[i] = Qs[bb][tq + 16 * i];
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) lacc[i][j] = fmaf(pr[i], qr[j], lacc[i][j]);
+      }
+      __syncthreads();
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) acc[i][j] += (double)lacc[i][j];
+  }
+  const double sc = p.g.gscale && birth < a.num_layers ? (double)p.g.gscale[birth] : 1.0;
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int pp = p0 + tp + 16 * i, qq = q0 + tq + 16 * j;
+      if (pp < Pd && qq < Qd) out[(size_t)pp * Qd + qq] = sc * acc[i][j];
+    }
+}
+
+// Loss rows and dL/dx (MB/utils.py): sc  0.5 ||x - x_true||^2;  lasso 0.5 (0.5 ||x A^T - y||^2) + lam ||x||_1.
+__global__ void __launch_bounds__(kThreads) ista_loss_kernel(const l2o_ista_loss_args a) {
+  extern __shared__ float4 smem_f4[];
+  float* xr = reinterpret_cast<float*>(smem_f4);
+  float* er = xr + a.n;
+  __shared__ float wsum[kWarps];
+  const int row = blockIdx.x, N = a.n, M = a.m, lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  for (int n = threadIdx.x; n < N; n += kThreads) xr[n] = a.x[(size_t)row * N + n];
+  __syncthreads();
+  float f = 0.f;
+  if (a.task == L2O_ISTA_TASK_SC) {
+    for (int n = threadIdx.x; n < N; n += kThreads) {
+      const float d = xr[n] - a.x_true[(size_t)row * a.ldx + n];
+      a.d_x[(size_t)row * N + n] = d;
+      f += 0.5f * d * d;
+    }
+  } else {
+    for (int i = w; i < M; i += kWarps) {
+      float v = 0.f;
+      for (int n = lane; n < N; n += 32) v = fmaf(xr[n], a.A[(size_t)i * N + n], v);
+      for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+      if (lane == 0) er[i] = v - a.y[(size_t)row * a.ldy + i];
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < M; i += kThreads) f += 0.25f * er[i] * er[i];
+    for (int n = threadIdx.x; n < N; n += kThreads) {
+      float v = 0.f;
+      for (int i = 0; i < M; ++i) v = fmaf(er[i], a.A[(size_t)i * N + n], v);
+      const float x = xr[n];
+      a.d_x[(size_t)row * N + n] = 0.5f * v + a.lam * (x > 0.f ? 1.f : (x < 0.f ? -1.f : 0.f));
+      f += a.lam * fabsf(x);
+    }
+  }
+  const float s = block_sum(f, wsum);
+  if (threadIdx.x == 0 && a.loss) a.loss[row] = (double)s;
+}
+
+int check_args(const l2o_ista_args* a) {
+  if (!a || (a->form != L2O_ISTA_LISTA && a->form != L2O_ISTA_COUPLED)) return L2O_E_INVALID;
+  if (a->batch <= 0 || a->m <= 0 || a->n <= 0 || a->num_layers <= 0 || a->k0 < 0 || a->k0 >= a->k1 ||
+      a->k1 > a->num_layers || a->share_W < 0 || a->share_W > 1 || a->ldy < a->m)
+    return L2O_E_INVALID;
+  if (!a->theta || !a->y) return L2O_E_INVALID;
+  if (a->form == L2O_ISTA_COUPLED && (!a->A || !a->W)) return L2O_E_INVALID;
+  if (a->form == L2O_ISTA_LISTA && (!a->B1 || (a->k1 > 1 && !a->W))) return L2O_E_INVALID;
+  const void* ptrs[] = {a->A, a->B1, a->W, a->theta, a->step, a->ss_rank, a->y, a->x_in, a->xs, a->zs, a->rs};
+  for (const void* q : ptrs)
+    if (misaligned(q, 4)) return L2O_E_INVALID;
+  if (a->m > kMaxDim || a->n > kMaxDim) return L2O_E_UNSUPPORTED;
+  if ((size_t)smem_plan(*a).total * sizeof(float) > 200 * 1024) return L2O_E_UNSUPPORTED;
+  return L2O_OK;
+}
+
+inline int clusters(const l2o_ista_args& a) { return (a.batch + kR - 1) / kR; }
+
+size_t scratch_bytes(const l2o_ista_args& a) {
+  const size_t L = (size_t)(a.k1 - a.k0);
+  return 4 * (L * a.batch * a.n + L * clusters(a) * kCl * 2);
+}
+
+}  // namespace ista
+}  // namespace l2o
+
+using namespace l2o::ista;
+
+extern "C" {
+
+int l2o_ista_workspace_bytes(const l2o_ista_args* a, size_t* bytes) {
+  if (!bytes) return L2O_E_INVALID;
+  if (int rc = check_args(a)) return rc;
+  *bytes = scratch_bytes(*a);
+  return L2O_OK;
+}
+
+int l2o_ista_fwd(const l2o_ista_args* a, void* stream) {
+  if (int rc = check_args(a)) return rc;
+  if (!a->xs) return L2O_E_INVALID;
+  const size_t smem = (size_t)smem_plan(*a).total * sizeof(float);
+  if (int rc = l2o::raise_smem_limit("l2o_ista_fwd", ista_fwd_kernel, smem)) return rc;
+  ista_fwd_kernel<<<clusters(*a) * kCl, kThreads, smem, (cudaStream_t)stream>>>(*a);
+  return l2o::after_launch("l2o_ista_fwd");
+}
+
+int l2o_ista_bwd(const l2o_ista_args* a, const l2o_ista_grads* g, void* stream) {
+  if (int rc = check_args(a)) return rc;
+  if (!g || !a->xs || !a->zs || !g->d_xk || !g->dtheta || !g->scratch) return L2O_E_INVALID;
+  if (a->ss_rank && !a->sel) return L2O_E_INVALID;
+  if (a->form == L2O_ISTA_COUPLED && !a->rs) return L2O_E_INVALID;
+  if (a->form == L2O_ISTA_LISTA && !g->dB1) return L2O_E_INVALID;
+  const void* f4[] = {g->d_xk, g->d_x_in, g->gscale, g->scratch};
+  for (const void* q : f4)
+    if (l2o::misaligned(q, 4)) return L2O_E_INVALID;
+  const void* f8[] = {g->dW, g->dB1, g->dtheta, g->dstep};
+  for (const void* q : f8)
+    if (l2o::misaligned(q, 8)) return L2O_E_INVALID;
+  Bwd p{*a, *g};
+  const size_t smem = (size_t)smem_plan(*a).total * sizeof(float);
+  if (int rc = l2o::raise_smem_limit("l2o_ista_bwd", ista_bwd_kernel, smem)) return rc;
+  const int nblk = clusters(*a) * kCl;
+  ista_bwd_kernel<<<nblk, kThreads, smem, (cudaStream_t)stream>>>(p);
+  if (int rc = l2o::after_launch("l2o_ista_bwd")) return rc;
+  const int nw = g->dW ? w_slots(*a) : 0, nb1 = a->form == L2O_ISTA_LISTA ? 1 : 0;
+  const int pd = a->form == L2O_ISTA_COUPLED ? a->m : a->n;
+  int tiles = ((pd + kTile - 1) / kTile) * ((a->n + kTile - 1) / kTile);
+  if (nb1) tiles = std::max(tiles, ((a->n + kTile - 1) / kTile) * ((a->m + kTile - 1) / kTile));
+  tiles = std::max(tiles, a->num_layers);
+  ista_grad_kernel<<<dim3(tiles, nw + nb1 + 1), kThreads, 0, (cudaStream_t)stream>>>(p, nblk);
+  return l2o::after_launch("l2o_ista_bwd");
+}
+
+int l2o_ista_loss_grad(const l2o_ista_loss_args* a, void* stream) {
+  if (!a || (a->task != L2O_ISTA_TASK_SC && a->task != L2O_ISTA_TASK_LASSO) || a->batch <= 0 || a->m <= 0 ||
+      a->n <= 0 || !a->x || !a->d_x)
+    return L2O_E_INVALID;
+  if (a->task == L2O_ISTA_TASK_SC && (!a->x_true || a->ldx < a->n)) return L2O_E_INVALID;
+  if (a->task == L2O_ISTA_TASK_LASSO && (!a->A || !a->y || a->ldy < a->m)) return L2O_E_INVALID;
+  const void* f4[] = {a->A, a->y, a->x_true, a->x, a->d_x};
+  for (const void* q : f4)
+    if (l2o::misaligned(q, 4)) return L2O_E_INVALID;
+  if (l2o::misaligned(a->loss, 8)) return L2O_E_INVALID;
+  const size_t smem = (size_t)(a->n + a->m) * sizeof(float);
+  if (smem > 200 * 1024) return L2O_E_UNSUPPORTED;
+  if (int rc = l2o::raise_smem_limit("l2o_ista_loss_grad", ista_loss_kernel, smem)) return rc;
+  ista_loss_kernel<<<a->batch, kThreads, smem, (cudaStream_t)stream>>>(*a);
+  return l2o::after_launch("l2o_ista_loss_grad");
+}
+
+}  // extern "C"
