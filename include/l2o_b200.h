@@ -175,6 +175,12 @@ int l2o_unroll_bwd_carry(l2o_handle h, const l2o_bwd_args* a, const l2o_bwd_carr
  * instantiation (DM net, in-kernel Rastrigin or diagonal quadratic, n % 64 == 0, T >= 1, plain output layer, ckpt and
  * g_rec both set or both NULL), 0 = the general one, L2O_E_UNSUPPORTED = not the tensor-core engine's call. */
 int l2o_tc_fwd_variant(l2o_handle h, const l2o_unroll_args* a);
+/* The tensor-core engine's weight image of theta, as the forward (with_transposed = 0: B1h | B1l | B2h | B2l) or the
+ * BPTT (1: + T1h | T1l | T2h | T2l) stages it in shared memory; K-major tf32 core-matrix order, DESIGN.md §3.2.  The
+ * B images hold the gate weights and biases scaled by -log2e (i, f, o) and -2 log2e (j), with the forget bias +1 in
+ * the bias row; the T images hold them unscaled.  img NULL: nothing is launched.  Returns the image's float count,
+ * or a negative status. */
+int64_t l2o_tc_weight_image(l2o_handle h, const float* theta, float* img, int32_t with_transposed, void* stream);
 
 /* TF-1.14 Adam on theta: k = 1-based step count. */
 int l2o_adam_step(float* theta, const double* dtheta, float* m, float* v, int64_t n, int32_t k, float lr,

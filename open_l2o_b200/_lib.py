@@ -24,7 +24,7 @@ ENGINE_AUTO, ENGINE_FFMA, ENGINE_TC = 0, 1, 2
 # every symbol include/l2o_b200.h declares (tests check the .so exports all of them)
 EXPORTS = [
     "l2o_net_create", "l2o_net_destroy", "l2o_net_set_engine", "l2o_theta_count", "l2o_state_floats", "l2o_workspace_bytes",
-    "l2o_step", "l2o_unroll_fwd", "l2o_unroll_bwd", "l2o_unroll_bwd_carry", "l2o_tc_fwd_variant", "l2o_adam_step", "l2o_log_and_sign", "l2o_lasso_grad",
+    "l2o_step", "l2o_unroll_fwd", "l2o_unroll_bwd", "l2o_unroll_bwd_carry", "l2o_tc_fwd_variant", "l2o_tc_weight_image", "l2o_adam_step", "l2o_log_and_sign", "l2o_lasso_grad",
     "l2o_confocal_grad",
     "l2o_dense_create", "l2o_dense_destroy", "l2o_dense_theta_count", "l2o_dense_state_floats", "l2o_dense_step",
     "l2o_dense_unroll_bwd",
@@ -246,6 +246,8 @@ def lib():
     L.l2o_unroll_bwd_carry.restype = C.c_int
     L.l2o_tc_fwd_variant.argtypes = [C.c_void_p, C.POINTER(UnrollArgs)]
     L.l2o_tc_fwd_variant.restype = C.c_int
+    L.l2o_tc_weight_image.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
+    L.l2o_tc_weight_image.restype = C.c_int64
     L.l2o_adam_step.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_float,
                                 C.c_float, C.c_float, C.c_float, C.c_void_p]
     L.l2o_adam_step.restype = C.c_int

@@ -209,6 +209,18 @@ __device__ __forceinline__ float ext_weight(const float* __restrict__ theta, boo
   if (in_h2) return theta[C::O_W2 + (kH + vec_unit(c, G::ColH2)) * C::G2 + col];
   return 0.f;
 }
+// Gate scales folded into the forward images B1 / B2: MMA gate column n delivers z' = -s_g (z + delta_g), the exponent
+// of sigma(z) = 1 / (1 + 2^(-log2e z)) and tanh(z) = 2 / (1 + 2^(-2 log2e z)) - 1, so the epilogues feed the
+// accumulators to ex2 without a multiply.  s_g = log2e for i, f, o and 2 log2e for j; delta_f = 1 is snt.LSTM's
+// forget bias (delta = 0 for the other gates), added to the bias row.  The dX images T1 / T2 stay unscaled: dZ is the
+// gradient with respect to the unscaled pre-activation z.
+constexpr float kLog2e = 1.4426950408889634f;
+__host__ __device__ constexpr float gate_scale(int gate) { return gate == 1 ? -2.f * kLog2e : -kLog2e; }
+constexpr int kGateF = 2;
+// sigma(z) and tanh(z) from the scaled pre-activations sigma: z' = -log2e z, tanh: z' = -2 log2e z
+__device__ __forceinline__ float sigmoid_scaled(float zs) { return rcp_approx(1.0f + ex2_approx(zs)); }
+__device__ __forceinline__ float tanh_scaled(float zs) { return fmaf(2.0f, rcp_approx(1.0f + ex2_approx(zs)), -1.0f); }
+
 // operand-row column of dX output column c of layer l2
 template <class C>
 __host__ __device__ constexpr int dx_operand_col(bool l2, int c) {
@@ -219,7 +231,7 @@ __host__ __device__ constexpr int dx_operand_col(bool l2, int c) {
 
 // Weight image: B1h | B1l | B2h | B2l (forward) and, with_transposed, T1h | T1l | T2h | T2l (BPTT dX contractions,
 // K = 80 gates in the physical order of dx_gate_col, N = N1 / N2 dX columns).  B_l rows = operand-row columns
-// 8 L_lLo .. 8 L_lHi - 1.
+// 8 L_lLo .. 8 L_lHi - 1, scaled by gate_scale (each value rounded once in fp32, then split into hi + lo).
 template <class C>
 __global__ void prep_weights_kernel(const float* __restrict__ theta, float* __restrict__ img, int with_transposed) {
   static_assert(C::H1 == kH && C::H2 == kH && (C::F <= 3 || C::FC), "tc engine: LSTM-20x2, F <= 3 or fc(20)");
@@ -234,7 +246,10 @@ __global__ void prep_weights_kernel(const float* __restrict__ theta, float* __re
       const bool l2 = e >= G::K1 * kN;
       const int ee = l2 ? e - G::K1 * kN : e;
       const int k = ee / kN, n = ee % kN;
-      w = ext_weight<C>(theta, l2, 8 * (l2 ? G::L2Lo : G::L1Lo) + k, n);
+      const int c = 8 * (l2 ? G::L2Lo : G::L1Lo) + k, gate = gate_ref_col(n) / kH;
+      w = ext_weight<C>(theta, l2, c, n);
+      if (c == G::ColOne && gate == kGateF) w += 1.0f;
+      w *= gate_scale(gate);
       hi = img + (l2 ? 2 * G::B1Floats : 0);
       off = l2 ? G::B2Floats : G::B1Floats;
       idx = img_index(k, n, kN);
@@ -306,21 +321,21 @@ __device__ __forceinline__ void mma3(float* d, const Frag<KB>& f, uint64_t bh, u
 __host__ __device__ constexpr int acc_idx(int s, int g, int rh) { return 4 * (2 * s + (g >> 1)) + 2 * rh + (g & 1); }
 
 // ------------------------------------------------------------------ epilogue helpers
-// One LSTM unit, pointwise, from the pre-activations (i, j, f, o) of the unit.  7 MUFU ops (5 ex2 + 2 rcp) instead of
-// the 10 of five separate sigmoid/tanh evaluations: the whole cell update shares ONE reciprocal,
+// One LSTM unit, pointwise, from the scaled pre-activations (i', j', f', o') of the unit (gate_scale: Ei = 2^i' etc.).
+// 7 MUFU ops (5 ex2 + 2 rcp) instead of the 10 of five separate sigmoid/tanh evaluations: the whole cell update shares
+// ONE reciprocal,
 //   c' = sigma(f+1) c + sigma(i) tanh(j) = [c (1+Ei)(1+Ej) + (1-Ej)(1+Ef)] / [(1+Ei)(1+Ej)(1+Ef)],
 // and tanh(c') sigma(o) = (1-Ec) / ((1+Ec)(1+Eo)) another.  The exponents are clamped to 2^40 so the triple product
 // stays finite (sigma / tanh are saturated to 1e-12 there).
-constexpr float kLog2e = 1.4426950408889634f;
 __device__ __forceinline__ void lstm_point_fwd(float zi, float zj, float zf, float zo, float& c, float& h) {
-  const float Ei = ex2_approx(fminf(-kLog2e * zi, 40.f));
-  const float Ej = ex2_approx(fminf(-2.f * kLog2e * zj, 40.f));
-  const float Qf = 1.0f + ex2_approx(fminf(fmaf(-kLog2e, zf, -kLog2e), 40.f));
+  const float Ei = ex2_approx(fminf(zi, 40.f));
+  const float Ej = ex2_approx(fminf(zj, 40.f));
+  const float Qf = 1.0f + ex2_approx(fminf(zf, 40.f));
   const float Pij = (1.0f + Ei) * (1.0f + Ej);
   const float cn = fmaf(c, Pij, (1.0f - Ej) * Qf) * rcp_approx(Pij * Qf);
   c = cn;
   const float Ec = ex2_approx(fminf(-2.f * kLog2e * cn, 63.f));
-  const float Eo = ex2_approx(fminf(-kLog2e * zo, 63.f));
+  const float Eo = ex2_approx(fminf(zo, 63.f));
   h = (1.0f - Ec) * rcp_approx((1.0f + Ec) * (1.0f + Eo));
 }
 // elu as the forward and backward kernels both evaluate it: a (a > 0) | expm1(a), with a short Taylor sum near zero

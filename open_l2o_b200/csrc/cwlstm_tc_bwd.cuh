@@ -68,10 +68,11 @@ __device__ __forceinline__ void prefetch_l2_bulk(const void* p, uint32_t bytes) 
 }
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
-// LSTM pointwise backward for one unit from the pre-activations (i, j, f, o) -> overwritten with dz; c: previous cell
+// LSTM pointwise backward for one unit from the scaled pre-activations (i', j', f', o') of the forward image
+// (gate_scale) -> overwritten with dz, the gradient with respect to the unscaled pre-activations; c: previous cell
 // state; dh: gradient of h'; dc: carry in (gradient of c') / out (gradient of c).  hn: h' (the output layer needs it).
 __device__ __forceinline__ void unit_bwd(float& zi, float& zj, float& zf, float& zo, float cprev, float dh, float& dc, float& hn) {
-  const float i = sigmoid_fast(zi), j = tanh_fast(zj), f = sigmoid_fast(zf + 1.0f), o = sigmoid_fast(zo);
+  const float i = sigmoid_scaled(zi), j = tanh_scaled(zj), f = sigmoid_scaled(zf), o = sigmoid_scaled(zo);
   const float cn = fmaf(f, cprev, i * j);
   const float tcn = tanh_fast(cn);
   hn = tcn * o;

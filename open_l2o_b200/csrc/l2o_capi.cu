@@ -218,6 +218,11 @@ int l2o_tc_fwd_variant(l2o_handle h, const l2o_unroll_args* a) {
   return l2o::tc_fwd_variant(h, *a);
 }
 
+int64_t l2o_tc_weight_image(l2o_handle h, const float* theta, float* img, int32_t with_transposed, void* stream) {
+  if (!h || (img && !theta) || l2o::misaligned(img, 16)) return L2O_E_INVALID;
+  return l2o::tc_weight_image(h, theta, img, with_transposed != 0, (cudaStream_t)stream);
+}
+
 int l2o_unroll_bwd(l2o_handle h, const l2o_bwd_args* a, void* stream) {
   if (!h || !a || a->n < 0 || a->T < 0 || !a->theta || !a->dtheta) return L2O_E_INVALID;
   if (a->T > 0 && !a->in_seq) return L2O_E_INVALID;

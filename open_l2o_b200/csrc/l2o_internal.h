@@ -79,6 +79,8 @@ void tc_release_image(l2o_net* h);   // hand the weight image back to the proces
 bool tc_fwd_ok(const l2o_net* h, const l2o_unroll_args& a);
 int tc_unroll_fwd(l2o_net* h, const l2o_unroll_args& a, cudaStream_t st);
 int tc_fwd_variant(const l2o_net* h, const l2o_unroll_args& a);   // l2o_tc_fwd_variant
+int64_t tc_weight_image(const l2o_net* h, const float* theta, float* img, bool with_transposed,
+                        cudaStream_t st);   // l2o_tc_weight_image
 bool tc_step_ok(const l2o_net* h, const l2o_step_args& a);
 int tc_step(l2o_net* h, const l2o_step_args& a, cudaStream_t st);
 bool tc_bwd_ok(const l2o_net* h, const l2o_bwd_args& a);

@@ -146,6 +146,23 @@ int tc_unroll_fwd(l2o_net* h, const l2o_unroll_args& a, cudaStream_t st) {
   return rc;
 }
 
+template <class C>
+static int64_t tc_image(const float* theta, float* img, bool with_transposed, cudaStream_t st) {
+  using G = tc::Geo<C>;
+  const int64_t floats = with_transposed ? G::AllFloats : G::FwdFloats;
+  if (img == nullptr) return floats;
+  tc::prep_weights_kernel<C><<<16, 256, 0, st>>>(theta, img, with_transposed ? 1 : 0);
+  if (int rc = after_launch("l2o_tc_weight_image")) return rc;
+  return floats;
+}
+
+int64_t tc_weight_image(const l2o_net* h, const float* theta, float* img, bool with_transposed, cudaStream_t st) {
+  if (h->cfg == 0) return tc_image<Cfg<L2O_PRE_IDENTITY, 1, 1, 20, 20>>(theta, img, with_transposed, st);
+  if (h->cfg == 1) return tc_image<Cfg<L2O_PRE_LOGSIGN, 1, 2, 20, 20>>(theta, img, with_transposed, st);
+  if (h->cfg == 2) return tc_image<Cfg<L2O_PRE_FC, 2, 20, 20, 20>>(theta, img, with_transposed, st);
+  return L2O_E_UNSUPPORTED;
+}
+
 int tc_fwd_variant(const l2o_net* h, const l2o_unroll_args& a) {
   if (!tc_supported(h->cfg) || !tc_fwd_ok(h, a)) return L2O_E_UNSUPPORTED;
   return tc_fwd_fast(h->cfg == 2, h->rt, a, nullptr) ? 1 : 0;
