@@ -51,15 +51,18 @@ def w_slot(form, W, k, share_W):
     return W[k] if form == COUPLED else W[k - 1]
 
 
-def forward(form, A, B1, W, theta, step, y, k1, share_W=False, ranks=None, sels=None, lives=None, zs_out=None):
-    """x_1 .. x_k1 and the support masks used (None per layer without support selection).  sels / lives: per-layer
-    masks to use in place of the computed support selection / |z| > theta classification.  zs_out: a list that
+def forward(form, A, B1, W, theta, step, y, k1, share_W=False, ranks=None, sels=None, lives=None, zs_out=None, k0=0,
+            x0=None):
+    """x_{k0+1} .. x_k1 of layers k0 .. k1-1 from x_{k0} = x0 (zeros when None), and the support masks used (None per
+    layer without support selection).  theta, step, ranks and the W slots are indexed by absolute layer; ranks[k] < 0
+    means soft shrinkage in layer k and ranks[k] >= N reads as N - 1.  sels / lives: masks to use in place of the
+    computed support selection / |z| > theta classification, one per layer of the pass.  zs_out: a list that
     receives every z_k."""
     B, N = y.shape[0], A.shape[1]
-    x = torch.zeros(B, N, dtype=y.dtype, device=y.device)
+    x = torch.zeros(B, N, dtype=y.dtype, device=y.device) if x0 is None else x0
     by = y @ B1.T if form == LISTA else None
     xs, used = [], []
-    for k in range(k1):
+    for k in range(k0, k1):
         s = 1.0 if step is None else step[k]
         if form == LISTA:
             z = by if k == 0 else by + s * (x @ w_slot(form, W, k, share_W).T)
@@ -67,14 +70,63 @@ def forward(form, A, B1, W, theta, step, y, k1, share_W=False, ranks=None, sels=
             z = x + s * ((y - x @ A.T) @ w_slot(form, W, k, share_W))
         if zs_out is not None:
             zs_out.append(z)
-        live = None if lives is None else lives[k]
-        if ranks is None:
+        live = None if lives is None else lives[k - k0]
+        rank = -1 if ranks is None else min(int(ranks[k]), N - 1)
+        if rank < 0:
             x, m = shrink_free(z, theta[k], live), None
         else:
-            x, m = shrink_ss(z, theta[k], int(ranks[k]), None if sels is None else sels[k], live)
+            x, m = shrink_ss(z, theta[k], rank, None if sels is None else sels[k - k0], live)
         xs.append(x)
         used.append(m)
     return xs, used
+
+
+def abs_sum_bound(form, A, B1, W, step, y, k1, share_W=False, k0=0, x0=None, d_xk=None):
+    """The largest sum of absolute terms over every GEMM, product and reduction that a pass [k0, k1) forms: forward
+    r_k, y B1^T, the W products and z_k; with d_xk, the backward's dx_k, ds_k and dtheta_k partials and the per-layer
+    dW / dB1 sums over the batch.  It bounds every partial sum in any order, since shrinkage never grows |z| and dz_k
+    is dx_{k+1} or 0.  Below 2^24, integer inputs keep all of them exact in fp32."""
+    ab = lambda t: None if t is None else t.abs()
+    A, B1, W, y = ab(A), ab(B1), ab(W), ab(y)
+    N = A.shape[1] if A is not None else B1.shape[0]
+    s = lambda k: 1.0 if step is None else abs(float(step[k]))
+    X = [torch.zeros(y.shape[0], N, dtype=y.dtype) if x0 is None else x0.abs()]
+    R, terms = [], []
+    by = y @ B1.T if form == LISTA else None
+    for k in range(k0, k1):
+        Wk = w_slot(form, W, k, share_W)
+        if form == LISTA:
+            u = (X[-1] @ Wk.T) if k > 0 else torch.zeros_like(by)
+            z = by + s(k) * u
+            terms += [by, u]
+        else:
+            r = y + X[-1] @ A.T
+            u = r @ Wk
+            z = X[-1] + s(k) * u
+            R.append(r)
+            terms += [r, u]
+        terms.append(z)
+        X.append(z)
+    if d_xk is not None:
+        D = d_xk.abs()
+        for k in range(k1 - 1, k0 - 1, -1):
+            l, Wk = k - k0, w_slot(form, W, k, share_W)
+            terms.append(D.sum().reshape(1))                                   # dtheta_k
+            if form == COUPLED:
+                u = D @ Wk.T
+                v = s(k) * u @ A
+                terms += [u, v, (R[l] * u).sum().reshape(1), s(k) * R[l].T @ D]   # ds_k, dW_k
+                D = D + v
+            else:
+                terms.append(D.T @ y)                                          # this layer's dB1 term
+                if k == 0:
+                    D = torch.zeros_like(D)
+                    continue
+                u = D @ Wk
+                terms += [u, (X[l] * u).sum().reshape(1), s(k) * D.T @ X[l]]      # ds_k, dW_k
+                D = s(k) * u
+            terms.append(D)
+    return max(float(t.max()) for t in terms)
 
 
 def sc_loss(x, x_true):

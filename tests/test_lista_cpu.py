@@ -9,6 +9,7 @@ import torch
 
 from open_l2o_b200 import _lib, lista, lista_train as lt
 from oracle import lista_oracle as lo
+from tests import lista_cases as lc
 
 
 def _ista(A, y, lam, K):
@@ -68,6 +69,78 @@ def test_percentile_rank_hand_cases():
     assert sel.tolist() == [[True, False, False, False, False, False]]
     x, _ = lo.shrink_ss(z, torch.tensor(0.2), 2)
     np.testing.assert_allclose(x.numpy(), [[5.0, -4.0, 2.8, 2.8, 0.8, 0.3]], rtol=1e-6)
+
+
+def _random_cell(form, M, N, K, share_W, seed):
+    g = torch.Generator().manual_seed(seed)
+    r = lambda *s: torch.randn(*s, generator=g, dtype=torch.float64)
+    S = 1 if share_W else (K if form == lo.COUPLED else K - 1)
+    A = r(M, N) / np.sqrt(M)
+    W = (A / 2 if form == lo.COUPLED else torch.eye(N, dtype=torch.float64) / 2) + 0.05 * r(S, M if form == lo.COUPLED
+                                                                                           else N, N)
+    return dict(A=A, B1=A.T / 2 if form == lo.LISTA else None, W=W, theta=0.1 + 0.05 * r(K).abs(),
+                step=1 + 0.2 * r(K), y=r(5, M))
+
+
+@pytest.mark.parametrize("form", [lo.LISTA, lo.COUPLED])
+@pytest.mark.parametrize("share_W", [False, True])
+def test_oracle_layer_ranges_and_per_layer_shrinkage(form, share_W):
+    M, N, K = 6, 9, 5
+    c = _random_cell(form, M, N, K, share_W, seed=form + 2 * share_W)
+    args = lambda: (form, c["A"], c["B1"], c["W"], c["theta"], c["step"], c["y"])
+    ranks = [2, -1, N - 1, N + 5, 0]
+    full, used = lo.forward(*args(), K, share_W, ranks)
+    assert used[1] is None and all(u is not None for i, u in enumerate(used) if i != 1)
+    for j in range(1, K):      # a pass [j, K) from x_j reproduces layers j .. K-1, bit for bit
+        part, pused = lo.forward(*args(), K, share_W, ranks, k0=j, x0=full[j - 1])
+        assert len(part) == K - j
+        for k in range(j, K):
+            assert torch.equal(part[k - j], full[k]), (j, k)
+            assert (pused[k - j] is None) == (used[k] is None)
+    # x0 = None is x_0 = 0; k0 = 0 with an explicit zero x0 is the same pass
+    z0, _ = lo.forward(*args(), K, share_W, ranks, x0=torch.zeros(5, N, dtype=torch.float64))
+    assert all(torch.equal(a, b) for a, b in zip(z0, full))
+    # a negative rank is soft shrinkage in that layer only
+    zs = []
+    xs, _ = lo.forward(*args(), 2, share_W, [-1, -1], zs_out=zs)
+    soft, _ = lo.forward(*args(), 2, share_W)
+    for k in range(2):
+        assert torch.equal(xs[k], soft[k]) and torch.equal(xs[k], lo.shrink_free(zs[k], c["theta"][k]))
+    # ranks >= N read as N - 1
+    _, a = lo.forward(*args(), K, share_W, [N - 1] * K)
+    _, b = lo.forward(*args(), K, share_W, [N + 5] * K)
+    assert all(torch.equal(u, v) for u, v in zip(a, b)) and any(bool(u.any()) for u in a)
+
+
+def test_abi_exact_inputs_keep_every_sum_exact():
+    """The premise of test_lista_abi_gpu's bit-exact tests, on every parametrization: the abs-sum bound of every sum
+    the kernels form stays below 2^24, so integer inputs give exact fp32 results; and the inputs reach the edges
+    they are there for: |z| == theta, z == 0 and -0.0, ties at the support-selection threshold just above theta (where
+    '>' against '>=' decides), and N - 1 against N - 2 changing a mask where the rank clamps."""
+    cases = [(lc.exact_case(*c), 0, lc.K) for c in lc.EXACT_CASES]
+    cases += [(lc.exact_case(f, (12, 16, 13), "clamp", "perlayer", seed=3), k0, k1) for f in (lo.LISTA, lo.COUPLED)
+              for k0, k1 in lc.RANGES]
+    cases.append((lc.exact_case(lo.LISTA, (24, 16, 13), "mixed", "perlayer", seed=5), 0, lc.K))
+    cases.append((lc.exact_case(lo.COUPLED, (24, 16, 13), "mixed", "perlayer", seed=5), 0, lc.K))
+    seen = dict(theta_ties=0, zeros=0, negative_zeros=0, rank_ties=0, clamp=0)
+    for P, k0, k1 in cases:
+        assert lc.exact_bound(P, k0, k1) < 2 ** 24
+        ref = lc.oracle(P, k0, k1, d_xk=None)
+        for l in range(k1 - k0):
+            z, th = ref["zs"][l], float(P["theta"][k0 + l])
+            seen["theta_ties"] += int((z.abs() == th).sum())
+            seen["zeros"] += int((z == 0).sum())
+            seen["negative_zeros"] += int(((z == 0) & torch.signbit(z)).sum())
+            if P["ranks"] is None or int(P["ranks"][k0 + l]) < 0:
+                continue
+            N = P["N"]
+            srt = z.abs().sort(dim=1, descending=True).values
+            thr = srt[:, min(int(P["ranks"][k0 + l]), N - 1)][:, None]
+            seen["rank_ties"] += int(((z.abs() == thr) & (z.abs() > th)).sum())
+            if N > 1 and int(P["ranks"][k0 + l]) >= N - 1:
+                seen["clamp"] += int(((z.abs() == srt[:, N - 2:N - 1]) & (z.abs() > srt[:, N - 1:]) &
+                                      (z.abs() > th)).sum())
+    assert all(v >= 10 for v in seen.values()), seen
 
 
 def test_keras_adam_one_step_closed_form():
@@ -228,6 +301,14 @@ def test_ista_abi_rejects_bad_arguments_without_gpu():
         _lib.L2O_OK
     assert L.l2o_ista_workspace_bytes(C.byref(_args(m=1024, n=1281, ldy=1024, **lista_args)), C.byref(nb)) == \
         _lib.L2O_E_UNSUPPORTED
+    # the largest plans of each form (run on the GPU by test_lista_abi_gpu) and their +1 neighbours in M and in N
+    largest = [({}, (1024, 1365)), ({}, (2048, 682)), ({}, (3, 2046)),
+               (lista_args, (1024, 1280)), (lista_args, (2048, 1024)), (lista_args, (4, 1535))]
+    for kw, (m, n) in largest:
+        assert L.l2o_ista_workspace_bytes(C.byref(_args(m=m, n=n, ldy=m, **kw)), C.byref(nb)) == _lib.L2O_OK, (m, n)
+        for mm, nn in ((m + 1, n), (m, n + 1)):
+            assert L.l2o_ista_workspace_bytes(C.byref(_args(m=mm, n=nn, ldy=mm, **kw)), C.byref(nb)) == \
+                _lib.L2O_E_UNSUPPORTED, (mm, nn)
     g = _lib.IstaGrads()
     assert L.l2o_ista_bwd(C.byref(_args()), C.byref(g), None) == _lib.L2O_E_INVALID          # no d_xk / dtheta
     g.d_xk = g.dtheta = g.scratch = 1 << 20
