@@ -482,20 +482,32 @@ int l2o_lrsgd_bwd(const l2o_lrsgd_bwd_args* a, void* stream);
  * Forms: L2O_ISTA_LISTA   z_k = y B1^T + s_k x_k W_k^T  (layer 0 has no W term); B1 [N][M], W slots [N][N], slot k-1
  *                         for layer k (one slot when share_W).
  *        L2O_ISTA_COUPLED z_k = x_k + s_k (y - x_k A^T) W_k;  W slots [M][N], slot k (one slot when share_W).
+ *        L2O_ISTA_LFISTA  z_k = y We^T + [k>=1] x_k Wg_k^T + [k>=2] x_{k-1} Wm_k^T       MB/models/lfista.py
+ *                         B1 = We [N][M], W = Wg slots and W2 = Wm slots [N][N], slot k-1 for layer k; no share_W,
+ *                         no step.  x_{k0-1} comes from s2_in.
+ *        L2O_ISTA_LAMP    v_k = y - x_k A^T + b_k v_{k-1}, b_k = ||x_k||_0 / M (b_0 = 0),  MB/models/lamp.py
+ *                         z_k = r_k = x_k + s_k v_k W_k, shrunk with the row's theta = max(sqrt(||v_k||^2 / M) lam_k,
+ *                         0); theta holds lam_k.  A, W slots [M][N] as the coupled form; rs records v_k.
+ *                         v_{k0-1} comes from s2_in.  The backward takes |r| >= theta (tf.maximum's tie rule) as live
+ *                         and gives a row with rvar = 0 no gradient through its theta.
  * x_{k+1} = sign(z) relu(|z| - theta_k); with ss_rank, entries with |z| > theta_k and |z| > t_b pass unshrunk, t_b
  * being row b's |z| at 0-based rank ss_rank[k] in descending order (the caller maps the percentile to the rank).
+ * LFISTA and LAMP take no ss_rank.  Their backward also carries the second state: d_s2 enters as its adjoint at the
+ * top of the pass and d_s2_in returns it at the bottom, so passes [0, j) and [j, K) compose as one.
  * The backward overwrites every gradient it is given (zero for layers outside [k0, k1)); gscale[j] multiplies the
  * gradient of every variable created with layer j (B1: layer 0; a shared W: its first layer).  L2O_E_UNSUPPORTED when
  * M or N > 2048 or when a CTA's shared-memory plan exceeds 200 KB: 4 (8 (M + 4N) + 2048) bytes in the LISTA form,
- * 4 (8 (2M + 3N) + 2048) in the coupled form (so the coupled form at M = 256, N = 512 needs 72 KB and at M = 1024 fits
- * N <= 1365); l2o_ista_loss_grad: 4 (M + N) bytes > 200 KB.  Float pointers 4-byte aligned, double pointers
+ * 4 (8 (2M + 3N) + 2048) in the coupled and LAMP forms (so the coupled form at M = 256, N = 512 needs 72 KB and at
+ * M = 1024 fits N <= 1365), 4 (8 (M + 5N) + 2048) in the LFISTA form; l2o_ista_loss_grad: 4 (M + N) bytes > 200 KB.  Float pointers 4-byte aligned, double pointers
  * 8-byte aligned (L2O_E_INVALID otherwise). */
 #define L2O_ISTA_LISTA 0
 #define L2O_ISTA_COUPLED 1
+#define L2O_ISTA_LFISTA 2
+#define L2O_ISTA_LAMP 3
 #define L2O_ISTA_TASK_SC 0
 #define L2O_ISTA_TASK_LASSO 1
 typedef struct {
-  int32_t form;            /* L2O_ISTA_LISTA or L2O_ISTA_COUPLED */
+  int32_t form;            /* L2O_ISTA_LISTA, _COUPLED, _LFISTA or _LAMP */
   int32_t batch, m, n;     /* > 0 */
   int32_t num_layers;      /* K: sizes theta, step, ss_rank and the W slots */
   int32_t k0, k1;          /* layers run: 0 <= k0 < k1 <= K */
@@ -515,6 +527,10 @@ typedef struct {
   float* rs;               /* [k1-k0][B][M] out: coupled r_k = y - x_k A^T, or NULL (required by the backward) */
   uint8_t* sel;            /* [k1-k0][B][N] out: 1 where support selection passed z through, or NULL (required by the
                               backward with ss_rank) */
+  const float* W2;         /* LFISTA: Wm slots [N][N], slot k-1 for layer k (slot 0 is never read) */
+  const float* s2_in;      /* the second state at k0: LFISTA x_{k0-1} [B][N], LAMP v_{k0-1} [B][M]; NULL: zeros */
+  float* rowrec;           /* LAMP: [k1-k0][B][2] out: sqrt(rvar_k) and b_k of each row, or NULL (required by the
+                              backward) */
 } l2o_ista_args;
 typedef struct {
   const float* d_xk;       /* [B][N] dL/dx_{k1} */
@@ -525,6 +541,9 @@ typedef struct {
   double* dstep;           /* [K] out, or NULL */
   const float* gscale;     /* [K] gradient multipliers by creation layer, or NULL: all 1 */
   void* scratch;           /* l2o_ista_workspace_bytes */
+  double* dW2;             /* LFISTA: Wm slots out, or NULL */
+  const float* d_s2;       /* optional: dL/dx_{k1-1} (LFISTA) or dL/dv_{k1-1} (LAMP) from beyond the pass */
+  float* d_s2_in;          /* optional out: dL/dx_{k0-1} (LFISTA) or dL/dv_{k0-1} (LAMP) */
 } l2o_ista_grads;
 typedef struct {
   int32_t task;            /* L2O_ISTA_TASK_SC: 0.5 ||x - x_true||^2;  LASSO: 0.5 (0.5 ||x A^T - y||^2) + lam ||x||_1 */

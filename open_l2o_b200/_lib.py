@@ -143,12 +143,13 @@ class IstaArgs(C.Structure):
     _fields_ = [("form", C.c_int32), ("batch", C.c_int32), ("m", C.c_int32), ("n", C.c_int32),
                 ("num_layers", C.c_int32), ("k0", C.c_int32), ("k1", C.c_int32), ("share_W", C.c_int32),
                 ("A", _fp), ("B1", _fp), ("W", _fp), ("theta", _fp), ("step", _fp), ("ss_rank", _fp), ("y", _fp),
-                ("ldy", C.c_int64), ("x_in", _fp), ("xs", _fp), ("zs", _fp), ("rs", _fp), ("sel", _fp)]
+                ("ldy", C.c_int64), ("x_in", _fp), ("xs", _fp), ("zs", _fp), ("rs", _fp), ("sel", _fp),
+                ("W2", _fp), ("s2_in", _fp), ("rowrec", _fp)]
 
 
 class IstaGrads(C.Structure):
     _fields_ = [("d_xk", _fp), ("d_x_in", _fp), ("dW", _fp), ("dB1", _fp), ("dtheta", _fp), ("dstep", _fp),
-                ("gscale", _fp), ("scratch", _fp)]
+                ("gscale", _fp), ("scratch", _fp), ("dW2", _fp), ("d_s2", _fp), ("d_s2_in", _fp)]
 
 
 class IstaLossArgs(C.Structure):

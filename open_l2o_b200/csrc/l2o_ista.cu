@@ -1,8 +1,9 @@
 // Model-based L2O's LISTA family (MB/ = Model_Base_L2O/ of the reference) — sm_90a kernels + C-ABI.
 //
-// Two cell forms over a batch of rows, layers k = k0 .. k1-1 (row-major: y [B,M], x [B,N], A [M,N]):
+// Four cell forms over a batch of rows, layers k = k0 .. k1-1 (row-major: y [B,M], x [B,N], A [M,N]):
 //   LISTA   (MB/models/lista.py:32-45)        z_k = y B1^T + s_k x_k W_k^T       (layer 0: no W term)
 //   coupled (lista_cp.py, lista_cpss.py, alista.py)  r_k = y - x_k A^T,  z_k = x_k + s_k r_k W_k
+//   LFISTA and LAMP, which also carry x_{k-1} or v_{k-1}: their own kernels, further down
 // then x_{k+1} = shrink(z_k): soft shrinkage sign(z) relu(|z| - theta_k) (MB/models/utils.py shrink_free), or support
 // selection (shrink_ss): entries with |z| > theta_k and |z| > the row's rank-q_k magnitude pass through unshrunk.
 //
@@ -550,19 +551,464 @@ __global__ void __launch_bounds__(kThreads) ista_loss_kernel(const l2o_ista_loss
   if (threadIdx.x == 0 && a.loss) a.loss[row] = (double)s;
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// The two-state recurrences: LFISTA carries x_{k-1} besides x_k, LAMP carries v_{k-1} and a per-row threshold.
+// Their own kernels, on the helpers above, so the four forms' kernels stay as they are.
+//   LFISTA (MB/models/lfista.py)  z_k = y We^T + [k>=1] x_k Wg_k^T + [k>=2] x_{k-1} Wm_k^T,  x_{k+1} = shrink(z_k)
+//   LAMP   (MB/models/lamp.py)    v_k = y - x_k A^T + b_k v_{k-1}  (b_k = ||x_k||_0 / M, b_0 = 0),
+//                                 r_k = x_k + s_k v_k W_k,  x_{k+1} = shrink(r_k, max(sqrt(||v_k||^2 / M) lam_k, 0))
+// One cluster owns kR rows for the pass, as above.  LFISTA: one exchange per layer (z_k), the x buffers rotate.
+// LAMP: an exchange of v_k (M slice) and one of r_k (N slice); every CTA forms ||v_k||^2 and ||x_k||_0 of each row
+// redundantly (a warp per row, in the same order everywhere), so all of them shrink with the same threshold.
+
+// Shared-memory plan of the two-state forms, in floats.  LFISTA: y, x_k, x_{k-1}, z double buffer, y We^T.  LAMP:
+// y, x_k, v (one buffer: a CTA writes v_k only into the other CTAs' slices of its own columns, after the barrier
+// that ends every read of v_{k-1} there), r double buffer.
+struct Smem2 {
+  int y, x, s, z, by, red, total;
+};
+__host__ __device__ inline Smem2 smem_plan2(const l2o_ista_args& a) {
+  Smem2 s;
+  s.y = 0;
+  s.x = s.y + kR * a.m;
+  s.s = s.x + kR * a.n;
+  s.z = s.s + kR * (a.form == L2O_ISTA_LFISTA ? a.n : a.m);
+  s.by = s.z + 2 * kR * a.n;
+  s.red = s.by + (a.form == L2O_ISTA_LFISTA ? kR * a.n : 0);
+  s.total = s.red + kThreads * kR;
+  return s;
+}
+
+__device__ __forceinline__ const float* wm_slot(const l2o_ista_args& a, int k) {
+  return a.W2 + (size_t)(k - 1) * a.n * a.n;
+}
+__device__ __forceinline__ const float* lamp_w(const l2o_ista_args& a, int k) {   // [M][N] slot k, as coupled
+  return a.W + (a.share_W ? 0 : (size_t)k * a.m * a.n);
+}
+
+// out[b][j] = sum_t (in0[b][t] W0[j][t] + in1[b][t] W1[j][t]): gemm_rows over two operand pairs in one loop.
+template <class F>
+__device__ __forceinline__ void gemm_rows2(const float* in0, const float* __restrict__ W0, const float* in1,
+                                           const float* __restrict__ W1, int ld, int T, int j0, int j1, F&& epi) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  for (int j = j0 + 2 * w; j < j1; j += 2 * kWarps) {
+    const bool two = j + 1 < j1;
+    const float *p0 = W0 + (size_t)j * ld, *q0 = W1 + (size_t)j * ld;
+    const float *p1 = two ? p0 + ld : p0, *q1 = two ? q0 + ld : q0;
+    float a0[kR], a1[kR];
+#pragma unroll
+    for (int b = 0; b < kR; ++b) a0[b] = a1[b] = 0.f;
+    for (int t = lane; t < T; t += 32) {
+      const float u0 = __ldg(p0 + t), u1 = __ldg(p1 + t), v0 = __ldg(q0 + t), v1 = __ldg(q1 + t);
+#pragma unroll
+      for (int b = 0; b < kR; ++b) {
+        const float x = in0[b * ld + t], xp = in1[b * ld + t];
+        a0[b] = fmaf(xp, v0, fmaf(x, u0, a0[b]));
+        a1[b] = fmaf(xp, v1, fmaf(x, u1, a1[b]));
+      }
+    }
+#pragma unroll
+    for (int b = 0; b < kR; ++b)
+#pragma unroll
+      for (int o = 16; o; o >>= 1) {
+        a0[b] += __shfl_xor_sync(0xffffffffu, a0[b], o);
+        a1[b] += __shfl_xor_sync(0xffffffffu, a1[b], o);
+      }
+#pragma unroll
+    for (int b = 0; b < kR; ++b) {
+      if (lane == b) epi(b, j, a0[b]);
+      if (two && lane == kR + b) epi(b, j + 1, a1[b]);
+    }
+  }
+}
+
+// Soft shrinkage, as the four forms do it.
+__device__ __forceinline__ float shrink1(float z, float th) {
+  const float m = fmaxf(fabsf(z) - th, 0.f);
+  return z > 0.f ? m : (z < 0.f ? -m : 0.f);
+}
+
+__global__ void __cluster_dims__(kCl, 1, 1) __launch_bounds__(kThreads)
+    ista2_fwd_kernel(const l2o_ista_args a) {
+  extern __shared__ float4 smem_f4[];
+  float* sm = reinterpret_cast<float*>(smem_f4);
+  cg::cluster_group cl = cg::this_cluster();
+  const int c = (int)cl.block_rank();
+  const int row0 = (blockIdx.x / kCl) * kR;
+  const int M = a.m, N = a.n, tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  const bool lamp = a.form == L2O_ISTA_LAMP;
+  const Smem2 P = smem_plan2(a);
+  float *ys = sm + P.y, *xs = sm + P.x, *s2 = sm + P.s, *by = sm + P.by, *red = sm + P.red;
+  __shared__ float thr[kR], bk[kR];
+  const Slice sm_ = slice_of(M, c), sn = slice_of(N, c);
+  const int S = lamp ? M : N;   // width of the second state
+
+  for (int e = tid; e < kR * M; e += kThreads) {
+    const int b = e / M, i = e % M, row = row0 + b;
+    ys[e] = row < a.batch ? a.y[(size_t)row * a.ldy + i] : 0.f;
+  }
+  for (int e = tid; e < kR * N; e += kThreads) {
+    const int b = e / N, n = e % N, row = row0 + b;
+    xs[e] = (a.x_in && row < a.batch) ? a.x_in[(size_t)row * N + n] : 0.f;
+  }
+  for (int e = tid; e < kR * S; e += kThreads) {
+    const int b = e / S, n = e % S, row = row0 + b;
+    s2[e] = (a.s2_in && row < a.batch) ? a.s2_in[(size_t)row * S + n] : 0.f;
+  }
+  __syncthreads();
+  if (!lamp) gemm_rows(ys, M, a.B1, M, M, sn.lo, sn.hi, [&](int b, int n, float v) { by[b * N + n] = v; });
+  cl.sync();   // every CTA of the cluster has started (and finished its prologue) before any remote write
+
+  for (int k = a.k0; k < a.k1; ++k) {
+    const int l = k - a.k0;
+    float* zb = sm + P.z + (l & 1) * kR * N;
+    auto put_z = [&](int b, int n, float z) {
+      for (int q = 0; q < kCl; ++q) cl.map_shared_rank(zb, q)[b * N + n] = z;
+    };
+    if (lamp) {
+      if (lane == 0) bk[w] = 0.f;
+      if (k > 0) {   // b_k = ||x_k||_0 / M, a warp per row
+        int cnt = 0;
+        for (int n = lane; n < N; n += 32) cnt += xs[w * N + n] != 0.f;
+        for (int o = 16; o; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+        if (lane == 0) bk[w] = (float)cnt / (float)M;
+      }
+      __syncthreads();
+      gemm_rows(xs, N, a.A, N, N, sm_.lo, sm_.hi, [&](int b, int i, float u) {
+        const float v = ys[b * M + i] - u + bk[b] * s2[b * M + i];
+        for (int q = 0; q < kCl; ++q) cl.map_shared_rank(s2, q)[b * M + i] = v;
+        if (a.rs && row0 + b < a.batch) a.rs[((size_t)l * a.batch + row0 + b) * M + i] = v;
+      });
+      cl.sync();
+      float ss = 0.f;   // ||v_k||^2 of row w
+      for (int i = lane; i < M; i += 32) ss = fmaf(s2[w * M + i], s2[w * M + i], ss);
+      for (int o = 16; o; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+      const float sq = sqrtf(ss / (float)M);
+      if (lane == 0) {
+        thr[w] = fmaxf(sq * a.theta[k], 0.f);
+        if (a.rowrec && c == 0 && row0 + w < a.batch) {
+          float* rr = a.rowrec + ((size_t)l * a.batch + row0 + w) * 2;
+          rr[0] = sq;
+          rr[1] = bk[w];
+        }
+      }
+      const float s = step_of(a, k);
+      gemm_cols(s2, M, lamp_w(a, k), N, M, sn.lo, sn.hi, red,
+                [&](int b, int n, float u) { put_z(b, n, xs[b * N + n] + s * u); });
+    } else {
+      auto z_of = [&](int b, int n, float u) { put_z(b, n, by[b * N + n] + u); };
+      if (k >= 2) gemm_rows2(xs, a.W + (size_t)(k - 1) * N * N, s2, wm_slot(a, k), N, N, sn.lo, sn.hi, z_of);
+      else if (k == 1) gemm_rows(xs, N, a.W, N, N, sn.lo, sn.hi, z_of);
+      else
+        for (int e = tid; e < kR * (sn.hi - sn.lo); e += kThreads) {
+          const int b = e / (sn.hi - sn.lo), n = sn.lo + e % (sn.hi - sn.lo);
+          put_z(b, n, by[b * N + n]);
+        }
+      if (lane == 0) thr[w] = a.theta[k];
+    }
+    cl.sync();
+    float* xn = lamp ? xs : s2;   // LFISTA: x_{k+1} replaces x_{k-1}, and the buffers swap roles
+    for (int e = tid; e < kR * N; e += kThreads) {
+      const int b = e / N, n = e % N, row = row0 + b;
+      const float z = zb[e], x = shrink1(z, thr[b]);
+      xn[e] = x;
+      if (n >= sn.lo && n < sn.hi && row < a.batch) {
+        const size_t o = ((size_t)l * a.batch + row) * N + n;
+        a.xs[o] = x;
+        if (a.zs) a.zs[o] = z;
+      }
+    }
+    if (!lamp) {
+      s2 = xs;
+      xs = xn;
+    }
+    __syncthreads();
+  }
+  cl.sync();   // no CTA leaves while another may still write into its shared memory
+}
+
+// x_{k-1} of pass layer l, for LFISTA's Wm term: the layer input two layers back.
+__device__ __forceinline__ const float* layer_input2(const l2o_ista_args& a, int l, int row) {
+  if (l == 0) return a.s2_in ? a.s2_in + (size_t)row * a.n : nullptr;
+  return layer_input(a, l - 1, row);
+}
+
+__global__ void __cluster_dims__(kCl, 1, 1) __launch_bounds__(kThreads) ista2_bwd_kernel(const Bwd p) {
+  extern __shared__ float4 smem_f4[];
+  float* sm = reinterpret_cast<float*>(smem_f4);
+  const l2o_ista_args& a = p.a;
+  cg::cluster_group cl = cg::this_cluster();
+  const int c = (int)cl.block_rank();
+  const int row0 = (blockIdx.x / kCl) * kR;
+  const int M = a.m, N = a.n, tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  const bool lamp = a.form == L2O_ISTA_LAMP;
+  const Smem2 P = smem_plan2(a);
+  // dx: dL/dx_{k+1} on the N slice.  s2: LFISTA the carry dL/dx_k from layer k+1's Wm term (N slice); LAMP dv, the
+  // full rows of dL/dv_k after the exchange (the own M slice holds the carry before it).
+  float *dx = sm + P.x, *s2 = sm + P.s, *red = sm + P.red;
+  __shared__ float wsum[kWarps], gpart[kCl][kR], gcoef[kR];
+  const Slice sm_ = slice_of(M, c), sn = slice_of(N, c);
+  const int ns = sn.hi - sn.lo;
+  const Slice ss_ = lamp ? sm_ : sn;
+  const int S = lamp ? M : N, nss = ss_.hi - ss_.lo;
+  float* dzr = dz_rec(p);
+  float* part = part_rec(p);
+  const int nblk = gridDim.x;
+
+  for (int e = tid; e < kR * ns; e += kThreads) {
+    const int b = e / ns, n = sn.lo + e % ns, row = row0 + b;
+    dx[b * N + n] = row < a.batch ? p.g.d_xk[(size_t)row * N + n] : 0.f;
+  }
+  for (int e = tid; e < kR * nss; e += kThreads) {
+    const int b = e / nss, j = ss_.lo + e % nss, row = row0 + b;
+    s2[b * S + j] = (p.g.d_s2 && row < a.batch) ? p.g.d_s2[(size_t)row * S + j] : 0.f;
+  }
+  cl.sync();   // every CTA of the cluster has started before any remote write
+  for (int k = a.k1 - 1; k >= a.k0; --k) {
+    const int l = k - a.k0;
+    float* zb = sm + P.z + (l & 1) * kR * N;
+    float dth = 0.f, ds = 0.f;
+    if (lamp) {
+      // dr = dx [r != 0, |r| >= theta_b] (tf.maximum sends the gradient to |r| - theta on ties); a warp per row, so
+      // the row's partial of g = dL/dtheta_b is summed in a fixed order.
+      const int row = row0 + w;
+      const bool ok = row < a.batch;
+      const float sq = ok ? a.rowrec[((size_t)l * a.batch + row) * 2] : 0.f;
+      const float th = fmaxf(sq * a.theta[k], 0.f);
+      float g = 0.f;
+      for (int n = sn.lo + lane; n < sn.hi; n += 32) {
+        float dr = 0.f;
+        if (ok) {
+          const size_t o = ((size_t)l * a.batch + row) * N + n;
+          const float r = a.zs[o], d = dx[w * N + n];
+          if (r != 0.f && fabsf(r) >= th) {
+            dr = d;
+            g -= r > 0.f ? d : -d;
+          }
+          dzr[o] = dr;
+        }
+        for (int q = 0; q < kCl; ++q) cl.map_shared_rank(zb, q)[w * N + n] = dr;
+      }
+      for (int o = 16; o; o >>= 1) g += __shfl_xor_sync(0xffffffffu, g, o);
+      if (lane < kCl) cl.map_shared_rank(&gpart[0][0], lane)[c * kR + w] = g;
+      cl.sync();
+      if (lane == 0) {
+        float gs = 0.f;
+        for (int q = 0; q < kCl; ++q) gs += gpart[q][w];
+        const float lk = a.theta[k];
+        // theta = max(sqrt(rvar) lam, 0): d theta / d v = lam v / (M sqrt(rvar)) where sqrt(rvar) lam >= 0; a row
+        // with rvar = 0 contributes nothing (TF's sqrt gradient would give inf * 0 there).
+        gcoef[w] = (sq * lk >= 0.f && sq > 0.f) ? gs * lk / ((float)M * sq) : 0.f;
+        if (c == 0 && sq * lk >= 0.f) dth = gs * sq;   // dlam_k, added by one CTA per cluster
+      }
+      __syncthreads();
+      const float s = step_of(a, k);
+      gemm_rows(zb, N, lamp_w(a, k), N, N, sm_.lo, sm_.hi, [&](int b, int i, float u) {
+        const int rw = row0 + b;
+        float dv = 0.f;
+        if (rw < a.batch) {
+          const float v = a.rs[((size_t)l * a.batch + rw) * M + i];
+          const float carry = k + 1 < a.k1 ? a.rowrec[((size_t)(l + 1) * a.batch + rw) * 2 + 1] * s2[b * M + i]
+                                           : s2[b * M + i];
+          ds += v * u;
+          dv = fmaf(s, u, fmaf(gcoef[b], v, carry));
+        }
+        for (int q = 0; q < kCl; ++q) cl.map_shared_rank(s2, q)[b * M + i] = dv;
+      });
+      cl.sync();
+      gemm_cols(s2, M, a.A, N, M, sn.lo, sn.hi, red, [&](int b, int n, float v) { dx[b * N + n] = zb[b * N + n] - v; });
+    } else {
+      const float th = a.theta[k];
+      for (int e = tid; e < kR * ns; e += kThreads) {
+        const int b = e / ns, n = sn.lo + e % ns, row = row0 + b;
+        float dz = 0.f;
+        if (row < a.batch) {
+          const size_t o = ((size_t)l * a.batch + row) * N + n;
+          const float z = a.zs[o], d = dx[b * N + n];
+          if (fabsf(z) > th && z != 0.f) {   // relu'(0) = 0 and sign'(z) = 0
+            dz = d;
+            dth -= z > 0.f ? d : -d;
+          }
+          dzr[o] = dz;
+        }
+        for (int q = 0; q < kCl; ++q) cl.map_shared_rank(zb, q)[b * N + n] = dz;
+      }
+      cl.sync();
+      // dx_k = dz_k Wg_k + carry;  the carry for x_{k-1} is dz_k Wm_k, local to the slice.
+      if (k >= 1)
+        gemm_cols(zb, N, a.W + (size_t)(k - 1) * N * N, N, N, sn.lo, sn.hi, red,
+                  [&](int b, int j, float u) { dx[b * N + j] = u + s2[b * N + j]; });
+      else
+        for (int e = tid; e < kR * ns; e += kThreads) dx[(e / ns) * N + sn.lo + e % ns] = s2[(e / ns) * N + sn.lo + e % ns];
+      if (k >= 2)
+        gemm_cols(zb, N, wm_slot(a, k), N, N, sn.lo, sn.hi, red, [&](int b, int j, float u) { s2[b * N + j] = u; });
+      else
+        for (int e = tid; e < kR * ns; e += kThreads) s2[(e / ns) * N + sn.lo + e % ns] = 0.f;
+      __syncthreads();
+    }
+    const float sth = block_sum(dth, wsum), sds = block_sum(ds, wsum);
+    if (tid == 0) {
+      part[((size_t)l * nblk + blockIdx.x) * 2 + 0] = sth;
+      part[((size_t)l * nblk + blockIdx.x) * 2 + 1] = sds;
+    }
+  }
+  if (p.g.d_x_in)
+    for (int e = tid; e < kR * ns; e += kThreads) {
+      const int b = e / ns, n = sn.lo + e % ns, row = row0 + b;
+      if (row < a.batch) p.g.d_x_in[(size_t)row * N + n] = dx[b * N + n];
+    }
+  if (p.g.d_s2_in)   // LFISTA: the carry dz_{k0} Wm_{k0};  LAMP: b_{k0} dv_{k0}
+    for (int e = tid; e < kR * nss; e += kThreads) {
+      const int b = e / nss, j = ss_.lo + e % nss, row = row0 + b;
+      if (row < a.batch)
+        p.g.d_s2_in[(size_t)row * S + j] = lamp ? a.rowrec[(size_t)row * 2 + 1] * s2[b * S + j] : s2[b * S + j];
+    }
+  cl.sync();
+}
+
+// The gradient launch of the two-state forms.  blockIdx.y walks, in order: LFISTA the Wg slots (nw), the Wm slots
+// (nw2) and dWe, or LAMP the W slots (nw); then the per-layer scalars (blockIdx.x = layer).
+// LFISTA slot g belongs to layer g + 1: dWg = dz^T x_k, dWm = dz^T x_{k-1} (0 at layer 1, which has no Wm term);
+// dWe = sum_k dz_k^T y.  LAMP: dW_k = s_k v_k^T dr_k, over the layers of the pass when W is shared.
+__global__ void __launch_bounds__(kThreads) ista2_grad_kernel(const Bwd p, int nblk_bwd, int nw, int nw2) {
+  const l2o_ista_args& a = p.a;
+  const int M = a.m, N = a.n, B = a.batch;
+  const bool lamp = a.form == L2O_ISTA_LAMP;
+  const int ne = lamp ? 0 : 1;
+  const float* dzr = dz_rec(p);
+  const int y_slot = blockIdx.y;
+  if (y_slot == nw + nw2 + ne) {   // per-layer scalars: dtheta (LAMP: dlam) and ds
+    const int k = blockIdx.x;
+    if (k >= a.num_layers) return;
+    const float* part = part_rec(p);
+    __shared__ double acc[2][kWarps];
+    double t = 0.0, s = 0.0;
+    if (k >= a.k0 && k < a.k1)
+      for (int i = threadIdx.x; i < nblk_bwd; i += kThreads) {
+        t += part[((size_t)(k - a.k0) * nblk_bwd + i) * 2];
+        s += part[((size_t)(k - a.k0) * nblk_bwd + i) * 2 + 1];
+      }
+    for (int o = 16; o; o >>= 1) {
+      t += __shfl_xor_sync(0xffffffffu, t, o);
+      s += __shfl_xor_sync(0xffffffffu, s, o);
+    }
+    if ((threadIdx.x & 31) == 0) acc[0][threadIdx.x >> 5] = t, acc[1][threadIdx.x >> 5] = s;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      t = s = 0.0;
+      for (int w = 0; w < kWarps; ++w) t += acc[0][w], s += acc[1][w];
+      const double sc = p.g.gscale ? (double)p.g.gscale[k] : 1.0;
+      p.g.dtheta[k] = sc * t;
+      if (p.g.dstep) p.g.dstep[k] = sc * s;
+    }
+    return;
+  }
+  // kind 0: LFISTA Wg / LAMP W;  1: LFISTA Wm;  2: LFISTA We
+  const int kind = y_slot < nw ? 0 : (y_slot < nw + nw2 ? 1 : 2);
+  const int g = kind == 0 ? y_slot : y_slot - nw;
+  int Pd = N, Qd = N, la = 0, lb = a.k1 - a.k0, birth = 0;
+  double* out;
+  if (kind == 2) {
+    Qd = M;
+    out = p.g.dB1;
+  } else if (lamp) {
+    const int k = a.share_W ? -1 : g;
+    Pd = M;
+    if (k >= 0) {
+      birth = k;
+      la = k >= a.k0 && k < a.k1 ? k - a.k0 : 0;
+      lb = k >= a.k0 && k < a.k1 ? la + 1 : 0;
+    }
+    out = p.g.dW + (size_t)g * M * N;
+  } else {
+    const int k = g + 1;
+    birth = k;
+    const bool in = k >= a.k0 && k < a.k1 && (kind == 0 || k >= 2);
+    la = in ? k - a.k0 : 0;
+    lb = in ? la + 1 : 0;
+    out = (kind == 0 ? p.g.dW : p.g.dW2) + (size_t)g * N * N;
+  }
+  const int tiles_q = (Qd + kTile - 1) / kTile, tiles = tiles_q * ((Pd + kTile - 1) / kTile);
+  if ((int)blockIdx.x >= tiles) return;
+  const int p0 = (blockIdx.x / tiles_q) * kTile, q0 = (blockIdx.x % tiles_q) * kTile;
+  __shared__ float Ps[kChunk][kTile], Qs[kChunk][kTile];
+  const int tp = threadIdx.x / 16, tq = threadIdx.x % 16;
+  double acc[4][4] = {};   // per-layer fp32 sums, added across layers in fp64
+  for (int l = la; l < lb; ++l) {
+    float lacc[4][4] = {};
+    const float coef = lamp ? step_of(a, a.k0 + l) : 1.f;
+    for (int b0 = 0; b0 < B; b0 += kChunk) {
+      for (int e = threadIdx.x; e < kChunk * kTile; e += kThreads) {
+        const int bb = e / kTile, j = e % kTile, row = b0 + bb;
+        float pv = 0.f, qv = 0.f;
+        if (row < B) {
+          const float* dz = dzr + ((size_t)l * B + row) * N;
+          if (lamp) {
+            if (p0 + j < Pd) pv = a.rs[((size_t)l * B + row) * M + p0 + j];
+            if (q0 + j < Qd) qv = dz[q0 + j];
+          } else {
+            if (p0 + j < Pd) pv = dz[p0 + j];
+            if (q0 + j < Qd) {
+              if (kind == 2) qv = a.y[(size_t)row * a.ldy + q0 + j];
+              else {
+                const float* xin = kind == 0 ? layer_input(a, l, row) : layer_input2(a, l, row);
+                qv = xin ? xin[q0 + j] : 0.f;
+              }
+            }
+          }
+        }
+        Ps[bb][j] = coef * pv;
+        Qs[bb][j] = qv;
+      }
+      __syncthreads();
+#pragma unroll
+      for (int bb = 0; bb < kChunk; ++bb) {
+        float pr[4], qr[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) pr[i] = Ps[bb][tp + 16 * i], qr[i] = Qs[bb][tq + 16 * i];
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) lacc[i][j] = fmaf(pr[i], qr[j], lacc[i][j]);
+      }
+      __syncthreads();
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) acc[i][j] += (double)lacc[i][j];
+  }
+  const double sc = p.g.gscale && birth < a.num_layers ? (double)p.g.gscale[birth] : 1.0;
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int pp = p0 + tp + 16 * i, qq = q0 + tq + 16 * j;
+      if (pp < Pd && qq < Qd) out[(size_t)pp * Qd + qq] = sc * acc[i][j];
+    }
+}
+
+inline bool two_state(const l2o_ista_args& a) { return a.form == L2O_ISTA_LFISTA || a.form == L2O_ISTA_LAMP; }
+inline int plan_floats(const l2o_ista_args& a) { return two_state(a) ? smem_plan2(a).total : smem_plan(a).total; }
+
 int check_args(const l2o_ista_args* a) {
-  if (!a || (a->form != L2O_ISTA_LISTA && a->form != L2O_ISTA_COUPLED)) return L2O_E_INVALID;
+  if (!a || a->form < L2O_ISTA_LISTA || a->form > L2O_ISTA_LAMP) return L2O_E_INVALID;
   if (a->batch <= 0 || a->m <= 0 || a->n <= 0 || a->num_layers <= 0 || a->k0 < 0 || a->k0 >= a->k1 ||
       a->k1 > a->num_layers || a->share_W < 0 || a->share_W > 1 || a->ldy < a->m)
     return L2O_E_INVALID;
   if (!a->theta || !a->y) return L2O_E_INVALID;
-  if (a->form == L2O_ISTA_COUPLED && (!a->A || !a->W)) return L2O_E_INVALID;
+  if ((a->form == L2O_ISTA_COUPLED || a->form == L2O_ISTA_LAMP) && (!a->A || !a->W)) return L2O_E_INVALID;
   if (a->form == L2O_ISTA_LISTA && (!a->B1 || (a->k1 > 1 && !a->W))) return L2O_E_INVALID;
-  const void* ptrs[] = {a->A, a->B1, a->W, a->theta, a->step, a->ss_rank, a->y, a->x_in, a->xs, a->zs, a->rs};
+  if (a->form == L2O_ISTA_LFISTA &&
+      (!a->B1 || (a->k1 > 1 && !a->W) || (a->k1 > 2 && !a->W2) || a->share_W || a->step))
+    return L2O_E_INVALID;
+  if (two_state(*a) && a->ss_rank) return L2O_E_INVALID;
+  const void* ptrs[] = {a->A,  a->B1, a->W,  a->theta, a->step,  a->ss_rank, a->y,     a->x_in,
+                        a->xs, a->zs, a->rs, a->W2,    a->s2_in, a->rowrec};
   for (const void* q : ptrs)
     if (misaligned(q, 4)) return L2O_E_INVALID;
   if (a->m > kMaxDim || a->n > kMaxDim) return L2O_E_UNSUPPORTED;
-  if ((size_t)smem_plan(*a).total * sizeof(float) > 200 * 1024) return L2O_E_UNSUPPORTED;
+  if ((size_t)plan_floats(*a) * sizeof(float) > 200 * 1024) return L2O_E_UNSUPPORTED;
   return L2O_OK;
 }
 
@@ -571,6 +1017,23 @@ inline int clusters(const l2o_ista_args& a) { return (a.batch + kR - 1) / kR; }
 size_t scratch_bytes(const l2o_ista_args& a) {
   const size_t L = (size_t)(a.k1 - a.k0);
   return 4 * (L * a.batch * a.n + L * clusters(a) * kCl * 2);
+}
+
+int bwd_two_state(const Bwd& p, cudaStream_t stream) {
+  const l2o_ista_args& a = p.a;
+  const size_t smem = (size_t)smem_plan2(a).total * sizeof(float);
+  if (int rc = l2o::raise_smem_limit("l2o_ista_bwd", ista2_bwd_kernel, smem)) return rc;
+  const int nblk = clusters(a) * kCl;
+  ista2_bwd_kernel<<<nblk, kThreads, smem, stream>>>(p);
+  if (int rc = l2o::after_launch("l2o_ista_bwd")) return rc;
+  const bool lamp = a.form == L2O_ISTA_LAMP;
+  const int slots = lamp ? (a.share_W ? 1 : a.num_layers) : a.num_layers - 1;
+  const int nw = p.g.dW ? slots : 0, nw2 = !lamp && p.g.dW2 ? slots : 0, ne = lamp ? 0 : 1;
+  const int tq = (a.n + kTile - 1) / kTile;
+  const int tiles = std::max({tq * (((lamp ? a.m : a.n) + kTile - 1) / kTile), tq * ((a.m + kTile - 1) / kTile),
+                              a.num_layers});
+  ista2_grad_kernel<<<dim3(tiles, nw + nw2 + ne + 1), kThreads, 0, stream>>>(p, nblk, nw, nw2);
+  return l2o::after_launch("l2o_ista_bwd");
 }
 
 }  // namespace ista
@@ -590,7 +1053,12 @@ int l2o_ista_workspace_bytes(const l2o_ista_args* a, size_t* bytes) {
 int l2o_ista_fwd(const l2o_ista_args* a, void* stream) {
   if (int rc = check_args(a)) return rc;
   if (!a->xs) return L2O_E_INVALID;
-  const size_t smem = (size_t)smem_plan(*a).total * sizeof(float);
+  const size_t smem = (size_t)plan_floats(*a) * sizeof(float);
+  if (two_state(*a)) {
+    if (int rc = l2o::raise_smem_limit("l2o_ista_fwd", ista2_fwd_kernel, smem)) return rc;
+    ista2_fwd_kernel<<<clusters(*a) * kCl, kThreads, smem, (cudaStream_t)stream>>>(*a);
+    return l2o::after_launch("l2o_ista_fwd");
+  }
   if (int rc = l2o::raise_smem_limit("l2o_ista_fwd", ista_fwd_kernel, smem)) return rc;
   ista_fwd_kernel<<<clusters(*a) * kCl, kThreads, smem, (cudaStream_t)stream>>>(*a);
   return l2o::after_launch("l2o_ista_fwd");
@@ -602,13 +1070,16 @@ int l2o_ista_bwd(const l2o_ista_args* a, const l2o_ista_grads* g, void* stream) 
   if (a->ss_rank && !a->sel) return L2O_E_INVALID;
   if (a->form == L2O_ISTA_COUPLED && !a->rs) return L2O_E_INVALID;
   if (a->form == L2O_ISTA_LISTA && !g->dB1) return L2O_E_INVALID;
-  const void* f4[] = {g->d_xk, g->d_x_in, g->gscale, g->scratch};
+  if (a->form == L2O_ISTA_LFISTA && !g->dB1) return L2O_E_INVALID;
+  if (a->form == L2O_ISTA_LAMP && (!a->rs || !a->rowrec)) return L2O_E_INVALID;
+  const void* f4[] = {g->d_xk, g->d_x_in, g->gscale, g->scratch, g->d_s2, g->d_s2_in};
   for (const void* q : f4)
     if (l2o::misaligned(q, 4)) return L2O_E_INVALID;
-  const void* f8[] = {g->dW, g->dB1, g->dtheta, g->dstep};
+  const void* f8[] = {g->dW, g->dB1, g->dtheta, g->dstep, g->dW2};
   for (const void* q : f8)
     if (l2o::misaligned(q, 8)) return L2O_E_INVALID;
   Bwd p{*a, *g};
+  if (two_state(*a)) return bwd_two_state(p, (cudaStream_t)stream);
   const size_t smem = (size_t)smem_plan(*a).total * sizeof(float);
   if (int rc = l2o::raise_smem_limit("l2o_ista_bwd", ista_bwd_kernel, smem)) return rc;
   const int nblk = clusters(*a) * kCl;

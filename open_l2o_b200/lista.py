@@ -1,5 +1,6 @@
 """Model-based L2O's LISTA family on the sm_90a kernels of ``csrc/l2o_ista.cu`` (MB/ = Model_Base_L2O/ of the
-reference): ``Lista``, ``ListaCp``, ``ListaCpss`` and ``Alista``, grown layer by layer with ``create_cell``.
+reference): ``Lista``, ``ListaCp``, ``ListaCpss``, ``Alista``, ``Lfista`` and ``Lamp``, grown layer by layer with
+``create_cell``.
 
 Every variable of a model lives in one fp32 arena on the device (its gradient in a matching fp64 arena), so one
 forward, one loss, one backward and one Adam launch train all layers at once; ``variables`` maps the reference's
@@ -11,6 +12,7 @@ handed (MB/models/lista.py:41-42), which raises in TensorFlow; here layer k uses
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 from typing import Dict, Optional
 
@@ -20,7 +22,7 @@ import torch
 from . import _lib
 from .engine import _ptr, _stream
 
-LISTA, COUPLED = 0, 1
+LISTA, COUPLED, LFISTA, LAMP = 0, 1, 2, 3
 TASK_SC, TASK_LASSO = 0, 1
 
 
@@ -65,7 +67,7 @@ def make_data(M: int, N: int, n, p: float = 0.1, noise: Optional[float] = None, 
 
 
 class _IstaModel:
-    """What the four models share: the variable arena, layer-wise growth and the kernel calls."""
+    """What the models share: the variable arena, layer-wise growth and the kernel calls."""
 
     form = COUPLED
 
@@ -119,6 +121,13 @@ class _IstaModel:
         else:
             self._specs += [(self.name + "_W%d" % (i + 1), A.shape, i, A) for i in range(self.T)]
 
+    def _theta_block(self):
+        """theta_1 .. theta_T (LAMP: lam_1 .. lam_T) as one span of the arena."""
+        return self._block(self.name + "_theta1", self.T)
+
+    def _theta_grad(self):
+        return self._grad_span(self.name + "_theta1", self.T)
+
     def _span(self, arena, vname, count):
         """The arena span of `count` consecutive variables starting at the one named `vname`."""
         v = self.variables[vname]
@@ -130,6 +139,10 @@ class _IstaModel:
 
     def _grad_span(self, vname, count):
         return self._span(self.grads, vname, count)
+
+    def _second(self):
+        """(W2, dW2) for the kernel arguments: LFISTA's Wm slots."""
+        return None, None
 
     def _weights(self):
         """(W pointer, dW span or None, B1, dB1, step, dstep) for the kernel arguments."""
@@ -170,7 +183,8 @@ class _IstaModel:
             b = {"xs": z(self.T, B, self.N)}
             if record:
                 b["zs"] = z(self.T, B, self.N)
-                b["rs"] = z(self.T, B, self.M) if self.form == COUPLED else None
+                b["rs"] = z(self.T, B, self.M) if self.form in (COUPLED, LAMP) else None
+                b["rowrec"] = z(self.T, B, 2) if self.form == LAMP else None
                 b["sel"] = z(self.T, B, self.N, dt=torch.uint8) if self.ss_rank is not None else None
                 b["d_xk"] = z(B, self.N)
                 b["loss"] = z(B, dt=torch.float64)
@@ -182,14 +196,14 @@ class _IstaModel:
         a = _lib.IstaArgs()
         a.form, a.batch, a.m, a.n, a.num_layers, a.k0, a.k1 = self.form, B, self.M, self.N, self.T, 0, k1
         a.share_W = int(self.one_W)
-        a.A, a.B1, a.W = _ptr(self.A), _ptr(B1), _ptr(W)
-        a.theta = _ptr(self._block(self.name + "_theta1", self.T))
+        a.A, a.B1, a.W, a.W2 = _ptr(self.A), _ptr(B1), _ptr(W), _ptr(self._second()[0])
+        a.theta = _ptr(self._theta_block())
         a.step = _ptr(step)
         a.ss_rank = None if self.ss_rank is None else _ptr(self.ss_rank, torch.int32, "ss_rank")
         a.y, a.ldy = y.data_ptr(), ldy
         a.xs = _ptr(bufs["xs"])
         if record:
-            a.zs, a.rs = _ptr(bufs["zs"]), _ptr(bufs["rs"])
+            a.zs, a.rs, a.rowrec = _ptr(bufs["zs"]), _ptr(bufs["rs"]), _ptr(bufs["rowrec"])
             a.sel = _ptr(bufs["sel"], torch.uint8, "sel")
         return a
 
@@ -238,7 +252,8 @@ class _IstaModel:
         g = _lib.IstaGrads()
         g.d_xk, g.d_x_in = _ptr(d_xk), _ptr(d_x_in)
         g.dW, g.dB1 = _ptr(dW, torch.float64, "dW"), _ptr(dB1, torch.float64, "dB1")
-        g.dtheta = _ptr(self._grad_span(self.name + "_theta1", self.T), torch.float64, "dtheta")
+        g.dW2 = _ptr(self._second()[1], torch.float64, "dW2")
+        g.dtheta = _ptr(self._theta_grad(), torch.float64, "dtheta")
         g.dstep = _ptr(dstep, torch.float64, "dstep")
         g.gscale = _ptr(gscale)
         g.scratch = _ptr(self._bufs[key])
@@ -309,3 +324,85 @@ class Alista(_IstaModel):
 
     def __init__(self, A, W, T, lam, q_per_layer, maxq, D=None, name="Alista", device="cuda"):
         super().__init__(A, T, lam, False, D, name, device, step_trainable=True, ss=(q_per_layer, maxq), W_const=W)
+
+
+def fista_momenta(T: int):
+    """m_0 .. m_{T-1} of MB/models/lfista.py: t = [1, 1], t_{i+2} = (1 + sqrt(1 + 4 t_{i+1}^2)) / 2,
+    m_i = (t_{i+1} - 1) / t_{i+2}."""
+    t, m = [1.0, 1.0], []
+    for _ in range(T):
+        t.append((1 + math.sqrt(1 + 4 * t[-1] ** 2.0)) / 2)
+        m.append((t[-2] - 1) / t[-1])
+    return m
+
+
+class Lfista(_IstaModel):
+    """LFISTA (MB/models/lfista.py): z_k = y We^T + x_k Wg_k^T + x_{k-1} Wm_k^T (Wg from layer 1, Wm from layer 2).
+    We = A^T / L is one variable shared by every layer; Wg_{k+1} = (1 + m_k) W and Wm_{k+1} = -m_k W with
+    W = I - We A.  ``Lfista_Wm2`` belongs to layer 1 but no layer reads it: its gradient is 0.  ``share_W`` is
+    accepted and ignored, as in the reference."""
+
+    form = LFISTA
+
+    def __init__(self, A, T, lam, share_W=False, D=None, name="Lfista", device="cuda"):
+        super().__init__(A, T, lam, False, D, name, device, step_trainable=False)
+
+    def _layout_W(self, A):
+        M, N = A.shape
+        B = (A.T.astype(np.float32) / np.float32(self.scale)).astype(np.float32)
+        W = (np.eye(N, dtype=np.float32) - B @ A).astype(np.float32)
+        m, nm = fista_momenta(self.T), self.name
+        self._specs.append((nm + "_We1", (N, M), 0, B))
+        self._specs += [(nm + "_Wg%d" % (i + 1), (N, N), i, (W * (1 + m[i])).astype(np.float32))
+                        for i in range(1, self.T)]
+        self._specs += [(nm + "_Wm%d" % (i + 1), (N, N), i, (-m[i] * W).astype(np.float32)) for i in range(1, self.T)]
+
+    def _second(self):
+        if self.T < 2:
+            return None, None
+        nm = self.name
+        return self._block(nm + "_Wm2", self.T - 1), self._grad_span(nm + "_Wm2", self.T - 1)
+
+    def _weights(self):
+        nm = self.name
+        B1, dB1 = self.variables[nm + "_We1"], self._grad_span(nm + "_We1", 1)
+        if self.T < 2:
+            return None, None, B1, dB1, None, None
+        return self._block(nm + "_Wg2", self.T - 1), self._grad_span(nm + "_Wg2", self.T - 1), B1, dB1, None, None
+
+
+class Lamp(_IstaModel):
+    """LAMP (MB/models/lamp.py): v_k = y - x_k A^T + b_k v_{k-1} (v_0 = y), b_k = ||x_k||_0 / M,
+    r_k = x_k + s_k v_k W_k, x_{k+1} = shrink(r_k, max(sqrt(||v_k||^2 / M) lam_k, 0)).  W_k = A / L initially, lam_k =
+    lam; the step sizes are trainable only with ``share_W`` (otherwise 1)."""
+
+    form = LAMP
+
+    def __init__(self, A, T, lam, share_W=False, D=None, name="Lamp", device="cuda"):
+        super().__init__(A, T, lam, share_W, D, name, device, step_trainable=share_W)
+
+    def _layout(self, A, W_const, step_trainable):
+        nm, T = self.name, self.T
+        self.W_const = None
+        W = (A.astype(np.float32) / np.float32(self.scale)).astype(np.float32)
+        if self.share_W:
+            self._specs.append((nm + "_W", A.shape, 0, W))
+        else:
+            self._specs += [(nm + "_W%d" % (i + 1), A.shape, i, W) for i in range(T)]
+        self._specs += [(nm + "_lam%d" % (i + 1), (1,), i, np.float32(self.lam)) for i in range(T)]
+        if step_trainable:
+            self._specs += [(nm + "_step_size%d" % (i + 1), (1,), i, np.float32(1.0)) for i in range(T)]
+
+    def _theta_block(self):
+        return self._block(self.name + "_lam1", self.T)
+
+    def _theta_grad(self):
+        return self._grad_span(self.name + "_lam1", self.T)
+
+    def __call__(self, inputs: torch.Tensor) -> torch.Tensor:
+        """The Keras model's output: [y, v_0, x_1, v_1, x_2, ..., v_{k-1}, x_k] (output_interval M + N)."""
+        y = inputs[:, :self.M].contiguous()
+        k = self.num_cells
+        xs = self.forward(y, k, record=True)
+        vs = self._bufs_for(y.shape[0], True)["rs"]
+        return torch.cat([y] + [t for i in range(k) for t in (vs[i], xs[i])], dim=1)

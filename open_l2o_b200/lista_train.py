@@ -103,8 +103,11 @@ def build_model(model_name, A, num_layers, model_lam, share_W, ss_q_per_layer, s
     if model_name == "alista":
         return lista.Alista(A, alista_W, num_layers, model_lam, ss_q_per_layer, ss_maxq, name="Alista",
                             device=device)
-    raise NotImplementedError("model %r is not built here (Step-LISTA, TiSTA, GLISTA, LFISTA, LAMP are out of scope)"
-                              % model_name)
+    if model_name == "lfista":
+        return lista.Lfista(A, num_layers, model_lam, share_W, name="Lfista", device=device)
+    if model_name == "lamp":
+        return lista.Lamp(A, num_layers, model_lam, share_W, name="Lamp", device=device)
+    raise NotImplementedError("model %r is not built here (Step-LISTA, TiSTA, GLISTA are out of scope)" % model_name)
 
 
 class KernelTrainer:
@@ -156,7 +159,8 @@ class KernelTrainer:
 
 
 def evaluate(model, data, task, lasso_lam, batch):
-    """Per-layer metric over `data` (mean over rows): NMSE in dB (EvalNMSE) or the Lasso objective (LassoObjective)."""
+    """Per-layer metric over `data` (mean over rows): NMSE in dB (EvalNMSE) or the Lasso objective (LassoObjective),
+    of each layer's x_k (for LAMP too, whose Keras output interleaves v_k)."""
     M, N, K = model.M, model.N, model.num_cells
     acc, rows = torch.zeros(K, dtype=torch.float64, device=data.device), 0
     for i in range(0, data.shape[0], batch):
@@ -230,7 +234,8 @@ def run(model_name="lista", task="sc", num_layers=16, model_lam=0.4, lasso_lam=0
 
 def main(argv=None):
     p = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
-    p.add_argument("--model_name", default="lista", choices=["lista", "lista_cp", "lista_cpss", "alista"])
+    p.add_argument("--model_name", default="lista", choices=["lista", "lista_cp", "lista_cpss", "alista", "lfista",
+                                                                   "lamp"])
     p.add_argument("--num_layers", type=int, default=16)
     p.add_argument("--model_lam", type=float, default=0.4)
     p.add_argument("--share_W", action="store_true")

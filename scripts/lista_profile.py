@@ -21,15 +21,21 @@ sys.path.insert(0, ROOT)
 from open_l2o_b200 import lista, lista_train as lt  # noqa: E402
 from open_l2o_b200.engine import adam_step  # noqa: E402
 from oracle import lista_oracle as lo  # noqa: E402
+from tests import lfista_lamp_cases as fc  # noqa: E402
 
 M, N, K = 256, 512, 16
 B_TRAIN, B_VAL = 128, 1024
 
 
 def flops(form, B, train, has_dw):
-    """GEMM FLOPs from shapes: coupled forward 4BMN per layer, backward 4BMN (+2BMN for dW); LISTA forward 2BMN
-    once (y B1^T) + 2BN^2 per layer with W, backward 2BN^2 (+2BN^2 for dW) per such layer + 2BMN for dB1."""
-    if form == lista.COUPLED:
+    """GEMM FLOPs from shapes: coupled and LAMP forward 4BMN per layer, backward 4BMN (+2BMN for dW); LISTA forward
+    2BMN once (y B1^T) + 2BN^2 per layer with W, backward 2BN^2 (+2BN^2 for dW) per such layer + 2BMN for dB1;
+    LFISTA as LISTA with K - 1 Wg and K - 2 Wm products."""
+    if form == lista.LFISTA:
+        nw = (K - 1) + (K - 2)
+        f = 2 * B * M * N + 2 * B * N * N * nw
+        return f + 4 * B * N * N * nw + 2 * B * M * N if train else f
+    if form in (lista.COUPLED, lista.LAMP):
         f = 4 * B * M * N * K
         return f + (4 + (2 if has_dw else 0)) * B * M * N * K if train else f
     f = 2 * B * M * N + 2 * B * N * N * (K - 1)
@@ -48,6 +54,8 @@ class TorchVersion:
 
     def forward(self, data, P=None):
         P, m, nm = P or self.P, self.m, self.m.name
+        if m.form in (lista.LFISTA, lista.LAMP):
+            return fc.model_forward(m, P, data[:, :M], K)
         if m.W_const is not None:
             W = m.W_const[None]
         elif m.share_W:
@@ -172,7 +180,7 @@ def main():
     p.add_argument("--reps", type=int, default=5)
     p.add_argument("--iters", type=int, default=50)
     p.add_argument("--out", default=os.path.join(ROOT, "scripts", "lista_profile_h100.json"))
-    p.add_argument("--models", default="lista,lista_cp,lista_cpss,alista")
+    p.add_argument("--models", default="lista,lista_cp,lista_cpss,alista,lfista,lamp")
     a = p.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("lista_profile.py measures on a GPU; none found")
