@@ -563,6 +563,61 @@ int l2o_ista_fwd(const l2o_ista_args* a, void* stream);
 int l2o_ista_bwd(const l2o_ista_args* a, const l2o_ista_grads* g, void* stream);
 int l2o_ista_loss_grad(const l2o_ista_loss_args* a, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * L2O-Minimax's Twin-L2O (MM = Model_Free_L2O/L2O-Minimax/Twin-L2O.py): two coordinate-wise optimizers, net 0 (min)
+ * and net 1 (max), each LSTMCell(2, H) -> LSTMCell(H, H) -> Linear(H, 1) (MM Optimizer, :676), alternating on a batch
+ * of B saddle-point problems of dim coordinates; R = B dim rows, row p dim + i is coordinate i of problem p.
+ *
+ *   l2o_minimax_fwd   iterations [t0, t1) of do_fit (MM :152-427), one launch.  Iteration t odd: net 0 updates u
+ *                     from [df/du, df/dv]; even: net 1 updates v from [df/dv, df/du], both at the current (u, v).
+ *                     The active net's h and c are multiplied by rescale before its cells.  Update: t < warm_end:
+ *                     x += sign(delta) lr[t-1], else x += delta out_mul.  l_t = f(u, v) after a min step, -f after
+ *                     a max step.
+ *   l2o_minimax_bwd   the gradient of sum_t coef[t-t0] weight[p] l_t(p) over the rows of [t0, t1) w.r.t. both nets'
+ *                     parameters, each l_t reached through its own update (t >= warm_end) and every later update's
+ *                     h/c chain inside [t0, t1): the states entering t0 are constants.  Two launches, deterministic.
+ *   l2o_minimax_image the forward's weight image of both nets from their torch-layout parameters (one launch).
+ *
+ * theta of one net, l2o_minimax_theta_count(H) = 12 H^2 + 25 H + 1 floats, in state_dict order: recurs.weight_ih
+ * [4H][2], recurs.weight_hh [4H][H], recurs.bias_ih [4H], recurs.bias_hh [4H], recurs2.weight_ih [4H][H],
+ * recurs2.weight_hh [4H][H], recurs2.bias_ih, recurs2.bias_hh, output.weight [H], output.bias [1] (gates i, f, g, o).
+ * Losses (MM ToyLoss, :612): 1 a u^2 - b v^2, 2 a u^2 - b v^2 + 2uv, 3 -b v sin(a pi u) (data [B][2] = (a, b),
+ * dim = 1), 4 u^T A v (data [B][dim][dim] = A).  L2O_E_UNSUPPORTED when H > 128, dim > 32 or losses 1-3 at dim > 1.
+ * Float pointers 4-byte aligned, double pointers 8-byte aligned (L2O_E_INVALID otherwise). */
+#define L2O_MINIMAX_MAX_HIDDEN 128
+#define L2O_MINIMAX_MAX_DIM 32
+typedef struct {
+  int32_t loss;            /* 1 .. 4 */
+  int32_t batch, dim, hidden;
+  int32_t t0, t1;          /* 1-based iterations run: 1 <= t0 < t1 */
+  int32_t warm_end;        /* >= 1: iterations t < warm_end take the sign step */
+  float out_mul, rescale;
+  const float* lr;         /* [warm_end - 1] sign-step sizes (required when t0 < warm_end) */
+  const float* theta;      /* [2][theta_count] torch-layout parameters (l2o_minimax_bwd) */
+  const float* image;      /* [2][l2o_minimax_image_floats] (l2o_minimax_fwd, l2o_minimax_bwd) */
+  const float* data;       /* losses 1-3: [B][2] (a, b); loss 4: [B][dim][dim] A */
+  float* u;                /* [R] in/out */
+  float* v;                /* [R] in/out */
+  float* state;            /* [2][4][R][H] in/out: h1, c1, h2, c2 of net 0, then of net 1 */
+  float* traj;             /* [t1-t0][R][2] out or NULL: u, v after each iteration */
+  float* ckpt;             /* [t1-t0][R][4H+2] out or NULL: the active net's inputs, h1, c1, h2, c2 before each
+                              iteration (required by the backward) */
+  float* dl;               /* [t1-t0][R] out or NULL: d l_t / d x_t of the updated x (required by the backward) */
+  float* lval;             /* [t1-t0][B] out or NULL: l_t of each problem */
+} l2o_minimax_args;
+typedef struct {
+  const float* coef;       /* [t1-t0] the weight of each l_t (0 where no gradient may pass) */
+  const float* weight;     /* [B] per-problem weights, or NULL: all 1 */
+  double* dtheta;          /* [2][theta_count] out (overwritten) */
+  void* scratch;           /* l2o_minimax_workspace_bytes */
+} l2o_minimax_grads;
+int64_t l2o_minimax_theta_count(int32_t hidden);
+int64_t l2o_minimax_image_floats(int32_t hidden);
+int l2o_minimax_image(const float* theta, float* image, int32_t hidden, void* stream);
+int l2o_minimax_workspace_bytes(const l2o_minimax_args* a, size_t* bytes);
+int l2o_minimax_fwd(const l2o_minimax_args* a, void* stream);
+int l2o_minimax_bwd(const l2o_minimax_args* a, const l2o_minimax_grads* g, void* stream);
+
 /* Number of this library's kernels launched so far in this process (bench.py's gpu_launches). */
 int64_t l2o_launch_count(void);
 const char* l2o_status_string(int status);

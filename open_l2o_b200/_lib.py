@@ -37,6 +37,8 @@ EXPORTS = [
     "l2o_tadam_theta_count", "l2o_tadam_state_floats", "l2o_tadam_step", "l2o_tadam_bwd", "l2o_lrsgd_step",
     "l2o_lrsgd_bwd",
     "l2o_ista_workspace_bytes", "l2o_ista_fwd", "l2o_ista_bwd", "l2o_ista_loss_grad",
+    "l2o_minimax_theta_count", "l2o_minimax_image_floats", "l2o_minimax_image", "l2o_minimax_workspace_bytes",
+    "l2o_minimax_fwd", "l2o_minimax_bwd",
 ]
 
 
@@ -156,6 +158,17 @@ class IstaLossArgs(C.Structure):
     _fields_ = [("task", C.c_int32), ("batch", C.c_int32), ("m", C.c_int32), ("n", C.c_int32), ("A", _fp),
                 ("y", _fp), ("ldy", C.c_int64), ("x_true", _fp), ("ldx", C.c_int64), ("x", _fp), ("lam", C.c_float),
                 ("d_x", _fp), ("loss", _fp)]
+
+
+class MinimaxArgs(C.Structure):
+    _fields_ = [("loss", C.c_int32), ("batch", C.c_int32), ("dim", C.c_int32), ("hidden", C.c_int32),
+                ("t0", C.c_int32), ("t1", C.c_int32), ("warm_end", C.c_int32), ("out_mul", C.c_float),
+                ("rescale", C.c_float), ("lr", _fp), ("theta", _fp), ("image", _fp), ("data", _fp), ("u", _fp),
+                ("v", _fp), ("state", _fp), ("traj", _fp), ("ckpt", _fp), ("dl", _fp), ("lval", _fp)]
+
+
+class MinimaxGrads(C.Structure):
+    _fields_ = [("coef", _fp), ("weight", _fp), ("dtheta", _fp), ("scratch", _fp)]
 
 
 class L2OError(RuntimeError):
@@ -311,6 +324,15 @@ def lib():
     L.l2o_ista_bwd.argtypes = [C.POINTER(IstaArgs), C.POINTER(IstaGrads), C.c_void_p]
     L.l2o_ista_loss_grad.argtypes = [C.POINTER(IstaLossArgs), C.c_void_p]
     for name in ("l2o_ista_workspace_bytes", "l2o_ista_fwd", "l2o_ista_bwd", "l2o_ista_loss_grad"):
+        getattr(L, name).restype = C.c_int
+    for name in ("l2o_minimax_theta_count", "l2o_minimax_image_floats"):
+        getattr(L, name).argtypes = [C.c_int32]
+        getattr(L, name).restype = C.c_int64
+    L.l2o_minimax_image.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
+    L.l2o_minimax_workspace_bytes.argtypes = [C.POINTER(MinimaxArgs), C.POINTER(C.c_size_t)]
+    L.l2o_minimax_fwd.argtypes = [C.POINTER(MinimaxArgs), C.c_void_p]
+    L.l2o_minimax_bwd.argtypes = [C.POINTER(MinimaxArgs), C.POINTER(MinimaxGrads), C.c_void_p]
+    for name in ("l2o_minimax_image", "l2o_minimax_workspace_bytes", "l2o_minimax_fwd", "l2o_minimax_bwd"):
         getattr(L, name).restype = C.c_int
     for name in ("l2o_status_string", "l2o_last_cuda_error", "l2o_version"):
         getattr(L, name).restype = C.c_char_p
