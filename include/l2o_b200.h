@@ -618,6 +618,71 @@ int l2o_minimax_workspace_bytes(const l2o_minimax_args* a, size_t* bytes);
 int l2o_minimax_fwd(const l2o_minimax_args* a, void* stream);
 int l2o_minimax_bwd(const l2o_minimax_args* a, const l2o_minimax_grads* g, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * The analytic families of L2O-Scale's problem zoo (SC/problems/problem_generator.py, SC/ =
+ * Model_Free_L2O/L2O-Scale/L2O-Scale-Training/): the objective and its gradient, or its Hessian times a vector, at
+ * one parameter vector x of n coordinates, in ONE launch.  Sums are fp64 in a fixed order (no atomics): the same
+ * input gives the same bits, eager or replayed from a CUDA graph.
+ *
+ *   l2o_zoo_value_grad  f(x) (fp64 sums, fp32 out) and out = df/dx    objective + tf.gradients (Problem.gradients, :329-350)
+ *   l2o_zoo_hvp         out = H(x) v, closed forms per family          tf.gradients(grads, params, grad_ys=v)
+ *
+ * Families (x flattened in the reference's parameter order):
+ *   QUADRATIC  0.5 ||A x - y||^2, A [n][n]            LASSO  QUADRATIC + p0 ||x||_1
+ *   BOWL       0.5 ||A x||^2, A [2][2] (y NULL)        NORM   (sum_i (|A x - y|_i + 1e-6)^p0)^(1/p0)
+ *   RASTRIGIN  mean_i(0.5 (A x - y)_i^2) - p0 c.cos(2 pi x) + p0 n^2   (y = b)
+ *   PROJECTION_QUADRATIC  sum_bi (x_i A_bi)^2           SUM_OF_QUADRATICS  sum_bi (x_i - A_bi)^2 - A_bi^2 + 1e-12
+ *   OUTWARD_SNAKE  sum_b A_b0 / (|x| + 1e-6) + sum_b,i>=1 ((x_i - pi cos x_(i-1)) A_bi)^2
+ *                  (A = the data batch [rows][n]: the three data families)
+ *   ISOTROPIC_QUADRATIC sum x^2   DEPENDENCY_CHAIN (n = ndim + 1)   MIN_MAX_WELL   and the 2-D test functions
+ *   ROSENBROCK .. MICHALEWICZ (n = 2).
+ * Matrix and data families with rows * n >= 65536 run on one cluster of 8 CTAs, each owning a block of A's rows (a
+ * row-block GEMV), the partial column sums exchanged through distributed shared memory and summed in rank order;
+ * every other problem runs on one CTA.  L2O_E_INVALID: NULL x / out (or v for l2o_zoo_hvp, A for the matrix and data
+ * families, y for QUADRATIC / LASSO / NORM / RASTRIGIN, c for RASTRIGIN), an unknown family, n or rows out of
+ * range for the family (matrix families: rows == n; BOWL and the 2-D functions: n == 2; DEPENDENCY_CHAIN,
+ * OUTWARD_SNAKE: n >= 2), NORM with p0 <= 0.  L2O_E_UNSUPPORTED: n > L2O_ZOO_MAX_N.
+ * The non-smooth points follow TensorFlow's gradients: sign(0) = 0 for |.|, sqrt'(0) = inf (Ackley at the origin,
+ * OUTWARD_SNAKE at x = 0 give NaN), ties of min / max share the gradient evenly. */
+#define L2O_ZOO_MAX_N 4096
+#define L2O_ZOO_QUADRATIC 0
+#define L2O_ZOO_LASSO 1
+#define L2O_ZOO_RASTRIGIN 2
+#define L2O_ZOO_BOWL 3
+#define L2O_ZOO_NORM 4
+#define L2O_ZOO_PROJECTION_QUADRATIC 5
+#define L2O_ZOO_SUM_OF_QUADRATICS 6
+#define L2O_ZOO_OUTWARD_SNAKE 7
+#define L2O_ZOO_ISOTROPIC_QUADRATIC 8
+#define L2O_ZOO_DEPENDENCY_CHAIN 9
+#define L2O_ZOO_MIN_MAX_WELL 10
+#define L2O_ZOO_ROSENBROCK 11
+#define L2O_ZOO_SADDLE 12
+#define L2O_ZOO_LOGSUMEXP 13
+#define L2O_ZOO_ACKLEY 14
+#define L2O_ZOO_BEALE 15
+#define L2O_ZOO_BOOTH 16
+#define L2O_ZOO_STYBLINSKI_TANG 17
+#define L2O_ZOO_MATYAS 18
+#define L2O_ZOO_BRANIN 19
+#define L2O_ZOO_MICHALEWICZ 20
+#define L2O_ZOO_NUM_FAMILIES 21
+typedef struct {
+  int32_t family;          /* L2O_ZOO_* */
+  int32_t n;               /* coordinates */
+  int32_t rows;            /* rows of A (matrix families: n, BOWL: 2; data families: the batch); else ignored */
+  float p0;                /* LASSO lambda, RASTRIGIN alpha, NORM power */
+  const float* x;          /* [n] */
+  const float* v;          /* [n] the direction (l2o_zoo_hvp) */
+  const float* A;          /* [rows][n] row-major: the matrix (W, BOWL's sqrt(H) R) or the data batch */
+  const float* y;          /* [rows] */
+  const float* c;          /* [n] RASTRIGIN's c */
+  float* f;                /* [1] out or NULL (l2o_zoo_value_grad) */
+  float* out;              /* [n] out: df/dx (l2o_zoo_value_grad) or H v (l2o_zoo_hvp) */
+} l2o_zoo_args;
+int l2o_zoo_value_grad(const l2o_zoo_args* a, void* stream);
+int l2o_zoo_hvp(const l2o_zoo_args* a, void* stream);
+
 /* Number of this library's kernels launched so far in this process (bench.py's gpu_launches). */
 int64_t l2o_launch_count(void);
 const char* l2o_status_string(int status);

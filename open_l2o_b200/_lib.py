@@ -39,6 +39,7 @@ EXPORTS = [
     "l2o_ista_workspace_bytes", "l2o_ista_fwd", "l2o_ista_bwd", "l2o_ista_loss_grad",
     "l2o_minimax_theta_count", "l2o_minimax_image_floats", "l2o_minimax_image", "l2o_minimax_workspace_bytes",
     "l2o_minimax_fwd", "l2o_minimax_bwd",
+    "l2o_zoo_value_grad", "l2o_zoo_hvp",
 ]
 
 
@@ -169,6 +170,18 @@ class MinimaxArgs(C.Structure):
 
 class MinimaxGrads(C.Structure):
     _fields_ = [("coef", _fp), ("weight", _fp), ("dtheta", _fp), ("scratch", _fp)]
+
+
+class ZooArgs(C.Structure):
+    _fields_ = [("family", C.c_int32), ("n", C.c_int32), ("rows", C.c_int32), ("p0", C.c_float), ("x", _fp),
+                ("v", _fp), ("A", _fp), ("y", _fp), ("c", _fp), ("f", _fp), ("out", _fp)]
+
+
+ZOO_MAX_N = 4096
+ZOO_FAMILIES = ["QUADRATIC", "LASSO", "RASTRIGIN", "BOWL", "NORM", "PROJECTION_QUADRATIC", "SUM_OF_QUADRATICS",
+                "OUTWARD_SNAKE", "ISOTROPIC_QUADRATIC", "DEPENDENCY_CHAIN", "MIN_MAX_WELL", "ROSENBROCK", "SADDLE",
+                "LOGSUMEXP", "ACKLEY", "BEALE", "BOOTH", "STYBLINSKI_TANG", "MATYAS", "BRANIN", "MICHALEWICZ"]
+ZOO = {name: i for i, name in enumerate(ZOO_FAMILIES)}   # the L2O_ZOO_* family ids
 
 
 class L2OError(RuntimeError):
@@ -333,6 +346,9 @@ def lib():
     L.l2o_minimax_fwd.argtypes = [C.POINTER(MinimaxArgs), C.c_void_p]
     L.l2o_minimax_bwd.argtypes = [C.POINTER(MinimaxArgs), C.POINTER(MinimaxGrads), C.c_void_p]
     for name in ("l2o_minimax_image", "l2o_minimax_workspace_bytes", "l2o_minimax_fwd", "l2o_minimax_bwd"):
+        getattr(L, name).restype = C.c_int
+    for name in ("l2o_zoo_value_grad", "l2o_zoo_hvp"):
+        getattr(L, name).argtypes = [C.POINTER(ZooArgs), C.c_void_p]
         getattr(L, name).restype = C.c_int
     for name in ("l2o_status_string", "l2o_last_cuda_error", "l2o_version"):
         getattr(L, name).restype = C.c_char_p
