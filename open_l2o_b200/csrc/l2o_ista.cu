@@ -50,6 +50,10 @@ __host__ __device__ inline Slice slice_of(int len, int c) {
   return {lo, min(len, lo + w)};
 }
 
+// The coupled form and LAMP apply W [M][N] to r_k (v_k); LISTA and LFISTA apply W [N][N] to x_k.
+__host__ __device__ inline bool w_on_r(const l2o_ista_args& a) {
+  return a.form == L2O_ISTA_COUPLED || a.form == L2O_ISTA_LAMP;
+}
 __device__ __forceinline__ const float* w_slot(const l2o_ista_args& a, int k) {
   if (a.form == L2O_ISTA_COUPLED) return a.W + (a.share_W ? 0 : (size_t)k * a.m * a.n);
   return a.W + (a.share_W ? 0 : (size_t)(k - 1) * a.n * a.n);
@@ -380,140 +384,6 @@ __global__ void __cluster_dims__(kCl, 1, 1) __launch_bounds__(kThreads) ista_bwd
   cl.sync();
 }
 
-// Weight slots of the gradient launch.  Returns the creation layer of slot g (its gradient multiplier's index) and
-// the range of pass layers [la, lb) that contribute to it; la >= lb: the slot's gradient is 0 in this pass.
-struct SlotInfo {
-  int birth, la, lb;
-};
-__host__ __device__ inline int w_slots(const l2o_ista_args& a) {
-  if (a.share_W) return 1;
-  return a.form == L2O_ISTA_COUPLED ? a.num_layers : a.num_layers - 1;
-}
-__device__ inline SlotInfo slot_info(const l2o_ista_args& a, int g) {
-  const int first = a.form == L2O_ISTA_COUPLED ? 0 : 1;   // the first layer with a W term
-  SlotInfo s;
-  if (a.share_W) {
-    s.birth = first;
-    s.la = max(a.k0, first) - a.k0;
-    s.lb = a.k1 - a.k0;
-  } else {
-    const int k = g + first;
-    s.birth = k;
-    s.la = k >= a.k0 && k < a.k1 ? k - a.k0 : 0;
-    s.lb = k >= a.k0 && k < a.k1 ? s.la + 1 : 0;
-  }
-  return s;
-}
-
-// blockIdx.y < w_slots: dW slot; == w_slots (LISTA): dB1; last: dtheta and ds (blockIdx.x = layer).
-// C[p][q] = scale * sum_{l in [la, lb)} c_l sum_b P_l[b][p] Q_l[b][q] over 64 x 64 tiles (4 x 4 per thread).
-__global__ void __launch_bounds__(kThreads) ista_grad_kernel(const Bwd p, int nblk_bwd) {
-  const l2o_ista_args& a = p.a;
-  const int M = a.m, N = a.n, B = a.batch;
-  const int nw = p.g.dW ? w_slots(a) : 0;
-  const int nb1 = a.form == L2O_ISTA_LISTA && p.g.dB1 ? 1 : 0;
-  const float* dzr = dz_rec(p);
-  const int y_slot = blockIdx.y;
-  if (y_slot == nw + nb1) {   // per-layer scalars
-    const int k = blockIdx.x;
-    if (k >= a.num_layers) return;
-    const float* part = part_rec(p);
-    __shared__ double acc[2][kWarps];
-    double t = 0.0, s = 0.0;
-    if (k >= a.k0 && k < a.k1)
-      for (int i = threadIdx.x; i < nblk_bwd; i += kThreads) {
-        t += part[((size_t)(k - a.k0) * nblk_bwd + i) * 2];
-        s += part[((size_t)(k - a.k0) * nblk_bwd + i) * 2 + 1];
-      }
-    for (int o = 16; o; o >>= 1) {
-      t += __shfl_xor_sync(0xffffffffu, t, o);
-      s += __shfl_xor_sync(0xffffffffu, s, o);
-    }
-    if ((threadIdx.x & 31) == 0) acc[0][threadIdx.x >> 5] = t, acc[1][threadIdx.x >> 5] = s;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      t = s = 0.0;
-      for (int w = 0; w < kWarps; ++w) t += acc[0][w], s += acc[1][w];
-      const double sc = p.g.gscale ? (double)p.g.gscale[k] : 1.0;
-      p.g.dtheta[k] = sc * t;
-      if (p.g.dstep) p.g.dstep[k] = sc * s;
-    }
-    return;
-  }
-  int Pd, Qd, la, lb, birth;
-  double* out;
-  const bool b1 = y_slot == nw;
-  if (b1) {   // dB1 [N][M] = sum_k dz_k^T y
-    Pd = N, Qd = M, la = 0, lb = a.k1 - a.k0, birth = 0;
-    out = p.g.dB1;
-  } else {
-    const SlotInfo si = slot_info(a, y_slot);
-    la = si.la, lb = si.lb, birth = si.birth;
-    if (a.form == L2O_ISTA_COUPLED) Pd = M, Qd = N;   // dW [M][N] = s r^T dz
-    else Pd = N, Qd = N;                              // dW [N][N] = s dz^T x
-    out = p.g.dW + (size_t)y_slot * Pd * Qd;
-  }
-  const int tiles_q = (Qd + kTile - 1) / kTile, tiles = tiles_q * ((Pd + kTile - 1) / kTile);
-  if ((int)blockIdx.x >= tiles) return;
-  const int p0 = (blockIdx.x / tiles_q) * kTile, q0 = (blockIdx.x % tiles_q) * kTile;
-  __shared__ float Ps[kChunk][kTile], Qs[kChunk][kTile];
-  const int tp = threadIdx.x / 16, tq = threadIdx.x % 16;
-  double acc[4][4] = {};   // per-layer fp32 sums, added across layers in fp64 (a shared W or B1 sums K of them)
-  for (int l = la; l < lb; ++l) {
-    float lacc[4][4] = {};
-    const int k = a.k0 + l;
-    const float coef = b1 ? 1.f : step_of(a, k);
-    for (int b0 = 0; b0 < B; b0 += kChunk) {
-      for (int e = threadIdx.x; e < kChunk * kTile; e += kThreads) {
-        const int bb = e / kTile, j = e % kTile, row = b0 + bb;
-        float pv = 0.f, qv = 0.f;
-        if (row < B) {
-          const float* dz = dzr + ((size_t)l * B + row) * N;
-          if (a.form == L2O_ISTA_COUPLED) {
-            if (p0 + j < Pd) pv = a.rs[((size_t)l * B + row) * M + p0 + j];
-            if (q0 + j < Qd) qv = dz[q0 + j];
-          } else {
-            if (p0 + j < Pd) pv = dz[p0 + j];
-            if (q0 + j < Qd) {
-              if (b1) qv = a.y[(size_t)row * a.ldy + q0 + j];
-              else {
-                const float* xin = layer_input(a, l, row);
-                qv = xin ? xin[q0 + j] : 0.f;
-              }
-            }
-          }
-        }
-        Ps[bb][j] = coef * pv;
-        Qs[bb][j] = qv;
-      }
-      __syncthreads();
-#pragma unroll
-      for (int bb = 0; bb < kChunk; ++bb) {
-        float pr[4], qr[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) pr[i] = Ps[bb][tp + 16 * i], qr[i] = Qs[bb][tq + 16 * i];
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-#pragma unroll
-          for (int j = 0; j < 4; ++j) lacc[i][j] = fmaf(pr[i], qr[j], lacc[i][j]);
-      }
-      __syncthreads();
-    }
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) acc[i][j] += (double)lacc[i][j];
-  }
-  const double sc = p.g.gscale && birth < a.num_layers ? (double)p.g.gscale[birth] : 1.0;
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int pp = p0 + tp + 16 * i, qq = q0 + tq + 16 * j;
-      if (pp < Pd && qq < Qd) out[(size_t)pp * Qd + qq] = sc * acc[i][j];
-    }
-}
-
 // Loss rows and dL/dx (MB/utils.py): sc  0.5 ||x - x_true||^2;  lasso 0.5 (0.5 ||x A^T - y||^2) + lam ||x||_1.
 __global__ void __launch_bounds__(kThreads) ista_loss_kernel(const l2o_ista_loss_args a) {
   extern __shared__ float4 smem_f4[];
@@ -553,7 +423,8 @@ __global__ void __launch_bounds__(kThreads) ista_loss_kernel(const l2o_ista_loss
 
 // ---------------------------------------------------------------------------------------------------------------
 // The two-state recurrences: LFISTA carries x_{k-1} besides x_k, LAMP carries v_{k-1} and a per-row threshold.
-// Their own kernels, on the helpers above, so the four forms' kernels stay as they are.
+// Their own forward and backward kernels, on the helpers above; the weight-gradient kernel further down serves every
+// form.
 //   LFISTA (MB/models/lfista.py)  z_k = y We^T + [k>=1] x_k Wg_k^T + [k>=2] x_{k-1} Wm_k^T,  x_{k+1} = shrink(z_k)
 //   LAMP   (MB/models/lamp.py)    v_k = y - x_k A^T + b_k v_{k-1}  (b_k = ||x_k||_0 / M, b_0 = 0),
 //                                 r_k = x_k + s_k v_k W_k,  x_{k+1} = shrink(r_k, max(sqrt(||v_k||^2 / M) lam_k, 0))
@@ -866,18 +737,51 @@ __global__ void __cluster_dims__(kCl, 1, 1) __launch_bounds__(kThreads) ista2_bw
   cl.sync();
 }
 
-// The gradient launch of the two-state forms.  blockIdx.y walks, in order: LFISTA the Wg slots (nw), the Wm slots
-// (nw2) and dWe, or LAMP the W slots (nw); then the per-layer scalars (blockIdx.x = layer).
-// LFISTA slot g belongs to layer g + 1: dWg = dz^T x_k, dWm = dz^T x_{k-1} (0 at layer 1, which has no Wm term);
-// dWe = sum_k dz_k^T y.  LAMP: dW_k = s_k v_k^T dr_k, over the layers of the pass when W is shared.
-__global__ void __launch_bounds__(kThreads) ista2_grad_kernel(const Bwd p, int nblk_bwd, int nw, int nw2) {
+// The weight slots of the gradient launch, in blockIdx.y order: the W slots (nw), LFISTA's Wm slots (nw2), then B1
+// (LFISTA: We).  Slot C [Pd][Qd] = gscale[birth] sum_{l in [la, lb)} c_l sum_b P_l[b][p] Q_l[b][q], c_l = s_k (1 for
+// B1), over the pass layers [la, lb) that have the slot's term (la >= lb: the slot's gradient is 0 in this pass):
+//   coupled, LAMP  dW_k = s_k r_k^T dz_k      (P = rs, Q = dz)
+//   LISTA, LFISTA  dW_k = s_k dz_k^T x_k      (P = dz, Q = x_k);   LFISTA dWm_k = dz_k^T x_{k-1}  (Q = x_{k-1})
+//   dB1 = sum_k dz_k^T y                      (P = dz, Q = y)
+enum : int { kRsDz, kDzX, kDzXm, kDzY };
+struct Slot {
+  double* out;
+  int Pd, Qd, la, lb, birth, op;
+};
+__host__ inline int w_slots(const l2o_ista_args& a) {
+  if (a.share_W) return 1;
+  return w_on_r(a) ? a.num_layers : a.num_layers - 1;
+}
+__device__ inline Slot grad_slot(const Bwd& p, int y, int nw, int nw2) {
+  const l2o_ista_args& a = p.a;
+  if (y >= nw + nw2) return {p.g.dB1, a.n, a.m, 0, a.k1 - a.k0, 0, kDzY};
+  const bool on_r = w_on_r(a), wm = y >= nw;
+  const int g = wm ? y - nw : y, first = on_r ? 0 : 1;   // first: the first layer with a W term
+  Slot s;
+  s.Pd = on_r ? a.m : a.n;
+  s.Qd = a.n;
+  s.op = on_r ? kRsDz : (wm ? kDzXm : kDzX);
+  s.out = (wm ? p.g.dW2 : p.g.dW) + (size_t)g * s.Pd * s.Qd;
+  if (a.share_W) {
+    s.birth = first;
+    s.la = max(a.k0, first) - a.k0;
+    s.lb = a.k1 - a.k0;
+  } else {
+    const int k = g + first;
+    const bool in = k >= a.k0 && k < a.k1 && (!wm || k >= 2);   // Wm_1 is never read
+    s.birth = k;
+    s.la = in ? k - a.k0 : 0;
+    s.lb = in ? s.la + 1 : 0;
+  }
+  return s;
+}
+
+// blockIdx.y < nw + nw2 + nb1: a weight slot, 64 x 64 output tiles (4 x 4 per thread); the last: dtheta and ds
+// (blockIdx.x = layer).  Held to 80 registers (3 CTAs per SM).
+__global__ void __launch_bounds__(kThreads, 3) ista_grad_kernel(const Bwd p, int nblk_bwd, int nw, int nw2, int nb1) {
   const l2o_ista_args& a = p.a;
   const int M = a.m, N = a.n, B = a.batch;
-  const bool lamp = a.form == L2O_ISTA_LAMP;
-  const int ne = lamp ? 0 : 1;
-  const float* dzr = dz_rec(p);
-  const int y_slot = blockIdx.y;
-  if (y_slot == nw + nw2 + ne) {   // per-layer scalars: dtheta (LAMP: dlam) and ds
+  if ((int)blockIdx.y == nw + nw2 + nb1) {   // per-layer scalars (LAMP: dlam)
     const int k = blockIdx.x;
     if (k >= a.num_layers) return;
     const float* part = part_rec(p);
@@ -903,55 +807,33 @@ __global__ void __launch_bounds__(kThreads) ista2_grad_kernel(const Bwd p, int n
     }
     return;
   }
-  // kind 0: LFISTA Wg / LAMP W;  1: LFISTA Wm;  2: LFISTA We
-  const int kind = y_slot < nw ? 0 : (y_slot < nw + nw2 ? 1 : 2);
-  const int g = kind == 0 ? y_slot : y_slot - nw;
-  int Pd = N, Qd = N, la = 0, lb = a.k1 - a.k0, birth = 0;
-  double* out;
-  if (kind == 2) {
-    Qd = M;
-    out = p.g.dB1;
-  } else if (lamp) {
-    const int k = a.share_W ? -1 : g;
-    Pd = M;
-    if (k >= 0) {
-      birth = k;
-      la = k >= a.k0 && k < a.k1 ? k - a.k0 : 0;
-      lb = k >= a.k0 && k < a.k1 ? la + 1 : 0;
-    }
-    out = p.g.dW + (size_t)g * M * N;
-  } else {
-    const int k = g + 1;
-    birth = k;
-    const bool in = k >= a.k0 && k < a.k1 && (kind == 0 || k >= 2);
-    la = in ? k - a.k0 : 0;
-    lb = in ? la + 1 : 0;
-    out = (kind == 0 ? p.g.dW : p.g.dW2) + (size_t)g * N * N;
-  }
+  const Slot sl = grad_slot(p, blockIdx.y, nw, nw2);
+  const int Pd = sl.Pd, Qd = sl.Qd;
+  const float* dzr = dz_rec(p);
   const int tiles_q = (Qd + kTile - 1) / kTile, tiles = tiles_q * ((Pd + kTile - 1) / kTile);
   if ((int)blockIdx.x >= tiles) return;
   const int p0 = (blockIdx.x / tiles_q) * kTile, q0 = (blockIdx.x % tiles_q) * kTile;
   __shared__ float Ps[kChunk][kTile], Qs[kChunk][kTile];
   const int tp = threadIdx.x / 16, tq = threadIdx.x % 16;
-  double acc[4][4] = {};   // per-layer fp32 sums, added across layers in fp64
-  for (int l = la; l < lb; ++l) {
+  double acc[4][4] = {};   // per-layer fp32 sums, added across layers in fp64 (a shared W or B1 sums K of them)
+  for (int l = sl.la; l < sl.lb; ++l) {
     float lacc[4][4] = {};
-    const float coef = lamp ? step_of(a, a.k0 + l) : 1.f;
+    const float coef = sl.op == kDzY ? 1.f : step_of(a, a.k0 + l);
     for (int b0 = 0; b0 < B; b0 += kChunk) {
       for (int e = threadIdx.x; e < kChunk * kTile; e += kThreads) {
         const int bb = e / kTile, j = e % kTile, row = b0 + bb;
         float pv = 0.f, qv = 0.f;
         if (row < B) {
           const float* dz = dzr + ((size_t)l * B + row) * N;
-          if (lamp) {
+          if (sl.op == kRsDz) {
             if (p0 + j < Pd) pv = a.rs[((size_t)l * B + row) * M + p0 + j];
             if (q0 + j < Qd) qv = dz[q0 + j];
           } else {
             if (p0 + j < Pd) pv = dz[p0 + j];
             if (q0 + j < Qd) {
-              if (kind == 2) qv = a.y[(size_t)row * a.ldy + q0 + j];
+              if (sl.op == kDzY) qv = a.y[(size_t)row * a.ldy + q0 + j];
               else {
-                const float* xin = kind == 0 ? layer_input(a, l, row) : layer_input2(a, l, row);
+                const float* xin = sl.op == kDzX ? layer_input(a, l, row) : layer_input2(a, l, row);
                 qv = xin ? xin[q0 + j] : 0.f;
               }
             }
@@ -978,13 +860,13 @@ __global__ void __launch_bounds__(kThreads) ista2_grad_kernel(const Bwd p, int n
 #pragma unroll
       for (int j = 0; j < 4; ++j) acc[i][j] += (double)lacc[i][j];
   }
-  const double sc = p.g.gscale && birth < a.num_layers ? (double)p.g.gscale[birth] : 1.0;
+  const double sc = p.g.gscale && sl.birth < a.num_layers ? (double)p.g.gscale[sl.birth] : 1.0;
 #pragma unroll
   for (int i = 0; i < 4; ++i)
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const int pp = p0 + tp + 16 * i, qq = q0 + tq + 16 * j;
-      if (pp < Pd && qq < Qd) out[(size_t)pp * Qd + qq] = sc * acc[i][j];
+      if (pp < Pd && qq < Qd) sl.out[(size_t)pp * Qd + qq] = sc * acc[i][j];
     }
 }
 
@@ -1013,27 +895,11 @@ int check_args(const l2o_ista_args* a) {
 }
 
 inline int clusters(const l2o_ista_args& a) { return (a.batch + kR - 1) / kR; }
+inline int tiles_of(int len) { return (len + kTile - 1) / kTile; }
 
 size_t scratch_bytes(const l2o_ista_args& a) {
   const size_t L = (size_t)(a.k1 - a.k0);
   return 4 * (L * a.batch * a.n + L * clusters(a) * kCl * 2);
-}
-
-int bwd_two_state(const Bwd& p, cudaStream_t stream) {
-  const l2o_ista_args& a = p.a;
-  const size_t smem = (size_t)smem_plan2(a).total * sizeof(float);
-  if (int rc = l2o::raise_smem_limit("l2o_ista_bwd", ista2_bwd_kernel, smem)) return rc;
-  const int nblk = clusters(a) * kCl;
-  ista2_bwd_kernel<<<nblk, kThreads, smem, stream>>>(p);
-  if (int rc = l2o::after_launch("l2o_ista_bwd")) return rc;
-  const bool lamp = a.form == L2O_ISTA_LAMP;
-  const int slots = lamp ? (a.share_W ? 1 : a.num_layers) : a.num_layers - 1;
-  const int nw = p.g.dW ? slots : 0, nw2 = !lamp && p.g.dW2 ? slots : 0, ne = lamp ? 0 : 1;
-  const int tq = (a.n + kTile - 1) / kTile;
-  const int tiles = std::max({tq * (((lamp ? a.m : a.n) + kTile - 1) / kTile), tq * ((a.m + kTile - 1) / kTile),
-                              a.num_layers});
-  ista2_grad_kernel<<<dim3(tiles, nw + nw2 + ne + 1), kThreads, 0, stream>>>(p, nblk, nw, nw2);
-  return l2o::after_launch("l2o_ista_bwd");
 }
 
 }  // namespace ista
@@ -1053,14 +919,10 @@ int l2o_ista_workspace_bytes(const l2o_ista_args* a, size_t* bytes) {
 int l2o_ista_fwd(const l2o_ista_args* a, void* stream) {
   if (int rc = check_args(a)) return rc;
   if (!a->xs) return L2O_E_INVALID;
+  const auto kernel = two_state(*a) ? ista2_fwd_kernel : ista_fwd_kernel;
   const size_t smem = (size_t)plan_floats(*a) * sizeof(float);
-  if (two_state(*a)) {
-    if (int rc = l2o::raise_smem_limit("l2o_ista_fwd", ista2_fwd_kernel, smem)) return rc;
-    ista2_fwd_kernel<<<clusters(*a) * kCl, kThreads, smem, (cudaStream_t)stream>>>(*a);
-    return l2o::after_launch("l2o_ista_fwd");
-  }
-  if (int rc = l2o::raise_smem_limit("l2o_ista_fwd", ista_fwd_kernel, smem)) return rc;
-  ista_fwd_kernel<<<clusters(*a) * kCl, kThreads, smem, (cudaStream_t)stream>>>(*a);
+  if (int rc = l2o::raise_smem_limit("l2o_ista_fwd", kernel, smem)) return rc;
+  kernel<<<clusters(*a) * kCl, kThreads, smem, (cudaStream_t)stream>>>(*a);
   return l2o::after_launch("l2o_ista_fwd");
 }
 
@@ -1079,18 +941,17 @@ int l2o_ista_bwd(const l2o_ista_args* a, const l2o_ista_grads* g, void* stream) 
   for (const void* q : f8)
     if (l2o::misaligned(q, 8)) return L2O_E_INVALID;
   Bwd p{*a, *g};
-  if (two_state(*a)) return bwd_two_state(p, (cudaStream_t)stream);
-  const size_t smem = (size_t)smem_plan(*a).total * sizeof(float);
-  if (int rc = l2o::raise_smem_limit("l2o_ista_bwd", ista_bwd_kernel, smem)) return rc;
+  const auto kernel = two_state(*a) ? ista2_bwd_kernel : ista_bwd_kernel;
+  const size_t smem = (size_t)plan_floats(*a) * sizeof(float);
+  if (int rc = l2o::raise_smem_limit("l2o_ista_bwd", kernel, smem)) return rc;
   const int nblk = clusters(*a) * kCl;
-  ista_bwd_kernel<<<nblk, kThreads, smem, (cudaStream_t)stream>>>(p);
+  kernel<<<nblk, kThreads, smem, (cudaStream_t)stream>>>(p);
   if (int rc = l2o::after_launch("l2o_ista_bwd")) return rc;
-  const int nw = g->dW ? w_slots(*a) : 0, nb1 = a->form == L2O_ISTA_LISTA ? 1 : 0;
-  const int pd = a->form == L2O_ISTA_COUPLED ? a->m : a->n;
-  int tiles = ((pd + kTile - 1) / kTile) * ((a->n + kTile - 1) / kTile);
-  if (nb1) tiles = std::max(tiles, ((a->n + kTile - 1) / kTile) * ((a->m + kTile - 1) / kTile));
-  tiles = std::max(tiles, a->num_layers);
-  ista_grad_kernel<<<dim3(tiles, nw + nb1 + 1), kThreads, 0, (cudaStream_t)stream>>>(p, nblk);
+  const int nw = g->dW ? w_slots(*a) : 0, nw2 = a->form == L2O_ISTA_LFISTA && g->dW2 ? w_slots(*a) : 0;
+  const int nb1 = a->form == L2O_ISTA_LISTA || a->form == L2O_ISTA_LFISTA ? 1 : 0;   // dB1 is required there
+  int tiles = std::max(tiles_of(w_on_r(*a) ? a->m : a->n) * tiles_of(a->n), a->num_layers);
+  if (nb1) tiles = std::max(tiles, tiles_of(a->n) * tiles_of(a->m));
+  ista_grad_kernel<<<dim3(tiles, nw + nw2 + nb1 + 1), kThreads, 0, (cudaStream_t)stream>>>(p, nblk, nw, nw2, nb1);
   return l2o::after_launch("l2o_ista_bwd");
 }
 
