@@ -683,6 +683,26 @@ typedef struct {
 int l2o_zoo_value_grad(const l2o_zoo_args* a, void* stream);
 int l2o_zoo_hvp(const l2o_zoo_args* a, void* stream);
 
+/* The Hessian form of k direction pairs (u_k, v_k) in ONE launch, closed forms per family:
+ *   q   = sum_k u_k^T H(x) v_k                 (fp64 sums, fp32 out; q may be NULL)
+ *   out = dq/dx = sum_k d3f(x)[u_k, v_k, .]    (exactly 0 for the families with a constant Hessian: QUADRATIC, LASSO,
+ *                                               BOWL, ISOTROPIC_QUADRATIC, PROJECTION_QUADRATIC, SUM_OF_QUADRATICS,
+ *                                               BOOTH, MATYAS, SADDLE)
+ * With U = V = Rademacher probes, q / k is Hutchinson's estimate of tr H and out / k its gradient; with k = 1 out is
+ * the x-adjoint of l2o_zoo_hvp (u = the adjoint of H v, v = the direction).  base carries the problem as for
+ * l2o_zoo_hvp (its v and f are not read; out receives dq/dx).  Same launch rule, argument rules and non-smooth
+ * conventions as l2o_zoo_hvp; in addition L2O_E_INVALID: NULL U, V or out, or k < 1; L2O_E_UNSUPPORTED:
+ * k > L2O_ZOO_MAX_PAIRS (q and out are sums over pairs: split k into chunks and add). */
+#define L2O_ZOO_MAX_PAIRS 10
+typedef struct {
+  l2o_zoo_args base;       /* the problem, x and out */
+  int32_t k;               /* direction pairs, 1 .. L2O_ZOO_MAX_PAIRS */
+  const float* U;          /* [k][n] */
+  const float* V;          /* [k][n]; may be U */
+  float* q;                /* [1] out or NULL */
+} l2o_zoo_form_args;
+int l2o_zoo_hess_form(const l2o_zoo_form_args* a, void* stream);
+
 /* Number of this library's kernels launched so far in this process (bench.py's gpu_launches). */
 int64_t l2o_launch_count(void);
 const char* l2o_status_string(int status);

@@ -39,7 +39,7 @@ EXPORTS = [
     "l2o_ista_workspace_bytes", "l2o_ista_fwd", "l2o_ista_bwd", "l2o_ista_loss_grad",
     "l2o_minimax_theta_count", "l2o_minimax_image_floats", "l2o_minimax_image", "l2o_minimax_workspace_bytes",
     "l2o_minimax_fwd", "l2o_minimax_bwd",
-    "l2o_zoo_value_grad", "l2o_zoo_hvp",
+    "l2o_zoo_value_grad", "l2o_zoo_hvp", "l2o_zoo_hess_form",
 ]
 
 
@@ -177,7 +177,12 @@ class ZooArgs(C.Structure):
                 ("v", _fp), ("A", _fp), ("y", _fp), ("c", _fp), ("f", _fp), ("out", _fp)]
 
 
+class ZooFormArgs(C.Structure):
+    _fields_ = [("base", ZooArgs), ("k", C.c_int32), ("U", _fp), ("V", _fp), ("q", _fp)]
+
+
 ZOO_MAX_N = 4096
+ZOO_MAX_PAIRS = 10
 ZOO_FAMILIES = ["QUADRATIC", "LASSO", "RASTRIGIN", "BOWL", "NORM", "PROJECTION_QUADRATIC", "SUM_OF_QUADRATICS",
                 "OUTWARD_SNAKE", "ISOTROPIC_QUADRATIC", "DEPENDENCY_CHAIN", "MIN_MAX_WELL", "ROSENBROCK", "SADDLE",
                 "LOGSUMEXP", "ACKLEY", "BEALE", "BOOTH", "STYBLINSKI_TANG", "MATYAS", "BRANIN", "MICHALEWICZ"]
@@ -350,6 +355,8 @@ def lib():
     for name in ("l2o_zoo_value_grad", "l2o_zoo_hvp"):
         getattr(L, name).argtypes = [C.POINTER(ZooArgs), C.c_void_p]
         getattr(L, name).restype = C.c_int
+    L.l2o_zoo_hess_form.argtypes = [C.POINTER(ZooFormArgs), C.c_void_p]
+    L.l2o_zoo_hess_form.restype = C.c_int
     for name in ("l2o_status_string", "l2o_last_cuda_error", "l2o_version"):
         getattr(L, name).restype = C.c_char_p
     L.l2o_status_string.argtypes = [C.c_int]

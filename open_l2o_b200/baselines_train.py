@@ -70,9 +70,10 @@ class _BaselineTrainer(MetaTrainerBase):
 
     def __init__(self, shapes: Sequence[Sequence[int]], theta: torch.Tensor, device="cuda:0", learning_rate=1e-6,
                  rms_decay=0.9, rms_epsilon=1e-20, gradient_clip=1e4, l2_reg=0.0, use_log_objective=True,
-                 use_numerator_epsilon=False, random_seed=None, use_second_derivatives=False):
+                 use_numerator_epsilon=False, random_seed=None, use_second_derivatives=False, **regularizer):
         super().__init__(shapes, theta, device, learning_rate, rms_decay, rms_epsilon, gradient_clip, l2_reg,
-                         use_log_objective, use_numerator_epsilon, None, random_seed, use_second_derivatives)
+                         use_log_objective, use_numerator_epsilon, None, random_seed, use_second_derivatives,
+                         **regularizer)
 
 
 class TrainableAdamTrainer(_BaselineTrainer):

@@ -145,10 +145,10 @@ class MetaTrainer(MetaTrainerBase):
     def __init__(self, shapes: Sequence[Sequence[int]], theta: Optional[torch.Tensor] = None, device="cuda:0",
                  learning_rate=1e-6, rms_decay=0.9, rms_epsilon=1e-20, gradient_clip=1e4, l2_reg=0.0,
                  use_log_objective=True, use_numerator_epsilon=False, init_lr_range=(1e-6, 1e-2), random_seed=None,
-                 use_second_derivatives=False):
+                 use_second_derivatives=False, **regularizer):
         super().__init__(shapes, _init_theta(random_seed) if theta is None else theta, device, learning_rate, rms_decay,
                          rms_epsilon, gradient_clip, l2_reg, use_log_objective, use_numerator_epsilon, init_lr_range,
-                         random_seed, use_second_derivatives)
+                         random_seed, use_second_derivatives, **regularizer)
         self.engine = _Engine(self.sizes, self.device)
 
     # ---- state ---------------------------------------------------------------------------------------------------

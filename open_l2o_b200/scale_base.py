@@ -20,6 +20,7 @@ import torch
 from . import _lib
 from ._lib import L2OError
 from .engine import _ptr, _stream
+from .scale_reg import Regularizer, check_options, reg_switch
 
 
 def theta_views(theta: torch.Tensor, spec: Sequence[Tuple[str, Tuple[int, ...]]]) -> Dict[str, torch.Tensor]:
@@ -219,12 +220,22 @@ class MetaTrainerBase(object):
     ``use_second_derivatives``: differentiate through the optimizee's gradients (the reference's
     ``TrainableOptimizer`` argument, default ``True`` there).  The trainers' default is ``False``, the first-order
     meta-gradient; the second-order one keeps the optimizee's double-backward graph of every step of an unroll alive
-    until the meta-gradient is taken."""
+    until the meta-gradient is taken.
+
+    The regularisers (``scale_reg``; all off by default, and off the trainer runs the plain loop):
+    ``reg_optimizee`` hands the optimizer the noise-free g~_t = d(f_t + beta reg_t)/dx_t instead of g_t (also in
+    ``evaluate``); ``reg_optimizer`` adds alpha sum_t reg_t to the scaled meta objective of the partial unrolls that
+    ``regularize_time`` / ``reg_scale`` switch on (``scale_reg.reg_switch``).  reg_t is ``reg_option`` at x_t with its
+    graph to x_t; imitation unrolls have no regulariser term."""
     what = ""
     theta_spec = None     # (name, shape) layout of theta for get_variables; None: one flat "theta"
+    regularizer = None    # a scale_reg.Regularizer when reg_optimizer or reg_optimizee is on
 
     def __init__(self, shapes, theta, device, learning_rate, rms_decay, rms_epsilon, gradient_clip, l2_reg,
-                 use_log_objective, use_numerator_epsilon, init_lr_range, random_seed, use_second_derivatives):
+                 use_log_objective, use_numerator_epsilon, init_lr_range, random_seed, use_second_derivatives,
+                 reg_optimizer=False, reg_optimizee=False, reg_option="hessian", hessian_itrs=10, alpha=5e-4,
+                 beta=1e-4, regularize_time="posterior", reg_scale=0.5):
+        check_options(reg_option, reg_optimizee, use_second_derivatives)
         if not torch.cuda.is_available():
             raise L2OError("%s meta-training needs a CUDA device (no CPU path)" % self.what)
         self.device = torch.device(device)
@@ -242,6 +253,10 @@ class MetaTrainerBase(object):
         self._gen = torch.Generator()
         if random_seed is not None:
             self._gen.manual_seed(int(random_seed))
+        self.reg_optimizer, self.reg_optimizee = bool(reg_optimizer), bool(reg_optimizee)
+        self.alpha, self.beta, self.regularize_time, self.reg_scale = alpha, beta, regularize_time, reg_scale
+        self.regularizer = Regularizer(reg_option, hessian_itrs, random_seed) \
+            if self.reg_optimizer or self.reg_optimizee else None
 
     def _split(self, flat):
         out, off = [], 0
@@ -280,9 +295,24 @@ class MetaTrainerBase(object):
             obj = obj.detach()
         return obj, (g if second else g.detach()).contiguous()
 
+    def _regularized_objective_and_gradient(self, objective: Callable, x: torch.Tensor):
+        """``_objective_and_gradient`` with the regulariser: (f(x_t), g, reg_t).  g is g~_t = d(f + beta reg)/dx_t
+        from the noise-free objective under ``reg_optimizee``, else the objective's own gradient; reg_t keeps its graph
+        to x_t when x_t depends on theta."""
+        second = self.use_second_derivatives and x.requires_grad
+        with torch.enable_grad():
+            xg = x if x.requires_grad else x.detach().requires_grad_(True)
+            obj = (getattr(objective, "clean", objective) if self.reg_optimizee else objective)(self._split(xg))
+            reg = self.regularizer(objective, xg, self._split, self._gen)
+            target = obj + self.beta * reg if self.reg_optimizee else obj
+            (g,) = torch.autograd.grad(target, xg, retain_graph=x.requires_grad, create_graph=second)
+        if not x.requires_grad:
+            obj, reg = obj.detach(), reg.detach()
+        return obj, (g if second else g.detach()).contiguous(), reg
+
     def unroll(self, objective: Callable, state, num_steps: int, theta: Optional[torch.Tensor] = None,
                obj_weights: Optional[Sequence[float]] = None, initial_obj: Optional[torch.Tensor] = None,
-               labels: Optional[torch.Tensor] = None, grads: Optional[torch.Tensor] = None):
+               labels: Optional[torch.Tensor] = None, grads: Optional[torch.Tensor] = None, regularize: bool = False):
         """``loop_body`` x num_steps (trainable_optimizer.py:263-401).  Returns (meta objective with its graph, the list
         of objective values, the final state with its graph).
 
@@ -291,12 +321,15 @@ class MetaTrainerBase(object):
         still drives its state, and the meta objective is ``sum_t w_t sum_i (upd_t,i - labels_t,i)^2 / 2 / N`` with
         ``w_t = 1 / num_steps`` by default (trainable_optimizer.py:383-389, SC/metaopt.py:407-408).  ``grads``
         ([num_steps, N]) are the optimizee gradients at the teacher-forced points, recorded by ``teacher_labels``: given,
-        the unroll replays them and evaluates no objective; None, it evaluates ``objective`` at each forced point."""
+        the unroll replays them and evaluates no objective; None, it evaluates ``objective`` at each forced point.
+
+        ``regularize``: this unroll adds alpha sum_t reg_t to its meta objective (with ``reg_optimizer``)."""
         if num_steps < 1:
             raise ValueError("an unroll needs at least one step")
         step = self._stepper(self.theta if theta is None else theta)
         x = state.x
-        objs, total = [], 0.0
+        objs, total, reg_total = [], 0.0, 0.0
+        regular = self.regularizer is not None and labels is None
         if obj_weights is not None:
             w = list(obj_weights)
         else:
@@ -305,7 +338,11 @@ class MetaTrainerBase(object):
             if grads is None:
                 # objective at x_t and its gradient: a constant of the meta-gradient (stop_gradient,
                 # trainable_optimizer.py:330-338) unless use_second_derivatives
-                obj, g = self._objective_and_gradient(objective, x)
+                if regular:
+                    obj, g, reg = self._regularized_objective_and_gradient(objective, x)
+                    reg_total = reg_total + reg
+                else:
+                    obj, g = self._objective_and_gradient(objective, x)
                 objs.append(obj)
             else:
                 g = grads[t]
@@ -323,16 +360,25 @@ class MetaTrainerBase(object):
         # normalised by the objective at the start of the SERIES of partial unrolls (trainable_optimizer.py:438-441)
         initial = objs[0].detach() if initial_obj is None else initial_obj
         meta = self.scale_objective(total, torch.stack([o.reshape(()) for o in objs]), initial)
+        if regular and regularize and self.reg_optimizer:   # added after scaling (trainable_optimizer.py:439-446)
+            meta = meta + self.alpha * reg_total
         return meta, objs, state
 
     # ---- meta step -------------------------------------------------------------------------------------------------
     def meta_gradient(self, objective: Callable, params: Sequence[torch.Tensor], num_steps: int,
                       log_learning_rate: Optional[torch.Tensor] = None, state=None,
-                      initial_obj: Optional[torch.Tensor] = None):
+                      initial_obj: Optional[torch.Tensor] = None, regularize: Optional[bool] = None):
         """(meta objective, d meta / d theta, objective values, final state) of one unroll — from ``params`` with a fresh
         optimizer state, or continuing from ``state`` (a detached state: truncated BPTT over partial unrolls).
-        ``log_learning_rate``: the initial learning-rate state handed to ``initial_state`` (drawn when None)."""
-        return self._meta_gradient(objective, params, num_steps, log_learning_rate, state, initial_obj=initial_obj)
+        ``log_learning_rate``: the initial learning-rate state handed to ``initial_state`` (drawn when None).
+        ``regularize``: whether the regulariser term is on for this unroll; None: ``regularize_time``'s rule for a
+        run of one unroll."""
+        if self.regularizer is None:
+            return self._meta_gradient(objective, params, num_steps, log_learning_rate, state, initial_obj=initial_obj)
+        if regularize is None:
+            regularize = reg_switch(self.regularize_time, 0, 1, self.reg_scale)
+        return self._meta_gradient(objective, params, num_steps, log_learning_rate, state, initial_obj=initial_obj,
+                                   regularize=regularize)
 
     def meta_gradient_mt(self, objective: Optional[Callable], params: Sequence[torch.Tensor], labels: torch.Tensor,
                          grads: Optional[torch.Tensor], log_learning_rate: Optional[torch.Tensor] = None, state=None):
@@ -389,9 +435,11 @@ class MetaTrainerBase(object):
     def _train_unrolls(self, objective, params, unroll_lens, log_learning_rate=None, obj_train_max_multiplier=-1.0):
         """``train_problem`` with one length per partial unroll."""
         state, initial, metas, values = None, None, [], []
-        for ln in unroll_lens:
+        for i, ln in enumerate(unroll_lens):
+            kw = {} if self.regularizer is None else \
+                dict(regularize=reg_switch(self.regularize_time, i, len(unroll_lens), self.reg_scale))
             meta, grad, objs, final = self.meta_gradient(objective, params, ln, log_learning_rate, state=state,
-                                                         initial_obj=initial)
+                                                         initial_obj=initial, **kw)
             if not all(math.isfinite(o) for o in objs):
                 break
             if initial is None:

@@ -35,6 +35,13 @@ _BOOL = dict(zero_init_lr_weights=True, use_relative_lr=True, use_extreme_indica
              use_grad_products=True, use_multiple_scale_decays=False, use_numerator_epsilon=False,
              learnable_inp_decay=True, learnable_rnn_init=True, if_cl=False, fix_unroll=False, if_mt=False)
 _INT["num_gradient_scales"] = 4
+# the regulariser (SC/optimizer/trainable_optimizer.py:34-41, problems/problem_generator.py:33-36, metaopt.py:63-66)
+_REG_BOOL = dict(reg_optimizer=False, reg_optimizee=False)
+_REG = dict(reg_option="hessian", hessian_itrs=10, alpha=5e-4, beta=1e-4, regularize_time="posterior", reg_scale=0.5)
+_INT["hessian_itrs"] = _REG["hessian_itrs"]
+_FLOAT.update(alpha=_REG["alpha"], beta=_REG["beta"], reg_scale=_REG["reg_scale"])
+_STR.update(reg_option=_REG["reg_option"], regularize_time=_REG["regularize_time"])
+_BOOL.update(_REG_BOOL)
 # HierarchicalRNN's constructor flags (SC/metarun.py:373-396)
 _HRNN_FLAGS = ("learnable_decay", "dynamic_output_scale", "use_attention", "use_log_objective", "num_gradient_scales",
                "zero_init_lr_weights", "use_log_means_squared", "use_relative_lr", "use_extreme_indicator",
@@ -159,6 +166,7 @@ def run(flags, out=sys.stdout, train_optimizer=None):
                           l2_reg=flags.l2_reg, rms_decay=flags.rms_decay, rms_epsilon=flags.rms_epsilon,
                           use_log_objective=flags.use_log_objective, use_numerator_epsilon=flags.use_numerator_epsilon,
                           use_second_derivatives=flags.use_second_derivatives, random_seed=flags.seed)
+    trainer_kwargs.update({name: getattr(flags, name) for name in list(_REG_BOOL) + list(_REG)})
 
     def make_trainer(shapes, theta):
         return opt.meta_trainer([torch.empty(s) for s in shapes], **trainer_kwargs)

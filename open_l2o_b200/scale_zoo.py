@@ -158,6 +158,23 @@ class ZooKernel(object):
         _lib.check(_lib.lib().l2o_zoo_hvp(C.byref(self.args(x, out, v=v)), _stream()), "l2o_zoo_hvp")
         return out
 
+    def hess_form(self, x, U, V=None):
+        """(q, dq/dx) with q = sum_k u_k^T H(x) v_k over the rows of U, V [k, n] (V None: V = U): one
+        ``l2o_zoo_hess_form`` launch per ``ZOO_MAX_PAIRS`` rows; the chunks' results are added."""
+        V = U if V is None else V
+        k, m = int(U.shape[0]), _lib.ZOO_MAX_PAIRS
+        q, out = None, None
+        for lo in range(0, k, m):
+            u = U[lo:lo + m].contiguous()
+            v = u if V is U else V[lo:lo + m].contiguous()
+            qc, oc = torch.empty((), device=x.device), torch.empty_like(x)
+            a = _lib.ZooFormArgs()
+            a.base = self.args(x, oc)
+            a.k, a.U, a.V, a.q = int(u.shape[0]), _ptr(u, name="U"), _ptr(v, name="V"), _ptr(qc, name="q")
+            _lib.check(_lib.lib().l2o_zoo_hess_form(C.byref(a), _stream()), "l2o_zoo_hess_form")
+            q, out = (qc, oc) if q is None else (q + qc, out + oc)
+        return q, out
+
 
 class _ZooValue(torch.autograd.Function):
     """f(x) from the kernel; backward: grad_out * g, with g a function of x whose backward is the kernel's H v."""
@@ -176,6 +193,8 @@ class _ZooValue(torch.autograd.Function):
 
 
 class _ZooGrad(torch.autograd.Function):
+    """g(x) = df/dx; backward: H(x) dg, itself differentiable in x and dg (``_ZooHvp``)."""
+
     @staticmethod
     def forward(ctx, x, g, z):
         ctx.save_for_backward(x)
@@ -183,10 +202,30 @@ class _ZooGrad(torch.autograd.Function):
         return g
 
     @staticmethod
-    @torch.autograd.function.once_differentiable
     def backward(ctx, dg):
         (x,) = ctx.saved_tensors
-        return ctx.z.hvp(x.detach().contiguous(), dg.contiguous()), None, None
+        return _ZooHvp.apply(x, dg, ctx.z), None, None
+
+
+class _ZooHvp(torch.autograd.Function):
+    """H(x) v from ``l2o_zoo_hvp``; backward: the x-adjoint d(u^T H v)/dx from ``l2o_zoo_hess_form`` (u = the
+    adjoint of H v) and the v-adjoint H u."""
+
+    @staticmethod
+    def forward(ctx, x, v, z):
+        ctx.save_for_backward(x, v)
+        ctx.z = z
+        return z.hvp(x.detach().contiguous(), v.detach().contiguous())
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, u):
+        x, v = ctx.saved_tensors
+        x, u = x.detach().contiguous(), u.contiguous()
+        dx = ctx.z.hess_form(x, u.view(1, -1), v.detach().contiguous().view(1, -1))[1] \
+            if ctx.needs_input_grad[0] else None
+        dv = ctx.z.hvp(x, u) if ctx.needs_input_grad[1] else None
+        return dx, dv, None
 
 
 def _flat(params):
@@ -729,17 +768,29 @@ class _GradNoise(torch.autograd.Function):
 def training_objective(problem: Problem, batch: Optional[Callable] = None, generator: Optional[torch.Generator] = None):
     """``objective(list of tensors) -> scalar`` for ``scale_base.train_optimizer``: the problem's objective at the
     batch ``batch()`` returns ((data, labels), or None for problems without data), with the problem's gradient noise
-    and dropout drawn from ``generator`` in the backward."""
+    and dropout drawn from ``generator`` in the backward.
+
+    For the regularisers (``scale_reg``), which need the noise-free gradient on the batch the step's objective saw, the
+    function also carries ``objective.problem``, ``objective.batch()`` (the last evaluation's (data, labels)) and
+    ``objective.clean(params)`` (the objective at a fresh batch without gradient noise or dropout)."""
     noisy = bool(problem.noise_stdev) or bool(problem.zero_probability)
     if noisy and generator is None:
         raise ValueError("a noisy or sparse-gradient problem needs a generator for its gradient noise")
+    last = [(None, None)]
 
-    def objective(params):
-        if noisy:
+    def evaluate(params, with_noise):
+        if with_noise:
             params = [_GradNoise.apply(p, float(problem.noise_stdev), float(problem.zero_probability), generator)
                       for p in params]
         data, labels = batch() if batch is not None else (None, None)
+        last[0] = (data, labels)
         return problem.objective(params, data, labels)
+
+    def objective(params):
+        return evaluate(params, noisy)
+    objective.problem = problem
+    objective.batch = lambda: last[0]
+    objective.clean = lambda params: evaluate(params, False)
     return objective
 
 
