@@ -15,9 +15,9 @@ backward 12 (g, d_update read, d_g written).  The HBM figure is the H100 SXM dat
 Prints one JSON line; the card name and power limit come from a read-only nvidia-smi query in the same run.
 """
 import argparse
-import json
 import math
 import os
+import statistics
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -25,7 +25,7 @@ sys.path.insert(0, ROOT)
 
 import torch  # noqa: E402
 
-from scripts.crnn_profile import card, time_ms  # noqa: E402
+from scripts.measure import alternate, card, emit, event_ms, graph_ms  # noqa: E402
 
 TADAM_FWD, TADAM_BWD, LRS_FWD, LRS_BWD = 36, 44, 12, 12
 HBM = 3.35e12
@@ -43,37 +43,6 @@ def torch_tadam_step(theta, g, st, x):
     x.sub_(upd)
 
 
-def graph_ms(fn, reps, replays=5):
-    """Device time per call of `fn`: `reps` calls captured into one CUDA graph, replayed `replays` times between CUDA
-    events (after a warm-up replay).  Launching from Python costs more than these kernels take at the ConvNet size, so
-    events around eager launches would time the host."""
-    for _ in range(3):
-        fn()
-    torch.cuda.synchronize()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        for _ in range(reps):
-            fn()
-    g.replay()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(replays):
-        g.replay()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / (reps * replays)
-
-
-def alternate(fa, fb, reps, rounds=5):
-    """Median per-call device times of fa and fb over `rounds` alternated windows."""
-    ta, tb = [], []
-    for _ in range(rounds):
-        ta.append(graph_ms(fa, reps))
-        tb.append(graph_ms(fb, reps))
-    return sorted(ta)[rounds // 2], sorted(tb)[rounds // 2]
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=50)
@@ -89,8 +58,7 @@ def main():
     from tests.helpers import HRNN_CONVNET
     import ctypes as C
     dev = "cuda:0"
-    name, power, clock = card()
-    res = dict(card=name, power_limit=power, max_sm_clock=clock, reps=args.reps)
+    res = dict(card=card(), reps=args.reps)
     net = ConvNet(*HRNN_CONVNET)
     n_conv = sum(int(math.prod(s)) for s in net.param_shapes)
     gen = torch.Generator(device=dev).manual_seed(0)
@@ -108,8 +76,10 @@ def main():
         torch.cuda.synchronize()
         rel = lambda a, b: float((a - b).abs().max() / b.abs().max())
         cmp = dict(x=rel(xa, xb), m=rel(sa[0], sb[0]), t=rel(sa[1], sb[1]), v=float((sa[2] - sb[2]).abs().max()))
-        k_ms, t_ms = alternate(lambda: tadam_step_launch(theta, g, sa, sa, x=xa), lambda: torch_tadam_step(theta, g, sb, xb),
-                               args.reps)
+        kernel_ms = lambda fn: graph_ms(fn, args.reps, 5, 3)   # noqa: E731
+        t = alternate({"kernel": lambda: tadam_step_launch(theta, g, sa, sa, x=xa),
+                       "torch": lambda: torch_tadam_step(theta, g, sb, xb)}, 5, kernel_ms)
+        k_ms, t_ms = statistics.median(t["kernel"]), statistics.median(t["torch"])
         d_new, d_upd = torch.randn(3, n, device=dev, generator=gen), torch.randn(n, device=dev, generator=gen)
         d_old, d_g = torch.empty(3, n, device=dev), torch.empty(n, device=dev)
         d_theta = torch.zeros(4, dtype=torch.float64, device=dev)
@@ -117,13 +87,13 @@ def main():
         planes[0].normal_(generator=gen)
         ba = _lib.TadamBwdArgs(n=n, theta=_p(theta), g=_p(g), state_old=_p(planes), d_state_new=_p(d_new),
                                d_update=_p(d_upd), d_state_old=_p(d_old), d_theta=d_theta.data_ptr(), d_g=_p(d_g))
-        b_ms = graph_ms(lambda: L.l2o_tadam_bwd(C.byref(ba), _stream()), args.reps)
+        b_ms = kernel_ms(lambda: L.l2o_tadam_bwd(C.byref(ba), _stream()))
         rates, itr = torch.full((1000,), 1e-3, device=dev), torch.zeros(2, dtype=torch.int32, device=dev)
-        ls_ms = graph_ms(lambda: lrsgd_step_launch(rates, g, itr=itr, x=xa), args.reps)
+        ls_ms = kernel_ms(lambda: lrsgd_step_launch(rates, g, itr=itr, x=xa))
         d_rates = torch.zeros(1000, dtype=torch.float64, device=dev)
         la = _lib.LrsgdBwdArgs(n=n, rates=_p(rates), n_steps=1000, itr=_p(itr, torch.int32), g=_p(g), d_update=_p(d_upd),
                                d_rates=d_rates.data_ptr(), d_g=_p(d_g))
-        lb_ms = graph_ms(lambda: L.l2o_lrsgd_bwd(C.byref(la), _stream()), args.reps)
+        lb_ms = kernel_ms(lambda: L.l2o_lrsgd_bwd(C.byref(la), _stream()))
         tb = lambda b, ms: n * b / ms / 1e9
         res[tag] = dict(n=n, tadam_step_ms=k_ms, tadam_step_TBps=tb(TADAM_FWD, k_ms),
                         tadam_step_hbm_share=tb(TADAM_FWD, k_ms) * 1e12 / HBM,
@@ -147,14 +117,10 @@ def main():
         for second in (False, True):
             tr = cls(shapes, theta=th, device=dev, use_second_derivatives=second)
             torch.cuda.reset_peak_memory_stats()
-            ms20 = time_ms(lambda: tr.meta_gradient(obj, p0, 20), max(3, args.reps // 10), warmup=1)
+            ms20 = event_ms(lambda: tr.meta_gradient(obj, p0, 20), max(3, args.reps // 10), 1)
             res["meta_gradient_T20_convnet_%s_%s" % (nm, "second" if second else "first")] = dict(
                 ms=ms20, peak_GB=torch.cuda.max_memory_allocated() / 1e9)
-    line = json.dumps(res)
-    print(line)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        open(os.path.join(args.out, "baselines_profile.json"), "w").write(line + "\n")
+    emit(res, args.out and os.path.join(args.out, "baselines_profile.json"))
 
 
 if __name__ == "__main__":

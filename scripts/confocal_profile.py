@@ -10,24 +10,16 @@ producer against torch autograd of the same loss.
     program past its two eager warm-up unrolls and CUDA-graph capture, --unrolls timed unrolls per round, alternated.
 The card's name and power limit are read in the same run."""
 import argparse
-import json
 import os
 import statistics
-import subprocess
 import sys
-import time
 
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from open_l2o_b200 import engine, meta, util  # noqa: E402
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader",
-                        "-i", str(torch.cuda.current_device())], capture_output=True, text=True)
-    return {"device": torch.cuda.get_device_name(), "nvidia_smi": q.stdout.strip()}
+from scripts.measure import alternate, card, emit, event_ms, wall_ms  # noqa: E402
 
 
 def program(fused, T):
@@ -40,18 +32,6 @@ def program(fused, T):
     sess = meta.Session()
     sess.run(ms.reset)
     return prog, sess, ms
-
-
-def time_calls(fn, n):
-    fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(n):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / n
 
 
 def main():
@@ -77,26 +57,18 @@ def main():
     f_a, g_a = autograd()
     agree = {"f_rel": abs(float(f_k) - float(f_a)) / abs(float(f_a)),
              "g_rel_maxnorm": float((g_k - g_a).abs().max() / g_a.abs().max())}
-    step = {"kernel_ms": [], "autograd_ms": []}
-    for _ in range(args.rounds):
-        step["kernel_ms"].append(time_calls(kernel, args.launches))
-        step["autograd_ms"].append(time_calls(autograd, args.launches))
+    step = alternate({"kernel_ms": kernel, "autograd_ms": autograd}, args.rounds,
+                     lambda fn: event_ms(fn, args.launches, 1))
 
     # (b) training unrolls
     def unroll(sess, ms):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        sess.run([ms.fx, ms.update, ms.step])
-        torch.cuda.synchronize()
-        return 1e3 * (time.perf_counter() - t0)
+        return wall_ms(lambda: sess.run([ms.fx, ms.update, ms.step]))
 
     for _ in range(3):   # two eager unrolls, then the capture of each program's graph
         unroll(sf, mf)
         unroll(sa, ma)
-    train = {"producer_unroll_ms": [], "autograd_unroll_ms": []}
-    for _ in range(args.rounds):
-        train["producer_unroll_ms"].append(statistics.median(unroll(sf, mf) for _ in range(args.unrolls)))
-        train["autograd_unroll_ms"].append(statistics.median(unroll(sa, ma) for _ in range(args.unrolls)))
+    train = alternate({"producer_unroll_ms": lambda: unroll(sf, mf), "autograd_unroll_ms": lambda: unroll(sa, ma)},
+                      args.rounds, lambda fn: statistics.median(fn() for _ in range(args.unrolls)))
 
     med = {k: statistics.median(v) for k, v in list(step.items()) + list(train.items())}
     res = {"card": card(), "shape": {"batch": B, "num_points": P, "roi": list(roi), "T": T},
@@ -104,10 +76,7 @@ def main():
            "step": step, "train_unroll": train, "median": med,
            "speedup": {"step": med["autograd_ms"] / med["kernel_ms"],
                        "train_unroll": med["autograd_unroll_ms"] / med["producer_unroll_ms"]}}
-    os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-    with open(args.out, "w") as f:
-        json.dump(res, f, indent=1)
-    print(json.dumps(res))
+    emit(res, args.out)
 
 
 if __name__ == "__main__":

@@ -12,9 +12,7 @@ MACs + 60 readout MACs.  Roofline figures are the H100 SXM data sheet's (3.35 TB
 Prints one JSON line; the card name and power limit come from a read-only nvidia-smi query in the same run.
 """
 import argparse
-import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -22,31 +20,11 @@ sys.path.insert(0, ROOT)
 
 import torch  # noqa: E402
 
+from scripts.measure import card, emit, event_ms  # noqa: E402
+
 FWD_BYTES, BWD_BYTES = 836, 4 * (103 + 103 + 1 + 1 + 103)
 FWD_FLOPS = 2 * (11 * 40 + 31 * 80 + 41 * 80 + 60)
 HBM, FP32 = 3.35e12, 67e12
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        return [s.strip() for s in q.split(",")]
-    except Exception as e:   # the numbers below still stand; say that the card could not be read
-        return ["unknown (%r)" % (e,), "", ""]
-
-
-def time_ms(fn, reps, warmup=5):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(reps):
-        fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / reps
 
 
 def main():
@@ -61,8 +39,7 @@ def main():
     from open_l2o_b200.scale_problems import ConvNet
     from tests.helpers import HRNN_CONVNET
     dev = "cuda:0"
-    name, power, clock = card()
-    res = dict(card=name, power_limit=power, max_sm_clock=clock, reps=args.reps)
+    res = dict(card=card(), reps=args.reps)
     n_conv = sum(int(torch.tensor(s).prod()) for s in ConvNet(*HRNN_CONVNET).param_shapes)
     gen = torch.Generator(device=dev).manual_seed(0)
     for tag, n in (("convnet", n_conv), ("32M", 32 * 2 ** 20)):
@@ -70,7 +47,7 @@ def main():
         x = torch.randn(n, device=dev, generator=gen)
         g = torch.randn(n, device=dev, generator=gen) * 0.1
         opt.apply_gradients([(g, x)])
-        ms = time_ms(lambda: step_launch(opt.theta, g, opt.state, opt.state, x=opt.x), args.reps)
+        ms = event_ms(lambda: step_launch(opt.theta, g, opt.state, opt.state, x=opt.x), args.reps, 5)
         res["fwd_%s" % tag] = dict(n=n, ms=ms, coord_per_s=n / ms * 1e3, achieved_TBps=n * FWD_BYTES / ms / 1e9,
                                    hbm_share=n * FWD_BYTES / ms * 1e3 / HBM,
                                    fp32_share=n * FWD_FLOPS / ms * 1e3 / FP32)
@@ -95,19 +72,15 @@ def main():
         ctx.saved_tensors = (th, planes, g)
         ctx.needs_input_grad = (True, True, False)
         ct._Step.backward(ctx, d_new, d_upd)
-    f_ms, b_ms = time_ms(fwd, args.reps), time_ms(bwd, args.reps)
+    f_ms, b_ms = event_ms(fwd, args.reps, 5), event_ms(bwd, args.reps, 5)
     res["train_step_convnet"] = dict(n=n, fwd_ms=f_ms, bwd_ms=b_ms, bwd_achieved_TBps=n * BWD_BYTES / b_ms / 1e9)
     # T = 20 unroll + meta-gradient on a quadratic over the ConvNet coordinate count
     tgt = torch.randn(n, device=dev, generator=gen)
     obj = lambda ps: ((ps[0] - tgt) ** 2).mean()
     p0 = [torch.randn(n, device=dev, generator=gen)]
-    ms20 = time_ms(lambda: tr.meta_gradient(obj, p0, 20), max(3, args.reps // 10), warmup=1)
+    ms20 = event_ms(lambda: tr.meta_gradient(obj, p0, 20), max(3, args.reps // 10), 1)
     res["meta_gradient_T20_convnet_ms"] = ms20
-    line = json.dumps(res)
-    print(line)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        open(os.path.join(args.out, "crnn_profile.json"), "w").write(line + "\n")
+    emit(res, args.out and os.path.join(args.out, "crnn_profile.json"))
 
 
 if __name__ == "__main__":

@@ -7,10 +7,8 @@ the card's name and power limit read in the same run.
     python scripts/lista_profile.py [--reps 5] [--iters 50]
 """
 import argparse
-import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
@@ -21,6 +19,7 @@ sys.path.insert(0, ROOT)
 from open_l2o_b200 import lista, lista_train as lt  # noqa: E402
 from open_l2o_b200.engine import adam_step  # noqa: E402
 from oracle import lista_oracle as lo  # noqa: E402
+from scripts.measure import alternate, card, emit, event_ms, graphed  # noqa: E402
 from tests import lfista_lamp_cases as fc  # noqa: E402
 
 M, N, K = 256, 512, 16
@@ -84,37 +83,6 @@ class TorchVersion:
             return self.forward(data)[-1]
 
 
-def timed(fn, iters):
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    fn()
-    torch.cuda.synchronize()
-    s.record()
-    for _ in range(iters):
-        fn()
-    e.record()
-    torch.cuda.synchronize()
-    return s.elapsed_time(e) * 1e3 / iters   # us
-
-
-def graphed(fn):
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(2):
-            fn()
-    torch.cuda.current_stream().wait_stream(s)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        fn()
-    return g.replay
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return {"torch_name": torch.cuda.get_device_name(0), "nvidia_smi": q.stdout.strip()}
-
-
 def profile(name, reps, iters):
     d = lista.make_data(M, N, (B_TRAIN, B_VAL, 1), seed=0)
     A = d["A"]
@@ -156,11 +124,9 @@ def profile(name, reps, iters):
 
     t_step, t_val = (lambda: tv.train_step(train)), (lambda: tv.val_pass(val))
     fns = {"kernel_step": k_step, "kernel_val": k_val, "torch_eager_step": t_step, "torch_eager_val": t_val,
-           "torch_graph_step": graphed(t_step), "torch_graph_val": graphed(t_val), "kernel_graph_step": graphed(k_step)}
-    res = {k: [] for k in fns}
-    for _ in range(reps):            # alternate the versions within each repetition
-        for k, f in fns.items():
-            res[k].append(timed(f, iters))
+           "torch_graph_step": graphed(t_step, 2), "torch_graph_val": graphed(t_val, 2),
+           "kernel_graph_step": graphed(k_step, 2)}
+    res = alternate(fns, reps, lambda f: 1e3 * event_ms(f, iters, 1))   # us
     m.params.copy_(start)
     out = {k: statistics.median(v) for k, v in res.items()}
     out["spread"] = {k: [min(v), max(v)] for k, v in res.items()}
@@ -195,10 +161,7 @@ def main():
               % (name, r["kernel_step"], r["torch_graph_step"], r["torch_eager_step"], r["kernel_val"],
                  r["torch_graph_val"], r["torch_eager_val"]), r["outputs"], flush=True)
     rec["card_after"] = card()
-    os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-    with open(a.out, "w") as f:
-        json.dump(rec, f, indent=1)
-    print(json.dumps(rec["card"]))
+    emit(rec, a.out)
 
 
 if __name__ == "__main__":

@@ -8,11 +8,9 @@ torch's.  Writes scripts/minimax_profile_h100.json (or --out) with the card's na
     python scripts/minimax_profile.py [--reps 5] [--iters 5]
 """
 import argparse
-import json
 import math
 import os
 import statistics
-import subprocess
 import sys
 
 import numpy as np
@@ -22,6 +20,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from open_l2o_b200 import minimax as mm, minimax_train as tr  # noqa: E402
+from scripts.measure import alternate, card, emit, event_ms, graphed  # noqa: E402
 
 CONFIGS = {"seesaw": dict(loss=3, hidden=50, dim=1), "matrix_game_dim5": dict(loss=4, hidden=80, dim=5)}
 B_TRAIN, B_EVAL, TRAIN_IT, EVAL_IT, UNROLL, META_LR, RESCALE = 128, 20, 100, 1000, 5, 1e-4, 1e-4
@@ -93,37 +92,6 @@ class TorchTwin:
         return u.detach(), v.detach()
 
 
-def timed(fn, iters):
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    fn()
-    torch.cuda.synchronize()
-    s.record()
-    for _ in range(iters):
-        fn()
-    e.record()
-    torch.cuda.synchronize()
-    return s.elapsed_time(e) / iters   # ms
-
-
-def graphed(fn):
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(2):
-            fn()
-    torch.cuda.current_stream().wait_stream(s)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        fn()
-    return g.replay
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return {"torch_name": torch.cuda.get_device_name(0), "nvidia_smi": q.stdout.strip()}
-
-
 def problems(loss, dim, B, seed):
     if loss == 4:
         return mm.make_matrix_game_data(dim, 0.5, 0.5, 1.0, B, seed)
@@ -173,11 +141,8 @@ def profile(name, reps, iters):
                 a, b = tt.do_fit(u0, v0, s0, it, train)
             tu.copy_(a), tv.copy_(b)
 
-        fns = {"kernel": k_run, "torch_eager": t_run, "torch_graph": graphed(t_run)}
-        res = {k: [] for k in fns}
-        for _ in range(reps):   # alternate the versions within each repetition
-            for k, f in fns.items():
-                res[k].append(timed(f, iters))
+        fns = {"kernel": k_run, "torch_eager": t_run, "torch_graph": graphed(t_run, 2)}
+        res = alternate(fns, reps, lambda f: event_ms(f, iters, 1))
         twin.theta.copy_(th0)
         twin.refresh()
         r = {k: statistics.median(v) for k, v in res.items()}
@@ -209,10 +174,7 @@ def main():
             print("%-17s %-5s kernel %8.3f ms  torch graph %8.3f  eager %8.3f" %
                   (name, mode, m["kernel"], m["torch_graph"], m["torch_eager"]), m["outputs"], flush=True)
     rec["card_after"] = card()
-    os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-    with open(a.out, "w") as f:
-        json.dump(rec, f, indent=1)
-    print(json.dumps(rec["card"]))
+    emit(rec, a.out)
 
 
 if __name__ == "__main__":

@@ -10,12 +10,9 @@ N that an imitation step adds (upd - label, its square-sum, x - label) for all T
 imitation meta-gradient is compared with one that re-evaluates the objective at the teacher-forced points.  The
 card's name and power limit are read in the same run."""
 import argparse
-import json
 import os
 import statistics
-import subprocess
 import sys
-import time
 
 import torch
 
@@ -24,22 +21,9 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from open_l2o_b200 import hrnn_train as ht  # noqa: E402
 from open_l2o_b200.scale_base import teacher_labels  # noqa: E402
 from open_l2o_b200.scale_problems import ConvNet  # noqa: E402
+from scripts.measure import alternate, card, emit, event_ms, wall_ms  # noqa: E402
 
 DEV = "cuda:0"
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader",
-                        "-i", str(torch.cuda.current_device())], capture_output=True, text=True)
-    return {"device": torch.cuda.get_device_name(), "nvidia_smi": q.stdout.strip()}
-
-
-def timed(fn):
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    fn()
-    torch.cuda.synchronize()
-    return 1e3 * (time.perf_counter() - t0)
 
 
 def main():
@@ -88,27 +72,15 @@ def main():
 
     for fn in (first_order, imitation, teacher, passes):   # warm-up of every shape
         fn()
-    times = {"first_order_ms": [], "imitation_ms": [], "teacher_labels_ms": []}
-    for _ in range(args.rounds):
-        times["first_order_ms"].append(statistics.median(timed(first_order) for _ in range(args.steps)))
-        times["imitation_ms"].append(statistics.median(timed(imitation) for _ in range(args.steps)))
-        times["teacher_labels_ms"].append(timed(teacher))
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.synchronize()
-    e0.record()
-    for _ in range(10):
-        passes()
-    e1.record()
-    torch.cuda.synchronize()
+    times = alternate({"first_order_ms": first_order, "imitation_ms": imitation, "teacher_labels_ms": teacher},
+                      args.rounds,
+                      lambda fn: statistics.median(wall_ms(fn) for _ in range(1 if fn is teacher else args.steps)))
     med = {k: statistics.median(v) for k, v in times.items()}
-    med["mt_passes_ms_per_unroll"] = e0.elapsed_time(e1) / 10
+    med["mt_passes_ms_per_unroll"] = event_ms(passes, 10, 0)
     res = {"card": card(), "shape": {"coordinates": N, "tensors": len(params0), "T": T, "batch": 128},
            "replay_vs_reevaluation": agree, "rounds": times, "median": med,
            "imitation_over_first_order": med["imitation_ms"] / med["first_order_ms"]}
-    os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-    with open(args.out, "w") as f:
-        json.dump(res, f, indent=1)
-    print(json.dumps(res))
+    emit(res, args.out)
 
 
 if __name__ == "__main__":

@@ -14,10 +14,8 @@ time is wall time up to a device synchronise).  Writes ``scale_reg_profile_h100.
     python scripts/scale_reg_profile.py [--reps 5] [--out path]
 """
 import argparse
-import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
@@ -27,40 +25,10 @@ sys.path.insert(0, ROOT)
 
 from open_l2o_b200 import hrnn_train as ht  # noqa: E402
 from open_l2o_b200 import scale_zoo as Z  # noqa: E402
+from scripts.measure import alternate, card, emit, event_ms  # noqa: E402
 
 DEV = "cuda"
 OPTIONS = ("hessian", "jacob", "hessian-ev", "hessian-esd")
-
-
-def gpu_info():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        q = ""
-    return {"device": torch.cuda.get_device_name(0), "nvidia_smi": q}
-
-
-def timed(fn, inner):
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(inner):
-        fn()
-    b.record()
-    b.synchronize()
-    return a.elapsed_time(b) / inner
-
-
-def alternate(variants, reps, inner, warm=2):
-    for fn in variants.values():
-        for _ in range(warm):
-            fn()
-    torch.cuda.synchronize()
-    times = {k: [] for k in variants}
-    for _ in range(reps):
-        for k, fn in variants.items():
-            times[k].append(timed(fn, inner))
-    return {k: statistics.median(v) for k, v in times.items()}
 
 
 def meta_step(problem, objective, option):
@@ -80,7 +48,7 @@ def main():
     ap.add_argument("--out", default=os.path.join(os.path.dirname(os.path.abspath(__file__)),
                                                   "scale_reg_profile_h100.json"))
     a = ap.parse_args()
-    res = {"gpu": gpu_info(), "reps": a.reps, "meta_step_ms": {}, "hess_form_ms": {}}
+    res = {"gpu": card(), "reps": a.reps, "meta_step_ms": {}, "hess_form_ms": {}}
     sets = {"optimization_test": Z.optimization_test_problems(), "quadratic": Z.quadratic_problems(),
             "large_quadratic": Z.quadratic_problems_large()}
     for set_name, entries in sets.items():
@@ -90,7 +58,8 @@ def main():
             for option in OPTIONS:
                 t = alternate({"kernel": meta_step(problem, Z.training_objective(problem), option),
                                "torch_eager": meta_step(problem, lambda ps, p=problem: p.torch_objective(ps), option)},
-                              a.reps, 1, warm=1)
+                              a.reps, lambda fn: event_ms(fn, 1, 0), warmup=1)
+                t = {k: statistics.median(v) for k, v in t.items()}
                 res["meta_step_ms"]["%s/%s" % (name, option)] = t
                 print(name, option, t, flush=True)
     for problem in (Z.Quadratic(2048, random_seed=0), Z.Norm(2048, random_seed=0, norm_power=3.)):
@@ -102,12 +71,12 @@ def main():
         def ten_hvp():
             for p in rows:
                 z.hvp(x, p)
-        t = alternate({"hess_form_k10": lambda: z.hess_form(x, P), "hvp_x10": ten_hvp}, max(a.reps, 10), 20)
+        t = alternate({"hess_form_k10": lambda: z.hess_form(x, P), "hvp_x10": ten_hvp}, max(a.reps, 10),
+                      lambda fn: event_ms(fn, 20, 0), warmup=2)
+        t = {k: statistics.median(v) for k, v in t.items()}
         res["hess_form_ms"][type(problem).__name__ + "(2048)"] = t
         print(type(problem).__name__, t, flush=True)
-    os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-    with open(a.out, "w") as f:
-        json.dump(res, f, indent=1)
+    emit(res, a.out)
 
 
 if __name__ == "__main__":

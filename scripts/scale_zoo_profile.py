@@ -15,7 +15,6 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
@@ -25,40 +24,9 @@ sys.path.insert(0, ROOT)
 
 from open_l2o_b200 import hrnn_train as ht  # noqa: E402
 from open_l2o_b200 import scale_zoo as Z  # noqa: E402
+from scripts.measure import alternate, card, emit, event_ms, graphed  # noqa: E402
 
 DEV = "cuda"
-
-
-def gpu_info():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        q = ""
-    return {"device": torch.cuda.get_device_name(0), "nvidia_smi": q}
-
-
-def timed(fn, inner):
-    """ms per call of fn over `inner` back-to-back calls, by CUDA events."""
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(inner):
-        fn()
-    b.record()
-    b.synchronize()
-    return a.elapsed_time(b) / inner
-
-
-def alternate(variants, reps, inner):
-    for fn in variants.values():   # warm-up: module loads, autograd caches, allocator
-        for _ in range(3):
-            fn()
-    torch.cuda.synchronize()
-    times = {k: [] for k in variants}
-    for _ in range(reps):
-        for k, fn in variants.items():
-            times[k].append(timed(fn, inner))
-    return {k: statistics.median(v) for k, v in times.items()}
 
 
 def objective_calls(problem, x, v, which, hvp):
@@ -74,20 +42,6 @@ def objective_calls(problem, x, v, which, hvp):
             return f, g, h
         return f, g
     return call
-
-
-def graphed(call):
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):   # warm up on a side stream before the capture, as torch.cuda.graph asks
-        for _ in range(3):
-            call()
-    torch.cuda.current_stream().wait_stream(side)
-    torch.cuda.synchronize()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        call()
-    return g.replay
 
 
 def meta_step(problem, which, second, unroll):
@@ -112,7 +66,7 @@ def main(argv=None):
                                                   "scale_zoo_profile_h100.json"))
     a = ap.parse_args(argv)
     assert torch.cuda.is_available(), "this profile needs a CUDA device"
-    res = {"gpu": gpu_info(), "reps": a.reps, "meta_reps": a.meta_reps, "unroll": a.unroll, "sets": {}}
+    res = {"gpu": card(), "reps": a.reps, "meta_reps": a.meta_reps, "unroll": a.unroll, "sets": {}}
     for set_name, entries in (("optimization_test_problems", Z.optimization_test_problems()),
                               ("quadratic_problems", Z.quadratic_problems())):
         rows = []
@@ -124,13 +78,15 @@ def main(argv=None):
             for hvp in (False, True):
                 kern = objective_calls(problem, x, v, "objective", hvp)
                 tor = objective_calls(problem, x, v, "torch_objective", hvp)
-                t = alternate({"kernel": kern, "torch_eager": tor, "torch_graph": graphed(tor)}, a.reps, 20)
-                row["hvp_ms" if hvp else "value_grad_ms"] = t
+                t = alternate({"kernel": kern, "torch_eager": tor, "torch_graph": graphed(tor, 3)}, a.reps,
+                              lambda fn: event_ms(fn, 20, 0), warmup=3)
+                row["hvp_ms" if hvp else "value_grad_ms"] = {k: statistics.median(v) for k, v in t.items()}
             for second in (False, True):
                 t = alternate({"kernel": meta_step(problem, "objective", second, a.unroll),
                                "torch_eager": meta_step(problem, "torch_objective", second, a.unroll)},
-                              a.meta_reps, 1)
-                row["meta_step_%s_ms" % ("second" if second else "first")] = t
+                              a.meta_reps, lambda fn: event_ms(fn, 1, 0), warmup=3)
+                row["meta_step_%s_ms" % ("second" if second else "first")] = {
+                    k: statistics.median(v) for k, v in t.items()}
             # the two objectives agree at the timed point
             fk, gk = objective_calls(problem, x, v, "objective", False)()
             ft, gt = objective_calls(problem, x, v, "torch_objective", False)()
@@ -142,10 +98,7 @@ def main(argv=None):
             total[key] = {k: sum(r[key][k] for r in rows) for k in rows[0][key]}
         res["sets"][set_name] = {"problems": rows, "sum_over_problems": total}
         print(json.dumps({set_name: total}), flush=True)
-    os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-    with open(a.out, "w") as f:
-        json.dump(res, f, indent=1)
-    print("wrote", a.out)
+    emit(res, a.out)
 
 
 if __name__ == "__main__":

@@ -12,42 +12,16 @@ Prints one JSON line; the card name and power limit come from a read-only nvidia
 """
 import argparse
 import ctypes as C
-import json
 import math
 import os
-import statistics
 import sys
-import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 import torch  # noqa: E402
 
-from scripts.crnn_profile import card  # noqa: E402
-
-
-def alternate(fns, rounds, reps):
-    """{name: [ms per launch in each round]} with the variants interleaved round by round."""
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    out = {k: [] for k in fns}
-    for k, fn in fns.items():   # warm-up
-        for _ in range(3):
-            fn()
-    torch.cuda.synchronize()
-    for _ in range(rounds):
-        for k, fn in fns.items():
-            a.record()
-            for _ in range(reps):
-                fn()
-            b.record()
-            torch.cuda.synchronize()
-            out[k].append(a.elapsed_time(b) / reps)
-    return out
-
-
-def summary(v):
-    return dict(min_ms=min(v), median_ms=statistics.median(v))
+from scripts.measure import alternate, card, emit, event_ms, summary, wall_ms  # noqa: E402
 
 
 def hrnn_kernel(sizes, reps, rounds, gen):
@@ -72,7 +46,7 @@ def hrnn_kernel(sizes, reps, rounds, gen):
     L, st = _lib.lib(), torch.cuda.current_stream().cuda_stream
     args = {k: _lib.HrnnBwdArgs(d_g=p, **ptrs) for k, p in (("without_d_g", None), ("with_d_g", d_g.data_ptr()))}
     fns = {k: (lambda a=a: L.l2o_hrnn_coord_bwd(eng._h, C.byref(a), st)) for k, a in args.items()}
-    return {k: summary(v) for k, v in alternate(fns, rounds, reps).items()}
+    return {k: summary(v) for k, v in alternate(fns, rounds, lambda f: event_ms(f, reps, 0), warmup=3).items()}
 
 
 def crnn_kernel(n, reps, rounds, gen):
@@ -92,7 +66,7 @@ def crnn_kernel(n, reps, rounds, gen):
     L, st = _lib.lib(), torch.cuda.current_stream().cuda_stream
     args = {k: _lib.CrnnBwdArgs(n=n, d_g=p, **ptrs) for k, p in (("without_d_g", None), ("with_d_g", d_g.data_ptr()))}
     fns = {k: (lambda a=a: L.l2o_crnn_bwd(C.byref(a), st)) for k, a in args.items()}
-    return {k: summary(v) for k, v in alternate(fns, rounds, reps).items()}
+    return {k: summary(v) for k, v in alternate(fns, rounds, lambda f: event_ms(f, reps, 0), warmup=3).items()}
 
 
 def meta_gradient_cost(which, rounds, gen, T=20, batch=128):
@@ -119,7 +93,7 @@ def meta_gradient_cost(which, rounds, gen, T=20, batch=128):
             tr = ct.MetaTrainer(shapes, theta=crnn_generic_theta(7), device=dev, use_second_derivatives=second)
             lr = torch.exp(u * 1.5 - 12.0)
         trainers["second_order" if second else "first_order"] = tr
-    res = {k: dict(wall_ms=[]) for k in trainers}
+    res = {k: {} for k in trainers}
     for k, tr in trainers.items():   # warm-up, then one call for the memory high-water mark
         tr.meta_gradient(obj, p0, T, lr)
         torch.cuda.synchronize()
@@ -131,16 +105,9 @@ def meta_gradient_cost(which, rounds, gen, T=20, batch=128):
         res[k]["peak_over_resident_GB"] = (torch.cuda.max_memory_allocated() - base) / 1e9
         res[k]["grad_finite"] = bool(torch.isfinite(g).all())
         del g
-    for _ in range(rounds):
-        for k, tr in trainers.items():
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            tr.meta_gradient(obj, p0, T, lr)
-            torch.cuda.synchronize()
-            res[k]["wall_ms"].append((time.perf_counter() - t0) * 1e3)
-    for k in res:
-        v = res[k].pop("wall_ms")
-        res[k].update(wall_min_ms=min(v), wall_median_ms=statistics.median(v), rounds=len(v))
+    fns = {k: (lambda tr=tr: tr.meta_gradient(obj, p0, T, lr)) for k, tr in trainers.items()}
+    for k, v in alternate(fns, rounds, wall_ms).items():
+        res[k].update({"wall_" + m: t for m, t in summary(v).items()}, rounds=len(v))
     return res
 
 
@@ -154,8 +121,7 @@ def main():
         raise SystemExit("second_order_profile.py measures on the GPU and needs a CUDA device")
     from open_l2o_b200.scale_problems import ConvNet
     from tests.helpers import HRNN_CONVNET
-    name, power, clock = card()
-    res = dict(card=name, power_limit=power, max_sm_clock=clock, reps=args.reps, rounds=args.rounds)
+    res = dict(card=card(), reps=args.reps, rounds=args.rounds)
     gen = torch.Generator(device="cuda:0").manual_seed(0)
     conv = [int(math.prod(s)) for s in ConvNet(*HRNN_CONVNET).param_shapes]
     big = [8 * 2 ** 20] * 4
@@ -167,11 +133,7 @@ def main():
     for which in ("hrnn", "crnn"):
         res["meta_gradient_T20_convnet_%s" % which] = meta_gradient_cost(which, args.rounds, gen)
         torch.cuda.empty_cache()
-    line = json.dumps(res)
-    print(line)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        open(os.path.join(args.out, "second_order_profile.json"), "w").write(line + "\n")
+    emit(res, args.out and os.path.join(args.out, "second_order_profile.json"))
 
 
 if __name__ == "__main__":

@@ -19,25 +19,18 @@ import gc
 import json
 import os
 import statistics
-import subprocess
 import sys
-import time
 
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from open_l2o_b200 import meta, problems, util  # noqa: E402
+from scripts.measure import alternate, card, event_ms, wall_ms  # noqa: E402
 
 DM = {"net": "CoordinateWiseDeepLSTM", "net_options": {"layers": (20, 20), "scale": 0.1}}
 RNNPROP = {"net": "RNNprop", "net_options": {"layers": (20, 20), "preprocess_name": "fc",
                                              "preprocess_options": {"dim": 20}, "scale": 0.01, "tanh_output": True}}
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader",
-                        "-i", str(torch.cuda.current_device())], capture_output=True, text=True)
-    return {"device": torch.cuda.get_device_name(), "nvidia_smi": q.stdout.strip()}
 
 
 class Program:
@@ -53,12 +46,10 @@ class Program:
         self.it = 0
 
     def unroll(self):
-        torch.cuda.synchronize()
-        t = time.perf_counter()
-        self.sess.run([self.ops.fx, self.ops.update, self.ops.step], feed_dict={self.opt.step_placeholder: self.it * self.T + 1})
-        torch.cuda.synchronize()
+        ms = wall_ms(lambda: self.sess.run([self.ops.fx, self.ops.update, self.ops.step],
+                                           feed_dict={self.opt.step_placeholder: self.it * self.T + 1}))
         self.it += 1
-        return 1e3 * (time.perf_counter() - t)
+        return ms
 
     def split(self, reps):
         """Median ms of the segmented backward alone (run eagerly on the last unroll's records, outside any captured
@@ -66,22 +57,17 @@ class Program:
         prog, ev = self.prog, []
         rec = prog._recompute
 
-        def timed(*a):
+        def timed_recompute(*a):   # events around each recompute inside the one backward
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
             rec(*a)
             e1.record()
             ev.append((e0, e1))
-        prog._recompute = timed
+        prog._recompute = timed_recompute
         back, recomp = [], []
         for _ in range(reps):
             ev.clear()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            prog._bptt()
-            e1.record()
-            torch.cuda.synchronize()
-            back.append(e0.elapsed_time(e1))
+            back.append(event_ms(prog._bptt, 1, 0))
             recomp.append(sum(a.elapsed_time(b) for a, b in ev))
         del prog._recompute
         return dict(ms_backward=med(back), ms_recompute=med(recomp),
@@ -111,24 +97,27 @@ def compare(name, cls, cfg, make_problem, T, S, reps):
     full = Program(cls, cfg, make_problem(), T, None)
     seg = Program(cls, cfg, make_problem(), T, S)
     assert not full.prog.segmented and seg.prog.segmented, name
-    t_full, t_seg, ddiff = [], [], 0.0
-    for i in range(reps + 2):
+    ddiff = [0.0]
+
+    def full_unroll():
         for k in full.prog.nets:
             seg.prog.nets[k].theta.copy_(full.prog.nets[k].theta)
             for s in ("m", "v"):
                 seg.prog.adam[k][s].copy_(full.prog.adam[k][s])
-        a = full.unroll()
-        b = seg.unroll()
+        return full.unroll()
+
+    def seg_unroll():
+        ms = seg.unroll()
         for k in full.prog.nets:
             d = full.prog.dtheta[k]
-            ddiff = max(ddiff, float((seg.prog.dtheta[k] - d).abs().max() / d.abs().max()))
-        if i >= 2:
-            t_full.append(a)
-            t_seg.append(b)
+            ddiff.append(float((seg.prog.dtheta[k] - d).abs().max() / d.abs().max()))
+        return ms
+    t = alternate({"full": full_unroll, "segmented": seg_unroll}, reps + 2, lambda fn: fn())
+    t_full, t_seg = t["full"][2:], t["segmented"][2:]   # past two warm-up unrolls
     out = dict(case=name, T=T, S=S, coords=full.prog.N, unrolls=reps, ms_full=med(t_full), ms_segmented=med(t_seg),
                ms_full_all=t_full, ms_segmented_all=t_seg,
                segments=seg.prog.plan.bounds, plan_bytes_full=full.prog.plan.bytes, plan_bytes_segmented=seg.prog.plan.bytes,
-               max_rel_dtheta_diff=ddiff, **seg.split(reps))
+               max_rel_dtheta_diff=max(ddiff), **seg.split(reps))
     del full
     release()
     out["peak_bytes_segmented"] = seg.peak_bytes(2)
