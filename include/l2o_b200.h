@@ -21,6 +21,7 @@
  *   l2o_log_and_sign                    preprocess.LogAndSign                          DM/preprocess.py:52-70
  *   l2o_lasso_grad                      problems.lasso(_fixed) loss + tf.gradients     DM/problems.py:103-175, DM/meta.py:322-329
  *   l2o_confocal_grad                   problems.confocal_microscopy_3d + tf.gradients DM/problems.py:701-956, DM/meta.py:322-329
+ *   l2o_mnist_grad                      problems.mnist (batch draw + MLP) + tf.gradients DM/problems.py:254-288, DM/meta.py:322-329
  *
  * Conventions: every pointer is a DEVICE pointer owned by the caller (PyTorch allocates); no hidden
  * allocation; `stream` is a cudaStream_t passed as void*; every entry returns 0 or a negative
@@ -275,6 +276,41 @@ typedef struct {
   double* f;            /* optional scalar: += f */
 } l2o_confocal_args;
 int l2o_confocal_grad(const l2o_confocal_args* a, void* stream);
+
+/*   l2o_mnist_grad  problems.mnist, DM/problems.py:254-288 + tf.gradients at DM/meta.py:322-329:
+ *                   f = mean_b xent(MLP(images[idx_b] * fp32(1/255)), labels[idx_b]) with a fresh batch of `batch`
+ *                   indices idx_b drawn uniformly from [0, num_examples) at every call (the reference's
+ *                   tf.random_uniform + tf.gather), g = df/dx.  The draw is Philox4x32-10 keyed by `seed` at the
+ *                   device counter *counter, which the call reads and advances by one; idx_b = (r * N) >> 32 of the
+ *                   32-bit draw r (bias at most N / 2^32).  x, scale and g are the arena of the MLP's variables in
+ *                   creation order: w0 [784][h0], b0 [h0], w1 [h0][h1], b1, ..., w_L [h_last][10], b_L [10].  Sigmoid
+ *                   or ReLU between layers, none after the last; theta = x (.) scale (optional, random-scaling trick as
+ *                   l2o_lasso_grad).  One thread-block cluster; deterministic (no atomics).  Limits: 1..4 hidden layers
+ *                   of width 1..64 and batch 1..1024; anything else is L2O_E_INVALID. */
+#define L2O_MNIST_INPUT 784
+#define L2O_MNIST_CLASSES 10
+#define L2O_MNIST_MAX_HIDDEN 4
+#define L2O_MNIST_MAX_WIDTH 64
+#define L2O_MNIST_MAX_BATCH 1024
+#define L2O_MNIST_SIGMOID 0
+#define L2O_MNIST_RELU 1
+typedef struct {
+  int32_t batch;          /* B */
+  int32_t num_examples;   /* N: rows of images / labels */
+  int32_t n_layers;       /* linear layers: hidden layers + 1 */
+  int32_t hidden[4];      /* widths of the hidden layers */
+  int32_t activation;     /* L2O_MNIST_SIGMOID | L2O_MNIST_RELU */
+  uint64_t seed;
+  int64_t* counter;       /* device scalar: read, then += 1 */
+  const uint8_t* images;  /* [N][784] raw pixels */
+  const uint8_t* labels;  /* [N], each < 10 */
+  const float* x;         /* the arena */
+  const float* scale;     /* optional, the arena's layout */
+  float* g;               /* the arena's layout */
+  double* f;              /* optional scalar: = f */
+  int32_t* idx_out;       /* optional [B]: the indices drawn */
+} l2o_mnist_args;
+int l2o_mnist_grad(const l2o_mnist_args* a, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * L2O-Scale HierarchicalRNN update step (SURVEY.md 8(f) row 1; BASELINE config #4).

@@ -25,7 +25,7 @@ ENGINE_AUTO, ENGINE_FFMA, ENGINE_TC = 0, 1, 2
 EXPORTS = [
     "l2o_net_create", "l2o_net_destroy", "l2o_net_set_engine", "l2o_theta_count", "l2o_state_floats", "l2o_workspace_bytes",
     "l2o_step", "l2o_unroll_fwd", "l2o_unroll_bwd", "l2o_unroll_bwd_carry", "l2o_tc_fwd_variant", "l2o_tc_weight_image", "l2o_adam_step", "l2o_log_and_sign", "l2o_lasso_grad",
-    "l2o_confocal_grad",
+    "l2o_confocal_grad", "l2o_mnist_grad",
     "l2o_dense_create", "l2o_dense_destroy", "l2o_dense_theta_count", "l2o_dense_state_floats", "l2o_dense_step",
     "l2o_dense_unroll_bwd",
     "l2o_launch_count", "l2o_status_string", "l2o_last_cuda_error", "l2o_version",
@@ -84,6 +84,16 @@ class LassoArgs(C.Structure):
 class ConfocalArgs(C.Structure):
     _fields_ = [("batch", C.c_int32), ("num_points", C.c_int32), ("roi", C.c_int32 * 3), ("x", _fp), ("sim", _fp),
                 ("scale", _fp), ("g", _fp), ("f", _fp)]
+
+
+class MnistArgs(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("num_examples", C.c_int32), ("n_layers", C.c_int32), ("hidden", C.c_int32 * 4),
+                ("activation", C.c_int32), ("seed", C.c_uint64), ("counter", _fp), ("images", _fp), ("labels", _fp),
+                ("x", _fp), ("scale", _fp), ("g", _fp), ("f", _fp), ("idx_out", _fp)]
+
+
+MNIST_INPUT, MNIST_CLASSES, MNIST_MAX_HIDDEN, MNIST_MAX_WIDTH, MNIST_MAX_BATCH = 784, 10, 4, 64, 1024
+MNIST_SIGMOID, MNIST_RELU = 0, 1
 
 
 class DenseDesc(C.Structure):
@@ -289,6 +299,8 @@ def lib():
     L.l2o_lasso_grad.restype = C.c_int
     L.l2o_confocal_grad.argtypes = [C.POINTER(ConfocalArgs), C.c_void_p]
     L.l2o_confocal_grad.restype = C.c_int
+    L.l2o_mnist_grad.argtypes = [C.POINTER(MnistArgs), C.c_void_p]
+    L.l2o_mnist_grad.restype = C.c_int
     L.l2o_dense_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(DenseDesc)]
     L.l2o_dense_create.restype = C.c_int
     L.l2o_dense_destroy.argtypes = [C.c_void_p]

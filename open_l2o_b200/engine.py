@@ -304,6 +304,46 @@ def confocal_grad(x, sim, g, batch, num_points, roi, f=None, scale=None):
     _lib.check(_lib.lib().l2o_confocal_grad(C.byref(a), _stream()), "l2o_confocal_grad")
 
 
+def mnist_fits(layers, batch) -> bool:
+    """Whether l2o_mnist_grad takes this MLP: 1..4 hidden layers of width 1..64 and a batch of 1..1024."""
+    layers = tuple(int(w) for w in layers)
+    return (1 <= len(layers) <= _lib.MNIST_MAX_HIDDEN and all(1 <= w <= _lib.MNIST_MAX_WIDTH for w in layers)
+            and 1 <= int(batch) <= _lib.MNIST_MAX_BATCH)
+
+
+def mnist_grad(images, labels, x, g, layers, batch, activation, seed, counter, f=None, scale=None, idx_out=None):
+    """f and df/dx of problems.mnist (DM/problems.py:254-288) at a fresh batch in one launch.  images [N, 784] and
+    labels [N] uint8; x, g and scale the flat arena of the MLP's variables in creation order (w0, b0, w1, b1, ...);
+    ``counter`` a one-element int64 device tensor the call reads and advances; writes f (fp64 scalar) and the indices
+    drawn into ``idx_out`` (int32 [batch]) if given."""
+    a = _lib.MnistArgs()
+    layers = tuple(int(w) for w in layers)
+    a.batch, a.num_examples, a.n_layers = int(batch), int(images.shape[0]), len(layers) + 1
+    for k, w in enumerate(layers[:_lib.MNIST_MAX_HIDDEN]):
+        a.hidden[k] = w
+    a.activation = {"sigmoid": _lib.MNIST_SIGMOID, "relu": _lib.MNIST_RELU}[activation]
+    a.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+    if images.numel() != a.num_examples * _lib.MNIST_INPUT or labels.numel() != a.num_examples:
+        raise L2OError("mnist_grad: images must be [N, 784] and labels [N]")
+    n = 0
+    k = _lib.MNIST_INPUT
+    for w in layers + (_lib.MNIST_CLASSES,):
+        n, k = n + (k + 1) * w, w
+    for name, t in (("x", x), ("g", g), ("scale", scale)):
+        if t is not None and t.numel() != n:
+            raise L2OError(f"mnist_grad: {name} has {t.numel()} elements, the MLP has {n}")
+    if idx_out is not None and idx_out.numel() != a.batch:
+        raise L2OError(f"mnist_grad: idx_out has {idx_out.numel()} elements, batch is {a.batch}")
+    if counter.numel() != 1:
+        raise L2OError("mnist_grad: counter must be one int64 element")
+    a.counter = _ptr(counter, torch.int64, "counter")
+    a.images, a.labels = _ptr(images, torch.uint8, "images"), _ptr(labels, torch.uint8, "labels")
+    a.x, a.scale, a.g = _ptr(x, name="x"), _ptr(scale, name="scale"), _ptr(g, name="g")
+    a.f = _ptr(f, torch.float64, "f")
+    a.idx_out = _ptr(idx_out, torch.int32, "idx_out")
+    _lib.check(_lib.lib().l2o_mnist_grad(C.byref(a), _stream()), "l2o_mnist_grad")
+
+
 _graph_replayed = 0  # kernels of this library launched through CUDA-graph replays (not visible to the C-side counter)
 
 

@@ -26,7 +26,7 @@ from . import engine as _engine
 from . import networks
 from .variables import variable_getter
 
-_PRODUCER_KINDS = ("lasso_batch", "mlp_xent", "confocal_psf")
+_PRODUCER_KINDS = ("lasso_batch", "mlp_xent", "confocal_psf", "mnist_mlp")
 MetaLoss = collections.namedtuple("MetaLoss", "loss, update, reset, fx, x")
 MetaStep = collections.namedtuple("MetaStep", "step, update, reset, fx, x")
 
@@ -254,10 +254,13 @@ class _Program(object):
         self.fused = getattr(make_loss, "fused", None) if os.environ.get("L2O_DISABLE_FUSED") != "1" else None
         one_net = len(self.runs) == 1 and self.runs[0].n == self.N
         if self.fused is not None and not (one_net and (len(self.variables) == 1 or
-                                                        self.fused.kind in ("mlp_xent", "confocal_psf"))):
+                                                        self.fused.kind in ("mlp_xent", "confocal_psf",
+                                                                            "mnist_mlp"))):
             self.fused = None
         if self.fused is not None and self.fused.kind == "confocal_psf" and not self._confocal_layout_ok(self.fused):
             self.fused = None   # the arena is not the kernel's [6P+1][B] row order: autograd, not a wrong layout
+        if self.fused is not None and self.fused.kind == "mnist_mlp" and not self._mnist_ok(self.fused):
+            self.fused = None   # a shape l2o_mnist_grad does not take, or not its arena order: the autograd path
         # "producer" optimizees (SURVEY.md 8(f) row 4): f and df/dx come from ONE library kernel per step instead of
         # torch autograd (~15 launches); the unroll stays step-at-a-time (the gradient couples coordinates) and is
         # captured into one CUDA graph like every external-gradient unroll
@@ -272,6 +275,16 @@ class _Program(object):
             self._confocal_sim = torch.zeros(len(names), self.variables[0]["shape"][0], device=self.device)
             for row, name in zip(self._confocal_sim, names):
                 self.const_vals[name] = row.view(shapes[name])
+        if self.producer is not None and self.producer.kind == "mnist_mlp":
+            # the split on the device (uploaded once per process, never reset), the seed and the device counter of the
+            # kernel's batch draws, and the indices of each evaluation of the unroll: T steps + the final loss
+            from .mnist_data import device_split
+            e = self.producer.extra
+            self.mnist_images, self.mnist_labels = device_split(e["data_dir"], e["mode"], self.device)
+            self.mnist_seed = optimizer.seed
+            self.mnist_counter = torch.zeros(1, dtype=torch.int64, device=self.device)
+            self.mnist_idx = torch.zeros(self.T + 1, e["batch_size"], dtype=torch.int32, device=self.device)
+        self._draw = 0
         self.adam = _adam_slots(self.nets)
         self.dtheta = {k: torch.zeros(net.theta.numel(), dtype=torch.float64, device=self.device)
                        for k, net in self.nets.items()}
@@ -294,6 +307,14 @@ class _Program(object):
                 [c["name"] for c in self.constants] == spec.extra["constants"] and
                 all(tuple(r["shape"]) == (B, 1) for r in self.variables + self.constants) and
                 [s.start for s in self.var_slices] == [j * B for j in range(len(self.variables))])
+
+    def _mnist_ok(self, spec):
+        """l2o_mnist_grad takes the MLP, and the arena holds w0, b0, w1, b1, ... in creation order."""
+        e = spec.extra
+        names = [n for i in range(len(e["layers"]) + 1) for n in ("mlp/linear_{}/w".format(i), "mlp/linear_{}/b".format(i))]
+        sizes = [int(np.prod(v["shape"])) for v in self.variables]
+        return (_engine.mnist_fits(e["layers"], e["batch_size"]) and [v["name"] for v in self.variables] == names and
+                [s.start for s in self.var_slices] == [int(sum(sizes[:j])) for j in range(len(sizes))])
 
     # ---- memory ---------------------------------------------------------------------------------
     def _alloc_workspaces(self, segment=None):
@@ -430,6 +451,12 @@ class _Program(object):
         elif p.kind == "confocal_psf":
             _engine.confocal_grad(Xflat, self._confocal_sim, g, self._confocal_sim.shape[1], p.extra["num_points"],
                                   p.extra["roi"], f=fx, scale=self.scale_flat if self.scale_active else None)
+        elif p.kind == "mnist_mlp":
+            # one draw per optimizee evaluation, recorded in row t of mnist_idx (T steps, then the final loss)
+            t, self._draw = self._draw, self._draw + 1
+            _engine.mnist_grad(self.mnist_images, self.mnist_labels, Xflat, g, p.extra["layers"], p.extra["batch_size"],
+                               p.extra["activation"], self.mnist_seed, self.mnist_counter, f=fx,
+                               scale=self.scale_flat if self.scale_active else None, idx_out=self.mnist_idx[min(t, self.T)])
         elif p.kind == "mlp_xent":
             from .problems import mlp_value_and_grad
             with torch.no_grad():
@@ -547,6 +574,7 @@ class _Program(object):
     def _forward_external(self, train, step0):
         T, Xw = self.T, self._Xw
         self._fused_regime = False
+        self._draw = 0
         Xw.copy_(self.X)
         fxs = []
         for r in self.runs:

@@ -21,6 +21,7 @@ class FusedSpec:
     kind: str        # "rastrigin_sep" | "quadratic_diag" | "quadratic_batch" (in-kernel, include/l2o_b200.h L2O_OPT_*)
                      # | "lasso_batch" (producer kernel l2o_lasso_grad: a = A / w, b = y, alpha = l1 weight)
                      # | "mlp_xent" (mlp_value_and_grad) | "confocal_psf" (producer kernel l2o_confocal_grad)
+                     # | "mnist_mlp" (producer kernel l2o_mnist_grad; extra: layers, activation, batch, split)
     var: str         # name of the trainable variable
     a: str           # constant names
     b: str
@@ -211,6 +212,43 @@ def mlp_value_and_grad(params, data, labels, activation, grads_out):
             dh = dz @ params[2 * i].t()
             dz = dh * hs[i] * (1.0 - hs[i]) if activation == "sigmoid" else dh * (hs[i] > 0).to(dh.dtype)
     return loss
+
+
+def mnist(layers, activation="sigmoid", batch_size=128, mode="train", data_dir="MNIST-data"):
+    """MNIST classification with a multi-layer perceptron (DM/problems.py:254-288): Sonnet's ``mlp/linear_{i}/w|b``,
+    both N(0, 0.01) (``_nn_initializers``), sigmoid or ReLU between layers, the mean sparse softmax cross entropy of a
+    fresh batch of ``batch_size`` examples drawn uniformly with replacement at EVERY evaluation.  The data is read from
+    ``data_dir`` (mnist_data; never downloaded) when the problem is made, and is not an optimizee variable: a reset
+    re-initialises the weights only, as the reference's ``tf.constant`` images are untouched by its reset."""
+    from . import mnist_data
+    if activation not in ("sigmoid", "relu"):
+        raise ValueError("{} activation not supported".format(activation))
+    if mode not in ("train", "validation", "test"):
+        raise ValueError("{} is not an MNIST split".format(mode))
+    layers = tuple(int(w) for w in layers)
+    num_examples = mnist_data.load_mnist(data_dir)[mode].num_examples
+    act = {"sigmoid": torch.sigmoid, "relu": torch.relu}[activation]
+
+    def build():
+        params, k = [], 784
+        for i, width in enumerate(layers + (10,)):
+            params.append(get_variable("mlp/linear_{}/w".format(i), shape=[k, width],
+                                       initializer=random_normal_initializer(stddev=0.01)))
+            params.append(get_variable("mlp/linear_{}/b".format(i), shape=[width],
+                                       initializer=random_normal_initializer(stddev=0.01)))
+            k = width
+        images, labels = mnist_data.device_split(data_dir, mode, params[0].device)
+        idx = torch.randint(0, num_examples, (batch_size,), device=images.device)
+        h = images.index_select(0, idx).float() * float(mnist_data.SCALE)
+        for i in range(len(params) // 2):
+            h = h @ params[2 * i] + params[2 * i + 1]
+            if i < len(layers):
+                h = act(h)
+        return torch.nn.functional.cross_entropy(h, labels.index_select(0, idx).long())
+    # producer kernel l2o_mnist_grad: the batch draw, forward and backward in one launch
+    build.fused = FusedSpec("mnist_mlp", "mlp/linear_0/w", "", "", extra=dict(
+        layers=layers, activation=activation, batch_size=int(batch_size), mode=mode, data_dir=data_dir))
+    return build
 
 
 _PSF_PARAMS = ("I", "x", "y", "z", "sigmaxy", "sigmaz")

@@ -82,8 +82,12 @@ def _cw20(path):
     return {"cw": {"net": "CoordinateWiseDeepLSTM", "net_options": {"layers": (20, 20)}, "net_path": path}}
 
 
-def get_config(problem_name, path=None, mode=None, num_hidden_layer=None, net_name=None):
-    """Returns problem configuration (DM/util.py:112-265) for the synthetic problems that exist offline."""
+_MNIST = {"mnist": ((20,), "sigmoid"), "mnist_relu": ((20,), "relu"), "mnist_deeper": ((20, 20), "sigmoid")}
+
+
+def get_config(problem_name, path=None, mode=None, num_hidden_layer=None, net_name=None, data_dir="MNIST-data"):
+    """Returns problem configuration (DM/util.py:112-265) for the synthetic problems and, from the MNIST files in
+    ``data_dir`` (never downloaded), the MNIST MLPs."""
     net_assignments = None
     if problem_name == "simple":
         problem = problems.simple()
@@ -104,6 +108,12 @@ def get_config(problem_name, path=None, mode=None, num_hidden_layer=None, net_na
     elif problem_name == "square_cos":
         problem = problems.square_cos(batch_size=128, num_dims=2)
         net_config = _cw20(path)
+    elif problem_name in _MNIST:                  # DM/util.py:145-163
+        if mode is None:
+            mode = "train" if path is None else "test"
+        layers, activation = _MNIST[problem_name]
+        problem = problems.mnist(layers=layers, activation=activation, mode=mode, data_dir=data_dir)
+        net_config = {"cw": get_default_net_config(path)}
     elif problem_name == "rastrigin_separable":   # BASELINE config #5
         problem = problems.rastrigin_separable(num_dims=1000000)
         net_config = _cw20(path)
