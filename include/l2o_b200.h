@@ -22,6 +22,7 @@
  *   l2o_lasso_grad                      problems.lasso(_fixed) loss + tf.gradients     DM/problems.py:103-175, DM/meta.py:322-329
  *   l2o_confocal_grad                   problems.confocal_microscopy_3d + tf.gradients DM/problems.py:701-956, DM/meta.py:322-329
  *   l2o_mnist_grad                      problems.mnist (batch draw + MLP) + tf.gradients DM/problems.py:254-288, DM/meta.py:322-329
+ *   l2o_mnist_conv_grad                 problems.mnist_conv (batch-norm ConvNet) + tf.gradients DM/problems.py:291-347, DM/meta.py:322-329
  *
  * Conventions: every pointer is a DEVICE pointer owned by the caller (PyTorch allocates); no hidden
  * allocation; `stream` is a cudaStream_t passed as void*; every entry returns 0 or a negative
@@ -311,6 +312,48 @@ typedef struct {
   int32_t* idx_out;       /* optional [B]: the indices drawn */
 } l2o_mnist_args;
 int l2o_mnist_grad(const l2o_mnist_args* a, void* stream);
+
+/*   l2o_mnist_conv_grad  problems.mnist_conv(batch_norm=True), DM/problems.py:291-347 + tf.gradients at
+ *                   DM/meta.py:322-329: f = mean_b xent(ConvNet(images[idx_b] * fp32(1/255)), labels[idx_b]) with a
+ *                   fresh batch drawn exactly as l2o_mnist_grad draws it (same seed / counter convention, same indices),
+ *                   g = df/dx.  The ConvNet (NHWC): conv 3x3 1->16 VALID + b1, batch norm, ReLU, max-pool 2x2/2;
+ *                   conv 5x5 16->32 VALID + b2, batch norm, ReLU, max-pool 2x2/2 ([9,9] -> [4,4]); flatten (h, w, c);
+ *                   fc 512->10 + bias, ReLU; batch norm in training mode with gamma = 1, beta = 0, eps 1e-3 and the
+ *                   biased variance over all B*H*W positions.  x, scale and g are the arena of the variables in creation
+ *                   order: conv_layer1/weights1 [3][3][1][16], conv_layer1/biases1 [16], conv_layer2/weights1
+ *                   [5][5][16][32], conv_layer2/biases1 [32], fc_weights [512][10], fc_bias [10] (18,122 floats);
+ *                   theta = x (.) scale (optional, random-scaling trick as l2o_lasso_grad).  One cooperative launch over
+ *                   the resident CTAs; bitwise deterministic on any SM count (no atomics).  `workspace` is caller-owned
+ *                   device memory of at least l2o_mnist_conv_workspace_bytes(batch) bytes, 16-byte aligned.  Limits:
+ *                   batch 1..1024; anything else, a null required pointer, a misaligned pointer or a short workspace
+ *                   is L2O_E_INVALID before any CUDA call. */
+#define L2O_MNIST_CONV_COORDS 18122
+#define L2O_MNIST_CONV_MAX_BATCH 1024
+typedef struct {
+  int32_t batch;          /* B */
+  int32_t num_examples;   /* N: rows of images / labels */
+  uint64_t seed;
+  int64_t* counter;       /* device scalar: read, then += 1 */
+  const uint8_t* images;  /* [N][784] raw pixels */
+  const uint8_t* labels;  /* [N], each < 10 */
+  const float* x;         /* the arena */
+  const float* scale;     /* optional, the arena's layout */
+  float* g;               /* the arena's layout */
+  double* f;              /* optional scalar: = f */
+  int32_t* idx_out;       /* optional [B]: the indices drawn */
+  void* workspace;        /* caller-owned, >= l2o_mnist_conv_workspace_bytes(batch) bytes */
+  size_t workspace_bytes;
+} l2o_mnist_conv_args;
+/* bytes of workspace l2o_mnist_conv_grad needs at this batch size; L2O_E_INVALID outside 1..1024 */
+int64_t l2o_mnist_conv_workspace_bytes(int32_t batch);
+/* byte offsets inside the workspace of what the last call's ReLU and max-pool decisions were made from, so that a
+ * caller can check g against a reference taking the same decisions: [0] z1 (fp32 [B][26][26][16], conv1 + b1),
+ * [1] z2 (fp32 [B][9][9][32], conv2 + b2), [2] bn (fp32 [96]: mu1 [16], rstd1 [16], mu2 [32], rstd2 [32]; the
+ * normalised value is (z - mu) * rstd in fp32), [3] dlogits (fp32 [B][16], zero where the logit's ReLU is off).
+ * L2O_E_INVALID outside 1..1024 or for a null off. */
+#define L2O_MNIST_CONV_LAYOUT 4
+int l2o_mnist_conv_workspace_layout(int32_t batch, int64_t* off);
+int l2o_mnist_conv_grad(const l2o_mnist_conv_args* a, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * L2O-Scale HierarchicalRNN update step (SURVEY.md 8(f) row 1; BASELINE config #4).

@@ -57,6 +57,28 @@ int occupancy_launch(const char* fn, K* kernel, int block, size_t smem, int64_t 
   return after_launch(fn);
 }
 
+// occupancy_launch as a cooperative launch (cudaLaunchAttributeCooperative, also valid for captured graph nodes): the
+// grid is at most the resident CTAs, so every CTA is running at once and the kernel may use cg::this_grid().sync().
+template <class... KArgs, class... Args>
+int cooperative_launch(const char* fn, void (*kernel)(KArgs...), int block, size_t smem, int64_t n, cudaStream_t st,
+                       const Args&... args) {
+  int grid = 0;
+  if (int rc = occupancy_grid(fn, (const void*)kernel, block, smem, n, grid)) return rc;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeCooperative;
+  attr[0].val.cooperative = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)grid);
+  cfg.blockDim = dim3((unsigned)block);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, args...);
+  if (e != cudaSuccess) return set_cuda_error(e, fn, "cudaLaunchKernelEx (cooperative)");
+  return after_launch(fn);
+}
+
 inline bool misaligned(const void* p, uintptr_t align) { return ((uintptr_t)p & (align - 1)) != 0; }
 
 // Does the byte range [p, p + bytes) share a byte with any of the ranges (q[k], qbytes[k])?  Null q[k] are skipped.

@@ -2,10 +2,8 @@
 //   f = mean_b xent(MLP(images[idx_b] / 255), labels[idx_b]),  idx_b ~ U[0, N) drawn afresh at every evaluation,
 // in ONE launch.  The optimizee step feeding the hot path (SURVEY.md 8(f) row 4), like l2o_lasso_grad.
 //
-// Batch indices.  Philox4x32-10 keyed by the 64-bit seed, counter (b, 0, c_lo, c_hi) for batch row b, where c is the
-// device int64 *counter the kernel reads and CTA rank 0 advances by one after the last cluster barrier; word 0 of the
-// output is the draw r and idx_b = (r * N) >> 32 (a 64-bit multiply-high: each index has probability within N / 2^32
-// of 1 / N).  Because the counter lives on the device, a captured CUDA graph draws a fresh batch on every replay.
+// Batch indices.  l2o_philox.cuh's draw at the device int64 *counter, which the kernel reads and CTA rank 0 advances by
+// one after the last cluster barrier.  Because the counter lives on the device, a captured CUDA graph draws a fresh batch on every replay.
 //
 // Design.  One cluster of kCl = 8 CTAs, CTA rank s owning batch rows [s R, s R + R), R = ceil(B / 8) (the last CTAs
 // may own fewer rows, or none).  Each CTA keeps its rows' hidden activations in shared memory, and later the dz of
@@ -24,6 +22,7 @@
 #include <cuda_runtime.h>
 
 #include "l2o_internal.h"
+#include "l2o_philox.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -86,29 +85,6 @@ bool make_plan(const l2o_mnist_args& a, Plan& p) {
   return true;
 }
 
-__device__ __forceinline__ float pixel(uint8_t v) {
-  // read_data_sets: images.astype(float32) * (1.0 / 255.0), the double constant rounded to fp32 first
-  return __fmul_rn((float)v, (float)(1.0 / 255.0));
-}
-
-// Philox4x32-10 (Salmon et al., SC'11), word 0 of the output block
-__device__ __forceinline__ uint32_t philox_w0(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0,
-                                              uint32_t k1) {
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    const uint32_t hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
-    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
-    const uint32_t n0 = hi1 ^ c1 ^ k0, n2 = hi0 ^ c3 ^ k1;
-    c0 = n0;
-    c1 = lo1;
-    c2 = n2;
-    c3 = lo0;
-    k0 += 0x9E3779B9u;
-    k1 += 0xBB67AE85u;
-  }
-  return c0;
-}
-
 __global__ void __cluster_dims__(kCl, 1, 1) __launch_bounds__(kThreads, 1) mnist_grad_kernel(const l2o_mnist_args a,
                                                                                           const Plan p) {
   extern __shared__ __align__(16) float sm[];
@@ -129,9 +105,7 @@ __global__ void __cluster_dims__(kCl, 1, 1) __launch_bounds__(kThreads, 1) mnist
   // ---- batch indices -------------------------------------------------------------------------------------------------
   const uint64_t ctr = (uint64_t)*a.counter;
   for (int r = tid; r < nrows; r += kThreads) {
-    const uint32_t w = philox_w0((uint32_t)(row0 + r), 0u, (uint32_t)ctr, (uint32_t)(ctr >> 32), (uint32_t)a.seed,
-                                 (uint32_t)(a.seed >> 32));
-    const int idx = (int)(((uint64_t)w * (uint64_t)a.num_examples) >> 32);
+    const int idx = l2o::batch_index(a.seed, ctr, row0 + r, a.num_examples);
     sidx[r] = idx;
     if (a.idx_out) a.idx_out[row0 + r] = idx;
   }
@@ -155,7 +129,7 @@ __global__ void __cluster_dims__(kCl, 1, 1) __launch_bounds__(kThreads, 1) mnist
         const uint8_t* xr = xc + r * kKC;
         float acc = c0 == 0 ? 0.f : z[o];
 #pragma unroll 8
-        for (int kk = 0; kk < kKC; ++kk) acc = fmaf(pixel(xr[kk]), wc[kk * W + j], acc);
+        for (int kk = 0; kk < kKC; ++kk) acc = fmaf(l2o::mnist_pixel(xr[kk]), wc[kk * W + j], acc);
         z[o] = acc;
       }
       __syncthreads();
@@ -241,7 +215,7 @@ __global__ void __cluster_dims__(kCl, 1, 1) __launch_bounds__(kThreads, 1) mnist
         for (int e = tid; e < nb * nk; e += kThreads) {
           const int r = e / nk, kk = e - r * nk, k = k0 + kk;
           float v = 1.f;
-          if (k < K) v = l == 0 ? pixel(a.images[(size_t)sI[r] * kIn + k]) : rA[(rb + r) * K + k];
+          if (k < K) v = l == 0 ? l2o::mnist_pixel(a.images[(size_t)sI[r] * kIn + k]) : rA[(rb + r) * K + k];
           sA[e] = v;
         }
         __syncthreads();

@@ -344,6 +344,55 @@ def mnist_grad(images, labels, x, g, layers, batch, activation, seed, counter, f
     _lib.check(_lib.lib().l2o_mnist_grad(C.byref(a), _stream()), "l2o_mnist_grad")
 
 
+def mnist_conv_fits(batch) -> bool:
+    """Whether l2o_mnist_conv_grad takes this batch size: 1..1024."""
+    return 1 <= int(batch) <= _lib.MNIST_CONV_MAX_BATCH
+
+
+def mnist_conv_workspace_bytes(batch) -> int:
+    """Bytes of device workspace l2o_mnist_conv_grad needs at this batch size (the library allocates nothing)."""
+    n = int(_lib.lib().l2o_mnist_conv_workspace_bytes(int(batch)))
+    if n < 0:
+        raise L2OError(f"mnist_conv_workspace_bytes: batch {batch} is outside 1..{_lib.MNIST_CONV_MAX_BATCH}")
+    return n
+
+
+def mnist_conv_workspace_layout(batch) -> dict:
+    """Byte offsets in the l2o_mnist_conv_grad workspace of z1, z2, the batch-norm constants and dlogits, the values
+    its ReLU and max-pool decisions come from (include/l2o_b200.h)."""
+    off = (C.c_int64 * _lib.MNIST_CONV_LAYOUT)()
+    _lib.check(_lib.lib().l2o_mnist_conv_workspace_layout(int(batch), off), "l2o_mnist_conv_workspace_layout")
+    return dict(zip(("z1", "z2", "bn", "dl"), (int(v) for v in off)))
+
+
+def mnist_conv_grad(images, labels, x, g, batch, seed, counter, workspace, f=None, scale=None, idx_out=None):
+    """f and df/dx of problems.mnist_conv (DM/problems.py:291-347, batch norm on) at a fresh batch in one launch.
+    images [N, 784] and labels [N] uint8; x, g and scale the flat 18,122-float arena of the ConvNet's variables in
+    creation order; ``counter`` a one-element int64 device tensor the call reads and advances (the batch is drawn as
+    mnist_grad draws it); ``workspace`` a uint8 device tensor of at least mnist_conv_workspace_bytes(batch) bytes;
+    writes f (fp64 scalar) and the indices drawn into ``idx_out`` (int32 [batch]) if given."""
+    a = _lib.MnistConvArgs()
+    a.batch, a.num_examples = int(batch), int(images.shape[0])
+    a.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+    if images.numel() != a.num_examples * _lib.MNIST_INPUT or labels.numel() != a.num_examples:
+        raise L2OError("mnist_conv_grad: images must be [N, 784] and labels [N]")
+    for name, t in (("x", x), ("g", g), ("scale", scale)):
+        if t is not None and t.numel() != _lib.MNIST_CONV_COORDS:
+            raise L2OError(f"mnist_conv_grad: {name} has {t.numel()} elements, the ConvNet has {_lib.MNIST_CONV_COORDS}")
+    if idx_out is not None and idx_out.numel() != a.batch:
+        raise L2OError(f"mnist_conv_grad: idx_out has {idx_out.numel()} elements, batch is {a.batch}")
+    if counter.numel() != 1:
+        raise L2OError("mnist_conv_grad: counter must be one int64 element")
+    a.counter = _ptr(counter, torch.int64, "counter")
+    a.images, a.labels = _ptr(images, torch.uint8, "images"), _ptr(labels, torch.uint8, "labels")
+    a.x, a.scale, a.g = _ptr(x, name="x"), _ptr(scale, name="scale"), _ptr(g, name="g")
+    a.f = _ptr(f, torch.float64, "f")
+    a.idx_out = _ptr(idx_out, torch.int32, "idx_out")
+    a.workspace = _ptr(workspace, torch.uint8, "workspace")
+    a.workspace_bytes = workspace.numel()
+    _lib.check(_lib.lib().l2o_mnist_conv_grad(C.byref(a), _stream()), "l2o_mnist_conv_grad")
+
+
 _graph_replayed = 0  # kernels of this library launched through CUDA-graph replays (not visible to the C-side counter)
 
 

@@ -26,7 +26,8 @@ from . import engine as _engine
 from . import networks
 from .variables import variable_getter
 
-_PRODUCER_KINDS = ("lasso_batch", "mlp_xent", "confocal_psf", "mnist_mlp")
+_PRODUCER_KINDS = ("lasso_batch", "mlp_xent", "confocal_psf", "mnist_mlp", "mnist_conv")
+_MNIST_KINDS = ("mnist_mlp", "mnist_conv")
 MetaLoss = collections.namedtuple("MetaLoss", "loss, update, reset, fx, x")
 MetaStep = collections.namedtuple("MetaStep", "step, update, reset, fx, x")
 
@@ -255,12 +256,14 @@ class _Program(object):
         one_net = len(self.runs) == 1 and self.runs[0].n == self.N
         if self.fused is not None and not (one_net and (len(self.variables) == 1 or
                                                         self.fused.kind in ("mlp_xent", "confocal_psf",
-                                                                            "mnist_mlp"))):
+                                                                            "mnist_mlp", "mnist_conv"))):
             self.fused = None
         if self.fused is not None and self.fused.kind == "confocal_psf" and not self._confocal_layout_ok(self.fused):
             self.fused = None   # the arena is not the kernel's [6P+1][B] row order: autograd, not a wrong layout
         if self.fused is not None and self.fused.kind == "mnist_mlp" and not self._mnist_ok(self.fused):
             self.fused = None   # a shape l2o_mnist_grad does not take, or not its arena order: the autograd path
+        if self.fused is not None and self.fused.kind == "mnist_conv" and not self._mnist_conv_ok(self.fused):
+            self.fused = None   # no batch norm, a batch l2o_mnist_conv_grad does not take, or not its arena order
         # "producer" optimizees (SURVEY.md 8(f) row 4): f and df/dx come from ONE library kernel per step instead of
         # torch autograd (~15 launches); the unroll stays step-at-a-time (the gradient couples coordinates) and is
         # captured into one CUDA graph like every external-gradient unroll
@@ -275,7 +278,7 @@ class _Program(object):
             self._confocal_sim = torch.zeros(len(names), self.variables[0]["shape"][0], device=self.device)
             for row, name in zip(self._confocal_sim, names):
                 self.const_vals[name] = row.view(shapes[name])
-        if self.producer is not None and self.producer.kind == "mnist_mlp":
+        if self.producer is not None and self.producer.kind in _MNIST_KINDS:
             # the split on the device (uploaded once per process, never reset), the seed and the device counter of the
             # kernel's batch draws, and the indices of each evaluation of the unroll: T steps + the final loss
             from .mnist_data import device_split
@@ -284,6 +287,9 @@ class _Program(object):
             self.mnist_seed = optimizer.seed
             self.mnist_counter = torch.zeros(1, dtype=torch.int64, device=self.device)
             self.mnist_idx = torch.zeros(self.T + 1, e["batch_size"], dtype=torch.int32, device=self.device)
+            if self.producer.kind == "mnist_conv":   # the ConvNet kernel's workspace, once per program
+                self.mnist_ws = torch.empty(_engine.mnist_conv_workspace_bytes(e["batch_size"]), dtype=torch.uint8,
+                                            device=self.device)
         self._draw = 0
         self.adam = _adam_slots(self.nets)
         self.dtheta = {k: torch.zeros(net.theta.numel(), dtype=torch.float64, device=self.device)
@@ -314,6 +320,16 @@ class _Program(object):
         names = [n for i in range(len(e["layers"]) + 1) for n in ("mlp/linear_{}/w".format(i), "mlp/linear_{}/b".format(i))]
         sizes = [int(np.prod(v["shape"])) for v in self.variables]
         return (_engine.mnist_fits(e["layers"], e["batch_size"]) and [v["name"] for v in self.variables] == names and
+                [s.start for s in self.var_slices] == [int(sum(sizes[:j])) for j in range(len(sizes))])
+
+    def _mnist_conv_ok(self, spec):
+        """l2o_mnist_conv_grad takes the ConvNet (batch norm on, its batch size), and the arena holds its six variables
+        in creation order."""
+        from .problems import MNIST_CONV_VARIABLES
+        e = spec.extra
+        sizes = [int(np.prod(v["shape"])) for v in self.variables]
+        return (e["batch_norm"] and _engine.mnist_conv_fits(e["batch_size"]) and
+                [(v["name"], tuple(v["shape"])) for v in self.variables] == list(MNIST_CONV_VARIABLES) and
                 [s.start for s in self.var_slices] == [int(sum(sizes[:j])) for j in range(len(sizes))])
 
     # ---- memory ---------------------------------------------------------------------------------
@@ -451,12 +467,17 @@ class _Program(object):
         elif p.kind == "confocal_psf":
             _engine.confocal_grad(Xflat, self._confocal_sim, g, self._confocal_sim.shape[1], p.extra["num_points"],
                                   p.extra["roi"], f=fx, scale=self.scale_flat if self.scale_active else None)
-        elif p.kind == "mnist_mlp":
+        elif p.kind in _MNIST_KINDS:
             # one draw per optimizee evaluation, recorded in row t of mnist_idx (T steps, then the final loss)
             t, self._draw = self._draw, self._draw + 1
-            _engine.mnist_grad(self.mnist_images, self.mnist_labels, Xflat, g, p.extra["layers"], p.extra["batch_size"],
-                               p.extra["activation"], self.mnist_seed, self.mnist_counter, f=fx,
-                               scale=self.scale_flat if self.scale_active else None, idx_out=self.mnist_idx[min(t, self.T)])
+            kw = dict(f=fx, scale=self.scale_flat if self.scale_active else None, idx_out=self.mnist_idx[min(t, self.T)])
+            if p.kind == "mnist_mlp":
+                _engine.mnist_grad(self.mnist_images, self.mnist_labels, Xflat, g, p.extra["layers"],
+                                   p.extra["batch_size"], p.extra["activation"], self.mnist_seed, self.mnist_counter,
+                                   **kw)
+            else:
+                _engine.mnist_conv_grad(self.mnist_images, self.mnist_labels, Xflat, g, p.extra["batch_size"],
+                                        self.mnist_seed, self.mnist_counter, self.mnist_ws, **kw)
         elif p.kind == "mlp_xent":
             from .problems import mlp_value_and_grad
             with torch.no_grad():

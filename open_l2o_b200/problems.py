@@ -22,6 +22,7 @@ class FusedSpec:
                      # | "lasso_batch" (producer kernel l2o_lasso_grad: a = A / w, b = y, alpha = l1 weight)
                      # | "mlp_xent" (mlp_value_and_grad) | "confocal_psf" (producer kernel l2o_confocal_grad)
                      # | "mnist_mlp" (producer kernel l2o_mnist_grad; extra: layers, activation, batch, split)
+                     # | "mnist_conv" (producer kernel l2o_mnist_conv_grad; extra: batch, split, batch_norm)
     var: str         # name of the trainable variable
     a: str           # constant names
     b: str
@@ -248,6 +249,55 @@ def mnist(layers, activation="sigmoid", batch_size=128, mode="train", data_dir="
     # producer kernel l2o_mnist_grad: the batch draw, forward and backward in one launch
     build.fused = FusedSpec("mnist_mlp", "mlp/linear_0/w", "", "", extra=dict(
         layers=layers, activation=activation, batch_size=int(batch_size), mode=mode, data_dir=data_dir))
+    return build
+
+
+MNIST_CONV_VARIABLES = (("conv_layer1/weights1", (3, 3, 1, 16)), ("conv_layer1/biases1", (16,)),
+                        ("conv_layer2/weights1", (5, 5, 16, 32)), ("conv_layer2/biases1", (32,)),
+                        ("fc_weights", (512, 10)), ("fc_bias", (10,)))
+
+
+def mnist_conv_forward(params, pixels, labels, batch_norm=True):
+    """The ConvNet of DM/problems.py:302-338 on a batch of fp32 pixels [B, 784]: NHWC semantics on torch's NCHW ops.
+    ``params`` are the six variables in creation order (HWIO conv weights)."""
+    w1, b1, w2, b2, wf, bf = params
+    F = torch.nn.functional
+    h = pixels.to(w1.dtype).reshape(-1, 1, 28, 28)
+    for w, b in ((w1, b1), (w2, b2)):
+        h = F.conv2d(h, w.permute(3, 2, 0, 1)) + b.reshape(1, -1, 1, 1)   # VALID, stride 1, then bias_add
+        if batch_norm:
+            # tf.layers.batch_normalization(training=True): batch mean and biased variance, eps 1e-3; its gamma / beta
+            # are not optimizee variables (DM/meta.py:88-99 patches tf.get_variable only), so they stay 1 and 0
+            h = F.batch_norm(h, None, None, training=True, eps=1e-3)
+        h = F.max_pool2d(F.relu(h), 2, 2)                   # VALID: 26 -> 13, 9 -> 4 (row and column 8 dropped)
+    h = h.permute(0, 2, 3, 1).reshape(h.shape[0], -1)     # tf.reshape([B, -1]) of NHWC: (h, w, c)
+    logits = F.relu(h @ wf + bf)                          # DM/problems.py:338: a ReLU on the logits
+    return F.cross_entropy(logits, labels.long())
+
+
+def mnist_conv(batch_norm=True, batch_size=128, mode="train", data_dir="MNIST-data"):
+    """MNIST classification with the batch-normalised ConvNet of DM/problems.py:291-347: conv 3x3 1->16 and conv 5x5
+    16->32 (VALID, each + bias, batch norm, ReLU, max-pool 2x2/2), fc 512->10 with a ReLU on the logits, the mean sparse
+    softmax cross entropy of a fresh batch of ``batch_size`` drawn uniformly with replacement at EVERY evaluation.  The
+    variables are the six of MNIST_CONV_VARIABLES (18,122 coordinates): weights N(0, 0.01), biases zero; batch norm's
+    gamma and beta are not among them.  The data come from ``data_dir`` as for ``mnist``."""
+    from . import mnist_data
+    if mode not in ("train", "validation", "test"):
+        raise ValueError("{} is not an MNIST split".format(mode))
+    num_examples = mnist_data.load_mnist(data_dir)[mode].num_examples
+
+    def build():
+        params = [get_variable(name, shape=list(shape),
+                               initializer=(random_normal_initializer(stddev=0.01) if len(shape) > 1 else
+                                            constant_initializer(0.0)))
+                  for name, shape in MNIST_CONV_VARIABLES]
+        images, labels = mnist_data.device_split(data_dir, mode, params[0].device)
+        idx = torch.randint(0, num_examples, (batch_size,), device=images.device)
+        pixels = images.index_select(0, idx).float() * float(mnist_data.SCALE)
+        return mnist_conv_forward(params, pixels, labels.index_select(0, idx), batch_norm)
+    # producer kernel l2o_mnist_conv_grad: the batch draw, forward and backward in one launch (batch norm on only)
+    build.fused = FusedSpec("mnist_conv", "conv_layer1/weights1", "", "", extra=dict(
+        batch_size=int(batch_size), mode=mode, data_dir=data_dir, batch_norm=bool(batch_norm)))
     return build
 
 

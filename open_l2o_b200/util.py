@@ -87,7 +87,7 @@ _MNIST = {"mnist": ((20,), "sigmoid"), "mnist_relu": ((20,), "relu"), "mnist_dee
 
 def get_config(problem_name, path=None, mode=None, num_hidden_layer=None, net_name=None, data_dir="MNIST-data"):
     """Returns problem configuration (DM/util.py:112-265) for the synthetic problems and, from the MNIST files in
-    ``data_dir`` (never downloaded), the MNIST MLPs."""
+    ``data_dir`` (never downloaded), the MNIST MLPs and ConvNet."""
     net_assignments = None
     if problem_name == "simple":
         problem = problems.simple()
@@ -113,6 +113,11 @@ def get_config(problem_name, path=None, mode=None, num_hidden_layer=None, net_na
             mode = "train" if path is None else "test"
         layers, activation = _MNIST[problem_name]
         problem = problems.mnist(layers=layers, activation=activation, mode=mode, data_dir=data_dir)
+        net_config = {"cw": get_default_net_config(path)}
+    elif problem_name == "mnist_conv":            # DM/util.py:164-169
+        if mode is None:
+            mode = "train" if path is None else "test"
+        problem = problems.mnist_conv(batch_norm=True, mode=mode, data_dir=data_dir)
         net_config = {"cw": get_default_net_config(path)}
     elif problem_name == "rastrigin_separable":   # BASELINE config #5
         problem = problems.rastrigin_separable(num_dims=1000000)
