@@ -75,18 +75,21 @@ def grad_v(kind, d, u, v):
 
 
 def do_fit(nets, kind, data, u0, v0, state0, unroll_unit, optim_it, rescale, out_mul=1.0, train=True,
-           meta_opts=None, select=None):
+           meta_opts=None, select=None, dtype=torch.float64):
     """One do_fit.  nets = (net_min, net_max); data[p] is (a, b) or A; u0, v0 [B][dim]; state0[n] = (h [2][R][H],
     c [2][R][H]).  meta_opts: the two torch.optim.Adam (or None: record gradients only).  select(t, traj_u) -> the
-    problems whose rewards enter the loss (curriculum), or None for all.
+    problems whose rewards enter the loss (curriculum), or None for all.  dtype: the precision of the variables, states
+    and problem data (the nets must already be in it); float32 gives the rounding error an fp32 implementation of the
+    same loop is entitled to.
     Returns per-iteration records (u, v, the [h1, c1, h2, c2] of both nets after the iteration, l_t) and per-segment gradients
     (a list over boundaries of [grads of net_min params, grads of net_max params], None where no path reached them)."""
     B, dim = len(u0), u0[0].numel()
     lr = sche_lr(optim_it)
-    u = [x.clone().double().requires_grad_(True) for x in u0]
-    v = [x.clone().double().requires_grad_(True) for x in v0]
-    hs = {n: [h.clone().double() for h in state0[n][0]] for n in (0, 1)}
-    cs = {n: [c.clone().double() for c in state0[n][1]] for n in (0, 1)}
+    data = [d.to(dtype) for d in data]
+    u = [x.clone().to(dtype).requires_grad_(True) for x in u0]
+    v = [x.clone().to(dtype).requires_grad_(True) for x in v0]
+    hs = {n: [h.clone().to(dtype) for h in state0[n][0]] for n in (0, 1)}
+    cs = {n: [c.clone().to(dtype) for c in state0[n][1]] for n in (0, 1)}
     reward = {0: [None] * B, 1: [None] * B}
     loss_prev = [0.0] * B
     recs, seg_grads = [], []
