@@ -12,7 +12,8 @@ with the same fetch semantics:
   * ``reset`` re-runs the initializers of state + x + constants (DM/meta.py:378-383).
 
 Two regimes (DESIGN.md): *fused* (separable optimizee evaluated in-kernel, one launch for all T steps) and
-*external-gradient* (torch autograd between single-step launches, state checkpointed in HBM).
+*external-gradient* (torch autograd, or a gradient producer of producers.py, between single-step launches, state
+checkpointed in HBM).
 """
 from __future__ import annotations
 
@@ -26,8 +27,6 @@ from . import engine as _engine
 from . import networks
 from .variables import variable_getter
 
-_PRODUCER_KINDS = ("lasso_batch", "mlp_xent", "confocal_psf", "mnist_mlp", "mnist_conv")
-_MNIST_KINDS = ("mnist_mlp", "mnist_conv")
 MetaLoss = collections.namedtuple("MetaLoss", "loss, update, reset, fx, x")
 MetaStep = collections.namedtuple("MetaStep", "step, update, reset, fx, x")
 
@@ -252,45 +251,14 @@ class _Program(object):
         self.var_slices, self.N, self.runs = plan_arena(self.variables, self.subsets, self.net_keys, self.nets)
         self.X = torch.zeros(self.N, device=self.device)
         self.const_vals = {}
-        self.fused = getattr(make_loss, "fused", None) if os.environ.get("L2O_DISABLE_FUSED") != "1" else None
-        one_net = len(self.runs) == 1 and self.runs[0].n == self.N
-        if self.fused is not None and not (one_net and (len(self.variables) == 1 or
-                                                        self.fused.kind in ("mlp_xent", "confocal_psf",
-                                                                            "mnist_mlp", "mnist_conv"))):
-            self.fused = None
-        if self.fused is not None and self.fused.kind == "confocal_psf" and not self._confocal_layout_ok(self.fused):
-            self.fused = None   # the arena is not the kernel's [6P+1][B] row order: autograd, not a wrong layout
-        if self.fused is not None and self.fused.kind == "mnist_mlp" and not self._mnist_ok(self.fused):
-            self.fused = None   # a shape l2o_mnist_grad does not take, or not its arena order: the autograd path
-        if self.fused is not None and self.fused.kind == "mnist_conv" and not self._mnist_conv_ok(self.fused):
-            self.fused = None   # no batch norm, a batch l2o_mnist_conv_grad does not take, or not its arena order
-        # "producer" optimizees (SURVEY.md 8(f) row 4): f and df/dx come from ONE library kernel per step instead of
-        # torch autograd (~15 launches); the unroll stays step-at-a-time (the gradient couples coordinates) and is
-        # captured into one CUDA graph like every external-gradient unroll
-        self.producer = None
-        if self.fused is not None and self.fused.kind in _PRODUCER_KINDS:
-            self.producer, self.fused = self.fused, None
-        if self.producer is not None and self.producer.kind == "confocal_psf":
-            # the simulated constants as row views of ONE [6P+1][B] buffer: reset_x refills them in place, so the kernel
-            # reads them with no packing launch per step and captured graphs stay valid
-            names = self.producer.extra["constants"]
-            shapes = {c["name"]: c["shape"] for c in self.constants}
-            self._confocal_sim = torch.zeros(len(names), self.variables[0]["shape"][0], device=self.device)
-            for row, name in zip(self._confocal_sim, names):
-                self.const_vals[name] = row.view(shapes[name])
-        if self.producer is not None and self.producer.kind in _MNIST_KINDS:
-            # the split on the device (uploaded once per process, never reset), the seed and the device counter of the
-            # kernel's batch draws, and the indices of each evaluation of the unroll: T steps + the final loss
-            from .mnist_data import device_split
-            e = self.producer.extra
-            self.mnist_images, self.mnist_labels = device_split(e["data_dir"], e["mode"], self.device)
-            self.mnist_seed = optimizer.seed
-            self.mnist_counter = torch.zeros(1, dtype=torch.int64, device=self.device)
-            self.mnist_idx = torch.zeros(self.T + 1, e["batch_size"], dtype=torch.int32, device=self.device)
-            if self.producer.kind == "mnist_conv":   # the ConvNet kernel's workspace, once per program
-                self.mnist_ws = torch.empty(_engine.mnist_conv_workspace_bytes(e["batch_size"]), dtype=torch.uint8,
-                                            device=self.device)
-        self._draw = 0
+        # both kernel regimes run one net over the whole arena; L2O_DISABLE_FUSED=1 turns both off (autograd, the
+        # reference the profile scripts and parity tests compare against)
+        enabled = os.environ.get("L2O_DISABLE_FUSED") != "1" and len(self.runs) == 1 and self.runs[0].n == self.N
+        fused, producer = getattr(make_loss, "fused", None), getattr(make_loss, "producer", None)
+        self.fused = fused if enabled and fused is not None and len(self.variables) == 1 else None
+        # a gradient producer (producers.py): f and df/dx from ONE library call per step instead of torch autograd
+        self.producer = (producer.bind(self) if enabled and producer is not None and
+                         producer.accepts(self.variables, self.var_slices, self.constants) else None)
         self.adam = _adam_slots(self.nets)
         self.dtheta = {k: torch.zeros(net.theta.numel(), dtype=torch.float64, device=self.device)
                        for k, net in self.nets.items()}
@@ -305,32 +273,6 @@ class _Program(object):
         self._graphs, self._eager_calls, self._graph_failed, self._graph_kernels = {}, {}, False, {}
         self._alloc_workspaces(optimizer.bptt_segment)
         self.reset()
-
-    def _confocal_layout_ok(self, spec):
-        """The arena and the constants are the [6P+1][B] rows l2o_confocal_grad reads, in its order."""
-        B = self.variables[0]["shape"][0]
-        return ([v["name"] for v in self.variables] == spec.extra["variables"] and
-                [c["name"] for c in self.constants] == spec.extra["constants"] and
-                all(tuple(r["shape"]) == (B, 1) for r in self.variables + self.constants) and
-                [s.start for s in self.var_slices] == [j * B for j in range(len(self.variables))])
-
-    def _mnist_ok(self, spec):
-        """l2o_mnist_grad takes the MLP, and the arena holds w0, b0, w1, b1, ... in creation order."""
-        e = spec.extra
-        names = [n for i in range(len(e["layers"]) + 1) for n in ("mlp/linear_{}/w".format(i), "mlp/linear_{}/b".format(i))]
-        sizes = [int(np.prod(v["shape"])) for v in self.variables]
-        return (_engine.mnist_fits(e["layers"], e["batch_size"]) and [v["name"] for v in self.variables] == names and
-                [s.start for s in self.var_slices] == [int(sum(sizes[:j])) for j in range(len(sizes))])
-
-    def _mnist_conv_ok(self, spec):
-        """l2o_mnist_conv_grad takes the ConvNet (batch norm on, its batch size), and the arena holds its six variables
-        in creation order."""
-        from .problems import MNIST_CONV_VARIABLES
-        e = spec.extra
-        sizes = [int(np.prod(v["shape"])) for v in self.variables]
-        return (e["batch_norm"] and _engine.mnist_conv_fits(e["batch_size"]) and
-                [(v["name"], tuple(v["shape"])) for v in self.variables] == list(MNIST_CONV_VARIABLES) and
-                [s.start for s in self.var_slices] == [int(sum(sizes[:j])) for j in range(len(sizes))])
 
     # ---- memory ---------------------------------------------------------------------------------
     def _alloc_workspaces(self, segment=None):
@@ -456,45 +398,13 @@ class _Program(object):
         """The optimizee variables of ``Xflat`` (default: the committed x) as host arrays in creation order."""
         return [v.cpu().numpy() for v in self._var_views(self.X if Xflat is None else Xflat)]
 
-    def _produce(self, Xflat):
-        """f(x) and df/dx from the fused producer kernel (one launch)."""
-        p = self.producer
-        g = torch.empty_like(Xflat)
-        fx = torch.zeros((), dtype=torch.float64, device=self.device)
-        if p.kind == "lasso_batch":
-            _engine.lasso_grad(self.const_vals[p.a], self.const_vals[p.b], Xflat, p.alpha, g, f=fx,
-                               scale=self.scale_flat if self.scale_active else None)
-        elif p.kind == "confocal_psf":
-            _engine.confocal_grad(Xflat, self._confocal_sim, g, self._confocal_sim.shape[1], p.extra["num_points"],
-                                  p.extra["roi"], f=fx, scale=self.scale_flat if self.scale_active else None)
-        elif p.kind in _MNIST_KINDS:
-            # one draw per optimizee evaluation, recorded in row t of mnist_idx (T steps, then the final loss)
-            t, self._draw = self._draw, self._draw + 1
-            kw = dict(f=fx, scale=self.scale_flat if self.scale_active else None, idx_out=self.mnist_idx[min(t, self.T)])
-            if p.kind == "mnist_mlp":
-                _engine.mnist_grad(self.mnist_images, self.mnist_labels, Xflat, g, p.extra["layers"],
-                                   p.extra["batch_size"], p.extra["activation"], self.mnist_seed, self.mnist_counter,
-                                   **kw)
-            else:
-                _engine.mnist_conv_grad(self.mnist_images, self.mnist_labels, Xflat, g, p.extra["batch_size"],
-                                        self.mnist_seed, self.mnist_counter, self.mnist_ws, **kw)
-        elif p.kind == "mlp_xent":
-            from .problems import mlp_value_and_grad
-            with torch.no_grad():
-                xs = Xflat * self.scale_flat if self.scale_active else Xflat    # f(x (.) scale), DM/meta_dm_train.py:384
-                fx = mlp_value_and_grad(self._var_views(xs), self.const_vals[p.a], self.const_vals[p.b],
-                                        p.extra["activation"], self._var_views(g)).double()
-                if self.scale_active:
-                    g.mul_(self.scale_flat)
-        else:
-            raise ValueError(p.kind)
-        return fx, g
-
-    def _value_and_grad(self, Xflat):
-        """f(x) and df/dx as a flat [N] tensor.  Each variable is its own autograd leaf (a view of the arena), so the
-        backward pass produces one gradient per variable and never materialises zero-filled [N] tensors."""
+    def _value_and_grad(self, Xflat, t=None):
+        """f(x) and df/dx as a flat [N] tensor at evaluation ``t`` of the unroll (0..T-1 the steps, T or None the final
+        loss).  A producer makes them in one call; otherwise each variable is its own autograd leaf (a view of the
+        arena), so the backward pass produces one gradient per variable and never materialises zero-filled [N]
+        tensors."""
         if self.producer is not None:
-            return self._produce(Xflat)
+            return self.producer(Xflat, self.scale_flat if self.scale_active else None, self.T if t is None else t)
         leaves = [v.detach().requires_grad_(True) for v in self._var_views(Xflat)]
         with torch.enable_grad():
             fx = self._loss_from_vars(leaves)
@@ -595,14 +505,13 @@ class _Program(object):
     def _forward_external(self, train, step0):
         T, Xw = self.T, self._Xw
         self._fused_regime = False
-        self._draw = 0
         Xw.copy_(self.X)
         fxs = []
         for r in self.runs:
             self._state_slot(r, 0).copy_(r.state)
             self._load_moments(r)
         for t in range(T):
-            fx, g = self._value_and_grad(Xw)
+            fx, g = self._value_and_grad(Xw, t)
             fxs.append(fx)
             for r in self.runs:
                 h = r.net.handle
@@ -620,15 +529,14 @@ class _Program(object):
                 h.step(r.net.theta, r.g_rec[t], self._state_slot(r, t), self._state_slot(r, t + 1),
                        x=Xw[r.off:r.off + r.n], reuse_weights=(t > 0), **kw)
         if train:
-            fx, g = self._value_and_grad(Xw)
+            fx, g = self._value_and_grad(Xw, T)
             for r in self.runs:
                 r.g_rec[T].copy_(g[r.off:r.off + r.n])
+        elif self.producer is not None:
+            fx = self._value_and_grad(Xw, T)[0]
         else:
-            if self.producer is not None:
-                fx = self._produce(Xw)[0]
-            else:
-                with torch.no_grad():
-                    fx = self._loss_at(Xw)
+            with torch.no_grad():
+                fx = self._loss_at(Xw)
         fxs.append(fx)
         for r in self.runs:
             r.state_final = self._state_slot(r, T)
@@ -835,11 +743,11 @@ class _MtTask(object):
             h.unroll_fwd(r.net.theta, n, T, work, in_seq=inp, ckpt=sb["ckpt"] if train else None, labels=lab,
                          imit_loss=self.il, n_total=self.n_total, delta_seq=sb["dseq"] if train else None, **kw)
             if train:  # the recorded deltas let the tensor-core BPTT run in imitation mode too
-                extra = dict(prog._bwd_extra(r), delta_seq=sb["dseq"])
+                bwd_kw = dict(prog._bwd_extra(r), delta_seq=sb["dseq"])
                 if "scratch" in sb:
-                    extra["scratch"] = sb["scratch"]
+                    bwd_kw["scratch"] = sb["scratch"]
                 h.unroll_bwd(r.net.theta, n, T, in_seq, sb["ckpt"], prog.dtheta[r.key], labels=lab, n_total=self.n_total,
-                             **extra)
+                             **bwd_kw)
             finals.append((work, moments))
         out = {}
         if "loss_mt" in kinds:

@@ -2,7 +2,7 @@
 ``build()`` that creates its tensors through ``get_variable`` and returns a scalar loss, exactly like
 DM/problems.py; gradients come from torch autograd on the device (the "external-gradient" regime) unless
 the builder carries a ``fused`` spec, in which case the unroll kernel evaluates the separable gradient
-in-kernel (the "fused" regime)."""
+in-kernel (the "fused" regime), or a ``producer`` (producers.py) that makes f and df/dx in one call."""
 from __future__ import annotations
 
 import math
@@ -11,26 +11,20 @@ from dataclasses import dataclass
 import numpy as np
 import torch
 
-from .engine import confocal_fits
+from . import producers
 from .variables import (constant_initializer, get_variable, ones_initializer, random_normal_initializer,
                         random_uniform_initializer)
 
 
 @dataclass
 class FusedSpec:
-    kind: str        # "rastrigin_sep" | "quadratic_diag" | "quadratic_batch" (in-kernel, include/l2o_b200.h L2O_OPT_*)
-                     # | "lasso_batch" (producer kernel l2o_lasso_grad: a = A / w, b = y, alpha = l1 weight)
-                     # | "mlp_xent" (mlp_value_and_grad) | "confocal_psf" (producer kernel l2o_confocal_grad)
-                     # | "mnist_mlp" (producer kernel l2o_mnist_grad; extra: layers, activation, batch, split)
-                     # | "mnist_conv" (producer kernel l2o_mnist_conv_grad; extra: batch, split, batch_norm)
-    var: str         # name of the trainable variable
+    """An optimizee the unroll kernel evaluates in-kernel: one launch for all T steps of its one variable."""
+    kind: str        # a key of engine.OPT_KINDS: "rastrigin_sep" | "quadratic_diag" | "quadratic_batch"
     a: str           # constant names
     b: str
     alpha: float = 10.0
     fscale: float = 1.0
     group: int = 0   # "quadratic_batch": coordinates per dense group
-    extra: dict = None   # producer-specific structure ("mlp_xent": activation, number of layers;
-                         # "confocal_psf": points, ROI, the trainable and the simulated names in kernel row order)
 
 
 def simple():
@@ -63,7 +57,7 @@ def quadratic(batch_size=128, num_dims=10, stddev=0.01):
     # kernels are throughput-bound: at BASELINE config #1's 1,280 coordinates a thread walks the whole LSTM serially
     # either way, and the graph-captured step-at-a-time path is measured faster (1.29 vs 1.63 ms per unroll).
     if num_dims <= 128 and batch_size * num_dims >= 16384:
-        build.fused = FusedSpec("quadratic_batch", "x", "w", "y", fscale=1.0 / batch_size, group=num_dims)
+        build.fused = FusedSpec("quadratic_batch", "w", "y", fscale=1.0 / batch_size, group=num_dims)
     return build
 
 
@@ -83,7 +77,7 @@ def lasso(batch_size=128, num_dims=10, stddev=0.01, l=0.005):
         y = get_variable("y", shape=[batch_size, num_dims, 1], initializer=random_uniform_initializer(),
                          trainable=False)
         return _lasso_loss(x, w, y, l)
-    build.fused = FusedSpec("lasso_batch", "x", "w", "y", alpha=float(l))   # producer kernel: f and df/dx in one launch
+    build.producer = producers.Lasso("x", "w", "y", alpha=float(l))
     return build
 
 
@@ -97,7 +91,7 @@ def lasso_fixed(data_A, data_b, stddev=0.01, l=0.005):
         w = get_variable("w", shape=list(a.shape), initializer=constant_initializer(a), trainable=False)
         y = get_variable("y", shape=list(b.shape), initializer=constant_initializer(b), trainable=False)
         return _lasso_loss(x, w, y, l)
-    build.fused = FusedSpec("lasso_batch", "x", "w", "y", alpha=float(l))   # producer kernel: f and df/dx in one launch
+    build.producer = producers.Lasso("x", "w", "y", alpha=float(l))
     return build
 
 
@@ -143,7 +137,7 @@ def rastrigin_separable(num_dims=1000000, alpha=10.0, stddev=1.0, normalize=True
         c = get_variable("c", shape=[n_loc], initializer=normal, trainable=False)
         fi = 0.5 * (x - b) ** 2 - alpha * c * torch.cos(two_pi * x) + alpha
         return fscale * torch.sum(fi)
-    build.fused = FusedSpec("rastrigin_sep", "x", "b", "c", alpha=float(alpha), fscale=fscale)
+    build.fused = FusedSpec("rastrigin_sep", "b", "c", alpha=float(alpha), fscale=fscale)
     return build
 
 
@@ -156,7 +150,7 @@ def quadratic_diag(num_dims=1280, stddev=0.01, normalize=True):
         w = get_variable("w", shape=[num_dims], initializer=random_uniform_initializer(0.5, 1.5), trainable=False)
         y = get_variable("y", shape=[num_dims], initializer=random_uniform_initializer(), trainable=False)
         return fscale * torch.sum((w * x - y) ** 2)
-    build.fused = FusedSpec("quadratic_diag", "x", "w", "y", fscale=fscale)
+    build.fused = FusedSpec("quadratic_diag", "w", "y", fscale=fscale)
     return build
 
 
@@ -183,8 +177,7 @@ def mlp(layers=(100,), in_dim=784, n_classes=10, batch_size=128, activation="sig
             k = width
         return torch.nn.functional.cross_entropy(h, labels.long())
     # analytic producer: f and df/dx without the autograd engine (mlp_value_and_grad below)
-    build.fused = FusedSpec("mlp_xent", "mlp", "data", "labels", extra=dict(activation=activation,
-                                                                           n_layers=len(tuple(layers)) + 1))
+    build.producer = producers.MlpXent(activation, n_layers=len(tuple(layers)) + 1)
     return build
 
 
@@ -246,9 +239,8 @@ def mnist(layers, activation="sigmoid", batch_size=128, mode="train", data_dir="
             if i < len(layers):
                 h = act(h)
         return torch.nn.functional.cross_entropy(h, labels.index_select(0, idx).long())
-    # producer kernel l2o_mnist_grad: the batch draw, forward and backward in one launch
-    build.fused = FusedSpec("mnist_mlp", "mlp/linear_0/w", "", "", extra=dict(
-        layers=layers, activation=activation, batch_size=int(batch_size), mode=mode, data_dir=data_dir))
+    build.producer = producers.MnistMlp(batch_size=int(batch_size), mode=mode, data_dir=data_dir, layers=layers,
+                                        activation=activation)
     return build
 
 
@@ -295,9 +287,8 @@ def mnist_conv(batch_norm=True, batch_size=128, mode="train", data_dir="MNIST-da
         idx = torch.randint(0, num_examples, (batch_size,), device=images.device)
         pixels = images.index_select(0, idx).float() * float(mnist_data.SCALE)
         return mnist_conv_forward(params, pixels, labels.index_select(0, idx), batch_norm)
-    # producer kernel l2o_mnist_conv_grad: the batch draw, forward and backward in one launch (batch norm on only)
-    build.fused = FusedSpec("mnist_conv", "conv_layer1/weights1", "", "", extra=dict(
-        batch_size=int(batch_size), mode=mode, data_dir=data_dir, batch_norm=bool(batch_norm)))
+    build.producer = producers.MnistConv(batch_size=int(batch_size), mode=mode, data_dir=data_dir,
+                                         batch_norm=bool(batch_norm), variables=MNIST_CONV_VARIABLES)
     return build
 
 
@@ -351,11 +342,9 @@ def confocal_microscopy_3d(batch_size=128, num_points=5, ROI=(28, 28, 28), stdde
         bg_sim = get_variable("bg_sim", shape=[batch_size, 1], initializer=random_uniform_initializer(), trainable=False)
         return torch.mean(torch.sum((y_pred + bg_var - _l2_normalize(y_sim + bg_sim)) ** 2, dim=1))
     # the separable PSF lets one kernel launch produce f and df/dx without forming the [batch, voxels] image in HBM
-    if confocal_fits(num_points, ROI):
-        names = ["%s_var_%d" % (n, i) for i in range(num_points) for n in _PSF_PARAMS] + ["bg_var"]
-        sims = [("y_sim%d" if n == "y" else n + "_sim_%d") % i for i in range(num_points) for n in _PSF_PARAMS]
-        build.fused = FusedSpec("confocal_psf", "I_var_0", "I_sim_0", "bg_sim",
-                                extra=dict(num_points=num_points, roi=ROI, variables=names, constants=sims + ["bg_sim"]))
+    names = ["%s_var_%d" % (n, i) for i in range(num_points) for n in _PSF_PARAMS] + ["bg_var"]
+    sims = [("y_sim%d" if n == "y" else n + "_sim_%d") % i for i in range(num_points) for n in _PSF_PARAMS]
+    build.producer = producers.Confocal(num_points, ROI, variables=names, constants=sims + ["bg_sim"])
     return build
 
 

@@ -48,10 +48,10 @@ def main():
 
     # (a) one step's f and df/dx
     p = pf.producer
-    B, P, roi = pf._confocal_sim.shape[1], p.extra["num_points"], p.extra["roi"]
+    B, P, roi = p.sim.shape[1], p.num_points, p.roi
     g = torch.empty_like(pf.X)
     fx = torch.zeros((), dtype=torch.float64, device=pf.X.device)
-    kernel = lambda: engine.confocal_grad(pf.X, pf._confocal_sim, g, B, P, roi, f=fx)   # noqa: E731
+    kernel = lambda: engine.confocal_grad(pf.X, p.sim, g, B, P, roi, f=fx)   # noqa: E731
     autograd = lambda: pa._value_and_grad(pa.X)   # noqa: E731
     f_k, g_k = pf._value_and_grad(pf.X)
     f_a, g_a = autograd()

@@ -74,7 +74,7 @@ def test_square_cos_oracle_equals_builder_loss():
     assert rel_err(co.square_cos_f(x, w, y, wcos), loss) <= 1e-6
 
 
-def test_get_config_entries():
+def test_get_config_entries_and_their_producers():
     from open_l2o_b200 import util
     cw = {"cw": {"net": "CoordinateWiseDeepLSTM", "net_options": {"layers": (20, 20)}, "net_path": None}}
     for name, (n_var, n_const, size) in {"confocal_microscopy_3d": (31, 31, 32), "square_cos": (1, 3, 256)}.items():
@@ -84,10 +84,10 @@ def test_get_config_entries():
         assert (len(var), len(const)) == (n_var, n_const)
         assert sum(t.numel() for _, _, t in var) == (size if name == "square_cos" else 31 * size)
     problem, _, _ = util.get_config("confocal_microscopy_3d")
-    assert problem.fused.kind == "confocal_psf" and problem.fused.extra["num_points"] == 5
-    assert problem.fused.extra["roi"] == (28, 28, 28)
+    assert problem.producer.kind == "confocal_psf" and problem.producer.num_points == 5
+    assert problem.producer.roi == (28, 28, 28)
     square, _, _ = util.get_config("square_cos")
-    assert getattr(square, "fused", None) is None
+    assert getattr(square, "fused", None) is None and getattr(square, "producer", None) is None
 
 
 def test_confocal_args_follow_the_header_field_order():

@@ -70,13 +70,13 @@ def _train_confocal(monkeypatch, disable_fused, graphs=True, T=20):
     return prog, (theta0, x0, sim0), out
 
 
-def test_confocal_training_producer_matches_autograd_and_oracle(monkeypatch):
+def test_confocal_bound_producer_matches_autograd_and_oracle(monkeypatch):
     T = 20
     prog, init, fused = _train_confocal(monkeypatch, False, T=T)
     assert prog.producer is not None and prog.producer.kind == "confocal_psf"
     # the simulated constants are rows of the one buffer the kernel reads
-    assert all(prog.const_vals[n].data_ptr() == prog._confocal_sim[k].data_ptr()
-               for k, n in enumerate(prog.producer.extra["constants"]))
+    assert all(prog.const_vals[n].data_ptr() == prog.producer.sim[k].data_ptr()
+               for k, n in enumerate(prog.producer.constants))
     prog_ag, init_ag, autograd = _train_confocal(monkeypatch, True, T=T)
     assert prog_ag.producer is None and not prog_ag._graph_failed and True in prog_ag._graphs
     assert all(torch.equal(a, b) for a, b in zip(init, init_ag))

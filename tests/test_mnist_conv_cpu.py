@@ -45,16 +45,16 @@ def _run(build, params=None):
     return made, loss, drawn[-1]
 
 
-def test_registry_matches_the_reference(tmp_path):
+def test_registry_producer_matches_the_reference(tmp_path):
     write_mnist(str(tmp_path))
     problem, net_config, assignments = util.get_config("mnist_conv", data_dir=str(tmp_path))
     assert assignments is None and net_config == {"cw": util.get_default_net_config(None)}
-    e = problem.fused.extra
-    assert problem.fused.kind == "mnist_conv" and e["batch_norm"] is True and e["batch_size"] == 128
-    assert e["mode"] == "train" and e["data_dir"] == str(tmp_path)
-    assert util.get_config("mnist_conv", path="/some/net", data_dir=str(tmp_path))[0].fused.extra["mode"] == "test"
+    p = problem.producer
+    assert p.kind == "mnist_conv" and p.batch_norm is True and p.batch_size == 128
+    assert p.mode == "train" and p.data_dir == str(tmp_path)
+    assert util.get_config("mnist_conv", path="/some/net", data_dir=str(tmp_path))[0].producer.mode == "test"
     assert util.get_config("mnist_conv", path="/some/net", mode="validation",
-                           data_dir=str(tmp_path))[0].fused.extra["mode"] == "validation"
+                           data_dir=str(tmp_path))[0].producer.mode == "validation"
     rp = util.get_config("mnist_conv", net_name="RNNprop", data_dir=str(tmp_path))[1]
     assert list(rp) == ["rp"] and rp["rp"]["net"] == "RNNprop"
     made, loss, idx = _run(problem)
@@ -123,10 +123,10 @@ def test_torch_build_equals_a_numpy_forward_of_the_spec(tmp_path):
     assert abs(float(loss) - ref) <= 1e-10 * abs(ref), (float(loss), ref)
 
 
-def test_without_batch_norm_builds_and_keeps_the_autograd_path(tmp_path):
+def test_without_batch_norm_builds_and_its_producer_keeps_the_flag(tmp_path):
     write_mnist(str(tmp_path))
     build = problems.mnist_conv(batch_norm=False, data_dir=str(tmp_path))
-    assert build.fused.extra["batch_norm"] is False
+    assert build.producer.batch_norm is False
     made, loss, _ = _run(build)
     assert list(made) == NAMES and np.isfinite(float(loss))
 

@@ -243,8 +243,8 @@ def _parity(data_dir, rnnprop, monkeypatch):
     for it in range(2):
         cost, xs, _, _ = sess.run([ms.fx, ms.x, ms.update, ms.step])
         torch.cuda.synchronize()
-        assert int(prog.mnist_counter) == (it + 1) * (T + 1)
-        rep.start(prog.mnist_idx.clone())
+        assert int(prog.producer.counter) == (it + 1) * (T + 1)
+        rep.start(prog.producer.idx.clone())
         with torch.device(DEV):
             res = tr.run_unroll(T)
         fx = prog.last_fx.cpu()
@@ -258,7 +258,7 @@ def _parity(data_dir, rnnprop, monkeypatch):
             images, labels = _split(data_dir)
             assert len(calls) == T + 1
             for t, (xc, ic, gc, dec) in enumerate(calls):
-                assert torch.equal(ic, prog.mnist_idx[t]) and torch.equal(gc, prog.runs[0].g_rec[t]), t
+                assert torch.equal(ic, prog.producer.idx[t]) and torch.equal(gc, prog.runs[0].g_rec[t]), t
                 _, g_ref, flips = fp64_grad(xc, images, labels, ic, dec)
                 assert flips <= MAX_FLIPS, (t, flips)
                 assert_grad_close(gc, g_ref, ("step", t))
@@ -268,7 +268,7 @@ def _parity(data_dir, rnnprop, monkeypatch):
 
 
 @pytest.mark.parametrize("rnnprop", [False, True])
-def test_mnist_conv_meta_training_matches_oracle(data_dir, rnnprop, monkeypatch):
+def test_mnist_conv_bound_producer_meta_training_matches_oracle(data_dir, rnnprop, monkeypatch):
     """get_config("mnist_conv"), T = 20, two unrolls: per-step fx, x and dtheta against the oracle replaying the
     engine's [T+1][B] recorded batches and gradients; the counter advances by T + 1 per unroll; and every gradient the
     first unroll recorded against fp64 autograd at the x and batch it was computed at."""
@@ -288,12 +288,12 @@ def _graph_run(data_dir, segment, unrolls=4, T=10):
     for it in range(unrolls):
         sess.run([ms.fx, ms.update, ms.step])
         torch.cuda.synchronize()
-        out.append((int(prog.mnist_counter), prog.mnist_idx.clone().cpu(),
+        out.append((int(prog.producer.counter), prog.producer.idx.clone().cpu(),
                     next(iter(prog.dtheta.values())).clone().cpu()))
     return prog, out
 
 
-def test_mnist_conv_graph_replay_draws_fresh_batches(data_dir):
+def test_mnist_conv_graph_replay_advances_the_producer_counter(data_dir):
     """Unrolls 3 and 4 replay one captured graph and still draw new batches; the counter advances by T + 1 per unroll
     with and without BPTT segments, whose recomputation draws nothing."""
     T = 10
@@ -311,7 +311,7 @@ def test_mnist_conv_graph_replay_draws_fresh_batches(data_dir):
         assert rel_err(seg[it][2], full[it][2]) <= REL_TOL, (it, rel_err(seg[it][2], full[it][2]))
 
 
-def test_mnist_conv_eval_epoch_draws_per_evaluation(data_dir):
+def test_mnist_conv_eval_epoch_producer_draws_per_evaluation(data_dir):
     """util.run_eval_epoch over a meta_loss of get_config("mnist_conv", mode="test"): T + 1 draws per unroll."""
     from open_l2o_b200 import meta, util
     T = 10
@@ -323,8 +323,8 @@ def test_mnist_conv_eval_epoch_draws_per_evaluation(data_dir):
     _, costs = util.run_eval_epoch(sess, cost_op, [update], 3)
     assert len(costs) == 3 and all(np.isfinite(costs))
     prog = optimizer.program
-    assert prog.producer.kind == "mnist_conv" and int(prog.mnist_counter) == 3 * (T + 1)
-    assert int(prog.mnist_idx.max()) < 1000   # the 1,000 test images of the fixture
+    assert prog.producer.kind == "mnist_conv" and int(prog.producer.counter) == 3 * (T + 1)
+    assert int(prog.producer.idx.max()) < 1000   # the 1,000 test images of the fixture
 
 
 def test_without_batch_norm_meta_trains_on_the_autograd_path(data_dir):

@@ -81,15 +81,15 @@ def _capture(build):
 
 @pytest.mark.parametrize("name,layers,act", [("mnist", (20,), "sigmoid"), ("mnist_relu", (20,), "relu"),
                                              ("mnist_deeper", (20, 20), "sigmoid")])
-def test_registry_matches_the_reference(tmp_path, name, layers, act):
+def test_registry_producer_matches_the_reference(tmp_path, name, layers, act):
     write_mnist(str(tmp_path))
     problem, net_config, assignments = util.get_config(name, data_dir=str(tmp_path))
     assert assignments is None and net_config == {"cw": util.get_default_net_config(None)}
-    e = problem.fused.extra
-    assert problem.fused.kind == "mnist_mlp" and e["layers"] == layers and e["activation"] == act
-    assert e["mode"] == "train" and e["batch_size"] == 128
-    assert util.get_config(name, path="/some/net", data_dir=str(tmp_path))[0].fused.extra["mode"] == "test"
-    assert util.get_config(name, path="/some/net", mode="validation", data_dir=str(tmp_path))[0].fused.extra["mode"] \
+    p = problem.producer
+    assert p.kind == "mnist_mlp" and p.layers == layers and p.activation == act
+    assert p.mode == "train" and p.batch_size == 128
+    assert util.get_config(name, path="/some/net", data_dir=str(tmp_path))[0].producer.mode == "test"
+    assert util.get_config(name, path="/some/net", mode="validation", data_dir=str(tmp_path))[0].producer.mode \
         == "validation"
     rp = util.get_config(name, net_name="RNNprop", data_dir=str(tmp_path))[1]
     assert list(rp) == ["rp"] and rp["rp"]["net"] == "RNNprop"

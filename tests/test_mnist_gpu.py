@@ -209,8 +209,8 @@ def _parity(data_dir, rnnprop):
     for it in range(2):
         cost, xs, _, _ = sess.run([ms.fx, ms.x, ms.update, ms.step])
         torch.cuda.synchronize()
-        assert int(prog.mnist_counter) == (it + 1) * (T + 1)
-        rep.start(prog.mnist_idx.clone())
+        assert int(prog.producer.counter) == (it + 1) * (T + 1)
+        rep.start(prog.producer.idx.clone())
         with torch.device(DEV):
             res = tr.run_unroll(T)
         fx = prog.last_fx.cpu()
@@ -229,7 +229,7 @@ def tr_cpu(tr):
 
 
 @pytest.mark.parametrize("rnnprop", [False, True])
-def test_mnist_meta_training_matches_oracle(data_dir, rnnprop):
+def test_mnist_bound_producer_meta_training_matches_oracle(data_dir, rnnprop):
     """get_config("mnist"), T = 20, two unrolls: per-step fx, x and dtheta against the oracle replaying the engine's
     [T+1][B] recorded batches; the counter advances by T + 1 per unroll."""
     _parity(data_dir, rnnprop)
@@ -248,12 +248,12 @@ def _graph_run(data_dir, segment, unrolls=4, T=10):
     for it in range(unrolls):
         sess.run([ms.fx, ms.update, ms.step])
         torch.cuda.synchronize()
-        out.append((int(prog.mnist_counter), prog.mnist_idx.clone().cpu(),
+        out.append((int(prog.producer.counter), prog.producer.idx.clone().cpu(),
                     next(iter(prog.dtheta.values())).clone().cpu()))
     return prog, out
 
 
-def test_mnist_graph_replay_draws_fresh_batches(data_dir):
+def test_mnist_graph_replay_advances_the_producer_counter(data_dir):
     """Unrolls 3 and 4 replay one captured graph and still draw new batches; the counter advances by T + 1 per unroll
     with and without BPTT segments, whose recomputation draws nothing; dtheta agrees up to summation order."""
     T = 10
@@ -271,7 +271,7 @@ def test_mnist_graph_replay_draws_fresh_batches(data_dir):
         assert rel_err(seg[it][2], full[it][2]) <= REL_TOL, (it, rel_err(seg[it][2], full[it][2]))
 
 
-def test_mnist_eval_epoch_draws_per_evaluation(data_dir):
+def test_mnist_eval_epoch_producer_draws_per_evaluation(data_dir):
     """util.run_eval_epoch over a meta_loss of get_config("mnist", path=...): test split, T + 1 draws per unroll."""
     from open_l2o_b200 import meta, util
     T = 10
@@ -283,8 +283,8 @@ def test_mnist_eval_epoch_draws_per_evaluation(data_dir):
     _, costs = util.run_eval_epoch(sess, cost_op, [update], 3)
     assert len(costs) == 3 and all(np.isfinite(costs))
     prog = optimizer.program
-    assert int(prog.mnist_counter) == 3 * (T + 1)
-    assert int(prog.mnist_idx.max()) < 1000   # the 1,000 test images of the fixture
+    assert int(prog.producer.counter) == 3 * (T + 1)
+    assert int(prog.producer.idx.max()) < 1000   # the 1,000 test images of the fixture
 
 
 def test_train_dm_runs_on_a_local_mnist(data_dir, tmp_path):
