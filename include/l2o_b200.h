@@ -23,6 +23,8 @@
  *   l2o_confocal_grad                   problems.confocal_microscopy_3d + tf.gradients DM/problems.py:701-956, DM/meta.py:322-329
  *   l2o_mnist_grad                      problems.mnist (batch draw + MLP) + tf.gradients DM/problems.py:254-288, DM/meta.py:322-329
  *   l2o_mnist_conv_grad                 problems.mnist_conv (batch-norm ConvNet) + tf.gradients DM/problems.py:291-347, DM/meta.py:322-329
+ *   l2o_cifar_conv_grad                 problems.cifar10 (batch-norm ConvNet) + tf.gradients DM/problems.py:369-458, DM/meta.py:322-329
+ *   l2o_nas_grad                        problems.NAS (batch-norm NAS cell) + tf.gradients DM/problems.py:540-634, DM/meta.py:322-329
  *
  * Conventions: every pointer is a DEVICE pointer owned by the caller (PyTorch allocates); no hidden
  * allocation; `stream` is a cudaStream_t passed as void*; every entry returns 0 or a negative
@@ -354,6 +356,88 @@ int64_t l2o_mnist_conv_workspace_bytes(int32_t batch);
 #define L2O_MNIST_CONV_LAYOUT 4
 int l2o_mnist_conv_workspace_layout(int32_t batch, int64_t* off);
 int l2o_mnist_conv_grad(const l2o_mnist_conv_args* a, void* stream);
+
+/*   l2o_cifar_conv_grad  problems.cifar10(batch_norm=True), DM/problems.py:369-458 + tf.gradients at
+ *                   DM/meta.py:322-329: f = mean_b xent(ConvNet(images[idx_b] / 255), labels[idx_b]) with a fresh batch
+ *                   drawn as l2o_mnist_grad draws it (same seed / counter convention; the indices are uniform over the
+ *                   N rows given), g = df/dx.  A pixel is fp32(p) / fp32(255), a correctly rounded division, read NHWC
+ *                   from the record's [3][32][32] planes.  The ConvNet (NHWC): conv 3x3 3->16 stride 2 VALID + b1
+ *                   ([32,32] -> [15,15]), batch norm, ReLU, max-pool 2x2/2 ([15,15] -> [7,7]); conv 5x5 16->32 stride 2
+ *                   VALID + b2 ([7,7] -> [2,2]), batch norm, ReLU, max-pool 2x2/2 ([2,2] -> [1,1]); the 32 channels;
+ *                   fc 32->10 + bias, ReLU; batch norm in training mode with gamma = 1, beta = 0, eps 1e-3 and the
+ *                   biased variance over all B*H*W positions.  x, scale and g are the arena of the variables in creation
+ *                   order: conv_layer1/weights1 [3][3][3][16], conv_layer1/biases1 [16], conv_layer2/weights1
+ *                   [5][5][16][32], conv_layer2/biases1 [32], fc_weights [32][10], fc_bias [10] (13,610 floats);
+ *                   theta = x (.) scale (optional, random-scaling trick as l2o_lasso_grad).  One cooperative launch over
+ *                   the resident CTAs; bitwise deterministic on any SM count (no atomics).  `workspace` is caller-owned
+ *                   device memory of at least l2o_cifar_conv_workspace_bytes(batch) bytes, 16-byte aligned.  Limits:
+ *                   batch 1..1024; anything else, a null required pointer, a misaligned pointer or a short workspace
+ *                   is L2O_E_INVALID before any CUDA call. */
+#define L2O_CIFAR_CONV_COORDS 13610
+#define L2O_CIFAR_CONV_MAX_BATCH 1024
+typedef struct {
+  int32_t batch;          /* B */
+  int32_t num_examples;   /* N: rows of images / labels */
+  uint64_t seed;
+  int64_t* counter;       /* device scalar: read, then += 1 */
+  const uint8_t* images;  /* [N][3][32][32] raw pixels, the record's plane order */
+  const uint8_t* labels;  /* [N], each < 10 */
+  const float* x;         /* the arena */
+  const float* scale;     /* optional, the arena's layout */
+  float* g;               /* the arena's layout */
+  double* f;              /* optional scalar: = f */
+  int32_t* idx_out;       /* optional [B]: the indices drawn */
+  void* workspace;        /* caller-owned, >= l2o_cifar_conv_workspace_bytes(batch) bytes */
+  size_t workspace_bytes;
+} l2o_cifar_conv_args;
+/* bytes of workspace l2o_cifar_conv_grad needs at this batch size; L2O_E_INVALID outside 1..1024 */
+int64_t l2o_cifar_conv_workspace_bytes(int32_t batch);
+/* byte offsets inside the workspace of what the last call's ReLU and max-pool decisions were made from, so that a
+ * caller can check g against a reference taking the same decisions: [0] z1 (fp32 [B][15][15][16], conv1 + b1),
+ * [1] z2 (fp32 [B][2][2][32], conv2 + b2), [2] bn (fp32 [96]: mu1 [16], rstd1 [16], mu2 [32], rstd2 [32]; the
+ * normalised value is (z - mu) * rstd in fp32), [3] dlogits (fp32 [B][16], zero where the logit's ReLU is off).
+ * L2O_E_INVALID outside 1..1024 or for a null off. */
+#define L2O_CIFAR_CONV_LAYOUT 4
+int l2o_cifar_conv_workspace_layout(int32_t batch, int64_t* off);
+int l2o_cifar_conv_grad(const l2o_cifar_conv_args* a, void* stream);
+
+/*   l2o_nas_grad     problems.NAS(batch_norm=True), DM/problems.py:540-634 + tf.gradients at DM/meta.py:322-329:
+ *                   f = mean_b xent(NAS(images[idx_b] / 255), labels[idx_b]), the batch and the pixels as
+ *                   l2o_cifar_conv_grad, g = df/dx.  The network (NHWC): every conv 3x3 SAME stride 1 + bias, batch norm,
+ *                   ReLU; node0 = conv(x, 3->16), n0o2 = conv(node0), node1 = conv(node0), n1o3 = conv(node1) (16->16);
+ *                   node2 = avgpool 3x3/1 SAME(node1) + n0o2, the average over the in-image cells of each window;
+ *                   node3 = node2 + n1o3 + node0; the mean over the 1024 positions; fc 16->10 + bias, ReLU.  Batch norm
+ *                   as l2o_cifar_conv_grad.  x, scale and g are the arena of the variables in creation order:
+ *                   node0/weights1 [3][3][3][16], node0/biases1 [16], then node0_onto_node2, node1 and node1_onto_node3,
+ *                   each weights1 [3][3][16][16] and biases1 [16], then fc_weights [16][10], fc_bias [10] (7,578 floats).
+ *                   One cooperative launch, seven grid barriers; bitwise deterministic on any SM count (no atomics).
+ *                   Workspace, alignment and limits (batch 1..1024) as l2o_cifar_conv_grad. */
+#define L2O_NAS_COORDS 7578
+#define L2O_NAS_MAX_BATCH 1024
+typedef struct {
+  int32_t batch;          /* B */
+  int32_t num_examples;   /* N: rows of images / labels */
+  uint64_t seed;
+  int64_t* counter;       /* device scalar: read, then += 1 */
+  const uint8_t* images;  /* [N][3][32][32] raw pixels, the record's plane order */
+  const uint8_t* labels;  /* [N], each < 10 */
+  const float* x;         /* the arena */
+  const float* scale;     /* optional, the arena's layout */
+  float* g;               /* the arena's layout */
+  double* f;              /* optional scalar: = f */
+  int32_t* idx_out;       /* optional [B]: the indices drawn */
+  void* workspace;        /* caller-owned, >= l2o_nas_workspace_bytes(batch) bytes */
+  size_t workspace_bytes;
+} l2o_nas_args;
+/* bytes of workspace l2o_nas_grad needs at this batch size; L2O_E_INVALID outside 1..1024 */
+int64_t l2o_nas_workspace_bytes(int32_t batch);
+/* byte offsets inside the workspace of what the last call's ReLU decisions were made from: [0] z0, [1] za (n0o2),
+ * [2] z1 (node1), [3] zb (n1o3), each fp32 [B][32][32][16], conv + bias before batch norm; [4] bn (fp32 [4][2][16]:
+ * mu and rstd of node0, n0o2, node1, n1o3 in that order; the normalised value is (z - mu) * rstd in fp32), [5] dlogits
+ * (fp32 [B][16], zero where the logit's ReLU is off).  L2O_E_INVALID outside 1..1024 or for a null off. */
+#define L2O_NAS_LAYOUT 6
+int l2o_nas_workspace_layout(int32_t batch, int64_t* off);
+int l2o_nas_grad(const l2o_nas_args* a, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * L2O-Scale HierarchicalRNN update step (SURVEY.md 8(f) row 1; BASELINE config #4).

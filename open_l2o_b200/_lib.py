@@ -26,7 +26,8 @@ EXPORTS = [
     "l2o_net_create", "l2o_net_destroy", "l2o_net_set_engine", "l2o_theta_count", "l2o_state_floats", "l2o_workspace_bytes",
     "l2o_step", "l2o_unroll_fwd", "l2o_unroll_bwd", "l2o_unroll_bwd_carry", "l2o_tc_fwd_variant", "l2o_tc_weight_image", "l2o_adam_step", "l2o_log_and_sign", "l2o_lasso_grad",
     "l2o_confocal_grad", "l2o_mnist_grad", "l2o_mnist_conv_workspace_bytes", "l2o_mnist_conv_workspace_layout",
-    "l2o_mnist_conv_grad",
+    "l2o_mnist_conv_grad", "l2o_cifar_conv_workspace_bytes", "l2o_cifar_conv_workspace_layout", "l2o_cifar_conv_grad",
+    "l2o_nas_workspace_bytes", "l2o_nas_workspace_layout", "l2o_nas_grad",
     "l2o_dense_create", "l2o_dense_destroy", "l2o_dense_theta_count", "l2o_dense_state_floats", "l2o_dense_step",
     "l2o_dense_unroll_bwd",
     "l2o_launch_count", "l2o_status_string", "l2o_last_cuda_error", "l2o_version",
@@ -104,6 +105,23 @@ class MnistConvArgs(C.Structure):
 
 
 MNIST_CONV_COORDS, MNIST_CONV_MAX_BATCH, MNIST_CONV_LAYOUT = 18122, 1024, 4
+
+
+class CifarConvArgs(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("num_examples", C.c_int32), ("seed", C.c_uint64), ("counter", _fp),
+                ("images", _fp), ("labels", _fp), ("x", _fp), ("scale", _fp), ("g", _fp), ("f", _fp), ("idx_out", _fp),
+                ("workspace", _fp), ("workspace_bytes", C.c_size_t)]
+
+
+CIFAR_INPUT = 3 * 32 * 32
+CIFAR_CONV_COORDS, CIFAR_CONV_MAX_BATCH, CIFAR_CONV_LAYOUT = 13610, 1024, 4
+
+
+class NasArgs(C.Structure):
+    _fields_ = CifarConvArgs._fields_
+
+
+NAS_COORDS, NAS_MAX_BATCH, NAS_LAYOUT = 7578, 1024, 6
 
 
 class DenseDesc(C.Structure):
@@ -317,6 +335,18 @@ def lib():
     L.l2o_mnist_conv_workspace_layout.restype = C.c_int
     L.l2o_mnist_conv_grad.argtypes = [C.POINTER(MnistConvArgs), C.c_void_p]
     L.l2o_mnist_conv_grad.restype = C.c_int
+    L.l2o_cifar_conv_workspace_bytes.argtypes = [C.c_int32]
+    L.l2o_cifar_conv_workspace_bytes.restype = C.c_int64
+    L.l2o_cifar_conv_workspace_layout.argtypes = [C.c_int32, C.POINTER(C.c_int64)]
+    L.l2o_cifar_conv_workspace_layout.restype = C.c_int
+    L.l2o_cifar_conv_grad.argtypes = [C.POINTER(CifarConvArgs), C.c_void_p]
+    L.l2o_cifar_conv_grad.restype = C.c_int
+    L.l2o_nas_workspace_bytes.argtypes = [C.c_int32]
+    L.l2o_nas_workspace_bytes.restype = C.c_int64
+    L.l2o_nas_workspace_layout.argtypes = [C.c_int32, C.POINTER(C.c_int64)]
+    L.l2o_nas_workspace_layout.restype = C.c_int
+    L.l2o_nas_grad.argtypes = [C.POINTER(NasArgs), C.c_void_p]
+    L.l2o_nas_grad.restype = C.c_int
     L.l2o_dense_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(DenseDesc)]
     L.l2o_dense_create.restype = C.c_int
     L.l2o_dense_destroy.argtypes = [C.c_void_p]

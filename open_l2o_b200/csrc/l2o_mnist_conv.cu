@@ -43,6 +43,7 @@
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>
 
+#include "l2o_bn.cuh"
 #include "l2o_internal.h"
 #include "l2o_philox.cuh"
 
@@ -131,62 +132,6 @@ struct Args {
   Ws w;
 };
 
-// per-channel sum over the threads of one CTA, tid = q * C + c: red[tid] = v, then thread c < C adds q = 0.. in order
-__device__ __forceinline__ double chan_sum(double* red, double v, int C) {
-  const int tid = threadIdx.x;
-  red[tid] = v;
-  __syncthreads();
-  double s = 0.0;
-  if (tid < C)
-    for (int q = 0; q < kThreads / C; ++q) s += red[q * C + tid];
-  __syncthreads();
-  return s;   // meaningful in threads tid < C
-}
-
-// the BN statistics of the batch from the per-image (mean, M2) of n positions each: Chan's formula for equal counts
-__device__ void merge_stats(const double2* st, int B, int C, int n, double* red, float* mu_out, float* rs_out,
-                            double* mu_tmp) {
-  const int tid = threadIdx.x, c = tid % C, k = tid / C, K = kThreads / C;
-  double s = 0.0;
-  for (int b = k; b < B; b += K) s += __ldcg(&st[(size_t)b * C + c].x);
-  s = chan_sum(red, s, C);
-  if (tid < C) mu_tmp[tid] = s / (double)B;
-  __syncthreads();
-  const double mu = mu_tmp[c];
-  double m2 = 0.0;
-  for (int b = k; b < B; b += K) {
-    const double2 v = __ldcg(&st[(size_t)b * C + c]);
-    const double d = v.x - mu;
-    m2 += v.y + (double)n * d * d;
-  }
-  m2 = chan_sum(red, m2, C);
-  if (tid < C) {
-    const double var = m2 / ((double)B * (double)n);   // biased, as fused training-mode batch norm
-    mu_out[tid] = (float)mu_tmp[tid];
-    rs_out[tid] = (float)(1.0 / sqrt(var + (double)kEps));
-  }
-  __syncthreads();
-}
-
-// the BN backward means: sum_b (sum dy, sum dy * yhat) / (B n)
-__device__ void merge_back(const double2* bk, int B, int C, int n, double* red, float* ma, float* mb) {
-  const int tid = threadIdx.x, c = tid % C, k = tid / C, K = kThreads / C;
-  double s = 0.0, t = 0.0;
-  for (int b = k; b < B; b += K) {
-    const double2 v = __ldcg(&bk[(size_t)b * C + c]);
-    s += v.x;
-    t += v.y;
-  }
-  s = chan_sum(red, s, C);
-  t = chan_sum(red, t, C);
-  if (tid < C) {
-    const double nn = (double)B * (double)n;
-    ma[tid] = (float)(s / nn);
-    mb[tid] = (float)(t / nn);
-  }
-  __syncthreads();
-}
-
 // BN1, ReLU and max-pool of image b from its z1 in the workspace: p1 and the maxima's window places in shared memory
 __device__ void pool1(const float* z1, float* sm) {
   const float* mu = sm + sPc;
@@ -271,7 +216,7 @@ __global__ void __launch_bounds__(kThreads, 1) mnist_conv_kernel(const Args args
       z1[p * kC1 + c] = z;
       s += (double)z;
     }
-    s = chan_sum(red, s, kC1);
+    s = l2o::chan_sum<kThreads>(red, s, kC1);
     if (tid < kC1) mu_tmp[tid] = s / (double)(kH1 * kH1);
     __syncthreads();
     const double m = mu_tmp[c];
@@ -280,11 +225,11 @@ __global__ void __launch_bounds__(kThreads, 1) mnist_conv_kernel(const Args args
       const double d = (double)sm[sU + p * kC1 + c] - m;
       m2 += d * d;
     }
-    m2 = chan_sum(red, m2, kC1);
+    m2 = l2o::chan_sum<kThreads>(red, m2, kC1);
     if (tid < kC1) w.st1[(size_t)b * kC1 + tid] = make_double2(mu_tmp[tid], m2);
   }
   grid.sync();
-  merge_stats(w.st1, B, kC1, kH1 * kH1, red, mu1, rs1, mu_tmp);
+  l2o::merge_stats<kThreads>(w.st1, B, kC1, kH1 * kH1, kEps, red, mu1, rs1, mu_tmp);
   if (blockIdx.x == 0 && tid < kC1) {   // every CTA holds the same values; CTA 0 records them for the caller
     w.bn[tid] = mu1[tid];
     w.bn[kC1 + tid] = rs1[tid];
@@ -339,7 +284,7 @@ __global__ void __launch_bounds__(kThreads, 1) mnist_conv_kernel(const Args args
     const int c = tid & (kC2 - 1), q = tid >> 5;
     double s = 0.0;
     for (int p = q; p < kH2 * kH2; p += kThreads / kC2) s += (double)sm[sZ2 + p * kC2 + c];
-    s = chan_sum(red, s, kC2);
+    s = l2o::chan_sum<kThreads>(red, s, kC2);
     if (tid < kC2) mu_tmp[tid] = s / (double)(kH2 * kH2);
     __syncthreads();
     const double m = mu_tmp[c];
@@ -348,11 +293,11 @@ __global__ void __launch_bounds__(kThreads, 1) mnist_conv_kernel(const Args args
       const double d = (double)sm[sZ2 + p * kC2 + c] - m;
       m2 += d * d;
     }
-    m2 = chan_sum(red, m2, kC2);
+    m2 = l2o::chan_sum<kThreads>(red, m2, kC2);
     if (tid < kC2) w.st2[(size_t)b * kC2 + tid] = make_double2(mu_tmp[tid], m2);
   }
   grid.sync();
-  merge_stats(w.st2, B, kC2, kH2 * kH2, red, mu2, rs2, mu_tmp);
+  l2o::merge_stats<kThreads>(w.st2, B, kC2, kH2 * kH2, kEps, red, mu2, rs2, mu_tmp);
   if (blockIdx.x == 0 && tid < kC2) {
     w.bn[2 * kC1 + tid] = mu2[tid];
     w.bn[2 * kC1 + kC2 + tid] = rs2[tid];
@@ -434,12 +379,12 @@ __global__ void __launch_bounds__(kThreads, 1) mnist_conv_kernel(const Args args
       s1 += (double)d;
       s2 += (double)d * (double)((z2[p * kC2 + c] - mu2[c]) * rs2[c]);
     }
-    s1 = chan_sum(red, s1, kC2);
-    s2 = chan_sum(red, s2, kC2);
+    s1 = l2o::chan_sum<kThreads>(red, s1, kC2);
+    s2 = l2o::chan_sum<kThreads>(red, s2, kC2);
     if (tid < kC2) w.bk2[(size_t)b * kC2 + tid] = make_double2(s1, s2);
   }
   grid.sync();
-  merge_back(w.bk2, B, kC2, kH2 * kH2, red, ma2, mb2);
+  l2o::merge_back<kThreads>(w.bk2, B, kC2, kH2 * kH2, red, ma2, mb2);
 
   // ---- 4: dz2; dW2 and db2 of the image; dp1 = conv2 transposed, routed to the pool1 maxima; BN1 backward sums ---
   for (int b = blockIdx.x; b < B; b += G) {
@@ -462,7 +407,7 @@ __global__ void __launch_bounds__(kThreads, 1) mnist_conv_kernel(const Args args
       const int c = tid & (kC2 - 1), q = tid >> 5;
       float s = 0.f;
       for (int p = q; p < kH2 * kH2; p += kThreads / kC2) s += sm[sZ2 + p * kC2 + c];
-      const double t = chan_sum(red, (double)s, kC2);
+      const double t = l2o::chan_sum<kThreads>(red, (double)s, kC2);
       if (tid < kC2) part[oB2 + tid] = (float)t;
     }
     {   // dW2[r][o], r = (kh * 5 + kw) * 16 + c: warp = 4 output channels, lane = rows lane + 32 k
@@ -549,12 +494,12 @@ __global__ void __launch_bounds__(kThreads, 1) mnist_conv_kernel(const Args args
       s1 += (double)sm[sDyc + e];
       s2 += (double)sm[sDyc + e] * (double)sm[sYs + e];
     }
-    s1 = chan_sum(red, s1, kC1);
-    s2 = chan_sum(red, s2, kC1);
+    s1 = l2o::chan_sum<kThreads>(red, s1, kC1);
+    s2 = l2o::chan_sum<kThreads>(red, s2, kC1);
     if (tid < kC1) w.bk1[(size_t)b * kC1 + tid] = make_double2(s1, s2);
   }
   grid.sync();
-  merge_back(w.bk1, B, kC1, kH1 * kH1, red, ma1, mb1);
+  l2o::merge_back<kThreads>(w.bk1, B, kC1, kH1 * kH1, red, ma1, mb1);
 
   // ---- 5: dz1; dW1 and db1 of the image -------------------------------------------------------------------------
   for (int b = blockIdx.x; b < B; b += G) {

@@ -1,5 +1,6 @@
-// The in-kernel minibatch draw of the MNIST producers (l2o_mnist_grad, l2o_mnist_conv_grad): both draw the same
-// indices for the same (seed, counter), so the MLPs and the ConvNet see one index stream.
+// The in-kernel minibatch draw of the dataset-backed producers (l2o_mnist_grad, l2o_mnist_conv_grad,
+// l2o_cifar_conv_grad): all draw the same indices for the same (seed, counter, N), so the MNIST MLPs and ConvNet see
+// one index stream, and the CIFAR-10 ConvNet draws from its split by the same rule.
 //
 // Batch row b of the evaluation at device counter c takes Philox4x32-10 keyed by the 64-bit seed at counter
 // (b, 0, c_lo, c_hi); word 0 of the output is the draw r and idx_b = (r * N) >> 32 (a 64-bit multiply-high: each
@@ -36,5 +37,8 @@ __device__ __forceinline__ int batch_index(uint64_t seed, uint64_t ctr, int row,
 
 // read_data_sets: images.astype(float32) * (1.0 / 255.0), the double constant rounded to fp32 first
 __device__ __forceinline__ float mnist_pixel(uint8_t v) { return __fmul_rn((float)v, (float)(1.0 / 255.0)); }
+
+// the CIFAR-10 reader's tf.math.divide(image, 255) on a float32 image: a correctly rounded fp32 division
+__device__ __forceinline__ float cifar_pixel(uint8_t v) { return __fdiv_rn((float)v, 255.f); }
 
 }  // namespace l2o

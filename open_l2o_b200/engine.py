@@ -393,6 +393,93 @@ def mnist_conv_grad(images, labels, x, g, batch, seed, counter, workspace, f=Non
     _lib.check(_lib.lib().l2o_mnist_conv_grad(C.byref(a), _stream()), "l2o_mnist_conv_grad")
 
 
+def cifar_conv_fits(batch) -> bool:
+    """Whether l2o_cifar_conv_grad takes this batch size: 1..1024."""
+    return 1 <= int(batch) <= _lib.CIFAR_CONV_MAX_BATCH
+
+
+def cifar_conv_workspace_bytes(batch) -> int:
+    """Bytes of device workspace l2o_cifar_conv_grad needs at this batch size (the library allocates nothing)."""
+    n = int(_lib.lib().l2o_cifar_conv_workspace_bytes(int(batch)))
+    if n < 0:
+        raise L2OError(f"cifar_conv_workspace_bytes: batch {batch} is outside 1..{_lib.CIFAR_CONV_MAX_BATCH}")
+    return n
+
+
+def cifar_conv_workspace_layout(batch) -> dict:
+    """Byte offsets in the l2o_cifar_conv_grad workspace of z1, z2, the batch-norm constants and dlogits, the values
+    its ReLU and max-pool decisions come from (include/l2o_b200.h)."""
+    off = (C.c_int64 * _lib.CIFAR_CONV_LAYOUT)()
+    _lib.check(_lib.lib().l2o_cifar_conv_workspace_layout(int(batch), off), "l2o_cifar_conv_workspace_layout")
+    return dict(zip(("z1", "z2", "bn", "dl"), (int(v) for v in off)))
+
+
+def _cifar_args(cls, name, coords, images, labels, x, g, batch, seed, counter, workspace, f, scale, idx_out):
+    """The checked argument struct of a CIFAR-10 producer (l2o_cifar_conv_grad, l2o_nas_grad)."""
+    a = cls()
+    a.batch, a.num_examples = int(batch), int(images.shape[0])
+    a.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+    if images.numel() != a.num_examples * _lib.CIFAR_INPUT or labels.numel() != a.num_examples:
+        raise L2OError(f"{name}: images must be [N, 3072] and labels [N]")
+    for what, t in (("x", x), ("g", g), ("scale", scale)):
+        if t is not None and t.numel() != coords:
+            raise L2OError(f"{name}: {what} has {t.numel()} elements, the network has {coords}")
+    if idx_out is not None and idx_out.numel() != a.batch:
+        raise L2OError(f"{name}: idx_out has {idx_out.numel()} elements, batch is {a.batch}")
+    if counter.numel() != 1:
+        raise L2OError(f"{name}: counter must be one int64 element")
+    a.counter = _ptr(counter, torch.int64, "counter")
+    a.images, a.labels = _ptr(images, torch.uint8, "images"), _ptr(labels, torch.uint8, "labels")
+    a.x, a.scale, a.g = _ptr(x, name="x"), _ptr(scale, name="scale"), _ptr(g, name="g")
+    a.f = _ptr(f, torch.float64, "f")
+    a.idx_out = _ptr(idx_out, torch.int32, "idx_out")
+    a.workspace = _ptr(workspace, torch.uint8, "workspace")
+    a.workspace_bytes = workspace.numel()
+    return a
+
+
+def cifar_conv_grad(images, labels, x, g, batch, seed, counter, workspace, f=None, scale=None, idx_out=None):
+    """f and df/dx of problems.cifar10 (DM/problems.py:369-458, batch norm on) at a fresh batch in one launch.
+    images [N, 3072] (each row the record's [3][32][32] planes) and labels [N] uint8; x, g and scale the flat
+    13,610-float arena of the ConvNet's variables in creation order; ``counter`` a one-element int64 device tensor the
+    call reads and advances (the batch is drawn as mnist_grad draws it); ``workspace`` a uint8 device tensor of at
+    least cifar_conv_workspace_bytes(batch) bytes; writes f (fp64 scalar) and the indices drawn into ``idx_out``
+    (int32 [batch]) if given."""
+    a = _cifar_args(_lib.CifarConvArgs, "cifar_conv_grad", _lib.CIFAR_CONV_COORDS, images, labels, x, g, batch, seed,
+                    counter, workspace, f, scale, idx_out)
+    _lib.check(_lib.lib().l2o_cifar_conv_grad(C.byref(a), _stream()), "l2o_cifar_conv_grad")
+
+
+def nas_fits(batch) -> bool:
+    """Whether l2o_nas_grad takes this batch size: 1..1024."""
+    return 1 <= int(batch) <= _lib.NAS_MAX_BATCH
+
+
+def nas_workspace_bytes(batch) -> int:
+    """Bytes of device workspace l2o_nas_grad needs at this batch size (the library allocates nothing)."""
+    n = int(_lib.lib().l2o_nas_workspace_bytes(int(batch)))
+    if n < 0:
+        raise L2OError(f"nas_workspace_bytes: batch {batch} is outside 1..{_lib.NAS_MAX_BATCH}")
+    return n
+
+
+def nas_workspace_layout(batch) -> dict:
+    """Byte offsets in the l2o_nas_grad workspace of the four pre-batch-norm maps, the batch-norm constants and
+    dlogits, the values its ReLU decisions come from (include/l2o_b200.h)."""
+    off = (C.c_int64 * _lib.NAS_LAYOUT)()
+    _lib.check(_lib.lib().l2o_nas_workspace_layout(int(batch), off), "l2o_nas_workspace_layout")
+    return dict(zip(("z0", "za", "z1", "zb", "bn", "dl"), (int(v) for v in off)))
+
+
+def nas_grad(images, labels, x, g, batch, seed, counter, workspace, f=None, scale=None, idx_out=None):
+    """f and df/dx of problems.nas (DM/problems.py:540-634, batch norm on) at a fresh batch in one launch; the
+    arguments as cifar_conv_grad's, x, g and scale the flat 7,578-float arena of the cell's variables in creation
+    order, ``workspace`` at least nas_workspace_bytes(batch) bytes."""
+    a = _cifar_args(_lib.NasArgs, "nas_grad", _lib.NAS_COORDS, images, labels, x, g, batch, seed, counter, workspace,
+                    f, scale, idx_out)
+    _lib.check(_lib.lib().l2o_nas_grad(C.byref(a), _stream()), "l2o_nas_grad")
+
+
 _graph_replayed = 0  # kernels of this library launched through CUDA-graph replays (not visible to the C-side counter)
 
 

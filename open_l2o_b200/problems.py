@@ -292,6 +292,103 @@ def mnist_conv(batch_norm=True, batch_size=128, mode="train", data_dir="MNIST-da
     return build
 
 
+CIFAR10_VARIABLES = (("conv_layer1/weights1", (3, 3, 3, 16)), ("conv_layer1/biases1", (16,)),
+                     ("conv_layer2/weights1", (5, 5, 16, 32)), ("conv_layer2/biases1", (32,)),
+                     ("fc_weights", (32, 10)), ("fc_bias", (10,)))
+
+
+def cifar10_forward(params, pixels, labels, batch_norm=True):
+    """The ConvNet of DM/problems.py:410-448 on a batch of fp32 NHWC pixels [B, 32, 32, 3]: NHWC semantics on torch's
+    NCHW ops.  ``params`` are the six variables in creation order (HWIO conv weights)."""
+    w1, b1, w2, b2, wf, bf = params
+    F = torch.nn.functional
+    h = pixels.to(w1.dtype).reshape(-1, 32, 32, 3).permute(0, 3, 1, 2)
+    for w, b in ((w1, b1), (w2, b2)):
+        h = F.conv2d(h, w.permute(3, 2, 0, 1), stride=2) + b.reshape(1, -1, 1, 1)   # VALID, stride 2, then bias_add
+        if batch_norm:   # training mode, gamma = 1, beta = 0, as mnist_conv_forward (DESIGN §3.18)
+            h = F.batch_norm(h, None, None, training=True, eps=1e-3)
+        h = F.max_pool2d(F.relu(h), 2, 2)                   # VALID: 15 -> 7 (row and column 14 dropped), 2 -> 1
+    h = h.permute(0, 2, 3, 1).reshape(h.shape[0], -1)     # tf.reshape([B, -1]) of NHWC: (h, w, c)
+    logits = F.relu(h @ wf + bf)                          # DM/problems.py:448: a ReLU on the logits
+    return F.cross_entropy(logits, labels.long())
+
+
+def cifar10(batch_norm=True, batch_size=128, mode="train", data_dir="cifar10"):
+    """CIFAR-10 classification with the batch-normalised ConvNet of DM/problems.py:369-458: conv 3x3 3->16 and conv
+    5x5 16->32 (stride 2, VALID, each + bias, batch norm, ReLU, max-pool 2x2/2), fc 32->10 with a ReLU on the logits,
+    the mean sparse softmax cross entropy of a fresh batch of ``batch_size`` drawn uniformly with replacement at EVERY
+    evaluation (the reference dequeues from a shuffling queue instead; DESIGN §3.18).  The variables are the six of
+    CIFAR10_VARIABLES (13,610 coordinates): weights N(0, 0.01), biases zero; batch norm's gamma and beta are not among
+    them.  The data come from the CIFAR-10 binary files in ``data_dir`` (cifar_data; never downloaded)."""
+    from . import cifar_data
+    num_examples = cifar_data.load_cifar10(data_dir, mode).num_examples
+
+    def build():
+        params = [get_variable(name, shape=list(shape),
+                               initializer=(random_normal_initializer(stddev=0.01) if len(shape) > 1 else
+                                            constant_initializer(0.0)))
+                  for name, shape in CIFAR10_VARIABLES]
+        images, labels = cifar_data.device_split(data_dir, mode, params[0].device)
+        idx = torch.randint(0, num_examples, (batch_size,), device=images.device)
+        pixels = cifar_data.device_values(images.device)[images.index_select(0, idx).long()]   # fp32(p) / fp32(255)
+        pixels = pixels.reshape(-1, 3, 32, 32).permute(0, 2, 3, 1)                            # the planes, NHWC
+        return cifar10_forward(params, pixels, labels.index_select(0, idx), batch_norm)
+    build.producer = producers.CifarConv(batch_size=int(batch_size), mode=mode, data_dir=data_dir,
+                                         batch_norm=bool(batch_norm), variables=CIFAR10_VARIABLES)
+    return build
+
+
+NAS_VARIABLES = tuple((scope + suffix, shape) for scope, cin in (("node0", 3), ("node0_onto_node2", 16), ("node1", 16),
+                                                                  ("node1_onto_node3", 16))
+                      for suffix, shape in (("/weights1", (3, 3, cin, 16)), ("/biases1", (16,)))) + \
+    (("fc_weights", (16, 10)), ("fc_bias", (10,)))
+
+
+def nas_forward(params, pixels, labels, batch_norm=True):
+    """The NAS cell network of DM/problems.py:584-625 on a batch of fp32 NHWC pixels [B, 32, 32, 3]: NHWC semantics on
+    torch's NCHW ops.  ``params`` are the ten variables in creation order (HWIO conv weights)."""
+    w0, b0, wa, ba, w1, b1, wb, bb, wf, bf = params
+    F = torch.nn.functional
+
+    def conv(h, w, b):   # 3x3 SAME stride 1 (pad 1), bias_add, batch norm as cifar10_forward, ReLU
+        h = F.conv2d(h, w.permute(3, 2, 0, 1), padding=1) + b.reshape(1, -1, 1, 1)
+        if batch_norm:
+            h = F.batch_norm(h, None, None, training=True, eps=1e-3)
+        return F.relu(h)
+    node0 = conv(pixels.to(w0.dtype).reshape(-1, 32, 32, 3).permute(0, 3, 1, 2), w0, b0)
+    node0_onto_node2 = conv(node0, wa, ba)
+    node1 = conv(node0, w1, b1)
+    node1_onto_node3 = conv(node1, wb, bb)
+    # tf.nn.avg_pool SAME divides by the in-image cells of each window (4 at a corner, 6 on an edge, 9 inside)
+    node2 = F.avg_pool2d(node1, 3, 1, padding=1, count_include_pad=False) + node0_onto_node2
+    node3 = node2 + node1_onto_node3 + node0
+    logits = F.relu(node3.mean(dim=(2, 3)) @ wf + bf)   # the mean over the 1024 positions per channel
+    return F.cross_entropy(logits, labels.long())
+
+
+def nas(batch_norm=True, batch_size=128, mode="train", data_dir="cifar10"):
+    """CIFAR-10 classification with the NAS cell of DM/problems.py:540-634: four 3x3 SAME convs (each + bias, batch
+    norm, ReLU) wired node0 -> {n0o2, node1}, node1 -> n1o3, node2 = avgpool3x3(node1) + n0o2, node3 = node2 + n1o3 +
+    node0, the mean over positions, fc 16->10 with a ReLU on the logits.  The variables are the ten of NAS_VARIABLES
+    (7,578 coordinates): weights N(0, 0.01), biases zero.  Data and batch draw as ``cifar10``."""
+    from . import cifar_data
+    num_examples = cifar_data.load_cifar10(data_dir, mode).num_examples
+
+    def build():
+        params = [get_variable(name, shape=list(shape),
+                               initializer=(random_normal_initializer(stddev=0.01) if len(shape) > 1 else
+                                            constant_initializer(0.0)))
+                  for name, shape in NAS_VARIABLES]
+        images, labels = cifar_data.device_split(data_dir, mode, params[0].device)
+        idx = torch.randint(0, num_examples, (batch_size,), device=images.device)
+        pixels = cifar_data.device_values(images.device)[images.index_select(0, idx).long()]   # fp32(p) / fp32(255)
+        pixels = pixels.reshape(-1, 3, 32, 32).permute(0, 2, 3, 1)                            # the planes, NHWC
+        return nas_forward(params, pixels, labels.index_select(0, idx), batch_norm)
+    build.producer = producers.Nas(batch_size=int(batch_size), mode=mode, data_dir=data_dir,
+                                   batch_norm=bool(batch_norm), variables=NAS_VARIABLES)
+    return build
+
+
 _PSF_PARAMS = ("I", "x", "y", "z", "sigmaxy", "sigmaz")
 
 

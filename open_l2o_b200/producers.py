@@ -11,8 +11,8 @@ from dataclasses import dataclass
 import numpy as np
 import torch
 
+from . import cifar_data, mnist_data
 from . import engine as _engine
-from .mnist_data import device_split
 
 
 def _names(records):
@@ -115,21 +115,27 @@ class Confocal(_Producer):
 
 
 @dataclass
-class _Mnist(_Producer):
-    """A fresh batch of ``batch_size`` from split ``mode`` of ``data_dir``, drawn in the kernel at every evaluation."""
+class _Minibatch(_Producer):
+    """A fresh batch of ``batch_size`` from split ``mode`` of ``data_dir``, drawn in the kernel at every evaluation
+    (l2o_philox.cuh).  ``device_split(data_dir, mode, device) -> (images, labels)`` is the dataset's loader."""
     batch_size: int
     mode: str
     data_dir: str
+    device_split = None
 
     def bind(self, prog):
         # the split on the device (uploaded once per process, never reset), the seed and the device counter of the
         # draws, and the indices each evaluation drew: row t of idx for step t, row T for the final loss
         bound = super().bind(prog)
-        bound.images, bound.labels = device_split(self.data_dir, self.mode, prog.device)
+        bound.images, bound.labels = self.device_split(self.data_dir, self.mode, prog.device)
         bound.seed = prog.opt.seed
         bound.counter = torch.zeros(1, dtype=torch.int64, device=prog.device)
         bound.idx = torch.zeros(prog.T + 1, self.batch_size, dtype=torch.int32, device=prog.device)
         return bound
+
+
+class _Mnist(_Minibatch):
+    device_split = staticmethod(mnist_data.device_split)
 
 
 @dataclass
@@ -172,4 +178,51 @@ class MnistConv(_Mnist):
         g, fx = _outputs(x)
         _engine.mnist_conv_grad(self.images, self.labels, x, g, self.batch_size, self.seed, self.counter, self.ws,
                                 f=fx, scale=scale, idx_out=self.idx[t])
+        return fx, g
+
+
+@dataclass
+class CifarConv(_Minibatch):
+    """problems.cifar10: l2o_cifar_conv_grad, when batch norm is on, it takes the batch, and the arena holds
+    ``variables`` (name, shape) in creation order."""
+    batch_norm: bool
+    variables: tuple
+    kind = "cifar_conv"
+    device_split = staticmethod(cifar_data.device_split)
+
+    def accepts(self, variables, var_slices, constants):
+        return (self.batch_norm and _engine.cifar_conv_fits(self.batch_size) and _creation_order(variables, var_slices)
+                and [(v["name"], tuple(v["shape"])) for v in variables] == list(self.variables))
+
+    def bind(self, prog):
+        bound = super().bind(prog)
+        bound.ws = torch.empty(_engine.cifar_conv_workspace_bytes(self.batch_size), dtype=torch.uint8,
+                               device=prog.device)
+        return bound
+
+    def __call__(self, x, scale, t):
+        g, fx = _outputs(x)
+        _engine.cifar_conv_grad(self.images, self.labels, x, g, self.batch_size, self.seed, self.counter, self.ws,
+                                f=fx, scale=scale, idx_out=self.idx[t])
+        return fx, g
+
+
+@dataclass
+class Nas(CifarConv):
+    """problems.nas: l2o_nas_grad, under the same conditions as CifarConv."""
+    kind = "nas"
+
+    def accepts(self, variables, var_slices, constants):
+        return (self.batch_norm and _engine.nas_fits(self.batch_size) and _creation_order(variables, var_slices)
+                and [(v["name"], tuple(v["shape"])) for v in variables] == list(self.variables))
+
+    def bind(self, prog):
+        bound = _Minibatch.bind(self, prog)
+        bound.ws = torch.empty(_engine.nas_workspace_bytes(self.batch_size), dtype=torch.uint8, device=prog.device)
+        return bound
+
+    def __call__(self, x, scale, t):
+        g, fx = _outputs(x)
+        _engine.nas_grad(self.images, self.labels, x, g, self.batch_size, self.seed, self.counter, self.ws,
+                         f=fx, scale=scale, idx_out=self.idx[t])
         return fx, g

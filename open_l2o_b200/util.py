@@ -85,9 +85,11 @@ def _cw20(path):
 _MNIST = {"mnist": ((20,), "sigmoid"), "mnist_relu": ((20,), "relu"), "mnist_deeper": ((20, 20), "sigmoid")}
 
 
-def get_config(problem_name, path=None, mode=None, num_hidden_layer=None, net_name=None, data_dir="MNIST-data"):
-    """Returns problem configuration (DM/util.py:112-265) for the synthetic problems and, from the MNIST files in
-    ``data_dir`` (never downloaded), the MNIST MLPs and ConvNet."""
+def get_config(problem_name, path=None, mode=None, num_hidden_layer=None, net_name=None, data_dir=None):
+    """Returns problem configuration (DM/util.py:112-265) for the synthetic problems and, from the dataset files in
+    ``data_dir`` (never downloaded), the MNIST MLPs and ConvNet and the CIFAR-10 ConvNet and NAS cell.  ``data_dir``
+    defaults to the directory the reference passes: "MNIST-data" for the MNIST problems, "cifar10" for cifar_conv and
+    nas."""
     net_assignments = None
     if problem_name == "simple":
         problem = problems.simple()
@@ -111,13 +113,27 @@ def get_config(problem_name, path=None, mode=None, num_hidden_layer=None, net_na
     elif problem_name in _MNIST:                  # DM/util.py:145-163
         if mode is None:
             mode = "train" if path is None else "test"
+        data_dir = "MNIST-data" if data_dir is None else data_dir
         layers, activation = _MNIST[problem_name]
         problem = problems.mnist(layers=layers, activation=activation, mode=mode, data_dir=data_dir)
         net_config = {"cw": get_default_net_config(path)}
     elif problem_name == "mnist_conv":            # DM/util.py:164-169
         if mode is None:
             mode = "train" if path is None else "test"
+        data_dir = "MNIST-data" if data_dir is None else data_dir
         problem = problems.mnist_conv(batch_norm=True, mode=mode, data_dir=data_dir)
+        net_config = {"cw": get_default_net_config(path)}
+    elif problem_name == "cifar_conv":            # DM/util.py:170-175
+        if mode is None:
+            mode = "train" if path is None else "test"
+        data_dir = "cifar10" if data_dir is None else data_dir
+        problem = problems.cifar10(batch_norm=True, mode=mode, data_dir=data_dir)
+        net_config = {"cw": get_default_net_config(path)}
+    elif problem_name == "nas":                   # DM/util.py:185-190
+        if mode is None:
+            mode = "train" if path is None else "test"
+        data_dir = "cifar10" if data_dir is None else data_dir
+        problem = problems.nas(batch_norm=True, mode=mode, data_dir=data_dir)
         net_config = {"cw": get_default_net_config(path)}
     elif problem_name == "rastrigin_separable":   # BASELINE config #5
         problem = problems.rastrigin_separable(num_dims=1000000)
