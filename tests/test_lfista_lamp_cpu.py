@@ -201,3 +201,54 @@ def test_two_state_abi_rejects_bad_arguments_without_gpu():
     assert L.l2o_ista_bwd(C.byref(_args(lista.LFISTA)), C.byref(g), None) == _lib.L2O_E_INVALID     # misaligned
     g.dW2, g.d_s2_in = None, fake + 2
     assert L.l2o_ista_bwd(C.byref(_args(lista.LAMP)), C.byref(g), None) == _lib.L2O_E_INVALID       # misaligned
+
+
+def test_exact_abi_problems_keep_every_sum_exact_in_fp32():
+    """Every exact problem of the C-ABI tests, over every layer range they run: each sum the kernels form stays below
+    2^24 units of its terms' granularity, so the kernels must reproduce the fp64 oracle bit for bit."""
+    for case in fc.EXACT2_CASES:
+        P = fc.exact_case2(case)
+        for k0, k1 in fc.RANGES2:
+            assert fc.exact_bound2(P, k0, k1) < 2 ** 24, (case, k0, k1)
+
+
+def test_exact_bound_counts_granularity():
+    """b_k = ||x_k||_0 / M makes LAMP's records dyadic: at M = 8 the granularity takes the bound past 2^24, where
+    the integers alone would stay far below it."""
+    P = fc.exact_problem2(lista.LAMP, 8, 5, 13, 0)
+    assert fc.exact_bound2(P) >= 2 ** 24
+    assert fc._gran(torch.tensor([3.0, -0.5, 0.25])) == 0.25 and fc._gran(torch.tensor([4.0, -0.0])) == 1.0
+
+
+@pytest.mark.parametrize("form,share_W", [(lista.LFISTA, False), (lista.LAMP, False), (lista.LAMP, True)])
+@pytest.mark.parametrize("a,b", fc.SPLITS2)
+def test_abi_oracle_three_way_split_composes_to_the_full_pass(form, share_W, a, b):
+    """oracle2 over [0, a), [a, b), [b, K) chained through x_in / s2_in forward and d_xk / d_s2 backward is the full
+    pass in fp64: records, d_x_in, d_s2_in and every gradient (the per-layer ones from the pass that runs the layer,
+    a shared W or We as the sum of the parts)."""
+    P = fc.generic_problem2(form, 9, 14, 5, share_W, seed=1)
+    g = torch.Generator().manual_seed(3)
+    P["x_in"] = 0.1 * torch.randn(P["B"], P["N"], generator=g)
+    P["s2_in"] = 0.1 * torch.randn(P["B"], fc._s2_width(P), generator=g)
+    P["d_s2"] = torch.randn(P["B"], fc._s2_width(P), generator=g)
+    full = fc.oracle2(P)
+    lo_f = fc.oracle2(P, 0, a, d_xk=None)
+    x_a, s_a = lo_f["xs"][-1], fc.s2_after(P, lo_f, P["x_in"])
+    mid_f = fc.oracle2(P, a, b, x_in=x_a, s2_in=s_a, d_xk=None)
+    x_b, s_b = mid_f["xs"][-1], fc.s2_after(P, mid_f, x_a)
+    hi = fc.oracle2(P, b, fc.K2, x_in=x_b, s2_in=s_b)
+    mid = fc.oracle2(P, a, b, x_in=x_a, s2_in=s_a, d_xk=hi["d_x_in"], d_s2=hi["d_s2_in"])
+    lo = fc.oracle2(P, 0, a, d_xk=mid["d_x_in"], d_s2=mid["d_s2_in"])
+    close = lambda u, v: torch.allclose(u, v, rtol=1e-12, atol=1e-12 * float(v.abs().max()))
+    for key in ("xs", "zs", "rs", "rowrec"):
+        if full[key] is not None:
+            assert close(torch.cat([lo[key], mid[key], hi[key]]), full[key]), key
+    assert close(lo["d_x_in"], full["d_x_in"]) and close(lo["d_s2_in"], full["d_s2_in"])
+    assert hi["d_s2_in"].abs().max() > 0      # the carry between passes is not trivially zero
+    for key in ("dW", "dW2", "dB1", "dtheta", "dstep"):
+        if full[key] is not None:
+            assert close(lo[key] + mid[key] + hi[key], full[key]), key
+    for key in ("dtheta", "dstep"):
+        if full[key] is not None:
+            for part, k0, k1 in ((lo, 0, a), (mid, a, b), (hi, b, fc.K2)):
+                assert not part[key][[k for k in range(fc.K2) if not k0 <= k < k1]].any(), (key, k0)
