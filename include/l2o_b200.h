@@ -849,7 +849,9 @@ int l2o_minimax_bwd(const l2o_minimax_args* a, const l2o_minimax_grads* g, void*
  * range for the family (matrix families: rows == n; BOWL and the 2-D functions: n == 2; DEPENDENCY_CHAIN,
  * OUTWARD_SNAKE: n >= 2), NORM with p0 <= 0.  L2O_E_UNSUPPORTED: n > L2O_ZOO_MAX_N.
  * The non-smooth points follow TensorFlow's gradients: sign(0) = 0 for |.|, sqrt'(0) = inf (Ackley at the origin,
- * OUTWARD_SNAKE at x = 0 give NaN), ties of min / max share the gradient evenly. */
+ * OUTWARD_SNAKE at x = 0 give NaN), ties of min / max share the gradient evenly.
+ * NORM at a residual r_i = 0 exactly: d sign / dr = 0, so row i adds no curvature (its H v and Hessian-form weight is 0).
+ * RASTRIGIN at a residual r_i = 0 exactly: tf.norm's r / |r| is NaN, so every entry of df/dx, H v, q and dq/dx is NaN. */
 #define L2O_ZOO_MAX_N 4096
 #define L2O_ZOO_QUADRATIC 0
 #define L2O_ZOO_LASSO 1

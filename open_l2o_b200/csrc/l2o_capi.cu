@@ -5,6 +5,7 @@
 #include <cmath>
 #include <cstdio>
 #include <map>
+#include <mutex>
 #include <new>
 #include <tuple>
 #include <utility>
@@ -76,8 +77,12 @@ int device_sms(const char* fn) {
   return sms;
 }
 
+// The limit belongs to the function in the device's context, which every host thread shares (torch's autograd calls
+// in from its device threads), so the record of it is one per process, under a lock.
 static int raise_smem_limit_on(const char* fn, int dev, const void* kernel, size_t smem) {
-  static thread_local std::map<std::pair<const void*, int>, size_t> limit;
+  static std::mutex mu;
+  static std::map<std::pair<const void*, int>, size_t> limit;
+  std::lock_guard<std::mutex> lock(mu);
   size_t& lim = limit[{kernel, dev}];
   if (smem <= lim) return L2O_OK;
   L2O_CUDA_TRY(fn, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

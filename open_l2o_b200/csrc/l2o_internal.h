@@ -32,9 +32,9 @@ namespace l2o {
 // l2o_last_cuda_error as "<fn>: <CUDA call>: <error string>" and returns L2O_E_CUDA.
 int set_cuda_error(cudaError_t e, const char* fn, const char* call);
 int device_sms(const char* fn);   // SM count of the current device (cached), 0 on failure
-// Raises kernel's dynamic shared-memory limit on the current device to at least smem.  Each thread remembers the
-// highest limit it set per kernel and device, so the limit is only ever raised: a lower one would break the
-// launches another thread sized for a higher one.
+// Raises kernel's dynamic shared-memory limit on the current device to at least smem.  The process remembers the
+// highest limit set per kernel and device, whichever thread set it, so the limit is only ever raised: a lower one
+// would break the launches another thread sized for a higher one.
 int raise_smem_limit(const char* fn, const void* kernel, size_t smem);
 // raise_smem_limit, then grid = min(ceil(n / block), occupancy x SMs) for (kernel, block, smem), the resident CTAs
 // cached per kernel, device, block and smem on each thread.  L2O_E_UNSUPPORTED when not one CTA fits on an SM.

@@ -308,7 +308,7 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(kThreads) zoo_kerne
   if (FORM && kind == kMatrix) {
     // pass 1: du_k = A_i.u_k, dv_k = A_i.v_k; q's row term P_i = sum_k du_k dv_k (NORM: the per-CTA sums S, B.P and
     // Wu_k = sum_i w_i du_k, Wv_k in this warp's slots of red, the row weights w, b, c P)
-    const bool norm = fam == L2O_ZOO_NORM;
+    const bool norm = fam == L2O_ZOO_NORM, rdot = norm || fam == L2O_ZOO_RASTRIGIN;   // rdot: needs A_i.x
     for (int t = tid; t < kWarps * kRed; t += kThreads) red[t] = 0.0;
     __syncthreads();
     double s[2] = {0.0, 0.0};
@@ -322,7 +322,7 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(kThreads) zoo_kerne
         for (int q = 0; q < kTile; ++q) du[q] = dv[q] = 0.0;
         for (int j = lane; j < n; j += 32) {
           const double u = (double)row[j];
-          if (norm && q0 == 0) ax = fma(u, (double)xs[j], ax);
+          if (rdot && q0 == 0) ax = fma(u, (double)xs[j], ax);
 #pragma unroll
           for (int q = 0; q < kTile; ++q) {
             if (q0 + q < K) {
@@ -343,18 +343,22 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(kThreads) zoo_kerne
             P = fma(du[q], dv[q], P);
           }
         }
-        if (!norm) continue;
-        if (q0 == 0) {
+        if (rdot && q0 == 0) {
 #pragma unroll
           for (int o = 16; o > 0; o >>= 1) ax += __shfl_xor_sync(0xffffffffu, ax, o);
           const double r = ax - (double)a.y[i];
-          const double ab = fabs(r) + 1e-6;   // |diff| + EPSILON
-          const double sg = r > 0.0 ? 1.0 : (r < 0.0 ? -1.0 : 0.0);
-          w = pow(ab, (double)p - 1.0) * sg;
-          b = pow(ab, (double)p - 2.0);
-          c = pow(ab, (double)p - 3.0) * sg;
-          s[0] += pow(ab, (double)p);
+          if (norm) {
+            const double ab = fabs(r) + 1e-6;   // |diff| + EPSILON
+            const double sg = r > 0.0 ? 1.0 : (r < 0.0 ? -1.0 : 0.0);
+            w = pow(ab, (double)p - 1.0) * sg;
+            b = pow(ab, (double)p - 2.0) * sg * sg;   // d sign / dr = 0: no curvature at r = 0
+            c = pow(ab, (double)p - 3.0) * sg;
+            s[0] += pow(ab, (double)p);
+          } else if (r == 0.0) {
+            P = __longlong_as_double(0x7ff8000000000000ll);   // as in H v: NaN through S0 into q and every out[j]
+          }
         }
+        if (!norm) continue;
         if (lane == 0) {
 #pragma unroll
           for (int q = 0; q < kTile; ++q) {
@@ -443,7 +447,7 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(kThreads) zoo_kerne
           u1 = (float)w;
           s[0] += pow(ab, (double)p);
           if (HVP) {
-            u2 = (float)(pow(ab, (double)p - 2.0) * av);
+            u2 = (float)(pow(ab, (double)p - 2.0) * sg * sg * av);   // d sign / dr = 0: no curvature at r = 0
             s[1] += w * av;
           }
         } else {
@@ -675,7 +679,7 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(kThreads) zoo_kerne
         const double cj = (double)a.c[j], ph = 2.0 * kPi * x;
         if (FORM) {
           const double P = pair_dot(fa, j);
-          o = -(double)p * 8.0 * kPi * kPi * kPi * cj * sin(ph) * P;
+          o = isnan(S0) ? S0 : -(double)p * 8.0 * kPi * kPi * kPi * cj * sin(ph) * P;   // S0 NaN: a zero residual
           t = (double)p * 4.0 * kPi * kPi * cj * cos(ph) * P;
           break;
         }

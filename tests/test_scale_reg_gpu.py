@@ -3,7 +3,6 @@ launch counts; the regularisers inside the five trainers' meta-gradients, kernel
 and scale_metarun with ``--reg_optimizer``."""
 import math
 
-import numpy as np
 import pytest
 import torch
 
@@ -11,6 +10,7 @@ from open_l2o_b200 import _lib
 from open_l2o_b200 import scale_zoo as Z
 from oracle import scale_reg_oracle as O
 from tests.test_scale_zoo_gpu import CASES, DATA_CASES
+from tests.zoo_cases import data_batch
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -67,9 +67,11 @@ def _tol(cls, kwargs):
 
 
 LARGE = [("Quadratic", (4096,), {}), ("Norm", (4096,), {"norm_power": 3.}), ("Rastrigin", (1024,), {})]
+# one Hessian-form case per family and size: LARGE's Norm(4096) at p = 3 stands for CASES' at p = 1.5
+FORM_CASES = [c for c in CASES if (c[0], c[1]) not in [(l[0], l[1]) for l in LARGE]] + LARGE
 
 
-@pytest.mark.parametrize("cls,args,kwargs", CASES + LARGE, ids=["%s%s" % (c, a) for c, a, _ in CASES + LARGE])
+@pytest.mark.parametrize("cls,args,kwargs", FORM_CASES, ids=["%s%s" % (c, a) for c, a, _ in FORM_CASES])
 def test_hess_form_matches_fp64_triple_autograd(cls, args, kwargs):
     for seed in (0, 1):
         problem = getattr(Z, cls)(*args, random_seed=seed, **kwargs) if cls != "IsotropicQuadratic" else \
@@ -81,11 +83,7 @@ def test_hess_form_matches_fp64_triple_autograd(cls, args, kwargs):
 def test_hess_form_data_families(cls, n, batch):
     for seed in (0, 1):
         problem = getattr(Z, cls)(n, random_seed=seed)
-        gen = np.random.RandomState(seed)
-        ds = Z.random_binary(n, batch, random_seed=seed) if cls == "OutwardSnake" else \
-            Z.random_symmetric(n, batch, random_seed=seed)
-        data = torch.as_tensor(ds.data[gen.permutation(batch)]).to(DEV)
-        _check(problem, cls, seed, data)
+        _check(problem, cls, seed, data_batch(cls, n, batch, seed).to(DEV))
 
 
 def test_hess_form_chunks_pairs_above_the_limit():

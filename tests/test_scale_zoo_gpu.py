@@ -8,6 +8,7 @@ import pytest
 import torch
 
 from open_l2o_b200 import scale_zoo as Z
+from tests.zoo_cases import BOUNDARY_CASES, BOUNDARY_DATA, DATA_FAMILIES, data_batch
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -57,7 +58,8 @@ CASES = ([("Quadratic", (n,), {}) for n in (1, 20, 100, 300, 2048)]
          + [("DependencyChain", (n,), {}) for n in (1, 20, 1000)]
          + [("MinMaxWell", (n,), {}) for n in (2, 64, 1000)]
          + [(c, (), {}) for c in ("Rosenbrock", "Saddle", "LogSumExp", "Ackley", "Beale", "Booth", "StyblinskiTang",
-                                  "Matyas", "Branin", "Michalewicz")])
+                                  "Matyas", "Branin", "Michalewicz")]
+         + BOUNDARY_CASES)
 
 
 @pytest.mark.parametrize("cls,args,kwargs", CASES, ids=["%s%s" % (c, a) for c, a, _ in CASES])
@@ -68,19 +70,14 @@ def test_analytic_family_matches_fp64_autograd(cls, args, kwargs):
         _check(problem, seed)
 
 
-DATA_CASES = [(c, n, b) for c in ("ProjectionQuadratic", "SumOfQuadratics", "OutwardSnake")
-              for n, b in ((12, 10), (64, 128), (300, 300))]
+DATA_CASES = [(c, n, b) for c in DATA_FAMILIES for n, b in [(12, 10), (64, 128), (300, 300)] + BOUNDARY_DATA]
 
 
 @pytest.mark.parametrize("cls,n,batch", DATA_CASES)
 def test_data_family_matches_fp64_autograd(cls, n, batch):
     for seed in SEEDS:
         problem = getattr(Z, cls)(n, random_seed=seed)
-        gen = np.random.RandomState(seed)
-        ds = Z.random_binary(n, batch, random_seed=seed) if cls == "OutwardSnake" else \
-            Z.random_symmetric(n, batch, random_seed=seed)
-        data = torch.as_tensor(ds.data[gen.permutation(batch)]).to(DEV)
-        _check(problem, seed, data)
+        _check(problem, seed, data_batch(cls, n, batch, seed).to(DEV))
 
 
 def test_wrappers_over_kernel_families():
