@@ -339,8 +339,8 @@ __global__ void __launch_bounds__(kTile) unroll_fwd_kernel(l2o_unroll_args a, Ne
 // ------------------------------------------------------------------------------------------
 // K3: BPTT.  Reverse-time sweep; gates recomputed from the checkpointed (h, c); per-coordinate
 // vectors staged to shared memory so the CTA can reduce dW = X^T dZ over its 128 coordinates with
-// a (row-group x col-group) thread tiling whose accumulators persist (in smem slots) over all
-// steps and tiles; flushed once per CTA with fp64 atomics.
+// a (row-group x col-group) thread tiling whose accumulators persist (in smem slots) over the
+// tile's steps; flushed once per tile with fp64 atomics.
 // ------------------------------------------------------------------------------------------
 __host__ __device__ constexpr int conflict_free_stride(int x) {  // multiple of 4 whose quarter is odd => float4 rows of
   int s = round4(x);                          // consecutive threads hit disjoint bank groups
@@ -389,7 +389,7 @@ __device__ __forceinline__ void dw_pass(const float* __restrict__ sIN, const flo
 
 // rows 0..KR-2 -> W[row][col] (row-major, NC columns) ; row KR-1 -> bias[col]
 template <int KR, int NC>
-__device__ __forceinline__ void dw_flush(const float* sAcc, double* __restrict__ dtheta, int o_w, int o_b, int tid) {
+__device__ __forceinline__ void dw_flush(float* sAcc, double* __restrict__ dtheta, int o_w, int o_b, int tid) {
   using G = PassGeom<KR, NC>;
   if (tid >= G::RG * G::NCG) return;
   const int r = tid / G::NCG, q = tid % G::NCG;
@@ -401,9 +401,10 @@ __device__ __forceinline__ void dw_flush(const float* sAcc, double* __restrict__
     for (int j = 0; j < 4; ++j) {
       const int col = 4 * q + j;
       if (col >= NC) continue;
-      const float v = sAcc[(rr * 4 + j) * kTile + tid];
+      float& v = sAcc[(rr * 4 + j) * kTile + tid];   // this thread's own accumulator (dw_pass's ownership)
       const int idx = (row < KR - 1) ? o_w + row * NC + col : o_b + col;
       atomicAdd(&dtheta[idx], (double)v);
+      v = 0.f;
     }
   }
 }
@@ -765,12 +766,13 @@ __global__ void __launch_bounds__(kTile) unroll_bwd_kernel(l2o_bwd_args a, NetRt
         cy.lam[i] = lam;
       }
     }
+    // drain the tile's accumulators (and zero them for the next tile): an fp32 sum over every tile a CTA walks was
+    // 1.2e-4 of the lstm_1 input rows' max-norm off the fp64 oracle at 270K coordinates and T = 100
+    if constexpr (C::H1 > 0) dw_flush<B::KR1, cmax(C::G1, 4)>(sACC + B::ACC1 * kTile, a.dtheta, C::O_W1, C::O_B1, tid);
+    if constexpr (C::H2 > 0) dw_flush<B::KR2, cmax(C::G2, 4)>(sACC + B::ACC2 * kTile, a.dtheta, C::O_W2, C::O_B2, tid);
+    dw_flush<B::KRO, 1>(sACC + B::ACCO * kTile, a.dtheta, C::O_WO, C::O_BO, tid);
+    if constexpr (C::FC) dw_flush<B::KRF, cmax(C::F, 4)>(sACC + B::ACCF * kTile, a.dtheta, C::O_WIN, C::O_BIN, tid);
   }
-  // flush the CTA's accumulators
-  if constexpr (C::H1 > 0) dw_flush<B::KR1, cmax(C::G1, 4)>(sACC + B::ACC1 * kTile, a.dtheta, C::O_W1, C::O_B1, tid);
-  if constexpr (C::H2 > 0) dw_flush<B::KR2, cmax(C::G2, 4)>(sACC + B::ACC2 * kTile, a.dtheta, C::O_W2, C::O_B2, tid);
-  dw_flush<B::KRO, 1>(sACC + B::ACCO * kTile, a.dtheta, C::O_WO, C::O_BO, tid);
-  if constexpr (C::FC) dw_flush<B::KRF, cmax(C::F, 4)>(sACC + B::ACCF * kTile, a.dtheta, C::O_WIN, C::O_BIN, tid);
 }
 
 }  // namespace l2o

@@ -9,8 +9,9 @@
 //             Both layers share ONE 64 x 80 accumulator: the operand rows of layer 2 ([h1n | h2p] in rows 0..39, 1 in
 //             row 63) and of layer 1 ([h1p | feature chunk] in rows 40..62) are disjoint (dw_row), and each layer's
 //             staged X^T keeps the other layer's rows at zero, so the two K = 64 contractions add into disjoint
-//             accumulator rows.  The accumulators are drained into the fp64 dtheta after every tile (bounded fp32
-//             accumulation length).  Both operands are staged as packed bf16 pairs with stmatrix (stage_x, stage_dz).
+//             accumulator rows.  The accumulators are drained every kDrainSteps steps into the warpgroup's fp32
+//             partial sums in global memory (round-to-nearest, see kDrainSteps), which go into the fp64 dtheta once,
+//             at the end of the kernel.  Both operands are staged as packed bf16 pairs with stmatrix (stage_x, stage_dz).
 // DM nets take the checkpoint rows from a shared-memory ring that TMA bulk copies fill one layer phase ahead (CkRing).
 // fc(20) nets (RNNProp) run the two layers as two passes over time (MODE 1: layer 2, exporting dX2[h1n] to the
 // caller's hand-over buffer; MODE 2: layer 1 with the fc layer's own gradient), DM nets both layers in one pass (MODE 0).
@@ -35,6 +36,15 @@ constexpr uint32_t kXbBytes = 8 * kXbLBO;
 // dW accumulator rows: 8-row blocks 0..4 hold layer 2 (MODE 2: layer 1's [h1p | e]), 5..7 layer 1 of DM nets (MODE 0),
 // row 63 the constant 1 of the blocks 0..4 operand (dw_row)
 constexpr int kBlkL1 = 5, kRowOne2 = 63;
+// The tensor cores' fp32 accumulation does not round to nearest, so the error of a wgmma accumulator grows with the
+// number of batches added into it rather than with its square root: accumulated over a whole 100-step tile, the identity
+// net's gate blocks of dtheta were up to 1.0e-4 of their max-norm off the fp64 oracle at 270K coordinates
+// (tests/test_dm_scale_gpu.py).  So every kDrainSteps steps each thread adds its accumulators into its own fp32 partial
+// sums (kDwPartFloats per warpgroup, [value][thread] so that a warp's adds are coalesced; red.add rounds to nearest) and
+// zeroes them; the partials reach the fp64 dtheta once per kernel, which takes far fewer fp64 atomics than a drain into
+// dtheta per tile.
+constexpr int kDrainSteps = 10;
+constexpr int kDwPartFloats = 128 * (kN / 2);
 
 // x = hi + lo for a pair of values (v0 in the low half): hi = bf16_rn(x), lo = bf16_rn(x - hi)
 __device__ __forceinline__ void split_bf16x2(float v0, float v1, uint32_t& hi, uint32_t& lo) {
@@ -144,7 +154,7 @@ constexpr int kFlImit = 1, kFlTanh = 2;
 // full, so the body tests no rows.
 template <class C, int MODE, bool CARRY, int FL, bool FULL>
 __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args a, NetRt rt, const float* __restrict__ img,
-                                                                    l2o_bwd_carry cy) {
+                                                                    float* __restrict__ dw_part, l2o_bwd_carry cy) {
   using G = Geo<C>;
   static_assert(MODE == 0 ? !C::FC : C::FC, "DM nets: one pass; fc nets: two passes");
   static_assert(MODE != 0 || C::F < 3, "the feature chunk leaves quad thread 3's slot of row 63 to layer 2's 1");
@@ -313,19 +323,16 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
     wg_commit();
     wg_wait<1>();   // dX done; the dW batch may still run (the next wait<0> retires it)
   };
-  auto flush_dw = [&]() {
+  // this thread's fp32 partial sums of its accumulator values (kDrainSteps): value k at part[128 k]
+  float* const part = dw_part + ((int64_t)blockIdx.x * kBwdWG + wg) * kDwPartFloats + (threadIdx.x & 127);
+#pragma unroll
+  for (int k = 0; k < kN / 2; ++k) atomicExch(part + 128 * k, 0.f);
+  auto drain_dw = [&]() {
     wg_wait<0>();
 #pragma unroll
-    for (int rh = 0; rh < 2; ++rh) {
-      const int r = dw_row<C, MODE>(kx + 8 * rh);
-#pragma unroll
-      for (int j = 0; j < kN / 8; ++j)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          float& v = dw[4 * j + 2 * rh + e];
-          if (r >= 0 && v != 0.f) atomicAdd(&a.dtheta[r + gate_ref_col(8 * j + 2 * q + e)], (double)v);
-          v = 0.f;
-        }
+    for (int k = 0; k < kN / 2; ++k) {
+      if (dw[k] != 0.f) atomicAdd(part + 128 * k, dw[k]);
+      dw[k] = 0.f;
     }
   };
 
@@ -365,7 +372,10 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
     A.template put<(G::ColOne & ~3)>(0, q == (G::ColOne & 3) ? 1.0f : 0.f);
     A.template put<(G::ColOne & ~3)>(1, q == (G::ColOne & 3) ? 1.0f : 0.f);
 
-    for (int t = T - 1; t >= 0; --t) {
+    // the dW accumulators are drained after every kDrainSteps steps, counted from the segment's end (so one sweep and
+    // a single carry segment group the sums alike), and after the tile's last step
+    for (int t_end = T; t_end > 0; t_end -= kDrainSteps) {
+    for (int t = t_end - 1; t >= 0 && t >= t_end - kDrainSteps; --t) {
       const float* ckr = ckt + kx * kH;   // this thread's row r0 of slot t (row r0 + 8 at + 8 kH)
       float z[kN / 2];
       float dh1n[2][kU];
@@ -561,6 +571,8 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
       ckt -= slot;
       tn -= n;
     }
+    drain_dw();
+    }
     if constexpr (CARRY) {
 #pragma unroll
       for (int rh = 0; rh < 2; ++rh) {
@@ -577,9 +589,20 @@ __global__ void __launch_bounds__(kBwdThreads, 1) unroll_bwd_kernel(l2o_bwd_args
         }
       }
     }
-    flush_dw();
   }
   wg_wait<0>();
+  // the partial sums into the fp64 dtheta (an atomic read: it follows this thread's adds to the same address)
+#pragma unroll
+  for (int rh = 0; rh < 2; ++rh) {
+    const int r = dw_row<C, MODE>(kx + 8 * rh);
+#pragma unroll
+    for (int j = 0; j < kN / 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const float v = atomicExch(part + 128 * (4 * j + 2 * rh + e), 0.f);
+        if (r >= 0 && v != 0.f) atomicAdd(&a.dtheta[r + gate_ref_col(8 * j + 2 * q + e)], (double)v);
+      }
+  }
   // ---- output layer (layer-2 passes) and fc layer (MODE 2) gradients: per-thread sums over the warp's rows -----------
   auto red8 = [&](float v) {   // sum over the 8 lanes with the same q
 #pragma unroll
@@ -621,7 +644,7 @@ int tc_launch_bwd(const char* fn, const NetRt& rt, const l2o_bwd_args& a, float*
   auto launch = [&](auto kern, size_t smem) {
     if (smem > 227 * 1024) return L2O_E_INVALID;
     if (int rc = raise_smem_limit(fn, kern, smem)) return rc;
-    kern<<<grid, tcb::kBwdThreads, smem, st>>>(a, rt, img, cy);
+    kern<<<grid, tcb::kBwdThreads, smem, st>>>(a, rt, img, img + tc::kImgMaxFloats, cy);
     return after_launch(fn);
   };
   // the layer-2 pass's instantiation for the output-layer flags of these arguments

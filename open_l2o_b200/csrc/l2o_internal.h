@@ -22,7 +22,7 @@ struct l2o_net {
   int64_t n_theta;
   int64_t state_floats;
   l2o::NetRt rt;
-  float* tc_img;   // device-side weight image of the tensor-core engine (owned; lazily allocated)
+  float* tc_img;   // device-side weight image of the tensor-core engine, then its BPTT dW partials (owned; lazy)
   int tc_img_dev;
   int tc_img_mode; // what the image currently holds: -1 nothing, 0 forward layout, 1 BPTT layout
 };

@@ -52,7 +52,12 @@ static int ensure_image(l2o_net* h, const char* fn) {
           break;
         }
     }
-    if (h->tc_img == nullptr) L2O_CUDA_TRY(fn, cudaMalloc(&h->tc_img, tc::kImgMaxFloats * sizeof(float)));
+    // the weight image, then the BPTT's fp32 dW partial sums: kDwPartFloats per warpgroup of a grid of at most one CTA
+    // per SM (the same size for every buffer of one device's free list)
+    const int sms = device_sms(fn);
+    if (sms <= 0) return L2O_E_CUDA;
+    const size_t floats = tc::kImgMaxFloats + (size_t)sms * tcb::kBwdWG * tcb::kDwPartFloats;
+    if (h->tc_img == nullptr) L2O_CUDA_TRY(fn, cudaMalloc(&h->tc_img, floats * sizeof(float)));
     h->tc_img_dev = dev;
     h->tc_img_mode = -1;
   }

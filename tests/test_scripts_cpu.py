@@ -50,7 +50,7 @@ def functions(t):
 def test_script_list():
     assert "measure" in NAMES and "tc_ab" in NAMES
     assert CHECKERS <= set(NAMES)
-    assert set(WITH_CLI) >= set(PROFILES) - {"tc_accuracy", "tc_accuracy_large"}
+    assert set(WITH_CLI) >= set(PROFILES) - {"tc_accuracy"}
 
 
 @pytest.mark.parametrize("name", IMPORTABLE)

@@ -3,10 +3,10 @@ forward's, and MetaOptimizer with forced segment lengths against the unsegmented
 
 The per-coordinate arithmetic of a chain of segments is the whole sweep's: the carried adjoint state and lambda pass
 through HBM exactly, and lambda keeps the summation order of one sweep.  So the carries a chain hands on are bitwise
-those of one sweep.  dtheta is not bitwise: both engines sum dW over a CTA's steps in fp32 before the fp64 atomics
-(the exact-fp32 engine in shared memory over the whole launch, the tensor-core engine per 64-coordinate tile), and a
-segment boundary ends such a sum early.  dtheta is therefore compared at DTHETA_TOL; a single segment with a zero carry
-groups every sum as l2o_unroll_bwd does and is compared at fp64-atomic reordering level."""
+those of one sweep.  dtheta is not bitwise: both engines sum dW in fp32 before the fp64 atomics (the exact-fp32 engine
+in shared memory per 128-coordinate tile, the tensor-core engine over the launch, in partial sums it feeds every 10 steps
+counted from the segment's end), and a segment boundary ends such a sum early.  dtheta is therefore compared at DTHETA_TOL; a single segment with a zero carry groups every sum as l2o_unroll_bwd does and is
+compared at fp64-atomic reordering level."""
 import numpy as np
 import pytest
 import torch
